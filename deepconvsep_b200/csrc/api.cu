@@ -63,9 +63,22 @@ int ensure_smem_attr_impl(const void* kernel, int bytes) {
   return DCS_OK;
 }
 
-int upload(const std::vector<float>& h, float** d) {
+int upload(const std::vector<float>& h, float** d, std::vector<void*>* owned) {
   DCS_CUDA(cudaMalloc((void**)d, h.size() * sizeof(float)));
+  if (owned) owned->push_back(*d);
   DCS_CUDA(cudaMemcpy(*d, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice));
+  return DCS_OK;
+}
+
+bool shape_is(const int64_t* s, int nd, int want_nd, int64_t a, int64_t b, int64_t c, int64_t d) {
+  return nd == want_nd && s[0] == a && s[1] == b && s[2] == c && s[3] == d;
+}
+
+int ensure_layout(dcs_ctx* ctx, NetSlot slot, size_t bytes, uint64_t sig, cudaStream_t st) {
+  bool grew = false;
+  DCS_TRY(ctx->net[slot].ensure(bytes, st, &grew));
+  if (!grew && ctx->net_sig[slot] != sig) DCS_CUDA(cudaMemsetAsync(ctx->net[slot].p, 0, ctx->net[slot].cap, st));
+  ctx->net_sig[slot] = sig;
   return DCS_OK;
 }
 
@@ -73,11 +86,10 @@ int upload(const std::vector<float>& h, float** d) {
 
 using namespace dcs;
 
-int64_t dcs_ctx::workspace_bytes() const {
-  size_t s = audio.cap + X.cap + mag.cap + S.cap + stems.cap + pcm_in.cap + pcm_out.cap + pcm_in2[0].cap + pcm_in2[1].cap +
-             pcm_out2[0].cap + pcm_out2[1].cap;
-  for (const auto& b : net) s += b.cap;
-  return (int64_t)s;
+// every device buffer of a context's workspace
+template <class Ctx, class F> static void for_each_buffer(Ctx* c, F f) {
+  for (auto* b : {&c->audio, &c->X, &c->mag, &c->S, &c->stems, &c->pcm_in[0], &c->pcm_in[1], &c->pcm_out[0], &c->pcm_out[1]}) f(*b);
+  for (auto& b : c->net) f(b);
 }
 
 extern "C" {
@@ -105,8 +117,6 @@ int dcs_create(int device, dcs_ctx** out) {
   c->num_sms = prop.multiProcessorCount;
   const char* dbg = getenv("DCS_DEBUG_SIMT_GEMM");
   c->debug_simt_gemm = dbg && dbg[0] == '1';
-  const char* sf = getenv("DCS_DEBUG_SMEM_FFT");
-  c->debug_smem_fft = sf && sf[0] == '1';
   *out = c;
   return DCS_OK;
 }
@@ -114,11 +124,8 @@ int dcs_create(int device, dcs_ctx** out) {
 int dcs_destroy(dcs_ctx* c) {
   if (!c) return DCS_OK;
   cudaSetDevice(c->device);
-  c->audio.release(); c->X.release(); c->mag.release(); c->S.release(); c->stems.release();
-  c->pcm_in.release(); c->pcm_out.release();
-  for (auto& b : c->net) b.release();
+  for_each_buffer(c, [](DevBuf& b) { b.release(); });
   for (int i = 0; i < 2; ++i) {
-    c->pcm_in2[i].release(); c->pcm_out2[i].release();
     if (c->ev_in[i]) cudaEventDestroy(c->ev_in[i]);
     if (c->ev_dec[i]) cudaEventDestroy(c->ev_dec[i]);
     if (c->ev_enc[i]) cudaEventDestroy(c->ev_enc[i]);
@@ -130,7 +137,11 @@ int dcs_destroy(dcs_ctx* c) {
   return DCS_OK;
 }
 
-int64_t dcs_workspace_bytes(const dcs_ctx* c) { return c ? c->workspace_bytes() : 0; }
+int64_t dcs_workspace_bytes(const dcs_ctx* c) {
+  int64_t s = 0;
+  if (c) for_each_buffer(c, [&s](const DevBuf& b) { s += (int64_t)b.cap; });
+  return s;
+}
 int64_t dcs_launch_count(const dcs_ctx* c) { return c ? c->launches : 0; }
 
 int dcs_set_spectrum_tap(dcs_ctx* c, dcs_complex* d_S, int64_t capacity) {
@@ -267,19 +278,13 @@ int dcs_model_nsources(const dcs_model* m) { return m ? m->nsrc : 0; }
 
 int dcs_model_destroy(dcs_model* m) {
   if (!m) return DCS_OK;
-  for (float* d : m->dev) cudaFree(d);
-  for (auto& w : m->sc.tW) tc_weight_destroy(&w);
-  tc_weight_destroy(&m->tW1f); tc_weight_destroy(&m->tW2c); tc_weight_destroy(&m->tWfc);
-  tc_weight_destroy(&m->tWdec); tc_weight_destroy(&m->tWt2);
+  for (void* d : m->dev) cudaFree(d);
   delete m;
   return DCS_OK;
 }
 
-static bool shape_is(const int64_t* s, int nd, int want_nd, int64_t a, int64_t b = 1, int64_t c = 1, int64_t d = 1) {
-  return nd == want_nd && s[0] == a && s[1] == b && s[2] == c && s[3] == d;
-}
-
 static int model_create_dsd(dcs_model* m, int nparams, const float* const* hp, const int64_t* shp, const int* nd) {
+  dcs_dsd& ds = m->dsd;
   const int F = m->F, tc = m->tc;
   // DSD100 / hiphopss: 1 input channel, 128-wide bottleneck, 3 decoders feeding 4 outputs
   // (separate_dsd.py:196-231); stereo / ILD: 2 input channels, 256-wide bottleneck, one decoder per
@@ -287,7 +292,7 @@ static int model_create_dsd(dcs_model* m, int nparams, const float* const* hp, c
   const bool ild = m->arch == DCS_ARCH_DSD_ILD;
   const int nch = ild ? 2 : 1, ndec = ild ? 4 : 3, nfc = ild ? 256 : 128, nout = 4 * nch;
   const int C1 = 50, C2 = 50, kh2 = tc / 2, h2 = tc - kh2 + 1, flat = C2 * h2;
-  m->C1 = C1; m->C2 = C2; m->kh2 = kh2; m->h2 = h2; m->nfc = nfc; m->ndec = ndec; m->nsrc = 4; m->nch = nch;
+  ds.C1 = C1; ds.C2 = C2; ds.kh2 = kh2; ds.h2 = h2; ds.nfc = nfc; ds.ndec = ndec; m->nsrc = 4; m->nch = nch;
   const int want = 8 + 2 * ndec + 1;
   if (nparams != want) { set_error("this DSD model needs %d parameter arrays, got %d (SURVEY.md App. A.4)", want, nparams); return DCS_EMODEL; }
   bool ok = shape_is(shp + 0, nd[0], 4, C1, nch, 1, F) && shape_is(shp + 4, nd[1], 1, C1) &&
@@ -299,13 +304,13 @@ static int model_create_dsd(dcs_model* m, int nparams, const float* const* hp, c
     ok = ok && shape_is(shp + 4 * (8 + 2 * d), nd[8 + 2 * d], 2, nfc, flat) && shape_is(shp + 4 * (9 + 2 * d), nd[9 + 2 * d], 1, flat);
   if (!ok) { set_error("DSD parameter shapes do not match feat_size=%d time_context=%d", F, tc); return DCS_EMODEL; }
   const int64_t ldf = dcs_padded_bins(2 * (F - 1));
-  m->ldw = ldf;
+  ds.ldw = ldf;
   const float *W1 = hp[0], *W2 = hp[3], *Wfc = hp[6];
   // channel pitch of the activation buffers: 52 floats, so that every row and every time step starts
   // on a 16-byte boundary (what the TMA-fed GEMM needs); the K index of each weight follows the
   // same pitch with zero rows at the two pad channels
   const int C1p = (C1 + 3) / 4 * 4, C2p = (C2 + 3) / 4 * 4, flatp = C2p * h2;
-  m->C1p = C1p; m->C2p = C2p;
+  ds.C1p = C1p; ds.C2p = C2p;
   // W1f: conv1 as a GEMM weight, K index = ch * F + bin; W1t: its transpose per input channel for K3
   std::vector<float> W1f((size_t)nch * ldf * C1, 0.f), W1t((size_t)nch * C1 * ldf, 0.f), b1(C1), W2c((size_t)kh2 * C1p * C2, 0.f),
       Wt2((size_t)kh2 * C2p * C1, 0.f), b2(C2), Wfcp((size_t)flatp * nfc, 0.f), Wdec((size_t)nfc * ndec * flatp, 0.f),
@@ -344,17 +349,14 @@ static int model_create_dsd(dcs_model* m, int nparams, const float* const* hp, c
   for (int ch = 0; ch < nch; ++ch)
     for (int sidx = 0; sidx < 4; ++sidx) bout[(size_t)ch * 4 + sidx] = hp[want - 1][sidx * nch + ch];
   struct { const std::vector<float>* h; float** d; } ups[] = {
-      {&W1f, &m->W1f}, {&b1, &m->b1}, {&W2c, &m->W2c}, {&b2, &m->b2}, {&Wfcp, &m->Wfc}, {&bfc, &m->bfc},
-      {&Wdec, &m->Wdec}, {&bdec, &m->bdec}, {&Wt2, &m->Wt2}, {&W1t, &m->W1t}, {&bout, &m->bout}};
-  for (auto& u : ups) {
-    DCS_TRY(upload(*u.h, u.d));
-    m->dev.push_back(*u.d);
-  }
-  DCS_TRY(tc_weight_create(W1f.data(), C1, nch * F, C1, &m->tW1f));
-  DCS_TRY(tc_weight_create(W2c.data(), C2, kh2 * C1p, C2, &m->tW2c));
-  DCS_TRY(tc_weight_create(Wfcp.data(), nfc, flatp, nfc, &m->tWfc));
-  DCS_TRY(tc_weight_create(Wdec.data(), ndec * flatp, nfc, ndec * flatp, &m->tWdec));
-  DCS_TRY(tc_weight_create(Wt2.data(), C1, kh2 * C2p, C1, &m->tWt2));
+      {&W1f, &ds.W1f}, {&b1, &ds.b1}, {&W2c, &ds.W2c}, {&b2, &ds.b2}, {&Wfcp, &ds.Wfc}, {&bfc, &ds.bfc},
+      {&Wdec, &ds.Wdec}, {&bdec, &ds.bdec}, {&Wt2, &ds.Wt2}, {&W1t, &ds.W1t}, {&bout, &ds.bout}};
+  for (auto& u : ups) DCS_TRY(upload(*u.h, u.d, &m->dev));
+  DCS_TRY(tc_weight_create(W1f.data(), C1, nch * F, C1, &ds.tW1f, &m->dev));
+  DCS_TRY(tc_weight_create(W2c.data(), C2, kh2 * C1p, C2, &ds.tW2c, &m->dev));
+  DCS_TRY(tc_weight_create(Wfcp.data(), nfc, flatp, nfc, &ds.tWfc, &m->dev));
+  DCS_TRY(tc_weight_create(Wdec.data(), ndec * flatp, nfc, ndec * flatp, &ds.tWdec, &m->dev));
+  DCS_TRY(tc_weight_create(Wt2.data(), C1, kh2 * C2p, C1, &ds.tWt2, &m->dev));
   return DCS_OK;
 }
 
@@ -390,64 +392,58 @@ static int run_gemm(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStre
   return ctx->debug_simt_gemm ? launch_gemm(ctx, d, st) : launch_gemm_tc(ctx, d, w, st);
 }
 
-// d_mag / d_X: nch planes [T][ldf] (plane strides mag_plane / x_plane; nch = 1: the DSD100 net);
-// d_S: masked spectra, plane (s * nch + ch) at (s * nch + ch) * src_stride
-static int dsd_forward(dcs_ctx* ctx, dcs_model* m, const float* d_mag, int64_t mag_plane, const float2* d_X, int64_t x_plane,
-                       int64_t T, int64_t ldf, int overlap, int patcher, float2* d_S, int64_t src_stride, cudaStream_t st) {
-  const int tc = m->tc, step = tc - overlap, C1 = m->C1, C2 = m->C2, kh2 = m->kh2, h2 = m->h2, nfc = m->nfc;
-  const int C1p = m->C1p, C2p = m->C2p;   // channel pitch of H1 / H2 / the padded decoder activations
-  const int nch = m->nch, ndec = m->ndec;
-  const int64_t P = dcs_num_patches(T, tc, overlap, patcher);
-  if (P == 0) {  // clip shorter than one patch: nothing is predicted, every stem is silence
-    for (int s = 0; s < m->nsrc * nch; ++s) DCS_CUDA(cudaMemsetAsync(d_S + s * src_stride, 0, (size_t)T * ldf * sizeof(float2), st));
-    return DCS_OK;
-  }
+// the DSD layer sequence: n.in holds nch magnitude planes (nch = 1: the DSD100 net); masked spectra plane
+// (s * nch + ch) at (s * nch + ch) * n.src_stride
+static int dsd_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaStream_t st) {
+  const dcs_dsd& ds = m->dsd;
+  const int tc = m->tc, step = n.step, C1 = ds.C1, C2 = ds.C2, kh2 = ds.kh2, h2 = ds.h2, nfc = ds.nfc;
+  const int C1p = ds.C1p, C2p = ds.C2p;   // channel pitch of H1 / H2 / the padded decoder activations
+  const int nch = m->nch, ndec = ds.ndec;
+  const int64_t T = n.T, ldf = n.ldf, P = n.P, Tp = n.Tp;
   DCS_REQUIRE(P * ndec * tc < (int64_t)1 << 31, "clip too long (%lld patches)", (long long)P);
-  const int64_t Tp = std::max<int64_t>(T, (P - 1) * step + tc);
   const int HP = h2 + 2 * (kh2 - 1), ldg = (C1 + 3) / 4 * 4;
-  DevBuf &bH1 = ctx->net[0], &bH2 = ctx->net[1], &bz = ctx->net[2], &bap = ctx->net[3], &bG = ctx->net[4];
-  const uint64_t sig = ((uint64_t)(m->arch + 1) << 48) ^ ((uint64_t)m->F << 24) ^ (uint64_t)(tc * 64);
   // zero on (re)allocation or layout change; afterwards only the interior (rows and the C of the
   // Cp channels) is ever written, so the zero padding persists
-  DCS_TRY(ensure_layout(ctx, 0, (size_t)Tp * C1p * 4, sig, st));
-  DCS_TRY(ensure_layout(ctx, 1, (size_t)(Tp - kh2 + 1) * C2p * 4, sig, st));
-  DCS_TRY(ensure_layout(ctx, 2, (size_t)P * nfc * 4, sig, st));
-  DCS_TRY(ensure_layout(ctx, 3, (size_t)P * ndec * HP * C2p * 4, sig, st));
+  DCS_TRY(ensure_layout(ctx, NET_H1, (size_t)Tp * C1p * 4, n.sig, st));
+  DCS_TRY(ensure_layout(ctx, NET_H2, (size_t)(Tp - kh2 + 1) * C2p * 4, n.sig, st));
+  DCS_TRY(ensure_layout(ctx, NET_Z, (size_t)P * nfc * 4, n.sig, st));
+  DCS_TRY(ensure_layout(ctx, NET_APAD, (size_t)P * ndec * HP * C2p * 4, n.sig, st));
   // G: the transposed conv2 output, patch-major [P][ndec][tc][ldg]
-  DCS_TRY(ensure_layout(ctx, 4, (size_t)P * ndec * tc * ldg * 4, sig, st));
-  float *H1 = bH1.as<float>(), *H2 = bH2.as<float>(), *z = bz.as<float>(), *ap = bap.as<float>(), *G = bG.as<float>();
+  DCS_TRY(ensure_layout(ctx, NET_G, (size_t)P * ndec * tc * ldg * 4, n.sig, st));
+  float *H1 = ctx->net[NET_H1].as<float>(), *H2 = ctx->net[NET_H2].as<float>(), *z = ctx->net[NET_Z].as<float>();
+  float *ap = ctx->net[NET_APAD].as<float>(), *G = ctx->net[NET_G].as<float>();
 
   // conv1 + both biases, once per frame (kernel height 1): H1[Tp][C1] = mag[T][nch x F] * W1f
-  GemmDesc g1 = gemm_plain(d_mag, ldf, m->W1f, C1, m->b1, H1, C1p, (int)Tp, C1, nch * m->F, 0);
-  if (nch > 1) { g1.k_seg = m->F; g1.k_ss = mag_plane; }   // one K segment per input channel plane
+  GemmDesc g1 = gemm_plain(n.in, ldf, ds.W1f, C1, ds.b1, H1, C1p, (int)Tp, C1, nch * m->F, 0);
+  if (nch > 1) { g1.k_seg = m->F; g1.k_ss = n.in_plane; }   // one K segment per input channel plane
   g1.a_valid_rows = (int)T;  // util patcher: frames beyond T are zero input
-  { ProfScope ps(ctx, "enc_conv1_gemm", st); DCS_TRY(run_gemm(ctx, g1, m->tW1f, st)); }
+  { ProfScope ps(ctx, "enc_conv1_gemm", st); DCS_TRY(run_gemm(ctx, g1, ds.tW1f, st)); }
   // conv2 + both biases, once per frame offset: rows overlap in H1 (stride C1p, length kh2*C1p)
-  GemmDesc g2 = gemm_plain(H1, C1p, m->W2c, C2, m->b2, H2, C2p, (int)(Tp - kh2 + 1), C2, kh2 * C1p, 0);
-  { ProfScope ps(ctx, "enc_conv2_gemm", st); DCS_TRY(run_gemm(ctx, g2, m->tW2c, st)); }
+  GemmDesc g2 = gemm_plain(H1, C1p, ds.W2c, C2, ds.b2, H2, C2p, (int)(Tp - kh2 + 1), C2, kh2 * C1p, 0);
+  { ProfScope ps(ctx, "enc_conv2_gemm", st); DCS_TRY(run_gemm(ctx, g2, ds.tW2c, st)); }
   // bottleneck: patch k reads H2 rows k*step .. k*step+h2-1 (contiguous h2*C2p floats)
-  GemmDesc g3 = gemm_plain(H2, (int64_t)step * C2p, m->Wfc, nfc, m->bfc, z, nfc, (int)P, nfc, h2 * C2p, 1);
-  { ProfScope ps(ctx, "bottleneck_gemm", st); DCS_TRY(run_gemm(ctx, g3, m->tWfc, st)); }
+  GemmDesc g3 = gemm_plain(H2, (int64_t)step * C2p, ds.Wfc, nfc, ds.bfc, z, nfc, (int)P, nfc, h2 * C2p, 1);
+  { ProfScope ps(ctx, "bottleneck_gemm", st); DCS_TRY(run_gemm(ctx, g3, ds.tWfc, st)); }
   // the decoder dense layers side by side, scattered into the zero-padded buffer
-  GemmDesc g4 = gemm_plain(z, nfc, m->Wdec, ndec * h2 * C2p, m->bdec, ap, (int64_t)ndec * HP * C2p, (int)P, ndec * h2 * C2p, nfc, 1);
+  GemmDesc g4 = gemm_plain(z, nfc, ds.Wdec, ndec * h2 * C2p, ds.bdec, ap, (int64_t)ndec * HP * C2p, (int)P, ndec * h2 * C2p, nfc, 1);
   g4.n_seg = h2 * C2p; g4.n_ss = (int64_t)HP * C2p; g4.c_col0 = (int64_t)(kh2 - 1) * C2p;
-  { ProfScope ps(ctx, "dec_dense_gemm", st); DCS_TRY(run_gemm(ctx, g4, m->tWdec, st)); }
+  { ProfScope ps(ctx, "dec_dense_gemm", st); DCS_TRY(run_gemm(ctx, g4, ds.tWdec, st)); }
   // InverseLayer(conv2): full correlation on the padded activations, rows (k, d, u)
   // Rows are ordered (u, k, d) -- u-major -- so that a 128-row tile holds one output position
   // u and can skip the taps that only see the zero padding (on average 8 of the 15).
-  GemmDesc g5 = gemm_plain(ap, 0, m->Wt2, C1, nullptr, G, ldg, (int)(P * ndec * tc), C1, kh2 * C2p, 0);
+  GemmDesc g5 = gemm_plain(ap, 0, ds.Wt2, C1, nullptr, G, ldg, (int)(P * ndec * tc), C1, kh2 * C2p, 0);
   g5.m_inner = (int)(P * ndec); g5.a_so = C2p; g5.a_si = (int64_t)HP * C2p;
   g5.cm_inner = (int)(P * ndec); g5.c_so = ldg; g5.c_si = (int64_t)tc * ldg;
   g5.kc_rows = (int)(P * ndec); g5.kc_unit = C2p; g5.kc_pad = kh2 - 1; g5.kc_n = h2; g5.kc_taps = kh2;
-  { ProfScope ps(ctx, "dec_convT2_gemm", st); DCS_TRY(run_gemm(ctx, g5, m->tWt2, st)); }
+  { ProfScope ps(ctx, "dec_convT2_gemm", st); DCS_TRY(run_gemm(ctx, g5, ds.tWt2, st)); }
   // InverseLayer(conv1) + bias + ReLU + mask + cross-fade + phase; the stereo net: once per channel
   // with that channel's conv1 weights, output biases and mixture STFT (trainCNN_ILD_DSD100.py:183-186)
   ProfScope ps(ctx, "dec_convT1_mask_xfade", st);
   for (int ch = 0; ch < nch; ++ch) {
     DsdMaskArgs a;
-    a.G = G; a.ldg = ldg; a.W1t = m->W1t + (int64_t)ch * C1 * m->ldw; a.ldw = (int)m->ldw; a.bout = m->bout + 4 * ch;
-    a.X = d_X + ch * x_plane; a.S = d_S + ch * src_stride;
-    a.ldf = ldf; a.src_stride = nch * src_stride; a.T = (int)T; a.P = (int)P; a.tc = tc; a.overlap = overlap; a.F = m->F;
+    a.G = G; a.ldg = ldg; a.W1t = ds.W1t + (int64_t)ch * C1 * ds.ldw; a.ldw = (int)ds.ldw; a.bout = ds.bout + 4 * ch;
+    a.X = n.X + ch * n.x_plane; a.S = n.S + ch * n.src_stride;
+    a.ldf = ldf; a.src_stride = nch * n.src_stride; a.T = (int)T; a.P = (int)P; a.tc = tc; a.overlap = n.overlap; a.F = m->F;
     a.ndec = ndec;
     if (!ctx->debug_simt_gemm && (tc + step - 1) / step <= 6) {
       DCS_REQUIRE(dsd_mask_tc_supported(a), "dsd_forward: tensor-core mask kernel does not take this shape");
@@ -459,65 +455,121 @@ static int dsd_forward(dcs_ctx* ctx, dcs_model* m, const float* d_mag, int64_t m
   return DCS_OK;
 }
 
-int dcs_separate_spec(dcs_ctx* ctx, dcs_model* m, const float* d_mag, const dcs_complex* d_X, int64_t T, int64_t ldf,
-                      int overlap, int patcher, dcs_complex* d_S, int64_t src_stride, void* stream) {
-  DCS_REQUIRE(ctx && m && d_mag && d_X && d_S, "dcs_separate_spec: NULL argument");
-  DCS_REQUIRE(T > 0 && ldf >= m->F && src_stride >= T * ldf, "dcs_separate_spec: bad shape");
+// the network stage of every entry point: the input planes (plane stride in_plane) and the mixture STFT
+// (channel stride x_plane) -> masked spectra, nsrc x nch planes of stride src_stride
+static int run_network(dcs_ctx* ctx, const dcs_model* m, const float* in, int64_t in_plane, const float2* X, int64_t x_plane,
+                       int64_t T, int64_t ldf, int overlap, int patcher, float2* S, int64_t src_stride, cudaStream_t st) {
+  const bool dsd = m->arch == DCS_ARCH_DSD || m->arch == DCS_ARCH_DSD_ILD;
+  NetCall n;
+  n.P = dcs_num_patches(T, m->tc, overlap, patcher);
+  if (n.P == 0) {  // clip shorter than one patch: nothing is predicted, every stem is silence
+    for (int s = 0; s < m->nsrc * m->nch; ++s) DCS_CUDA(cudaMemsetAsync(S + s * src_stride, 0, (size_t)T * ldf * sizeof(float2), st));
+    return DCS_OK;
+  }
+  n.in = in; n.in_plane = in_plane; n.X = X; n.x_plane = x_plane; n.S = S; n.src_stride = src_stride;
+  n.T = T; n.ldf = ldf; n.overlap = overlap; n.step = m->tc - overlap;
+  n.Tp = std::max<int64_t>(T, (n.P - 1) * n.step + m->tc);
+  // the zero-padded slots are re-zeroed when the model changes; those of the 30-channel nets also when the overlap does
+  n.sig = ((uint64_t)(m->arch + 1) << 48) ^ ((uint64_t)m->F << 24) ^ (uint64_t)(m->tc * 64 + (dsd ? 0 : overlap));
+  return dsd ? dsd_forward(ctx, m, n, st) : sconv_forward(ctx, m, n, st);
+}
+
+// arch: the architecture an entry point serves, -1 for the single-channel nets
+static int check_model(const char* fn, const dcs_ctx* ctx, const dcs_model* m, int arch, int overlap, int patcher) {
+  DCS_REQUIRE(ctx && m, "%s: NULL argument", fn);
+  const bool mono = m->arch != DCS_ARCH_DSD_ILD && m->arch != DCS_ARCH_BACH10_SCORE;
+  DCS_REQUIRE(arch < 0 ? mono : m->arch == arch, "%s does not serve architecture %d: use %s", fn, m->arch,
+              m->arch == DCS_ARCH_DSD_ILD ? "dcs_separate_audio_stereo"
+              : m->arch == DCS_ARCH_BACH10_SCORE ? "dcs_separate_audio_score / dcs_separate_spec_channels"
+                                                 : "dcs_separate_audio / dcs_separate_spec");
   DCS_REQUIRE(overlap >= 0 && overlap < m->tc, "overlap %d must be in [0, time_context=%d)", overlap, m->tc);
   DCS_REQUIRE(patcher == DCS_PATCHER_STANDALONE || patcher == DCS_PATCHER_UTIL, "unknown patcher %d", patcher);
-  DCS_CUDA(cudaSetDevice(ctx->device));
-  switch (m->arch) {
-    case DCS_ARCH_DSD:
-      return dsd_forward(ctx, m, d_mag, 0, (const float2*)d_X, 0, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
-                         (cudaStream_t)stream);
-    case DCS_ARCH_DSD_ILD:
-      DCS_REQUIRE(false, "the stereo network takes two input channels: use dcs_separate_audio_stereo");
-    case DCS_ARCH_IKALA:
-    case DCS_ARCH_IKALA_NOPOOL:
-    case DCS_ARCH_BACH10:
-      return sconv_forward(ctx, m, d_mag, 0, (const float2*)d_X, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
-                           (cudaStream_t)stream);
-    case DCS_ARCH_BACH10_SCORE:
-      DCS_REQUIRE(false, "the score-informed network takes 4 input channels: use dcs_separate_spec_channels / dcs_separate_audio_score");
+  return DCS_OK;
+}
+
+// the check every clip entry point makes before it queues anything: a clip of L samples (audio planes in_stride
+// apart) into stems out_stride apart
+static int check_clip(const char* fn, const dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int arch, const void* in,
+                      const void* out, int64_t L, int64_t in_stride, int64_t out_stride, int overlap, int patcher) {
+  DCS_TRY(check_model(fn, ctx, m, arch, overlap, patcher));
+  DCS_REQUIRE(p && in && out, "%s: NULL argument", fn);
+  DCS_REQUIRE(p->N / 2 + 1 == m->F, "%s: frame size %d does not give the model's %d bins", fn, p->N, m->F);
+  DCS_REQUIRE(L > 0 && in_stride >= L && out_stride >= L, "%s: bad length / stride", fn);
+  return DCS_OK;
+}
+
+// the workspace of a clip of L samples: nch STFT planes, nsrc x nch masked spectra, the score-informed net's input
+// channels; with `staged` also the device copies of host audio and stems
+static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, bool staged, cudaStream_t st) {
+  const int64_t plane = dcs_num_frames(L, p->hop) * dcs_padded_bins(p->N);
+  DCS_TRY(ctx->X.ensure((size_t)m->nch * plane * sizeof(float2), st));
+  DCS_TRY(ctx->mag.ensure((size_t)m->nch * plane * sizeof(float), st));
+  DCS_TRY(ctx->S.ensure((size_t)m->nsrc * m->nch * plane * sizeof(float2), st));
+  if (m->arch == DCS_ARCH_BACH10_SCORE) DCS_TRY(ctx->net[NET_CHANS].ensure((size_t)m->sc.nch * plane * sizeof(float), st));
+  if (staged) {
+    DCS_TRY(ctx->audio.ensure((size_t)L * sizeof(float), st));
+    DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * L * sizeof(float), st));
   }
-  DCS_REQUIRE(false, "architecture %d has no CUDA path yet", m->arch);
+  return DCS_OK;
+}
+
+// one clip, device to device: nch audio planes (audio_stride apart) -> nsrc x nch stem planes; d_filters: the
+// score filters that form the score-informed net's input channels
+static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,
+                         const float* d_filters, float scale_factor, int overlap, int patcher, float* d_stems,
+                         int64_t stem_stride, cudaStream_t st) {
+  DCS_TRY(size_workspace(ctx, m, p, L, false, st));
+  const int nch = m->nch;
+  const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
+  float2 *X = ctx->X.as<float2>(), *S = ctx->S.as<float2>();
+  float* mag = ctx->mag.as<float>();
+  {
+    ProfScope ps(ctx, "stft_fwd", st);   // compute_transform: one STFT per channel (transform.py:105-119)
+    for (int ch = 0; ch < nch; ++ch)
+      DCS_TRY(launch_stft(p, d_audio + ch * audio_stride, L, X + ch * plane, mag + ch * plane, nullptr, scale_factor, ldf, st));
+  }
+  const float* in = mag;
+  if (d_filters) {
+    float* chans = ctx->net[NET_CHANS].as<float>();
+    ProfScope ps(ctx, "score_channels", st);
+    DCS_TRY(launch_channel_mul(ctx, mag, d_filters, chans, plane, m->sc.nch, st));
+    in = chans;
+  }
+  DCS_TRY(run_network(ctx, m, in, plane, X, plane, T, ldf, overlap, patcher, S, plane, st));
+  DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * nch * plane, st));
+  ProfScope ps(ctx, "istft_ola", st);
+  return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc * nch, T, ldf, plane, d_stems, L, stem_stride, st);
+}
+
+int dcs_separate_spec(dcs_ctx* ctx, dcs_model* m, const float* d_mag, const dcs_complex* d_X, int64_t T, int64_t ldf,
+                      int overlap, int patcher, dcs_complex* d_S, int64_t src_stride, void* stream) {
+  DCS_TRY(check_model("dcs_separate_spec", ctx, m, -1, overlap, patcher));
+  DCS_REQUIRE(d_mag && d_X && d_S, "dcs_separate_spec: NULL argument");
+  DCS_REQUIRE(T > 0 && ldf >= m->F && src_stride >= T * ldf, "dcs_separate_spec: bad shape");
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  return run_network(ctx, m, d_mag, 0, (const float2*)d_X, 0, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
+                     (cudaStream_t)stream);
 }
 
 int dcs_separate_spec_channels(dcs_ctx* ctx, dcs_model* m, const float* d_in, int64_t in_plane, const dcs_complex* d_X,
                                int64_t T, int64_t ldf, int overlap, int patcher, dcs_complex* d_S, int64_t src_stride,
                                void* stream) {
-  DCS_REQUIRE(ctx && m && d_in && d_X && d_S, "dcs_separate_spec_channels: NULL argument");
-  DCS_REQUIRE(m->arch == DCS_ARCH_BACH10_SCORE, "dcs_separate_spec_channels: architecture %d has a single input channel", m->arch);
+  DCS_TRY(check_model("dcs_separate_spec_channels", ctx, m, DCS_ARCH_BACH10_SCORE, overlap, patcher));
+  DCS_REQUIRE(d_in && d_X && d_S, "dcs_separate_spec_channels: NULL argument");
   DCS_REQUIRE(T > 0 && ldf >= m->F && src_stride >= T * ldf && in_plane >= T * ldf, "dcs_separate_spec_channels: bad shape");
-  DCS_REQUIRE(overlap >= 0 && overlap < m->tc, "overlap %d must be in [0, time_context=%d)", overlap, m->tc);
-  DCS_REQUIRE(patcher == DCS_PATCHER_STANDALONE || patcher == DCS_PATCHER_UTIL, "unknown patcher %d", patcher);
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return sconv_forward(ctx, m, d_in, in_plane, (const float2*)d_X, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
-                       (cudaStream_t)stream);
+  return run_network(ctx, m, d_in, in_plane, (const float2*)d_X, 0, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
+                     (cudaStream_t)stream);
 }
 
 int dcs_separate_audio_score(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t L, const float* d_filters,
                              float scale_factor, int overlap, int patcher, float* d_stems, int64_t stem_stride, void* stream) {
-  DCS_REQUIRE(ctx && m && p && d_audio && d_filters && d_stems, "dcs_separate_audio_score: NULL argument");
-  DCS_REQUIRE(m->arch == DCS_ARCH_BACH10_SCORE, "dcs_separate_audio_score: needs the score-informed architecture");
-  DCS_REQUIRE(L > 0 && stem_stride >= L && p->N / 2 + 1 == m->F, "dcs_separate_audio_score: bad length / frame size");
-  cudaStream_t st = (cudaStream_t)stream;
+  DCS_TRY(check_clip("dcs_separate_audio_score", ctx, m, p, DCS_ARCH_BACH10_SCORE, d_audio, d_stems, L, L, stem_stride,
+                     overlap, patcher));
+  DCS_REQUIRE(d_filters, "dcs_separate_audio_score: NULL filters");
   DCS_CUDA(cudaSetDevice(ctx->device));
-  const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
-  DCS_TRY(ctx->X.ensure((size_t)plane * sizeof(float2), st));
-  DCS_TRY(ctx->mag.ensure((size_t)plane * sizeof(float), st));
-  DCS_TRY(ctx->S.ensure((size_t)m->nsrc * plane * sizeof(float2), st));
-  DCS_TRY(ctx->net[7].ensure((size_t)4 * plane * sizeof(float), st));
-  float2* X = ctx->X.as<float2>();
-  float* mag = ctx->mag.as<float>();
-  float2* S = ctx->S.as<float2>();
-  float* chans = ctx->net[7].as<float>();
-  { ProfScope ps(ctx, "stft_fwd", st); DCS_TRY(launch_stft(p, d_audio, L, X, mag, nullptr, scale_factor, ldf, st)); }
-  { ProfScope ps(ctx, "score_channels", st); DCS_TRY(launch_channel_mul(ctx, mag, d_filters, chans, plane, 4, st)); }
-  DCS_TRY(sconv_forward(ctx, m, chans, plane, X, T, ldf, overlap, patcher, S, plane, st));
-  DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * plane, st));
-  ProfScope ps(ctx, "istft_ola", st);
-  return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc, T, ldf, plane, d_stems, L, stem_stride, st);
+  return separate_clip(ctx, m, p, d_audio, L, L, d_filters, scale_factor, overlap, patcher, d_stems, stem_stride,
+                       (cudaStream_t)stream);
 }
 
 int dcs_gemm_f32(dcs_ctx* ctx, int engine, const float* d_A, int64_t lda, const float* h_B, int64_t ldb,
@@ -560,30 +612,11 @@ int dcs_gemm_f32(dcs_ctx* ctx, int engine, const float* d_A, int64_t lda, const 
 
 int dcs_separate_audio_stereo(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,
                               float scale_factor, int overlap, int patcher, float* d_stems, int64_t stem_stride, void* stream) {
-  DCS_REQUIRE(ctx && m && p && d_audio && d_stems, "dcs_separate_audio_stereo: NULL argument");
-  DCS_REQUIRE(m->arch == DCS_ARCH_DSD_ILD, "dcs_separate_audio_stereo: needs the stereo / ILD architecture");
-  DCS_REQUIRE(L > 0 && stem_stride >= L && audio_stride >= L && p->N / 2 + 1 == m->F, "dcs_separate_audio_stereo: bad length / frame size");
-  DCS_REQUIRE(overlap >= 0 && overlap < m->tc, "overlap %d must be in [0, time_context=%d)", overlap, m->tc);
-  DCS_REQUIRE(patcher == DCS_PATCHER_STANDALONE || patcher == DCS_PATCHER_UTIL, "unknown patcher %d", patcher);
-  cudaStream_t st = (cudaStream_t)stream;
+  DCS_TRY(check_clip("dcs_separate_audio_stereo", ctx, m, p, DCS_ARCH_DSD_ILD, d_audio, d_stems, L, audio_stride, stem_stride,
+                     overlap, patcher));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  const int nch = m->nch;
-  const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
-  DCS_TRY(ctx->X.ensure((size_t)nch * plane * sizeof(float2), st));
-  DCS_TRY(ctx->mag.ensure((size_t)nch * plane * sizeof(float), st));
-  DCS_TRY(ctx->S.ensure((size_t)m->nsrc * nch * plane * sizeof(float2), st));
-  float2* X = ctx->X.as<float2>();
-  float* mag = ctx->mag.as<float>();
-  float2* S = ctx->S.as<float2>();
-  {
-    ProfScope ps(ctx, "stft_fwd", st);   // compute_transform: one STFT per channel (transform.py:105-119)
-    for (int ch = 0; ch < nch; ++ch)
-      DCS_TRY(launch_stft(p, d_audio + ch * audio_stride, L, X + ch * plane, mag + ch * plane, nullptr, scale_factor, ldf, st));
-  }
-  DCS_TRY(dsd_forward(ctx, m, mag, plane, X, plane, T, ldf, overlap, patcher, S, plane, st));
-  DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * nch * plane, st));
-  ProfScope ps(ctx, "istft_ola", st);
-  return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc * nch, T, ldf, plane, d_stems, L, stem_stride, st);
+  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
+                       (cudaStream_t)stream);
 }
 
 int dcs_xcorr_lags(dcs_ctx* ctx, const float* const* h_a, const float* const* h_b, int npairs, int64_t num_samples, int flen,
@@ -595,60 +628,32 @@ int dcs_xcorr_lags(dcs_ctx* ctx, const float* const* h_a, const float* const* h_
 
 int dcs_separate_audio(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t L, float scale_factor,
                        int overlap, int patcher, float* d_stems, int64_t stem_stride, void* stream) {
-  DCS_REQUIRE(ctx && m && p && d_audio && d_stems, "dcs_separate_audio: NULL argument");
-  DCS_REQUIRE(L > 0 && stem_stride >= L, "dcs_separate_audio: bad length");
-  DCS_REQUIRE(p->N / 2 + 1 == m->F, "frame size %d does not give the model's %d bins", p->N, m->F);
-  cudaStream_t st = (cudaStream_t)stream;
+  DCS_TRY(check_clip("dcs_separate_audio", ctx, m, p, -1, d_audio, d_stems, L, L, stem_stride, overlap, patcher));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N);
-  DCS_TRY(ctx->X.ensure((size_t)T * ldf * sizeof(float2), st));
-  DCS_TRY(ctx->mag.ensure((size_t)T * ldf * sizeof(float), st));
-  DCS_TRY(ctx->S.ensure((size_t)m->nsrc * T * ldf * sizeof(float2), st));
-  float2* X = ctx->X.as<float2>();
-  float* mag = ctx->mag.as<float>();
-  float2* S = ctx->S.as<float2>();
-  { ProfScope ps(ctx, "stft_fwd", st); DCS_TRY(launch_stft(p, d_audio, L, X, mag, nullptr, scale_factor, ldf, st)); }
-  DCS_TRY(dcs_separate_spec(ctx, m, mag, (const dcs_complex*)X, T, ldf, overlap, patcher, (dcs_complex*)S, T * ldf, stream));
-  DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * T * ldf, st));
-  ProfScope ps(ctx, "istft_ola", st);
-  return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc, T, ldf, T * ldf, d_stems, L, stem_stride, st);
+  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
+                       (cudaStream_t)stream);
 }
 
 int dcs_separate_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* h_audio, int64_t L, float scale_factor,
                       int overlap, int patcher, float* h_stems, int64_t stem_stride, void* stream) {
-  DCS_REQUIRE(ctx && m && h_audio && h_stems && L > 0 && stem_stride >= L, "dcs_separate_host: bad argument");
+  DCS_TRY(check_clip("dcs_separate_host", ctx, m, p, -1, h_audio, h_stems, L, L, stem_stride, overlap, patcher));
   cudaStream_t st = (cudaStream_t)stream;
   DCS_CUDA(cudaSetDevice(ctx->device));
-  DCS_TRY(ctx->audio.ensure((size_t)L * sizeof(float), st));
-  DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * L * sizeof(float), st));
+  DCS_TRY(size_workspace(ctx, m, p, L, true, st));
   DCS_CUDA(cudaMemcpyAsync(ctx->audio.p, h_audio, (size_t)L * sizeof(float), cudaMemcpyHostToDevice, st));
-  DCS_TRY(dcs_separate_audio(ctx, m, p, ctx->audio.as<float>(), L, scale_factor, overlap, patcher, ctx->stems.as<float>(), L, stream));
+  DCS_TRY(separate_clip(ctx, m, p, ctx->audio.as<float>(), L, L, nullptr, scale_factor, overlap, patcher, ctx->stems.as<float>(), L, st));
   DCS_CUDA(cudaMemcpy2DAsync(h_stems, (size_t)stem_stride * sizeof(float), ctx->stems.p, (size_t)L * sizeof(float),
                              (size_t)L * sizeof(float), m->nsrc, cudaMemcpyDeviceToHost, st));
   DCS_CUDA(cudaStreamSynchronize(st));
   return DCS_OK;
 }
 
+// one clip is a batch of one: the same checks, staging and kernels as every clip of dcs_separate_batch_pcm16_host
 int dcs_separate_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const int16_t* h_pcm, int64_t L, int channels,
                             int downmix, float scale_factor, int overlap, int patcher, int16_t* h_out,
                             int64_t out_stride, void* stream) {
-  DCS_REQUIRE(ctx && m && h_pcm && h_out && L > 0 && out_stride >= L, "dcs_separate_pcm16_host: bad argument");
-  DCS_REQUIRE(channels >= 1 && channels <= 8 && downmix >= 0 && downmix <= 2, "bad channels/downmix");
-  DCS_REQUIRE(downmix == 0 || channels >= 2 || channels == 1, "downmix needs two channels");
-  cudaStream_t st = (cudaStream_t)stream;
-  DCS_CUDA(cudaSetDevice(ctx->device));
-  DCS_TRY(ctx->pcm_in.ensure((size_t)L * channels * sizeof(int16_t), st));
-  DCS_TRY(ctx->pcm_out.ensure((size_t)m->nsrc * L * sizeof(int16_t), st));
-  DCS_TRY(ctx->audio.ensure((size_t)L * sizeof(float), st));
-  DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * L * sizeof(float), st));
-  DCS_CUDA(cudaMemcpyAsync(ctx->pcm_in.p, h_pcm, (size_t)L * channels * sizeof(int16_t), cudaMemcpyHostToDevice, st));
-  DCS_TRY(launch_pcm_decode(ctx, ctx->pcm_in.as<int16_t>(), L, channels, downmix, ctx->audio.as<float>(), st));
-  DCS_TRY(dcs_separate_audio(ctx, m, p, ctx->audio.as<float>(), L, scale_factor, overlap, patcher, ctx->stems.as<float>(), L, stream));
-  DCS_TRY(launch_pcm_encode(ctx, ctx->stems.as<float>(), L, m->nsrc, L, ctx->pcm_out.as<int16_t>(), L, st));
-  DCS_CUDA(cudaMemcpy2DAsync(h_out, (size_t)out_stride * sizeof(int16_t), ctx->pcm_out.p, (size_t)L * sizeof(int16_t),
-                             (size_t)L * sizeof(int16_t), m->nsrc, cudaMemcpyDeviceToHost, st));
-  DCS_CUDA(cudaStreamSynchronize(st));
-  return DCS_OK;
+  return dcs_separate_batch_pcm16_host(ctx, m, p, 1, &h_pcm, &L, channels, downmix, scale_factor, overlap, patcher, &h_out,
+                                       &out_stride, stream);
 }
 
 // Multi-clip scheduler: the clips of a batch run through ONE context as a three-stage pipeline -- H2D of clip i+1
@@ -670,19 +675,19 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, c
     const int64_t L = num_samples[i];
     // H2D of clip i: its staging buffer is free once the decode of clip i-2 has read it
     if (i >= 2) DCS_CUDA(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_dec[b], 0));
-    DCS_CUDA(cudaMemcpyAsync(ctx->pcm_in2[b].p, h_pcm[i], (size_t)L * channels * sizeof(int16_t), cudaMemcpyHostToDevice, ctx->s_h2d));
+    DCS_CUDA(cudaMemcpyAsync(ctx->pcm_in[b].p, h_pcm[i], (size_t)L * channels * sizeof(int16_t), cudaMemcpyHostToDevice, ctx->s_h2d));
     DCS_CUDA(cudaEventRecord(ctx->ev_in[b], ctx->s_h2d));
     // kernels of clip i
     DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_in[b], 0));
-    DCS_TRY(launch_pcm_decode(ctx, ctx->pcm_in2[b].as<int16_t>(), L, channels, downmix, ctx->audio.as<float>(), st));
+    DCS_TRY(launch_pcm_decode(ctx, ctx->pcm_in[b].as<int16_t>(), L, channels, downmix, ctx->audio.as<float>(), st));
     DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
-    DCS_TRY(dcs_separate_audio(ctx, m, p, ctx->audio.as<float>(), L, scale_factor, overlap, patcher, ctx->stems.as<float>(), L, (void*)st));
+    DCS_TRY(separate_clip(ctx, m, p, ctx->audio.as<float>(), L, L, nullptr, scale_factor, overlap, patcher, ctx->stems.as<float>(), L, st));
     if (i >= 2) DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_out[b], 0));     // D2H of clip i-2 has drained the output staging
-    DCS_TRY(launch_pcm_encode(ctx, ctx->stems.as<float>(), L, m->nsrc, L, ctx->pcm_out2[b].as<int16_t>(), L, st));
+    DCS_TRY(launch_pcm_encode(ctx, ctx->stems.as<float>(), L, m->nsrc, L, ctx->pcm_out[b].as<int16_t>(), L, st));
     DCS_CUDA(cudaEventRecord(ctx->ev_enc[b], st));
     // D2H of clip i
     DCS_CUDA(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_enc[b], 0));
-    DCS_CUDA(cudaMemcpy2DAsync(h_out[i], (size_t)out_strides[i] * sizeof(int16_t), ctx->pcm_out2[b].p, (size_t)L * sizeof(int16_t),
+    DCS_CUDA(cudaMemcpy2DAsync(h_out[i], (size_t)out_strides[i] * sizeof(int16_t), ctx->pcm_out[b].p, (size_t)L * sizeof(int16_t),
                                (size_t)L * sizeof(int16_t), m->nsrc, cudaMemcpyDeviceToHost, ctx->s_d2h));
     DCS_CUDA(cudaEventRecord(ctx->ev_out[b], ctx->s_d2h));
   }
@@ -695,13 +700,14 @@ int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int n
   DCS_REQUIRE(ctx && m && p && h_pcm && num_samples && h_out && out_strides && nclips >= 0, "dcs_separate_batch_pcm16_host: bad argument");
   DCS_REQUIRE(channels >= 1 && channels <= 8 && downmix >= 0 && downmix <= 2, "bad channels/downmix");
   if (nclips == 0) return DCS_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  DCS_CUDA(cudaSetDevice(ctx->device));
   int64_t Lmax = 0;
   for (int i = 0; i < nclips; ++i) {
     DCS_REQUIRE(h_pcm[i] && h_out[i] && num_samples[i] > 0 && out_strides[i] >= num_samples[i], "clip %d: bad buffer / length", i);
     Lmax = std::max(Lmax, num_samples[i]);
   }
+  DCS_TRY(check_clip("dcs_separate_batch_pcm16_host", ctx, m, p, -1, h_pcm, h_out, Lmax, Lmax, Lmax, overlap, patcher));
+  cudaStream_t st = (cudaStream_t)stream;
+  DCS_CUDA(cudaSetDevice(ctx->device));
   // each resource on its own: a call that failed half-way through this block must not leave later calls with null handles
   if (!ctx->s_h2d) DCS_CUDA(cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
   if (!ctx->s_d2h) DCS_CUDA(cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking));
@@ -713,18 +719,11 @@ int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int n
   }
   // every buffer at the size of the longest clip before the pipeline starts: a grow-only buffer that had to be
   // re-allocated mid-batch would synchronise the stream
-  for (int b = 0; b < 2; ++b) {
-    DCS_TRY(ctx->pcm_in2[b].ensure((size_t)Lmax * channels * sizeof(int16_t), st));
-    DCS_TRY(ctx->pcm_out2[b].ensure((size_t)m->nsrc * Lmax * sizeof(int16_t), st));
+  for (int b = 0; b < std::min(nclips, 2); ++b) {
+    DCS_TRY(ctx->pcm_in[b].ensure((size_t)Lmax * channels * sizeof(int16_t), st));
+    DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * Lmax * sizeof(int16_t), st));
   }
-  DCS_TRY(ctx->audio.ensure((size_t)Lmax * sizeof(float), st));
-  DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * Lmax * sizeof(float), st));
-  {
-    const int64_t T = dcs_num_frames(Lmax, p->hop), ldf = dcs_padded_bins(p->N);
-    DCS_TRY(ctx->X.ensure((size_t)T * ldf * sizeof(float2), st));
-    DCS_TRY(ctx->mag.ensure((size_t)T * ldf * sizeof(float), st));
-    DCS_TRY(ctx->S.ensure((size_t)m->nsrc * T * ldf * sizeof(float2), st));
-  }
+  DCS_TRY(size_workspace(ctx, m, p, Lmax, true, st));
   const int rc = batch_pipeline(ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, scale_factor, overlap, patcher,
                                 h_out, out_strides, st);
   // drain everything, success or not, before the host buffers go back to the caller

@@ -82,15 +82,15 @@ int launch_xcorr_lags(dcs_ctx* ctx, const float* const* h_a, const float* const*
   DCS_REQUIRE(nspans64 <= 0x7fffffff, "xcorr: signal too long");
   const int nspans = (int)nspans64;
   const size_t ptr_bytes = (size_t)npairs * sizeof(float*);
-  DCS_TRY(ctx->net[9].ensure(2 * ptr_bytes + (size_t)npairs * nlags * sizeof(double) + 16, st));
-  DCS_TRY(ctx->net[10].ensure((size_t)npairs * nspans * XC_LAGS * sizeof(double), st));
-  uint8_t* base = ctx->net[9].as<uint8_t>();
+  DCS_TRY(ctx->net[NET_XC_PTRS].ensure(2 * ptr_bytes + (size_t)npairs * nlags * sizeof(double) + 16, st));
+  DCS_TRY(ctx->net[NET_XC_PARTIAL].ensure((size_t)npairs * nspans * XC_LAGS * sizeof(double), st));
+  uint8_t* base = ctx->net[NET_XC_PTRS].as<uint8_t>();
   const float** dA = reinterpret_cast<const float**>(base);
   const float** dB = reinterpret_cast<const float**>(base + ptr_bytes);
   double* d_out = reinterpret_cast<double*>(base + (2 * ptr_bytes + 15) / 16 * 16);
   DCS_CUDA(cudaMemcpyAsync(dA, h_a, ptr_bytes, cudaMemcpyHostToDevice, st));
   DCS_CUDA(cudaMemcpyAsync(dB, h_b, ptr_bytes, cudaMemcpyHostToDevice, st));
-  double* partial = ctx->net[10].as<double>();
+  double* partial = ctx->net[NET_XC_PARTIAL].as<double>();
   xcorr_partial_kernel<<<dim3((unsigned)nspans, (unsigned)npairs), XC_THREADS, 0, st>>>(dA, dB, L, flen, partial, nspans);
   DCS_CHECK_LAUNCH();
   ctx->launches++;

@@ -53,6 +53,18 @@ struct DevBuf {
   template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
+// the context's scratch buffers beyond the clip buffers: the network's activations, the score-informed
+// channel planes and the scratch of single launchers
+enum NetSlot {
+  NET_H1, NET_H2, NET_Z, NET_APAD, NET_G,   // both families: conv1, conv2, bottleneck, padded decoder, conv2^T
+  NET_POOLED, NET_TIE,                      // max-pool net: pooled activations and tie bits
+  NET_CHANS,                                // score-informed net: the 4 input channel planes
+  NET_SPLITK,                               // split-K partial sums of the tensor-core GEMM
+  NET_XC_PTRS, NET_XC_PARTIAL,              // dcs_xcorr_lags
+  NET_XTAB,                                 // DSD mask kernel's frame table
+  NET_SLOTS
+};
+
 }  // namespace dcs
 
 struct dcs_prof_rec {
@@ -66,21 +78,19 @@ struct dcs_ctx {
   int64_t launches = 0;
   bool prof_on = false;
   bool debug_simt_gemm = false;
-  bool debug_smem_fft = false;
   std::vector<dcs_prof_rec> prof;
-  // workspace of one in-flight pipeline
-  dcs::DevBuf audio, X, mag, S, stems, pcm_in, pcm_out;
+  // workspace of one in-flight pipeline (api.cu walks every buffer for dcs_destroy / dcs_workspace_bytes)
+  dcs::DevBuf audio, X, mag, S, stems;
+  dcs::DevBuf net[dcs::NET_SLOTS];
+  uint64_t net_sig[dcs::NET_SLOTS] = {0};   // layout signature of what each net[] buffer currently holds
   // multi-clip scheduler (dcs_separate_batch_pcm16_host): copy streams, double-buffered staging, hand-over events
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
   cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_dec[2] = {nullptr, nullptr}, ev_enc[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
-  dcs::DevBuf pcm_in2[2], pcm_out2[2];
-  dcs::DevBuf net[12];
-  uint64_t net_sig[12] = {0};   // layout signature of what each net[] buffer currently holds
+  dcs::DevBuf pcm_in[2], pcm_out[2];
   float2* tap = nullptr;        // dcs_set_spectrum_tap: copy of the masked spectra the iSTFT consumed
   int64_t tap_cap = 0;
   uint8_t* pool_tap = nullptr;  // dcs_set_pool_tap: copy of the max-pool tie bits of the forward pass
   int64_t pool_tap_cap = 0;
-  int64_t workspace_bytes() const;
 };
 
 struct dcs_stft {
@@ -118,33 +128,48 @@ struct TcWeight {
 }  // namespace dcs
 
 // ---- model (device-resident network)
+struct dcs_dsd {     // DSD100 / hiphopss and the stereo / ILD net
+  int C1, C2, kh2, h2, nfc, ndec;
+  int C1p, C2p;   // channel pitch of the activation buffers (multiple of 4 floats)
+  int64_t ldw;
+  float *W1f, *b1, *W2c, *b2, *Wfc, *bfc, *Wdec, *bdec, *Wt2, *W1t, *bout;   // W1t is [nch][C1][ldw], bout [nch][4]
+  // tensor-core copies of the GEMM weights (K-major, 3xTF32 split)
+  dcs::TcWeight tW1f, tW2c, tWfc, tWdec, tWt2;
+};
 struct dcs_sconv {   // strided-conv1 families: iKala (pool / no pool), Bach10
-  int nch, sw1, J, pool, WP, kh2, kw2, h2, w2, HP, WPP, ndec, nfc, rule;
+  int nch, sw1, J, pool, WP, kh2, kw2, h2, w2, HP, WPP, ndec, nfc, rule;   // nch: input planes of the network
   dcs::TcWeight tW[8];                 // 0 conv1, 1 conv2, 2 fc, 3 convT2, 4.. decoder dense layers
   float *b1, *b2, *bfc, *bdec[4], *bout, *Wsc;
 };
 struct dcs_model {
   dcs_ctx* ctx;
   int arch, F, tc, nsrc;
-  // DSD dims
-  int C1, C2, kh2, h2, nfc, ndec;
-  int C1p, C2p;   // channel pitch of the activation buffers (multiple of 4 floats)
-  int nch = 1;    // input channels (2: stereo / ILD net); W1t is [nch][C1][ldw], bout [nch][4]
-  int64_t ldw;
-  std::vector<float*> dev;  // owned device arrays
-  float *W1f, *b1, *W2c, *b2, *Wfc, *bfc, *Wdec, *bdec, *Wt2, *W1t, *bout;
-  // tensor-core copies of the GEMM weights (K-major, 3xTF32 split)
-  dcs::TcWeight tW1f, tW2c, tWfc, tWdec, tWt2;
+  int nch = 1;    // audio channels of a clip; the stems are nsrc x nch planes (2: stereo / ILD net)
+  dcs_dsd dsd;
   dcs_sconv sc;
+  std::vector<void*> dev;   // every device allocation of the model, tensor-core weights included
 };
 namespace dcs {
-int upload(const std::vector<float>& h, float** d);
+// owned: a list the allocation is recorded in (a model's, which dcs_model_destroy frees)
+int upload(const std::vector<float>& h, float** d, std::vector<void*>* owned = nullptr);
 int model_create_sconv(dcs_model* m, int nparams, const float* const* hp, const int64_t* shp, const int* nd);
-// d_in: nch planes [T][ldf] (plane stride in_plane elements; nch = 1: the scaled magnitude)
-int sconv_forward(dcs_ctx* ctx, dcs_model* m, const float* d_in, int64_t in_plane, const float2* d_X, int64_t T, int64_t ldf,
-                  int overlap, int patcher, float2* d_S, int64_t src_stride, cudaStream_t st);
-// (re)zero a workspace buffer whenever what it holds changes layout: zero padding is relied upon
-int ensure_layout(dcs_ctx* ctx, int idx, size_t bytes, uint64_t sig, cudaStream_t st);
+bool shape_is(const int64_t* s, int nd, int want_nd, int64_t a, int64_t b = 1, int64_t c = 1, int64_t d = 1);
+
+// one call of the network stage (run_network, api.cu): the network's input planes [T][ldf] (plane c at
+// in + c * in_plane), the mixture STFT (channel c at X + c * x_plane) -> the masked spectra, plane p at S + p * src_stride
+struct NetCall {
+  const float* in; int64_t in_plane;
+  const float2* X; int64_t x_plane;
+  float2* S; int64_t src_stride;
+  int64_t T, ldf;
+  int64_t P, Tp;    // patches (> 0) and the frames they span
+  int overlap, step;
+  uint64_t sig;     // layout signature of the zero-padded slots for this model and overlap
+};
+// the layer sequence of the 30-channel nets (DSD's: api.cu)
+int sconv_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaStream_t st);
+// (re)zero a workspace slot whenever what it holds changes layout: zero padding is relied upon
+int ensure_layout(dcs_ctx* ctx, NetSlot slot, size_t bytes, uint64_t sig, cudaStream_t st);
 }  // namespace dcs
 
 // ---- kernel launchers (each returns a DCS_* code) ---------------------------------------------
@@ -156,7 +181,6 @@ int launch_istft(dcs_stft* plan, const float2* d_S, const float* d_mag, const fl
                  float polar_scale, int nsrc, int64_t T, int64_t ldf, int64_t src_stride, float* d_out,
                  int64_t Lout, int64_t out_stride, cudaStream_t st);
 
-bool stft_reg_supported(int N);
 int launch_stft_reg(dcs_stft* plan, const float* d_audio, int64_t L, float2* d_X, float* d_mag, float* d_phase,
                     float mag_scale, int64_t ldf, int64_t nframes, cudaStream_t st);
 bool istft_reg_supported(const dcs_stft* plan, const float* d_out, int64_t out_stride);
@@ -192,7 +216,7 @@ GemmDesc gemm_plain(const float* A, int64_t lda, const float* B, int64_t ldb, co
                     int64_t ldc, int M, int N, int K, int relu);
 int launch_gemm(dcs_ctx* ctx, const GemmDesc& d, cudaStream_t st);
 
-int tc_weight_create(const float* B_rowmajor, int64_t ldb, int K, int N, TcWeight* out);
+int tc_weight_create(const float* B_rowmajor, int64_t ldb, int K, int N, TcWeight* out, std::vector<void*>* owned = nullptr);
 void tc_weight_destroy(TcWeight* w);
 int launch_gemm_tc(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStream_t st);
 

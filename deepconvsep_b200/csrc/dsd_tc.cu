@@ -243,8 +243,8 @@ static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t
   const int gpc = (num_groups + chunks - 1) / chunks;
   dim3 grid((unsigned)m_tiles, (unsigned)((num_groups + gpc - 1) / gpc));
   const int Tpad = num_groups * MT::FRAMES;
-  DCS_TRY(ctx->net[11].ensure((size_t)Tpad * MT_SLOTS * sizeof(float4), st));
-  float4* xtab = ctx->net[11].as<float4>();
+  DCS_TRY(ctx->net[NET_XTAB].ensure((size_t)Tpad * MT_SLOTS * sizeof(float4), st));
+  float4* xtab = ctx->net[NET_XTAB].as<float4>();
   dsd_xfade_table_kernel<<<(unsigned)ceil_div64((int64_t)Tpad * MT_SLOTS, 256), 256, 0, st>>>(xtab, a.T, Tpad, a.P, a.tc, a.overlap);
   DCS_CHECK_LAUNCH();
   ctx->launches++;

@@ -237,7 +237,7 @@ __global__ void splitk_reduce_kernel(const GemmDesc d, const float* __restrict__
 }
 
 // ---- host side ------------------------------------------------------------------------------
-int tc_weight_create(const float* B, int64_t ldb, int K, int N, TcWeight* out) {
+int tc_weight_create(const float* B, int64_t ldb, int K, int N, TcWeight* out, std::vector<void*>* owned) {
   // B[k][n] row-major (ld = ldb) -> K-major Bt[n][k], zero padded to Np x Kp, split hi/lo
   const int Kp = (K + KSTAGE - 1) / KSTAGE * KSTAGE, Np = (N + 63) / 64 * 64;  // the widest tile reads 64 rows
   std::vector<float> hi((size_t)Np * Kp, 0.f), lo((size_t)Np * Kp, 0.f);
@@ -254,6 +254,7 @@ int tc_weight_create(const float* B, int64_t ldb, int K, int N, TcWeight* out) {
     }
   out->K = K; out->N = N; out->Kp = Kp; out->Np = Np;
   DCS_CUDA(cudaMalloc((void**)&out->hi, 2 * hi.size() * sizeof(float)));   // one allocation: [hi; lo]
+  if (owned) owned->push_back(out->hi);
   out->lo = out->hi + hi.size();
   DCS_CUDA(cudaMemcpy(out->hi, hi.data(), hi.size() * sizeof(float), cudaMemcpyHostToDevice));
   DCS_CUDA(cudaMemcpy(out->lo, lo.data(), lo.size() * sizeof(float), cudaMemcpyHostToDevice));
@@ -285,8 +286,8 @@ static int launch_tc(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStr
   float* partial = nullptr;
   const int ldp = (d.N + 3) / 4 * 4;
   if (splits > 1) {
-    DCS_TRY(ctx->net[8].ensure((size_t)splits * d.M * ldp * sizeof(float), st));
-    partial = ctx->net[8].as<float>();
+    DCS_TRY(ctx->net[NET_SPLITK].ensure((size_t)splits * d.M * ldp * sizeof(float), st));
+    partial = ctx->net[NET_SPLITK].as<float>();
   }
   dim3 grid((unsigned)m_tiles, (unsigned)n_tiles, (unsigned)splits);
   if (splits > 1)

@@ -18,18 +18,6 @@
 
 namespace dcs {
 
-int ensure_layout(dcs_ctx* ctx, int idx, size_t bytes, uint64_t sig, cudaStream_t st) {
-  bool grew = false;
-  DCS_TRY(ctx->net[idx].ensure(bytes, st, &grew));
-  if (!grew && ctx->net_sig[idx] != sig) DCS_CUDA(cudaMemsetAsync(ctx->net[idx].p, 0, ctx->net[idx].cap, st));
-  ctx->net_sig[idx] = sig;
-  return DCS_OK;
-}
-
-static bool shp_is(const int64_t* s, int nd, int want_nd, int64_t a, int64_t b = 1, int64_t c = 1, int64_t d = 1) {
-  return nd == want_nd && s[0] == a && s[1] == b && s[2] == c && s[3] == d;
-}
-
 int model_create_sconv(dcs_model* m, int nparams, const float* const* hp, const int64_t* shp, const int* nd) {
   dcs_sconv& c = m->sc;
   const int F = m->F, tc = m->tc, C = 30, CP = 32, KW = 30;
@@ -59,12 +47,12 @@ int model_create_sconv(dcs_model* m, int nparams, const float* const* hp, const 
   if (!ndec_params) ndec_params = ndec;
   const int want = 8 + 2 * ndec_params + 1, nout = ndec_params * c.nch == 16 ? 16 : m->nsrc;
   if (nparams != want) { set_error("architecture %d needs %d parameter arrays, got %d", m->arch, want, nparams); return DCS_EMODEL; }
-  bool ok = shp_is(shp + 0, nd[0], 4, C, c.nch, 1, KW) && shp_is(shp + 4, nd[1], 1, C) && shp_is(shp + 8, nd[2], 1, C) &&
-            shp_is(shp + 12, nd[3], 4, C, C, kh2, kw2) && shp_is(shp + 16, nd[4], 1, C) && shp_is(shp + 20, nd[5], 1, C) &&
-            shp_is(shp + 24, nd[6], 2, flat, c.nfc) && shp_is(shp + 28, nd[7], 1, c.nfc) &&
-            shp_is(shp + 4 * (want - 1), nd[want - 1], 1, nout);
+  bool ok = shape_is(shp + 0, nd[0], 4, C, c.nch, 1, KW) && shape_is(shp + 4, nd[1], 1, C) && shape_is(shp + 8, nd[2], 1, C) &&
+            shape_is(shp + 12, nd[3], 4, C, C, kh2, kw2) && shape_is(shp + 16, nd[4], 1, C) && shape_is(shp + 20, nd[5], 1, C) &&
+            shape_is(shp + 24, nd[6], 2, flat, c.nfc) && shape_is(shp + 28, nd[7], 1, c.nfc) &&
+            shape_is(shp + 4 * (want - 1), nd[want - 1], 1, nout);
   for (int d = 0; d < ndec_params && ok; ++d)
-    ok = shp_is(shp + 4 * (8 + 2 * d), nd[8 + 2 * d], 2, c.nfc, flat) && shp_is(shp + 4 * (9 + 2 * d), nd[9 + 2 * d], 1, flat);
+    ok = shape_is(shp + 4 * (8 + 2 * d), nd[8 + 2 * d], 2, c.nfc, flat) && shape_is(shp + 4 * (9 + 2 * d), nd[9 + 2 * d], 1, flat);
   if (!ok) { set_error("parameter shapes do not match architecture %d with feat_size=%d time_context=%d", m->arch, F, tc); return DCS_EMODEL; }
 
   const float *W1 = hp[0], *W2 = hp[3], *Wfc = hp[6];
@@ -86,9 +74,9 @@ int model_create_sconv(dcs_model* m, int nparams, const float* const* hp, const 
           B2[(((size_t)(kh2 - 1 - p) * kw2 + (kw2 - 1 - q)) * CP + ci) * C + fo] = v;  // out channel fo <- in ci
           Bt2[(((size_t)p * kw2 + q) * CP + fo) * C + ci] = v;                        // InverseLayer: in fo -> out ci
         }
-  DCS_TRY(tc_weight_create(B1.data(), C, nch * KW, C, &c.tW[0]));
-  DCS_TRY(tc_weight_create(B2.data(), C, (int)K2, C, &c.tW[1]));
-  DCS_TRY(tc_weight_create(Bt2.data(), C, (int)K2, C, &c.tW[3]));
+  DCS_TRY(tc_weight_create(B1.data(), C, nch * KW, C, &c.tW[0], &m->dev));
+  DCS_TRY(tc_weight_create(B2.data(), C, (int)K2, C, &c.tW[1], &m->dev));
+  DCS_TRY(tc_weight_create(Bt2.data(), C, (int)K2, C, &c.tW[3], &m->dev));
   {  // bottleneck: rows permuted from Lasagne's (f', i, v) flattening to (i, v, f' padded to 32)
     std::vector<float> Bfc((size_t)flatp * c.nfc, 0.f);
     for (int f = 0; f < C; ++f)
@@ -96,7 +84,7 @@ int model_create_sconv(dcs_model* m, int nparams, const float* const* hp, const 
         for (int v = 0; v < w2; ++v)
           memcpy(&Bfc[(((size_t)i * w2 + v) * CP + f) * c.nfc], &Wfc[(((size_t)f * h2 + i) * w2 + v) * c.nfc],
                  c.nfc * sizeof(float));
-    DCS_TRY(tc_weight_create(Bfc.data(), c.nfc, (int)flatp, c.nfc, &c.tW[2]));
+    DCS_TRY(tc_weight_create(Bfc.data(), c.nfc, (int)flatp, c.nfc, &c.tW[2], &m->dev));
   }
   for (int d = 0; d < ndec; ++d) {  // decoder dense layers: columns permuted the same way
     const float* Wd = hp[8 + 2 * d];
@@ -109,9 +97,8 @@ int model_create_sconv(dcs_model* m, int nparams, const float* const* hp, const 
           bb[col] = bd[src];
           for (int o = 0; o < c.nfc; ++o) Bd[(size_t)o * flatp + col] = Wd[(size_t)o * flat + src];
         }
-    DCS_TRY(tc_weight_create(Bd.data(), flatp, c.nfc, (int)flatp, &c.tW[4 + d]));
-    DCS_TRY(upload(bb, &c.bdec[d]));
-    m->dev.push_back(c.bdec[d]);
+    DCS_TRY(tc_weight_create(Bd.data(), flatp, c.nfc, (int)flatp, &c.tW[4 + d], &m->dev));
+    DCS_TRY(upload(bb, &c.bdec[d], &m->dev));
   }
   // K3s filter banks (one per conv1 input channel): w[ch][dd][f][r] = W1[f][ch][KW-1-r-sw1*dd]
   const int ND = (KW + c.sw1 - 1) / c.sw1;
@@ -125,49 +112,39 @@ int model_create_sconv(dcs_model* m, int nparams, const float* const* hp, const 
         }
   std::vector<float> bfc(hp[7], hp[7] + c.nfc), bout(hp[want - 1], hp[want - 1] + m->nsrc);
   struct { const std::vector<float>* h; float** d; } ups[] = {{&b1, &c.b1}, {&b2, &c.b2}, {&bfc, &c.bfc}, {&bout, &c.bout}, {&Wsc, &c.Wsc}};
-  for (auto& u : ups) {
-    DCS_TRY(upload(*u.h, u.d));
-    m->dev.push_back(*u.d);
-  }
+  for (auto& u : ups) DCS_TRY(upload(*u.h, u.d, &m->dev));
   return DCS_OK;
 }
 
-int sconv_forward(dcs_ctx* ctx, dcs_model* m, const float* d_in, int64_t in_plane, const float2* d_X, int64_t T, int64_t ldf,
-                  int overlap, int patcher, float2* d_S, int64_t src_stride, cudaStream_t st) {
+int sconv_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaStream_t st) {
   const dcs_sconv& c = m->sc;
-  const int tc = m->tc, step = tc - overlap, CP = 32, C = 30;
+  const int tc = m->tc, step = n.step, CP = 32, C = 30;
   const int J = c.J, WP = c.WP, kh2 = c.kh2, kw2 = c.kw2, h2 = c.h2, w2 = c.w2, HP = c.HP, WPP = c.WPP, ndec = c.ndec;
-  const int64_t P = dcs_num_patches(T, tc, overlap, patcher);
-  if (P == 0) {
-    for (int s = 0; s < m->nsrc; ++s) DCS_CUDA(cudaMemsetAsync(d_S + s * src_stride, 0, (size_t)T * ldf * sizeof(float2), st));
-    return DCS_OK;
-  }
-  const int64_t Tp = std::max<int64_t>(T, (P - 1) * step + tc);
+  const int64_t T = n.T, ldf = n.ldf, P = n.P, Tp = n.Tp;
   const int64_t U = Tp - kh2 + 1;  // conv2 output rows
   DCS_REQUIRE(P * ndec * tc * WP < ((int64_t)1 << 31) && Tp * J < ((int64_t)1 << 31), "clip too long for 32-bit row indices");
-  const uint64_t sig = ((uint64_t)(m->arch + 1) << 48) ^ ((uint64_t)m->F << 24) ^ (uint64_t)(tc * 64 + overlap);
   const int64_t flatp = (int64_t)h2 * w2 * CP;
-  DCS_TRY(ensure_layout(ctx, 0, (size_t)Tp * J * CP * 4, sig, st));
-  DCS_TRY(ensure_layout(ctx, 1, (size_t)U * w2 * CP * 4, sig, st));
-  DCS_TRY(ensure_layout(ctx, 2, (size_t)P * c.nfc * 4, sig, st));
-  DCS_TRY(ensure_layout(ctx, 3, ((size_t)P * ndec * HP * WPP + kw2 + 1) * CP * 4, sig, st));
-  DCS_TRY(ensure_layout(ctx, 4, (size_t)P * ndec * tc * WP * CP * 4, sig, st));
-  float *H1 = ctx->net[0].as<float>(), *H2 = ctx->net[1].as<float>(), *z = ctx->net[2].as<float>();
-  float *ap = ctx->net[3].as<float>(), *G = ctx->net[4].as<float>();
+  DCS_TRY(ensure_layout(ctx, NET_H1, (size_t)Tp * J * CP * 4, n.sig, st));
+  DCS_TRY(ensure_layout(ctx, NET_H2, (size_t)U * w2 * CP * 4, n.sig, st));
+  DCS_TRY(ensure_layout(ctx, NET_Z, (size_t)P * c.nfc * 4, n.sig, st));
+  DCS_TRY(ensure_layout(ctx, NET_APAD, ((size_t)P * ndec * HP * WPP + kw2 + 1) * CP * 4, n.sig, st));
+  DCS_TRY(ensure_layout(ctx, NET_G, (size_t)P * ndec * tc * WP * CP * 4, n.sig, st));
+  float *H1 = ctx->net[NET_H1].as<float>(), *H2 = ctx->net[NET_H2].as<float>(), *z = ctx->net[NET_Z].as<float>();
+  float *ap = ctx->net[NET_APAD].as<float>(), *G = ctx->net[NET_G].as<float>();
   float* Hp = H1;
   uint8_t* tie = nullptr;
   if (c.pool) {
-    DCS_TRY(ensure_layout(ctx, 5, (size_t)Tp * WP * CP * 4, sig, st));
-    DCS_TRY(ensure_layout(ctx, 6, (size_t)Tp * WP * CP, sig, st));
-    Hp = ctx->net[5].as<float>();
-    tie = ctx->net[6].as<uint8_t>();
+    DCS_TRY(ensure_layout(ctx, NET_POOLED, (size_t)Tp * WP * CP * 4, n.sig, st));
+    DCS_TRY(ensure_layout(ctx, NET_TIE, (size_t)Tp * WP * CP, n.sig, st));
+    Hp = ctx->net[NET_POOLED].as<float>();
+    tie = ctx->net[NET_TIE].as<uint8_t>();
   }
 
   {  // conv1 + biases: rows (t, j) are 30-sample windows of the magnitude frame, stride sw1
     ProfScope ps(ctx, "enc_conv1_gemm", st);
-    GemmDesc g = gemm_plain(d_in, 0, nullptr, C, c.b1, H1, CP, (int)(Tp * J), C, 30 * c.nch, 0);
+    GemmDesc g = gemm_plain(n.in, 0, nullptr, C, c.b1, H1, CP, (int)(Tp * J), C, 30 * c.nch, 0);
     g.m_inner = J; g.a_so = ldf; g.a_si = c.sw1;
-    g.k_seg = 30; g.k_ss = in_plane;      // one 30-tap segment per input channel
+    g.k_seg = 30; g.k_ss = n.in_plane;      // one 30-tap segment per input channel
     g.a_valid_rows = (int)(T * J);
     DCS_TRY(launch_gemm_tc(ctx, g, c.tW[0], st));
   }
@@ -214,8 +191,8 @@ int sconv_forward(dcs_ctx* ctx, dcs_model* m, const float* d_in, int64_t in_plan
     DCS_TRY(launch_gemm_tc(ctx, g, c.tW[3], st));
   }
   SconvMaskArgs a;
-  a.arch = m->arch; a.G = G; a.tie = tie; a.W = c.Wsc; a.bout = c.bout; a.X = d_X; a.S = d_S;
-  a.ldf = ldf; a.src_stride = src_stride; a.T = (int)T; a.P = (int)P; a.tc = tc; a.overlap = overlap; a.F = m->F;
+  a.arch = m->arch; a.G = G; a.tie = tie; a.W = c.Wsc; a.bout = c.bout; a.X = n.X; a.S = n.S;
+  a.ldf = ldf; a.src_stride = n.src_stride; a.T = (int)T; a.P = (int)P; a.tc = tc; a.overlap = n.overlap; a.F = m->F;
   a.J = J; a.WP = WP;
   ProfScope ps(ctx, "dec_convT1_mask_xfade", st);
   if (!ctx->debug_simt_gemm) {

@@ -192,13 +192,11 @@ int launch_stft(dcs_stft* p, const float* d_audio, int64_t L, float2* d_X, float
   const int64_t T = dcs_num_frames(L, p->hop);
   DCS_REQUIRE(ldf >= p->N / 2 + 1, "ldf %lld < F %d", (long long)ldf, p->N / 2 + 1);
   DCS_REQUIRE(ldf - (p->N / 2 + 1) <= 16, "ldf %lld pads more than 16 columns", (long long)ldf);
-  if (stft_reg_supported(p->N) && !p->ctx->debug_smem_fft)
-    return launch_stft_reg(p, d_audio, L, d_X, d_mag, d_phase, mag_scale, ldf, T, st);
   switch (p->N) {
     case 256: return launch_stft_n<256>(p, d_audio, L, d_X, d_mag, d_phase, mag_scale, ldf, T, st);
     case 512: return launch_stft_n<512>(p, d_audio, L, d_X, d_mag, d_phase, mag_scale, ldf, T, st);
-    case 1024: return launch_stft_n<1024>(p, d_audio, L, d_X, d_mag, d_phase, mag_scale, ldf, T, st);
-    case 2048: return launch_stft_n<2048>(p, d_audio, L, d_X, d_mag, d_phase, mag_scale, ldf, T, st);
+    case 1024:
+    case 2048: return launch_stft_reg(p, d_audio, L, d_X, d_mag, d_phase, mag_scale, ldf, T, st);
     case 4096: return launch_stft_n<4096>(p, d_audio, L, d_X, d_mag, d_phase, mag_scale, ldf, T, st);
   }
   DCS_REQUIRE(false, "unsupported frame size %d", p->N);
@@ -228,7 +226,7 @@ int launch_istft(dcs_stft* p, const float2* d_S, const float* d_mag, const float
                  int64_t out_stride, cudaStream_t st) {
   DCS_REQUIRE(Lout <= (T - 1) * p->hop + p->N - p->N / 2, "num_out %lld exceeds the istft length", (long long)Lout);
   if (Lout <= 0 || nsrc <= 0) return DCS_OK;
-  if (d_S && istft_reg_supported(p, d_out, out_stride) && !p->ctx->debug_smem_fft && ldf % 2 == 0 &&
+  if (d_S && istft_reg_supported(p, d_out, out_stride) && ldf % 2 == 0 &&
       src_stride % 2 == 0 && ((uintptr_t)d_S % 16 == 0) && ldf >= (p->N / 2 + 2) / 2 * 2)
     return launch_istft_reg(p, d_S, nsrc, T, ldf, src_stride, d_out, Lout, out_stride, st);
 #define DCS_ISTFT_CASE(NN) \

@@ -12,7 +12,6 @@
 //     coalesced, and the window shifts.  No shared accumulator, no atomics: the summation order
 //     is the reference's (ascending frame index) and the result is run-to-run deterministic.
 //     N/hop - 1 halo frames are recomputed at the start of each span.
-#include <stdlib.h>
 #include "common.cuh"
 #include "fft_reg.cuh"
 
@@ -242,8 +241,6 @@ istft_reg_kernel(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int
   }
 }
 
-bool stft_reg_supported(int N) { return N == 1024 || N == 2048; }
-
 int launch_stft_reg(dcs_stft* p, const float* d_audio, int64_t L, float2* d_X, float* d_mag, float* d_phase,
                     float mag_scale, int64_t ldf, int64_t nframes, cudaStream_t st) {
   const int fpg = 4;
@@ -284,10 +281,8 @@ static int launch_istft_reg_t(dcs_stft* p, const float2* d_S, int nsrc, int64_t 
   const int hop = 64 * HS;
   const int64_t num_hops = ceil_div64(Lout, hop);
   // hops per group: as long as possible (each group recomputes N/hop-1 halo frames) while every SM
-  // still gets its resident warps: ONE full wave of equal-sized groups (DCS_DEBUG_ISTFT_WAVES=2:
-  // the earlier two-wave split)
-  static const int waves = [] { const char* e = getenv("DCS_DEBUG_ISTFT_WAVES"); return e && e[0] == '2' ? 2 : 1; }();
-  const int64_t target_groups = (int64_t)p->ctx->num_sms * (ISTFT_THREADS / 32) * (32 / T) * waves;
+  // still gets its resident warps: ONE full wave of equal-sized groups
+  const int64_t target_groups = (int64_t)p->ctx->num_sms * (ISTFT_THREADS / 32) * (32 / T);
   int64_t hpg = ceil_div64((int64_t)nsrc * num_hops, target_groups);
   if (hpg < 12) hpg = 12;
   if (hpg > 64) hpg = 64;

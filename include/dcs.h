@@ -150,7 +150,8 @@ int dcs_separate_spec_channels(dcs_ctx* ctx, dcs_model* model, const float* d_in
                                const dcs_complex* d_X, int64_t num_frames, int64_t ldf, int overlap,
                                int patcher, dcs_complex* d_S, int64_t src_stride, void* stream);
 /* whole path on device buffers: d_filters float[4][T][ldf] (ldf = dcs_padded_bins(N), pad columns
- * arbitrary), d_audio float[L] -> d_stems float[4][stem_stride] */
+ * arbitrary), d_audio float[L] -> d_stems float[4][stem_stride].  Like every separation entry point it checks
+ * its arguments (overlap in [0, time_context) included) before anything is queued. */
 int dcs_separate_audio_score(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const float* d_audio,
                              int64_t num_samples, const float* d_filters, float scale_factor, int overlap,
                              int patcher, float* d_stems, int64_t stem_stride, void* stream);
@@ -209,8 +210,9 @@ int dcs_separate_pcm16_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, cons
  * dcs_separate_pcm16_host.  h_pcm[i]: int16[num_samples[i]][channels] (pinned for real overlap), h_out[i]:
  * int16[nsrc][out_strides[i]].  Order the clips longest first if their lengths differ much (grow-only workspace).
  * Synchronises before returning -- also when it returns an error: every copy in flight has drained, so the host
- * buffers are the caller's again (outputs of clips after the failure are undefined).  Arguments are validated
- * before anything is queued (DCS_EINVAL names the offending clip). */
+ * buffers are the caller's again (outputs of clips after the failure are undefined).  Every argument is checked
+ * before anything is queued: buffers and lengths of each clip (DCS_EINVAL names the offending clip), the plan's
+ * N/2+1 against the model's bins, overlap in [0, time_context), the patcher, and a single-channel architecture. */
 int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, int nclips,
                                   const int16_t* const* h_pcm, const int64_t* num_samples, int channels, int downmix,
                                   float scale_factor, int overlap, int patcher, int16_t* const* h_out,

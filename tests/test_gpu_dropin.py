@@ -173,3 +173,51 @@ def test_batch_scheduler_matches_per_clip_calls():
         sep.separate_pcm16_batch([clips[0], np.zeros((0, 2), dtype=np.int16)])
     again = sep.separate_pcm16_batch(clips[:2])
     assert np.array_equal(again[0], want[0]) and np.array_equal(again[1], want[1])
+
+
+def test_refused_calls_queue_nothing():
+    """A call with bad arguments is refused before it queues any work: the launch count stays where it was, and the
+    context then still gives the same bits.  Covers the batch scheduler (overlap, frame size, score-informed model),
+    the mono entry point with a stereo model and the score-informed entry point with overlap = time_context."""
+    import ctypes as C
+    from deepconvsep_b200.engine import Separator, Model, Stft
+    from deepconvsep_b200._lib import DcsError, check
+    params = nets.make_synthetic_params("dsd", 513, seed=12)
+    sep = Separator(params, frame_size=1024, hop=512, window="hanning", overlap=25)
+    lib, ctx = sep.lib, sep.ctx
+    mix, _ = pipeline.synth_mixture(1.0, 61)
+    clip = np.round(mix * 30000).astype(np.int16)
+    want = sep.separate_pcm16(clip)
+    L = clip.size
+    Ls = np.array([L], dtype=np.int64)
+    out16 = np.empty((4, L), dtype=np.int16)
+    pin, pout = (C.c_void_p * 1)(clip.ctypes.data), (C.c_void_p * 1)(out16.ctypes.data)
+    stereo = Model(ctx, nets.make_synthetic_params("dsd_ild", 513, seed=3), arch="dsd_ild", feat_size=513)
+    score = Model(ctx, nets.make_synthetic_params("bach10_score", 129, seed=3), arch="bach10_score", feat_size=129)
+    plan2048, plan256 = Stft(ctx, 2048, 512, "hanning"), Stft(ctx, 256, 128, "blackmanharris")
+    dev = torch.device("cuda", ctx.device)
+    x = torch.as_tensor(mix.astype(np.float32), device=dev)
+    stems = torch.empty((8, L), dtype=torch.float32, device=dev)
+    filters = torch.zeros((4, plan256.num_frames(L), plan256.ldf), dtype=torch.float32, device=dev)
+
+    def batch(model, plan, overlap):
+        return lib.dcs_separate_batch_pcm16_host(ctx.handle, model.handle, plan.handle, 1, pin, Ls.ctypes.data, 1, 0,
+                                                 C.c_float(0.3), overlap, 0, pout, Ls.ctypes.data, None)
+
+    refused = {
+        "batch, overlap = time_context": lambda: batch(sep.model, sep.stft, sep.model.tc),
+        "batch, plan of another frame size": lambda: batch(sep.model, plan2048, 25),
+        "batch, score-informed model": lambda: batch(score, plan256, 25),
+        "audio, stereo model": lambda: lib.dcs_separate_audio(ctx.handle, stereo.handle, sep.stft.handle, x.data_ptr(), L,
+                                                              C.c_float(0.3), 25, 0, stems.data_ptr(), L, None),
+        "score, overlap = time_context": lambda: lib.dcs_separate_audio_score(
+            ctx.handle, score.handle, plan256.handle, x.data_ptr(), L, filters.data_ptr(), C.c_float(0.2), score.tc, 1,
+            stems.data_ptr(), L, None),
+    }
+    for name, call in refused.items():
+        torch.cuda.synchronize(dev)
+        n0 = ctx.launch_count()
+        with pytest.raises(DcsError):
+            check(call())
+        assert ctx.launch_count() == n0, name
+    assert np.array_equal(sep.separate_pcm16(clip), want)

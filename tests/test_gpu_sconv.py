@@ -124,6 +124,38 @@ def test_score_informed_bach10():
         sep.separate(mix)          # the single-channel entry point must refuse this architecture
 
 
+def test_separate_spec_channels_matches_audio_score():
+    """dcs_separate_spec_channels on the four channel planes (score filter x scaled magnitude) and the mixture STFT of a
+    clip gives the masked spectra dcs_separate_audio_score records for the same clip, bit for bit."""
+    from deepconvsep_b200.engine import Separator, _ptr
+    from deepconvsep_b200._lib import check
+    F, N, hop = 129, 256, 128
+    params = nets.make_synthetic_params("bach10_score", F, seed=8)
+    mix, _ = pipeline.synth_mixture(1.0, 91)
+    T = dsp.num_frames(mix.size, hop)
+    rng = np.random.default_rng(4)
+    raw = np.full((4, T, F), 1e-18, dtype=np.float32)
+    for j in range(4):
+        for _ in range(6):
+            t0, b0 = rng.integers(0, T - 40), rng.integers(1, F - 12)
+            raw[j, t0:t0 + 40, b0:b0 + 8] = 1.0
+    filters = (raw / raw.sum(axis=0)).astype(np.float32)
+    sep = Separator(params, arch="bach10_score", frame_size=N, hop=hop, window="blackmanharris", overlap=25,
+                    patcher="util", scale_factor=0.2, feat_size=F)
+    _, tapped = sep.separate_tapped(mix, filters)
+    dev, ldf = sep.stft.dev, sep.stft.ldf
+    X, mag = sep.stft.forward(torch.as_tensor(mix.astype(np.float32), device=dev), mag_scale=0.2)
+    fd = torch.zeros((4, T, ldf), dtype=torch.float32, device=dev)
+    fd[:, :, :F] = torch.as_tensor(filters, device=dev)
+    chans = (fd * mag).contiguous()
+    S = torch.empty((4, T, ldf), dtype=torch.complex64, device=dev)
+    check(sep.lib.dcs_separate_spec_channels(sep.ctx.handle, sep.model.handle, _ptr(chans), T * ldf, _ptr(X), T, ldf,
+                                             sep.overlap, sep.patcher, _ptr(S), T * ldf, None))
+    torch.cuda.synchronize(dev)
+    got = S[:, :, :F].cpu().numpy()
+    assert np.abs(tapped).max() > 0 and np.array_equal(got, tapped)
+
+
 @pytest.mark.parametrize("arch,F,N,hop,win,overlap,seconds", [("bach10", 257, 512, 256, "blackmanharris", 25, 1.5),
                                                               ("bach10_score", 129, 256, 128, "blackmanharris", 25, 1.0),
                                                               ("ikala", 513, 1024, 512, "hanning", 20, 3.0),
