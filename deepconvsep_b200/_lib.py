@@ -51,6 +51,9 @@ _SIGS = {
     "dcs_separate_batch_pcm16_host": (C.c_int, [_p, _p, _p, C.c_int, _p, _p, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _p, _p, _p]),
     "dcs_separate_pcm16_host": (C.c_int, [_p, _p, _p, _p, _i64, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int,
                                            _p, _i64, _p]),
+    "dcs_separate_audio_keep_channels": (C.c_int, [_p, _p, _p, _p, _i64, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
+    "dcs_separate_batch_pcm16_keep_channels_host": (C.c_int, [_p, _p, _p, C.c_int, _p, _p, C.c_float, C.c_int, C.c_int,
+                                                              _p, _p, _p]),
 }
 
 _lib = None

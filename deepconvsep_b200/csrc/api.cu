@@ -437,36 +437,50 @@ static int dsd_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaS
   g5.kc_rows = (int)(P * ndec); g5.kc_unit = C2p; g5.kc_pad = kh2 - 1; g5.kc_n = h2; g5.kc_taps = kh2;
   { ProfScope ps(ctx, "dec_convT2_gemm", st); DCS_TRY(run_gemm(ctx, g5, ds.tWt2, st)); }
   // InverseLayer(conv1) + bias + ReLU + mask + cross-fade + phase; the stereo net: once per channel
-  // with that channel's conv1 weights, output biases and mixture STFT (trainCNN_ILD_DSD100.py:183-186)
+  // with that channel's conv1 weights, output biases and mixture STFT (trainCNN_ILD_DSD100.py:183-186).
+  // n.nx = 2 (DSD100 net, keep-channels): the downmix's masks times the STFT of each channel, planes (s * 2 + c) --
+  // one tensor-core launch for both channels, or the FFMA kernel once per channel
   ProfScope ps(ctx, "dec_convT1_mask_xfade", st);
+  const bool tc_path = !ctx->debug_simt_gemm && (tc + step - 1) / step <= 6;   // else the FFMA kernel: > 6 patches
+  const int nplanes = nch * n.nx;                                               // per frame, cross-check
   for (int ch = 0; ch < nch; ++ch) {
     DsdMaskArgs a;
     a.G = G; a.ldg = ldg; a.W1t = ds.W1t + (int64_t)ch * C1 * ds.ldw; a.ldw = (int)ds.ldw; a.bout = ds.bout + 4 * ch;
-    a.X = n.X + ch * n.x_plane; a.S = n.S + ch * n.src_stride;
-    a.ldf = ldf; a.src_stride = nch * n.src_stride; a.T = (int)T; a.P = (int)P; a.tc = tc; a.overlap = n.overlap; a.F = m->F;
+    a.ldf = ldf; a.T = (int)T; a.P = (int)P; a.tc = tc; a.overlap = n.overlap; a.F = m->F;
     a.ndec = ndec;
-    if (!ctx->debug_simt_gemm && (tc + step - 1) / step <= 6) {
+    a.x_plane = n.x_plane;
+    if (tc_path && n.nx == 2) {
+      a.X = n.X; a.S = n.S; a.src_stride = n.src_stride; a.nx = 2;
       DCS_REQUIRE(dsd_mask_tc_supported(a), "dsd_forward: tensor-core mask kernel does not take this shape");
       DCS_TRY(launch_dsd_mask_tc(ctx, a, st));
-    } else {
-      DCS_TRY(launch_dsd_mask(ctx, a, st));   // FFMA kernel: > 6 patches per frame, cross-check
+      continue;
+    }
+    for (int c = 0; c < n.nx; ++c) {   // ch + c: the channel (nch and n.nx are never both 2)
+      a.X = n.X + (ch + c) * n.x_plane; a.S = n.S + (ch + c) * n.src_stride; a.src_stride = nplanes * n.src_stride; a.nx = 1;
+      if (tc_path) {
+        DCS_REQUIRE(dsd_mask_tc_supported(a), "dsd_forward: tensor-core mask kernel does not take this shape");
+        DCS_TRY(launch_dsd_mask_tc(ctx, a, st));
+      } else {
+        DCS_TRY(launch_dsd_mask(ctx, a, st));
+      }
     }
   }
   return DCS_OK;
 }
 
 // the network stage of every entry point: the input planes (plane stride in_plane) and the mixture STFT
-// (channel stride x_plane) -> masked spectra, nsrc x nch planes of stride src_stride
+// (channel stride x_plane) -> masked spectra, nsrc x nch planes of stride src_stride; nx = 2 (DSD100 net only): the
+// masks applied to two mixture channels, nsrc x 2 planes (source, channel)
 static int run_network(dcs_ctx* ctx, const dcs_model* m, const float* in, int64_t in_plane, const float2* X, int64_t x_plane,
-                       int64_t T, int64_t ldf, int overlap, int patcher, float2* S, int64_t src_stride, cudaStream_t st) {
+                       int nx, int64_t T, int64_t ldf, int overlap, int patcher, float2* S, int64_t src_stride, cudaStream_t st) {
   const bool dsd = m->arch == DCS_ARCH_DSD || m->arch == DCS_ARCH_DSD_ILD;
   NetCall n;
   n.P = dcs_num_patches(T, m->tc, overlap, patcher);
   if (n.P == 0) {  // clip shorter than one patch: nothing is predicted, every stem is silence
-    for (int s = 0; s < m->nsrc * m->nch; ++s) DCS_CUDA(cudaMemsetAsync(S + s * src_stride, 0, (size_t)T * ldf * sizeof(float2), st));
+    for (int s = 0; s < m->nsrc * m->nch * nx; ++s) DCS_CUDA(cudaMemsetAsync(S + s * src_stride, 0, (size_t)T * ldf * sizeof(float2), st));
     return DCS_OK;
   }
-  n.in = in; n.in_plane = in_plane; n.X = X; n.x_plane = x_plane; n.S = S; n.src_stride = src_stride;
+  n.in = in; n.in_plane = in_plane; n.X = X; n.x_plane = x_plane; n.nx = nx; n.S = S; n.src_stride = src_stride;
   n.T = T; n.ldf = ldf; n.overlap = overlap; n.step = m->tc - overlap;
   n.Tp = std::max<int64_t>(T, (n.P - 1) * n.step + m->tc);
   // the zero-padded slots are re-zeroed when the model changes; those of the 30-channel nets also when the overlap does
@@ -499,34 +513,46 @@ static int check_clip(const char* fn, const dcs_ctx* ctx, const dcs_model* m, co
 }
 
 // the workspace of a clip of L samples: nch STFT planes, nsrc x nch masked spectra, the score-informed net's input
-// channels; with `staged` also the device copies of host audio and stems
-static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, bool staged, cudaStream_t st) {
+// channels; with `staged` also the device copies of host audio and stems.  keep (keep-channels mode of the DSD100
+// net): two STFT planes, one magnitude plane, nsrc x 2 spectra; staged: three audio planes (downmix, left, right)
+static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, bool staged, bool keep,
+                          cudaStream_t st) {
   const int64_t plane = dcs_num_frames(L, p->hop) * dcs_padded_bins(p->N);
-  DCS_TRY(ctx->X.ensure((size_t)m->nch * plane * sizeof(float2), st));
+  const int nx = keep ? 2 : m->nch;   // mixture STFT planes = stem planes per source
+  DCS_TRY(ctx->X.ensure((size_t)nx * plane * sizeof(float2), st));
   DCS_TRY(ctx->mag.ensure((size_t)m->nch * plane * sizeof(float), st));
-  DCS_TRY(ctx->S.ensure((size_t)m->nsrc * m->nch * plane * sizeof(float2), st));
+  DCS_TRY(ctx->S.ensure((size_t)m->nsrc * nx * plane * sizeof(float2), st));
   if (m->arch == DCS_ARCH_BACH10_SCORE) DCS_TRY(ctx->net[NET_CHANS].ensure((size_t)m->sc.nch * plane * sizeof(float), st));
   if (staged) {
-    DCS_TRY(ctx->audio.ensure((size_t)L * sizeof(float), st));
-    DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * L * sizeof(float), st));
+    DCS_TRY(ctx->audio.ensure((size_t)(keep ? 3 : 1) * L * sizeof(float), st));
+    DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * (keep ? 2 : 1) * L * sizeof(float), st));
   }
   return DCS_OK;
 }
 
 // one clip, device to device: nch audio planes (audio_stride apart) -> nsrc x nch stem planes; d_filters: the
-// score filters that form the score-informed net's input channels
+// score filters that form the score-informed net's input channels.  d_mono (keep-channels mode, DSD100 net): the
+// downmix of the two audio planes; the network sees its magnitude, its masks are applied to the STFT of each
+// channel -> nsrc x 2 stem planes ordered (source, channel)
 static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,
-                         const float* d_filters, float scale_factor, int overlap, int patcher, float* d_stems,
-                         int64_t stem_stride, cudaStream_t st) {
-  DCS_TRY(size_workspace(ctx, m, p, L, false, st));
-  const int nch = m->nch;
+                         const float* d_filters, const float* d_mono, float scale_factor, int overlap, int patcher,
+                         float* d_stems, int64_t stem_stride, cudaStream_t st) {
+  const bool keep = d_mono != nullptr;
+  DCS_TRY(size_workspace(ctx, m, p, L, false, keep, st));
+  const int nch = m->nch, nx = keep ? 2 : 1;
   const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
   float2 *X = ctx->X.as<float2>(), *S = ctx->S.as<float2>();
   float* mag = ctx->mag.as<float>();
   {
     ProfScope ps(ctx, "stft_fwd", st);   // compute_transform: one STFT per channel (transform.py:105-119)
-    for (int ch = 0; ch < nch; ++ch)
-      DCS_TRY(launch_stft(p, d_audio + ch * audio_stride, L, X + ch * plane, mag + ch * plane, nullptr, scale_factor, ldf, st));
+    if (keep) {
+      DCS_TRY(launch_stft(p, d_mono, L, nullptr, mag, nullptr, scale_factor, ldf, st));
+      for (int c = 0; c < 2; ++c)
+        DCS_TRY(launch_stft(p, d_audio + c * audio_stride, L, X + c * plane, nullptr, nullptr, scale_factor, ldf, st));
+    } else {
+      for (int ch = 0; ch < nch; ++ch)
+        DCS_TRY(launch_stft(p, d_audio + ch * audio_stride, L, X + ch * plane, mag + ch * plane, nullptr, scale_factor, ldf, st));
+    }
   }
   const float* in = mag;
   if (d_filters) {
@@ -535,10 +561,10 @@ static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const fl
     DCS_TRY(launch_channel_mul(ctx, mag, d_filters, chans, plane, m->sc.nch, st));
     in = chans;
   }
-  DCS_TRY(run_network(ctx, m, in, plane, X, plane, T, ldf, overlap, patcher, S, plane, st));
-  DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * nch * plane, st));
+  DCS_TRY(run_network(ctx, m, in, plane, X, plane, nx, T, ldf, overlap, patcher, S, plane, st));
+  DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * nch * nx * plane, st));
   ProfScope ps(ctx, "istft_ola", st);
-  return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc * nch, T, ldf, plane, d_stems, L, stem_stride, st);
+  return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc * nch * nx, T, ldf, plane, d_stems, L, stem_stride, st);
 }
 
 int dcs_separate_spec(dcs_ctx* ctx, dcs_model* m, const float* d_mag, const dcs_complex* d_X, int64_t T, int64_t ldf,
@@ -547,7 +573,7 @@ int dcs_separate_spec(dcs_ctx* ctx, dcs_model* m, const float* d_mag, const dcs_
   DCS_REQUIRE(d_mag && d_X && d_S, "dcs_separate_spec: NULL argument");
   DCS_REQUIRE(T > 0 && ldf >= m->F && src_stride >= T * ldf, "dcs_separate_spec: bad shape");
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return run_network(ctx, m, d_mag, 0, (const float2*)d_X, 0, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
+  return run_network(ctx, m, d_mag, 0, (const float2*)d_X, 0, 1, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
                      (cudaStream_t)stream);
 }
 
@@ -558,7 +584,7 @@ int dcs_separate_spec_channels(dcs_ctx* ctx, dcs_model* m, const float* d_in, in
   DCS_REQUIRE(d_in && d_X && d_S, "dcs_separate_spec_channels: NULL argument");
   DCS_REQUIRE(T > 0 && ldf >= m->F && src_stride >= T * ldf && in_plane >= T * ldf, "dcs_separate_spec_channels: bad shape");
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return run_network(ctx, m, d_in, in_plane, (const float2*)d_X, 0, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
+  return run_network(ctx, m, d_in, in_plane, (const float2*)d_X, 0, 1, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
                      (cudaStream_t)stream);
 }
 
@@ -568,7 +594,7 @@ int dcs_separate_audio_score(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const floa
                      overlap, patcher));
   DCS_REQUIRE(d_filters, "dcs_separate_audio_score: NULL filters");
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return separate_clip(ctx, m, p, d_audio, L, L, d_filters, scale_factor, overlap, patcher, d_stems, stem_stride,
+  return separate_clip(ctx, m, p, d_audio, L, L, d_filters, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
                        (cudaStream_t)stream);
 }
 
@@ -615,7 +641,7 @@ int dcs_separate_audio_stereo(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const flo
   DCS_TRY(check_clip("dcs_separate_audio_stereo", ctx, m, p, DCS_ARCH_DSD_ILD, d_audio, d_stems, L, audio_stride, stem_stride,
                      overlap, patcher));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
+  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
                        (cudaStream_t)stream);
 }
 
@@ -630,7 +656,7 @@ int dcs_separate_audio(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_a
                        int overlap, int patcher, float* d_stems, int64_t stem_stride, void* stream) {
   DCS_TRY(check_clip("dcs_separate_audio", ctx, m, p, -1, d_audio, d_stems, L, L, stem_stride, overlap, patcher));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
+  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
                        (cudaStream_t)stream);
 }
 
@@ -639,9 +665,9 @@ int dcs_separate_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* h_au
   DCS_TRY(check_clip("dcs_separate_host", ctx, m, p, -1, h_audio, h_stems, L, L, stem_stride, overlap, patcher));
   cudaStream_t st = (cudaStream_t)stream;
   DCS_CUDA(cudaSetDevice(ctx->device));
-  DCS_TRY(size_workspace(ctx, m, p, L, true, st));
+  DCS_TRY(size_workspace(ctx, m, p, L, true, false, st));
   DCS_CUDA(cudaMemcpyAsync(ctx->audio.p, h_audio, (size_t)L * sizeof(float), cudaMemcpyHostToDevice, st));
-  DCS_TRY(separate_clip(ctx, m, p, ctx->audio.as<float>(), L, L, nullptr, scale_factor, overlap, patcher, ctx->stems.as<float>(), L, st));
+  DCS_TRY(separate_clip(ctx, m, p, ctx->audio.as<float>(), L, L, nullptr, nullptr, scale_factor, overlap, patcher, ctx->stems.as<float>(), L, st));
   DCS_CUDA(cudaMemcpy2DAsync(h_stems, (size_t)stem_stride * sizeof(float), ctx->stems.p, (size_t)L * sizeof(float),
                              (size_t)L * sizeof(float), m->nsrc, cudaMemcpyDeviceToHost, st));
   DCS_CUDA(cudaStreamSynchronize(st));
@@ -662,10 +688,13 @@ int dcs_separate_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const int16
 // process per file (examples/dsd100/separate_multiple.ipynb cell 3); per clip this is the wav contract of train_auto
 // (separate_dsd.py:275-287,307-309), exactly dcs_separate_pcm16_host.  Host buffers should be pinned.
 // the pipelined loop of dcs_separate_batch_pcm16_host; on any failure the caller drains the copy streams before it
-// returns, because the copies in flight read and write the user's host buffers
+// returns, because the copies in flight read and write the user's host buffers.  keep (keep-channels mode, 2 channels):
+// the clip is decoded into (downmix, left, right) planes, the stems are encoded as interleaved [L][2] per source
 static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
-                          const int64_t* num_samples, int channels, int downmix, float scale_factor, int overlap,
+                          const int64_t* num_samples, int channels, int downmix, bool keep, float scale_factor, int overlap,
                           int patcher, int16_t* const* h_out, const int64_t* out_strides, cudaStream_t st) {
+  const int w = keep ? 2 : 1;   // int16 values per sample of a stem
+  float *audio = ctx->audio.as<float>(), *stems = ctx->stems.as<float>();
   // the copy streams start after whatever the caller queued on `st` (and after the memsets of fresh buffers)
   DCS_CUDA(cudaEventRecord(ctx->ev_dec[0], st));
   DCS_CUDA(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_dec[0], 0));
@@ -679,25 +708,36 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, c
     DCS_CUDA(cudaEventRecord(ctx->ev_in[b], ctx->s_h2d));
     // kernels of clip i
     DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_in[b], 0));
-    DCS_TRY(launch_pcm_decode(ctx, ctx->pcm_in[b].as<int16_t>(), L, channels, downmix, ctx->audio.as<float>(), st));
-    DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
-    DCS_TRY(separate_clip(ctx, m, p, ctx->audio.as<float>(), L, L, nullptr, scale_factor, overlap, patcher, ctx->stems.as<float>(), L, st));
+    if (keep) {
+      DCS_TRY(launch_pcm_decode_keep(ctx, ctx->pcm_in[b].as<int16_t>(), L, audio, st));
+      DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
+      DCS_TRY(separate_clip(ctx, m, p, audio + L, L, L, nullptr, audio, scale_factor, overlap, patcher, stems, L, st));
+    } else {
+      DCS_TRY(launch_pcm_decode(ctx, ctx->pcm_in[b].as<int16_t>(), L, channels, downmix, audio, st));
+      DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
+      DCS_TRY(separate_clip(ctx, m, p, audio, L, L, nullptr, nullptr, scale_factor, overlap, patcher, stems, L, st));
+    }
     if (i >= 2) DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_out[b], 0));     // D2H of clip i-2 has drained the output staging
-    DCS_TRY(launch_pcm_encode(ctx, ctx->stems.as<float>(), L, m->nsrc, L, ctx->pcm_out[b].as<int16_t>(), L, st));
+    if (keep)
+      DCS_TRY(launch_pcm_encode_keep(ctx, stems, L, m->nsrc, L, ctx->pcm_out[b].as<int16_t>(), st));
+    else
+      DCS_TRY(launch_pcm_encode(ctx, stems, L, m->nsrc, L, ctx->pcm_out[b].as<int16_t>(), L, st));
     DCS_CUDA(cudaEventRecord(ctx->ev_enc[b], st));
     // D2H of clip i
     DCS_CUDA(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_enc[b], 0));
-    DCS_CUDA(cudaMemcpy2DAsync(h_out[i], (size_t)out_strides[i] * sizeof(int16_t), ctx->pcm_out[b].p, (size_t)L * sizeof(int16_t),
-                               (size_t)L * sizeof(int16_t), m->nsrc, cudaMemcpyDeviceToHost, ctx->s_d2h));
+    DCS_CUDA(cudaMemcpy2DAsync(h_out[i], (size_t)w * out_strides[i] * sizeof(int16_t), ctx->pcm_out[b].p,
+                               (size_t)w * L * sizeof(int16_t), (size_t)w * L * sizeof(int16_t), m->nsrc, cudaMemcpyDeviceToHost,
+                               ctx->s_d2h));
     DCS_CUDA(cudaEventRecord(ctx->ev_out[b], ctx->s_d2h));
   }
   return DCS_OK;
 }
 
-int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
-                                  const int64_t* num_samples, int channels, int downmix, float scale_factor, int overlap,
-                                  int patcher, int16_t* const* h_out, const int64_t* out_strides, void* stream) {
-  DCS_REQUIRE(ctx && m && p && h_pcm && num_samples && h_out && out_strides && nclips >= 0, "dcs_separate_batch_pcm16_host: bad argument");
+// the checks, resources and drain of both int16 batch entry points around batch_pipeline
+static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
+                      const int64_t* num_samples, int channels, int downmix, bool keep, float scale_factor, int overlap,
+                      int patcher, int16_t* const* h_out, const int64_t* out_strides, cudaStream_t st) {
+  DCS_REQUIRE(ctx && m && p && h_pcm && num_samples && h_out && out_strides && nclips >= 0, "%s: bad argument", fn);
   DCS_REQUIRE(channels >= 1 && channels <= 8 && downmix >= 0 && downmix <= 2, "bad channels/downmix");
   if (nclips == 0) return DCS_OK;
   int64_t Lmax = 0;
@@ -705,8 +745,7 @@ int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int n
     DCS_REQUIRE(h_pcm[i] && h_out[i] && num_samples[i] > 0 && out_strides[i] >= num_samples[i], "clip %d: bad buffer / length", i);
     Lmax = std::max(Lmax, num_samples[i]);
   }
-  DCS_TRY(check_clip("dcs_separate_batch_pcm16_host", ctx, m, p, -1, h_pcm, h_out, Lmax, Lmax, Lmax, overlap, patcher));
-  cudaStream_t st = (cudaStream_t)stream;
+  DCS_TRY(check_clip(fn, ctx, m, p, keep ? DCS_ARCH_DSD : -1, h_pcm, h_out, Lmax, Lmax, Lmax, overlap, patcher));
   DCS_CUDA(cudaSetDevice(ctx->device));
   // each resource on its own: a call that failed half-way through this block must not leave later calls with null handles
   if (!ctx->s_h2d) DCS_CUDA(cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
@@ -721,10 +760,10 @@ int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int n
   // re-allocated mid-batch would synchronise the stream
   for (int b = 0; b < std::min(nclips, 2); ++b) {
     DCS_TRY(ctx->pcm_in[b].ensure((size_t)Lmax * channels * sizeof(int16_t), st));
-    DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * Lmax * sizeof(int16_t), st));
+    DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * (keep ? 2 : 1) * Lmax * sizeof(int16_t), st));
   }
-  DCS_TRY(size_workspace(ctx, m, p, Lmax, true, st));
-  const int rc = batch_pipeline(ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, scale_factor, overlap, patcher,
+  DCS_TRY(size_workspace(ctx, m, p, Lmax, true, keep, st));
+  const int rc = batch_pipeline(ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, keep, scale_factor, overlap, patcher,
                                 h_out, out_strides, st);
   // drain everything, success or not, before the host buffers go back to the caller
   const cudaError_t e0 = cudaStreamSynchronize(ctx->s_h2d), e1 = cudaStreamSynchronize(ctx->s_d2h), e2 = cudaStreamSynchronize(st);
@@ -733,6 +772,39 @@ int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int n
   DCS_CUDA(e1);
   DCS_CUDA(e2);
   return DCS_OK;
+}
+
+int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
+                                  const int64_t* num_samples, int channels, int downmix, float scale_factor, int overlap,
+                                  int patcher, int16_t* const* h_out, const int64_t* out_strides, void* stream) {
+  return batch_host("dcs_separate_batch_pcm16_host", ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, false,
+                    scale_factor, overlap, patcher, h_out, out_strides, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------------ keep-channels (DSD100 net)
+int dcs_separate_batch_pcm16_keep_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips,
+                                                const int16_t* const* h_pcm, const int64_t* num_samples, float scale_factor,
+                                                int overlap, int patcher, int16_t* const* h_out, const int64_t* out_strides,
+                                                void* stream) {
+  return batch_host("dcs_separate_batch_pcm16_keep_channels_host", ctx, m, p, nclips, h_pcm, num_samples, 2, 1, true,
+                    scale_factor, overlap, patcher, h_out, out_strides, (cudaStream_t)stream);
+}
+
+int dcs_separate_audio_keep_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride,
+                                     int64_t L, float scale_factor, int overlap, int patcher, float* d_stems,
+                                     int64_t stem_stride, void* stream) {
+  DCS_TRY(check_clip("dcs_separate_audio_keep_channels", ctx, m, p, DCS_ARCH_DSD, d_audio, d_stems, L, audio_stride,
+                     stem_stride, overlap, patcher));
+  cudaStream_t st = (cudaStream_t)stream;
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  DCS_TRY(ctx->audio.ensure((size_t)L * sizeof(float), st));
+  float* mono = ctx->audio.as<float>();
+  {
+    ProfScope ps(ctx, "downmix", st);
+    DCS_TRY(launch_downmix2(ctx, d_audio, audio_stride, L, mono, st));
+  }
+  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, mono, scale_factor, overlap, patcher, d_stems,
+                       stem_stride, st);
 }
 
 }  // extern "C"

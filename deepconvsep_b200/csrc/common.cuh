@@ -160,6 +160,7 @@ bool shape_is(const int64_t* s, int nd, int want_nd, int64_t a, int64_t b = 1, i
 struct NetCall {
   const float* in; int64_t in_plane;
   const float2* X; int64_t x_plane;
+  int nx;           // mixture channels the masks apply to (2: DSD100 net in keep-channels mode, planes (s * 2 + c))
   float2* S; int64_t src_stride;
   int64_t T, ldf;
   int64_t P, Tp;    // patches (> 0) and the frames they span
@@ -226,12 +227,15 @@ struct DsdMaskArgs {
   const float* W1t;    // [50][ldw]  W1t[c][b] = conv1.W[c,0,0,F-1-b]
   int ldw;
   const float* bout;   // [4]
-  const float2* X;     // [T][ldf]
-  float2* S;           // [4][T][ldf]
+  const float2* X;     // [nx][T][ldf], channel c at X + c * x_plane
+  float2* S;           // [4][nx][T][ldf]: source s, channel c at S + (s * nx + c) * src_stride
   int64_t ldf, src_stride;
   int T, P, tc, overlap, F;
   int ndec;            // 3: DSD100 (4th output = decoder 2, all-zero bins get 1/4); 4: one decoder per source,
                        //    all-zero bins get 0 (stereo / ILD net, one launch per channel)
+  int nx;              // mixture channels the masks are applied to: 1, or 2 (DSD100 net, stereo stems from the
+                       //    downmix's masks; tensor-core kernel only)
+  int64_t x_plane;
 };
 int launch_dsd_mask(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st);
 bool dsd_mask_tc_supported(const DsdMaskArgs& a);
@@ -260,5 +264,11 @@ int launch_pcm_decode(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int channel
                       cudaStream_t st);
 int launch_pcm_encode(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int64_t stem_stride, int16_t* d_out,
                       int64_t out_stride, cudaStream_t st);
+// stereo stems: interleaved int16 [L][2] -> three float planes L apart (downmix, left, right); float left / right planes
+// -> the downmix; nsrc x 2 stem planes (source, channel) -> int16 [nsrc][L][2], source s at d_out + s * 2 * L
+int launch_pcm_decode_keep(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, float* d_planes, cudaStream_t st);
+int launch_downmix2(dcs_ctx* ctx, const float* d_audio, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st);
+int launch_pcm_encode_keep(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int64_t stem_stride, int16_t* d_out,
+                           cudaStream_t st);
 
 }  // namespace dcs

@@ -42,6 +42,8 @@ constexpr int MT_A_BYTES = 4 * MT_A_SUB;           // hi k0-31, hi k32-63, lo k0
 //           separate_dsd.py:228,258-266), 8 frames per group, 144 columns (two m64n72k8 halves);
 // NDEC = 4: the stereo / ILD net, one launch per input channel (one decoder per source, all-zero bins get 0,
 //           trainCNN_ILD_DSD100.py:99-106,183-186), 4 frames per group, 96 columns (two m64n48k8 halves).
+// NX: mixture channels the cross-faded masks are applied to -- 1, or 2 with NDEC = 3 (stereo stems from the masks of
+//     the downmix: the same m times each channel's X; GEMM, gather and cross-fade run once).
 // Value v = slot * NDEC + decoder.  Fragment (tc.cuh): d[4j + 2i + e] = D[16w + l/4 + 8i][8j + 2(l%4) + e].
 //   NDEC = 3: column 8v + f          -> thread holds frames f = 2(l%4) + e, all v: d[4v + 2i + e]
 //   NDEC = 4: column 8(v/2) + 2f + v%2 -> thread holds frame f = l%4, all v:     d[4(v/2) + 2i + v%2]
@@ -121,7 +123,7 @@ __device__ __forceinline__ void mask_store_b(uint8_t* sB, int tid, const float4 
   }
 }
 
-template <int NDEC>
+template <int NDEC, int NX>
 __global__ void __launch_bounds__(MT_THREADS, 1)
 dsd_mask_tc_kernel(const DsdMaskArgs a, const float4* __restrict__ xtab, int num_groups, int num_items) {
   using MT = MaskTile<NDEC>;
@@ -186,7 +188,7 @@ dsd_mask_tc_kernel(const DsdMaskArgs a, const float4* __restrict__ xtab, int num
       }
     }
 
-    // ---- while they run: this item's X, B of item w + 1 into stage s^1, global loads of item w + 2
+    // ---- while they run: this item's X (of every channel), B of item w + 1 into stage s^1, global loads of item w + 2
     int bin[2];
     bool bok[2];
 #pragma unroll
@@ -194,14 +196,16 @@ dsd_mask_tc_kernel(const DsdMaskArgs a, const float4* __restrict__ xtab, int num
       bin[i] = tile * MT_BINS + row0 + 8 * i;
       bok[i] = bin[i] < a.F;
     }
-    float2 x[TF][2];
+    float2 x[NX][TF][2];
 #pragma unroll
-    for (int e = 0; e < TF; ++e) {
-      const int t = g * FRAMES + MT::thread_frame(lane, e);
+    for (int c = 0; c < NX; ++c)
 #pragma unroll
-      for (int i = 0; i < 2; ++i)
-        x[e][i] = (bok[i] && t < a.T) ? a.X[(int64_t)t * a.ldf + bin[i]] : make_float2(0.f, 0.f);
-    }
+      for (int e = 0; e < TF; ++e) {
+        const int t = g * FRAMES + MT::thread_frame(lane, e);
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+          x[c][e][i] = (bok[i] && t < a.T) ? a.X[c * a.x_plane + (int64_t)t * a.ldf + bin[i]] : make_float2(0.f, 0.f);
+      }
     if (w + 1 < w_end) {
       mask_store_b<NDEC>(sB + (s ^ 1) * MT::B_BYTES, tid, rb);
       fence_proxy_async();
@@ -249,22 +253,25 @@ dsd_mask_tc_kernel(const DsdMaskArgs a, const float4* __restrict__ xtab, int num
         }
       }
     }
+    // source s, channel c at S + (s * NX + c) * src_stride
 #pragma unroll
-    for (int e = 0; e < TF; ++e) {
-      const int t = g * FRAMES + MT::thread_frame(lane, e);
+    for (int c = 0; c < NX; ++c)
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        if (bok[i] && t < a.T) {
-          const float2 xx = x[e][i];
-          const float* mm = m[e][i];
-          const int64_t o = (int64_t)t * a.ldf + bin[i];
-          a.S[o] = make_float2(mm[0] * xx.x, mm[0] * xx.y);
-          a.S[o + a.src_stride] = make_float2(mm[1] * xx.x, mm[1] * xx.y);
-          a.S[o + 2 * a.src_stride] = make_float2(mm[2] * xx.x, mm[2] * xx.y);
-          a.S[o + 3 * a.src_stride] = make_float2(mm[3] * xx.x, mm[3] * xx.y);
+      for (int e = 0; e < TF; ++e) {
+        const int t = g * FRAMES + MT::thread_frame(lane, e);
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          if (bok[i] && t < a.T) {
+            const float2 xx = x[c][e][i];
+            const float* mm = m[e][i];
+            const int64_t o = (int64_t)t * a.ldf + bin[i] + c * a.src_stride;
+            a.S[o] = make_float2(mm[0] * xx.x, mm[0] * xx.y);
+            a.S[o + NX * a.src_stride] = make_float2(mm[1] * xx.x, mm[1] * xx.y);
+            a.S[o + 2 * NX * a.src_stride] = make_float2(mm[2] * xx.x, mm[2] * xx.y);
+            a.S[o + 3 * NX * a.src_stride] = make_float2(mm[3] * xx.x, mm[3] * xx.y);
+          }
         }
       }
-    }
   }
 }
 
@@ -292,15 +299,15 @@ __global__ void dsd_xfade_table_kernel(float4* __restrict__ tab, int T, int Tpad
 
 bool dsd_mask_tc_supported(const DsdMaskArgs& a) {
   const int step = a.tc - a.overlap;
-  return step > 0 && (a.ndec == 3 || a.ndec == 4) && (a.tc + step - 1) / step <= MT_SLOTS && a.ldg % 4 == 0 && a.ldg >= 52 &&
+  return step > 0 && (a.ndec == 3 || a.ndec == 4) && (a.nx == 1 || (a.nx == 2 && a.ndec == 3)) && (a.tc + step - 1) / step <= MT_SLOTS && a.ldg % 4 == 0 && a.ldg >= 52 &&
          ((uintptr_t)a.G % 16 == 0);
 }
 
 // all F bins; the last 128-bin tile holds only the Nyquist bin (F = 2^k + 1)
-template <int NDEC>
+template <int NDEC, int NX>
 static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st) {
   using MT = MaskTile<NDEC>;
-  DCS_TRY(ensure_smem_attr(dsd_mask_tc_kernel<NDEC>, MT::SMEM));
+  DCS_TRY(ensure_smem_attr(dsd_mask_tc_kernel<NDEC, NX>, MT::SMEM));
   const int m_tiles = (a.F + MT_BINS - 1) / MT_BINS;
   const int num_groups = (a.T + MT::FRAMES - 1) / MT::FRAMES;
   const int num_items = m_tiles * num_groups;
@@ -311,7 +318,7 @@ static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t
   dsd_xfade_table_kernel<<<(unsigned)ceil_div64((int64_t)Tpad * MT_SLOTS, 256), 256, 0, st>>>(xtab, a.T, Tpad, a.P, a.tc, a.overlap);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
-  dsd_mask_tc_kernel<NDEC><<<(unsigned)ctas, MT_THREADS, MT::SMEM, st>>>(a, xtab, num_groups, num_items);
+  dsd_mask_tc_kernel<NDEC, NX><<<(unsigned)ctas, MT_THREADS, MT::SMEM, st>>>(a, xtab, num_groups, num_items);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;
@@ -320,7 +327,8 @@ static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t
 int launch_dsd_mask_tc(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st) {
   if (a.T <= 0) return DCS_OK;
   DCS_REQUIRE(dsd_mask_tc_supported(a), "dsd_mask_tc: unsupported shape");
-  return a.ndec == 4 ? launch_dsd_mask_tc_t<4>(ctx, a, st) : launch_dsd_mask_tc_t<3>(ctx, a, st);
+  if (a.ndec == 4) return launch_dsd_mask_tc_t<4, 1>(ctx, a, st);
+  return a.nx == 2 ? launch_dsd_mask_tc_t<3, 2>(ctx, a, st) : launch_dsd_mask_tc_t<3, 1>(ctx, a, st);
 }
 
 }  // namespace dcs

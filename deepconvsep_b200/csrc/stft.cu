@@ -175,6 +175,37 @@ __global__ void pcm_encode_kernel(const float* __restrict__ stems, int64_t L, in
   out[(int64_t)s * out_stride + i] = (int16_t)(int)v;
 }
 
+// keep-channels mode: interleaved int16 [L][2] -> planes (downmix, left, right), L apart; the downmix is the
+// expression of pcm_decode_kernel's downmix 1, so the network sees what the mono call would see
+__global__ void pcm_decode_keep_kernel(const int16_t* __restrict__ pcm, int64_t L, float* __restrict__ planes) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= L) return;
+  const float maxv = 32767.0f;
+  const float l = (float)pcm[2 * i] / maxv, r = (float)pcm[2 * i + 1] / maxv;
+  planes[i] = (l + r) * 0.5f;
+  planes[L + i] = l;
+  planes[2 * L + i] = r;
+}
+
+// float left / right planes (stride apart) -> their downmix, the same expression
+__global__ void downmix2_kernel(const float* __restrict__ audio, int64_t stride, int64_t L, float* __restrict__ mono) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= L) return;
+  mono[i] = (audio[i] + audio[stride + i]) * 0.5f;
+}
+
+// stem planes (source s, channel c) at stems + (2 s + c) * stem_stride -> int16 [nsrc][L][2] (what writeAudioScipy
+// writes for a 2-channel stem), the truncation rule of pcm_encode_kernel
+__global__ void pcm_encode_keep_kernel(const float* __restrict__ stems, int64_t L, int64_t stem_stride,
+                                       int16_t* __restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= L) return;
+  const int s = blockIdx.y;
+  const float l = stems[(int64_t)(2 * s) * stem_stride + i] * 32767.0f;
+  const float r = stems[(int64_t)(2 * s + 1) * stem_stride + i] * 32767.0f;
+  reinterpret_cast<short2*>(out + (int64_t)s * 2 * L)[i] = make_short2((int16_t)(int)l, (int16_t)(int)r);
+}
+
 template <int N>
 static int launch_stft_n(dcs_stft* p, const float* d_audio, int64_t L, float2* d_X, float* d_mag, float* d_phase,
                          float mag_scale, int64_t ldf, int64_t T, cudaStream_t st) {
@@ -246,6 +277,33 @@ int launch_pcm_decode(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int channel
                       cudaStream_t st) {
   if (L <= 0) return DCS_OK;
   pcm_decode_kernel<<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(d_pcm, L, channels, downmix, d_audio);
+  DCS_CHECK_LAUNCH();
+  ctx->launches++;
+  return DCS_OK;
+}
+
+int launch_pcm_decode_keep(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, float* d_planes, cudaStream_t st) {
+  if (L <= 0) return DCS_OK;
+  pcm_decode_keep_kernel<<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(d_pcm, L, d_planes);
+  DCS_CHECK_LAUNCH();
+  ctx->launches++;
+  return DCS_OK;
+}
+
+int launch_downmix2(dcs_ctx* ctx, const float* d_audio, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st) {
+  if (L <= 0) return DCS_OK;
+  downmix2_kernel<<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(d_audio, audio_stride, L, d_mono);
+  DCS_CHECK_LAUNCH();
+  ctx->launches++;
+  return DCS_OK;
+}
+
+int launch_pcm_encode_keep(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int64_t stem_stride, int16_t* d_out,
+                           cudaStream_t st) {
+  if (L <= 0) return DCS_OK;
+  DCS_REQUIRE((uintptr_t)d_out % 4 == 0, "pcm_encode_keep: output not 4-byte aligned");
+  dim3 grid((unsigned)ceil_div64(L, 256), (unsigned)nsrc);
+  pcm_encode_keep_kernel<<<grid, 256, 0, st>>>(d_stems, L, stem_stride, d_out);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;

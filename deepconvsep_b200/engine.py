@@ -257,8 +257,12 @@ class Separator(object):
                                               _stream_ptr(None, self.ctx.device)))
         return out
 
-    def separate_pcm16(self, pcm, downmix=1, out=None):
-        """int16 wav samples [L] or [L, channels] -> int16 [nsrc, L] (train_auto's wav contract)."""
+    def separate_pcm16(self, pcm, downmix=1, out=None, keep_channels=False):
+        """int16 wav samples [L] or [L, channels] -> int16 [nsrc, L] (train_auto's wav contract).
+        keep_channels=True (DSD100 / hiphopss net, stereo [L, 2] in): int16 [nsrc, L, 2] stereo stems, see
+        separate_keep_channels."""
+        if keep_channels:
+            return self.separate_pcm16_batch([pcm], outs=None if out is None else [out], keep_channels=True)[0]
         p = np.ascontiguousarray(pcm, dtype=np.int16)
         L = p.shape[0]
         ch = 1 if p.ndim == 1 else p.shape[1]
@@ -269,14 +273,17 @@ class Separator(object):
                                                     self.patcher, out.ctypes.data, L, _stream_ptr(None, self.ctx.device)))
         return out
 
-    def separate_pcm16_batch(self, clips, downmix=1, outs=None):
+    def separate_pcm16_batch(self, clips, downmix=1, outs=None, keep_channels=False):
         """Several clips through the context's multi-clip scheduler (dcs_separate_batch_pcm16_host): H2D of clip i+1,
         the kernels of clip i and D2H of clip i-1 overlap.  clips: list of int16 arrays [L] or [L, channels] (same
-        channel count; pinned for real overlap) -> list of int16 [nsrc, L]."""
+        channel count; pinned for real overlap) -> list of int16 [nsrc, L].  keep_channels=True: stereo clips
+        [L, 2] -> list of int16 [nsrc, L, 2] (dcs_separate_batch_pcm16_keep_channels_host)."""
         ps = [np.ascontiguousarray(c, dtype=np.int16) for c in clips]
         n = len(ps)
         if n == 0:
             return []
+        if keep_channels:
+            return self._pcm16_batch_keep_channels(ps, outs)
         ch = 1 if ps[0].ndim == 1 else ps[0].shape[1]
         assert all((1 if p_.ndim == 1 else p_.shape[1]) == ch for p_ in ps), "all clips must have the same channel count"
         Ls = np.array([p_.shape[0] for p_ in ps], dtype=np.int64)
@@ -289,6 +296,22 @@ class Separator(object):
                                                           Ls.ctypes.data, ch, int(downmix if ch > 1 else 0), self.scale_factor,
                                                           self.overlap, self.patcher, pout, Ls.ctypes.data,
                                                           _stream_ptr(None, self.ctx.device)))
+        return outs
+
+    def _pcm16_batch_keep_channels(self, ps, outs):
+        for p_ in ps:
+            if p_.ndim != 2 or p_.shape[1] != 2:
+                raise ValueError("keep_channels needs stereo int16 clips [L, 2], got shape %r" % (p_.shape,))
+        n = len(ps)
+        Ls = np.array([p_.shape[0] for p_ in ps], dtype=np.int64)
+        if outs is None:
+            outs = [np.empty((self.nsrc, int(L), 2), dtype=np.int16) for L in Ls]
+        assert all(o.dtype == np.int16 and o.shape == (self.nsrc, int(L), 2) and o.flags.c_contiguous for o, L in zip(outs, Ls))
+        pin = (C.c_void_p * n)(*[p_.ctypes.data for p_ in ps])
+        pout = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
+        _lib.check(self.lib.dcs_separate_batch_pcm16_keep_channels_host(
+            self.ctx.handle, self.model.handle, self.stft.handle, n, pin, Ls.ctypes.data, self.scale_factor, self.overlap,
+            self.patcher, pout, Ls.ctypes.data, _stream_ptr(None, self.ctx.device)))
         return outs
 
     # ---- device buffers (torch tensors) ----
@@ -351,16 +374,41 @@ class Separator(object):
             return outd
         return np.ascontiguousarray(outd.cpu().numpy().reshape(self.nsrc, 2, L).transpose(2, 0, 1))
 
-    def separate_tapped(self, audio, filters=None, pool=False):
-        """Parity-test entry: the same pipeline as separate() / separate_score() / separate_stereo() with
-        the spectrum tap on (dcs_set_spectrum_tap) -> (stems as that call returns them, masked spectra
-        complex64 numpy [nplanes, T, F] -- the tensors the inverse STFT of THIS call consumed).
+    def separate_keep_channels(self, audio, out=None, stream=None):
+        """Stereo stems from the DSD100 / hiphopss network (dcs_separate_audio_keep_channels): the network sees the
+        downmix (l + r) * 0.5, its soft masks are applied to each channel's STFT and inverted with that channel's
+        phase.  audio float [L, 2] (numpy) or [2, L] (cuda tensor) -> float32 [L, nsrc, 2] (numpy, the layout of
+        separate_stereo) or the device planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out)."""
+        import torch
+        host = not hasattr(audio, "is_cuda")
+        if host:
+            a = np.asarray(audio, dtype=np.float32)
+            if a.ndim != 2 or a.shape[1] != 2:
+                raise ValueError("keep-channels separation needs stereo audio [L, 2], got shape %r" % (a.shape,))
+            x = torch.as_tensor(np.ascontiguousarray(a.T), device=self.stft.dev)
+        else:
+            x = audio.contiguous()
+            assert x.dim() == 2 and x.shape[0] == 2 and x.dtype == torch.float32
+        L = x.shape[1]
+        outd = out if (out is not None and not host) else torch.empty((self.nsrc * 2, L), dtype=torch.float32, device=x.device)
+        _lib.check(self.lib.dcs_separate_audio_keep_channels(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x),
+                                                             x.stride(0), L, self.scale_factor, self.overlap, self.patcher,
+                                                             _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
+        if not host:
+            return outd
+        return np.ascontiguousarray(outd.cpu().numpy().reshape(self.nsrc, 2, L).transpose(2, 0, 1))
+
+    def separate_tapped(self, audio, filters=None, pool=False, keep_channels=False):
+        """Parity-test entry: the same pipeline as separate() / separate_score() / separate_stereo() /
+        separate_keep_channels() (keep_channels=True) with the spectrum tap on (dcs_set_spectrum_tap) -> (stems as
+        that call returns them, masked spectra complex64 numpy [nplanes, T, F] -- the tensors the inverse STFT of THIS
+        call consumed, (source, channel) planes for the stereo outputs).
         pool=True (max-pool net): also the tie bits uint8 [T, WP, 32] of this call (dcs_set_pool_tap)."""
         import torch
         a = np.asarray(audio)
         L = a.shape[0]
         T = self.stft.num_frames(L)
-        nplanes = self.nsrc * (2 if self.model.arch == "dsd_ild" else 1)
+        nplanes = self.nsrc * (2 if self.model.arch == "dsd_ild" or keep_channels else 1)
         tap = torch.zeros((nplanes, T, self.stft.ldf), dtype=torch.complex64, device=self.stft.dev)
         _lib.check(self.lib.dcs_set_spectrum_tap(self.ctx.handle, _ptr(tap), tap.numel()))
         bits = None
@@ -370,7 +418,9 @@ class Separator(object):
             bits = torch.zeros((T, WP, 32), dtype=torch.uint8, device=self.stft.dev)
             _lib.check(self.lib.dcs_set_pool_tap(self.ctx.handle, _ptr(bits), bits.numel()))
         try:
-            if self.model.arch == "bach10_score":
+            if keep_channels:
+                out = self.separate_keep_channels(a)
+            elif self.model.arch == "bach10_score":
                 out = self.separate_score(a, filters)
             elif self.model.arch == "dsd_ild":
                 out = self.separate_stereo(a)

@@ -42,19 +42,44 @@ def decode(audioObj, family):
     return a if a.ndim == 1 else a[:, 0]
 
 
+def check_keep_channels(family, audioObj=None, filein=""):
+    """keep_channels (stereo stems from the masks of the downmix) exists for the DSD100 / hiphopss network and 2-channel
+    recordings only: raises ValueError with the reason otherwise."""
+    if family != "dsd":
+        raise ValueError("--keep-channels: only the DSD100 / hiphopss network keeps the stereo channels, not %s" % family)
+    if audioObj is not None and (audioObj.ndim != 2 or audioObj.shape[1] != 2):
+        raise ValueError("--keep-channels needs a 2-channel recording; %s has %d channel(s)"
+                         % (filein, 1 if audioObj.ndim == 1 else audioObj.shape[1]))
+
+
 def run(family, filein, outdir, model, scale_factor, time_context, overlap, batch_size, input_size, frame_size, hop,
-        out_name, window=None, device=0, slot=0):
+        out_name, window=None, device=0, slot=0, keep_channels=False):
     """wav in -> one int16 wav per source in `outdir`.  `batch_size` is accepted for signature
-    compatibility; the CUDA path has no patch batches."""
+    compatibility; the CUDA path has no patch batches.  keep_channels (DSD100 / hiphopss, 2-channel wav): one
+    2-channel wav per source -- the soft masks of the downmix applied to each channel."""
     d = dict(FAMILY_DEFAULTS[family])
     if window is not None:
         d["window"] = window
+    if keep_channels:
+        check_keep_channels(family)
     sampleRate, audioObj = scipy.io.wavfile.read(filein)
     if sampleRate != 44100:
         print("Sample rate is not 44100")        # separate_dsd.py:313
         return None
     arch = None if family in ("ikala",) else family
-    if isinstance(device, (list, tuple)):
+    if keep_channels:
+        check_keep_channels(family, audioObj, filein)
+        if isinstance(device, (list, tuple)):
+            raise ValueError("--keep-channels separates each recording on one device; give several files for several devices")
+        sep = get_separator(model, arch, frame_size, hop, d["window"], scale_factor, time_context, overlap, input_size,
+                            device=device, slot=slot)
+        if audioObj.dtype == np.int16:
+            stems16 = sep.separate_pcm16(audioObj, keep_channels=True)             # [nsrc, L, 2], int16 path on the GPU
+        else:
+            maxv = np.finfo(audioObj.dtype).max if np.issubdtype(audioObj.dtype, np.floating) else np.iinfo(audioObj.dtype).max
+            stems = sep.separate_keep_channels(audioObj.astype('float') / maxv)    # [L, nsrc, 2]
+            stems16 = (stems.transpose(1, 0, 2).astype(np.float64) * np.iinfo(np.int16).max).astype('int16')
+    elif isinstance(device, (list, tuple)):
         # one recording over several GPUs: hop- and patch-aligned segments with margins, one host thread per device,
         # the stitched stems are those of the whole-clip call (deepconvsep_b200.longclip)
         from .. import longclip
@@ -83,10 +108,11 @@ def run(family, filein, outdir, model, scale_factor, time_context, overlap, batc
 
 
 # ---- command line shared by the separate_*.py scripts ------------------------------------------------------
-LONG_OPTS = ["ifile=", "odir=", "mfile=", "frame-size=", "window=", "devices=", "batch-clips="]
+LONG_OPTS = ["ifile=", "odir=", "mfile=", "frame-size=", "window=", "devices=", "batch-clips=", "keep-channels"]
 EXTRA_USAGE = ("  optional: --frame-size N (STFT frame, feat_size = N/2+1)  --window hanning|blackmanharris|sinebell\n"
                "            --devices 0,1,...  --batch-clips K (clips in flight per device); with these, -i may be a directory of wavs\n"
-               "            (one wav and several devices: the recording itself is cut into segments over the devices)")
+               "            (one wav and several devices: the recording itself is cut into segments over the devices)\n"
+               "            --keep-channels (DSD100 / hiphopss, 2-channel wavs): 2-channel stems, the downmix's masks on each channel")
 
 
 def parse_cli(argv, usage):
@@ -99,7 +125,8 @@ def parse_cli(argv, usage):
         print(usage)
         print(EXTRA_USAGE)
         sys.exit(2)
-    o = {"inputfile": None, "outdir": None, "model": None, "frame_size": None, "window": None, "devices": None, "batch_clips": 1}
+    o = {"inputfile": None, "outdir": None, "model": None, "frame_size": None, "window": None, "devices": None, "batch_clips": 1,
+         "keep_channels": False}
     for opt, arg in opts:
         if opt == "-h":
             print(usage)
@@ -119,18 +146,33 @@ def parse_cli(argv, usage):
             o["devices"] = [int(x) for x in arg.split(",") if x != ""]
         elif opt == "--batch-clips":
             o["batch_clips"] = max(1, int(arg))
+        elif opt == "--keep-channels":
+            o["keep_channels"] = True
     if o["inputfile"] is None or o["outdir"] is None or o["model"] is None:
         print(usage)
         sys.exit(2)
     return o
 
 
-def cli_main(argv, usage, train_auto_default, run_one):
+def cli_main(argv, usage, train_auto_default, run_one, family=None):
     """`train_auto_default(inputfile, outdir, model)` = the script's literal reference call (no extra flag given);
-    `run_one(filein, outdir, model, frame_size, window, device, slot, several_clips)` = the same with the overrides."""
+    `run_one(filein, outdir, model, frame_size, window, device, slot, several_clips)` = the same with the overrides
+    (with --keep-channels also keep_channels=True; only the DSD100 / hiphopss script, family "dsd", takes it)."""
+    import sys
     o = parse_cli(argv, usage)
+    if o["keep_channels"]:
+        try:
+            check_keep_channels(family)
+        except ValueError as e:
+            sys.exit(str(e))
+        base = run_one
+
+        def run_one(*args):
+            return base(*args, keep_channels=True)
     plain = o["frame_size"] is None and o["window"] is None and o["devices"] is None and o["batch_clips"] == 1 \
         and not os.path.isdir(o["inputfile"])
+    if plain and o["keep_channels"]:
+        return run_one(o["inputfile"], o["outdir"], o["model"], None, None, 0, 0, False)
     if plain:
         return train_auto_default(o["inputfile"], o["outdir"], o["model"])
     if os.path.isdir(o["inputfile"]):

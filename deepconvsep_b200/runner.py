@@ -81,7 +81,12 @@ def _num_samples(path):
 
 
 def separate_dataset(family, testdir, outdir, model, scale_factor=0.3, time_context=30, rank=0, world_size=1, device=0,
-                     **overrides):
+                     keep_channels=False, **overrides):
+    """keep_channels (family dsd): 2-channel stems in the same layout -- the soft masks of the downmix applied to each
+    channel of the mixture (Separator.separate_keep_channels), so that a multichannel evaluation scores real stereo
+    images."""
+    if keep_channels and family != "dsd":
+        raise ValueError("--keep-channels is for --family dsd (the stereo / ILD net, dsd_ild, is stereo already)")
     cfg = dict(TRAINER[family], **overrides)
     params = load_model(model) if isinstance(model, str) else model
     sep = Separator(params, arch=None if family == "ikala" else family, frame_size=cfg["frameSize"], hop=cfg["hopSize"],
@@ -95,9 +100,11 @@ def separate_dataset(family, testdir, outdir, model, scale_factor=0.3, time_cont
         wav, outs = jobs[idx]
         audioObj, sampleRate, bitrate = util.readAudioScipy(wav)
         assert sampleRate == 44100, "Sample rate needs to be 44100"
-        if family == "dsd_ild":                              # both channels in, stereo stems out
-            assert audioObj.ndim == 2 and audioObj.shape[1] == 2, "the stereo / ILD network needs 2-channel mixtures"
-            sep_audio = sep.separate_stereo(audioObj)        # [nsamples, nsrc, 2]
+        if family == "dsd_ild" or keep_channels:             # both channels in, stereo stems out
+            assert audioObj.ndim == 2 and audioObj.shape[1] == 2, "%s needs 2-channel mixtures" % (
+                "--keep-channels" if keep_channels else "the stereo / ILD network")
+            # [nsamples, nsrc, 2]
+            sep_audio = sep.separate_keep_channels(audioObj) if keep_channels else sep.separate_stereo(audioObj)
             for i, path in enumerate(outs):
                 os.makedirs(os.path.dirname(path), exist_ok=True)
                 util.writeAudioScipy(path, sep_audio[:, i, :].astype(np.float64), sampleRate, bitrate)
@@ -124,7 +131,11 @@ def main(argv=None):
     ap.add_argument("--out", required=True)
     ap.add_argument("--model", required=True)
     ap.add_argument("--scale-factor", type=float, default=0.3)
+    ap.add_argument("--keep-channels", action="store_true",
+                    help="--family dsd: 2-channel stems, the soft masks of the downmix applied to each channel")
     args = ap.parse_args(argv)
+    if args.keep_channels and args.family != "dsd":
+        ap.error("--keep-channels is for --family dsd")
     world, rank, local = (int(os.environ.get(k, d)) for k, d in (("WORLD_SIZE", "1"), ("RANK", "0"), ("LOCAL_RANK", "0")))
     if world > 1:
         import torch
@@ -135,7 +146,7 @@ def main(argv=None):
     import time
     t0 = time.time()
     secs, njobs = separate_dataset(args.family, args.db, args.out, args.model, args.scale_factor, rank=rank,
-                                   world_size=world, device=local)
+                                   world_size=world, device=local, keep_channels=args.keep_channels)
     tot, ms, _ = reduce_stats(secs, (time.time() - t0) * 1e3)
     if rank == 0:
         print("separated %d files, %.1f audio-s in %.2f s (%.0f x real time) on %d GPU(s)" % (njobs, tot, ms / 1e3,

@@ -72,7 +72,8 @@ int64_t dcs_launch_count(const dcs_ctx* ctx);
 
 /* Inspection tap (used by the parity tests): while set, every dcs_separate_audio* / *_host call on this ctx
  * also copies the blended masked spectra its inverse STFT consumed -- complex[nplanes][T][ldf],
- * ldf = dcs_padded_bins(N), nplanes = nsrc (x 2 channels for the stereo net) -- to d_S (capacity in
+ * ldf = dcs_padded_bins(N), nplanes = nsrc (x 2 channels, ordered (source, channel), for the stereo net and for
+ * dcs_separate_*keep_channels*) -- to d_S (capacity in
  * elements; the call fails if it is too small).  d_S = NULL switches it off.  These are the tensors
  * `overlapadd_multi(...)/scale * exp(j*phase)` of separate_dsd.py:301-304. */
 int dcs_set_spectrum_tap(dcs_ctx* ctx, dcs_complex* d_S, int64_t capacity);
@@ -217,6 +218,27 @@ int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan
                                   const int16_t* const* h_pcm, const int64_t* num_samples, int channels, int downmix,
                                   float scale_factor, int overlap, int patcher, int16_t* const* h_out,
                                   const int64_t* out_strides, void* stream);
+
+/* ---- keep-channels mode of the DSD100 / hiphopss network (DCS_ARCH_DSD only) ------------------------------ */
+/* Stereo stems from the mono network: the network sees the downmix mono = (l + r) * 0.5f (fp32, the downmix 1 of
+ * dcs_separate_pcm16_host), so its blended soft masks M_s are those of the mono call (separate_dsd.py:282-304); each
+ * is applied to the STFT X_c of channel c and inverted with that channel's phase: plane (s*2 + c) = iSTFT(M_s * X_c).
+ * With l == r every channel equals the mono call's stem; (stem_L + stem_R) / 2 equals it up to STFT rounding.
+ * d_audio float[2][audio_stride] (left, right; first num_samples valid) -> d_stems float[nsrc*2][stem_stride], plane
+ * (s*2 + c) = source s, channel c (the layout of dcs_separate_audio_stereo).  Other architectures are refused before
+ * anything is queued (the stereo / ILD net: dcs_separate_audio_stereo).  With the spectrum tap set, it holds nsrc*2
+ * planes ordered (source, channel). */
+int dcs_separate_audio_keep_channels(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const float* d_audio,
+                                     int64_t audio_stride, int64_t num_samples, float scale_factor, int overlap,
+                                     int patcher, float* d_stems, int64_t stem_stride, void* stream);
+/* the same on int16 stereo clips through the multi-clip scheduler of dcs_separate_batch_pcm16_host:
+ * h_pcm[i] int16[num_samples[i]][2] -> h_out[i] + s*2*out_strides[i] = source s as int16 [num_samples[i]][2]
+ * interleaved (what util.writeAudioScipy writes for a 2-channel stem, util.py:56-58), (int16)(stem*32767) per
+ * sample as in dcs_separate_pcm16_host.  Channels are decoded as pcm/32767 (fp32) and downmixed as above. */
+int dcs_separate_batch_pcm16_keep_channels_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, int nclips,
+                                                const int16_t* const* h_pcm, const int64_t* num_samples,
+                                                float scale_factor, int overlap, int patcher, int16_t* const* h_out,
+                                                const int64_t* out_strides, void* stream);
 
 #ifdef __cplusplus
 }
