@@ -26,6 +26,8 @@ _SIGS = {
     "dcs_launch_count": (_i64, [_p]),
     "dcs_set_spectrum_tap": (C.c_int, [_p, _p, _i64]),
     "dcs_set_pool_tap": (C.c_int, [_p, _p, _i64]),
+    "dcs_set_wiener": (C.c_int, [_p, C.c_int]),
+    "dcs_wiener_stereo": (C.c_int, [_p, _p, _i64, _p, _i64, C.c_int, _i64, _i64, C.c_int, C.c_int, _p]),
     "dcs_profile": (C.c_int, [_p, C.c_int]),
     "dcs_profile_read": (C.c_int, [_p, C.c_char_p, C.c_int, _p, C.c_int]),
     "dcs_stft_plan": (C.c_int, [_p, C.c_int, C.c_int, _p, _p, C.POINTER(_p)]),

@@ -88,7 +88,7 @@ using namespace dcs;
 
 // every device buffer of a context's workspace
 template <class Ctx, class F> static void for_each_buffer(Ctx* c, F f) {
-  for (auto* b : {&c->audio, &c->X, &c->mag, &c->S, &c->stems, &c->pcm_in[0], &c->pcm_in[1], &c->pcm_out[0], &c->pcm_out[1]}) f(*b);
+  for (auto* b : {&c->audio, &c->X, &c->mag, &c->S, &c->stems, &c->pcm_in[0], &c->pcm_in[1], &c->pcm_out[0], &c->pcm_out[1], &c->wiener}) f(*b);
   for (auto& b : c->net) f(b);
 }
 
@@ -148,6 +148,13 @@ int dcs_set_spectrum_tap(dcs_ctx* c, dcs_complex* d_S, int64_t capacity) {
   DCS_REQUIRE(c != nullptr && capacity >= 0, "dcs_set_spectrum_tap: bad argument");
   c->tap = (float2*)d_S;
   c->tap_cap = d_S ? capacity : 0;
+  return DCS_OK;
+}
+
+int dcs_set_wiener(dcs_ctx* c, int iterations) {
+  DCS_REQUIRE(c != nullptr, "dcs_set_wiener: NULL ctx");
+  DCS_REQUIRE(iterations >= 0, "dcs_set_wiener: iterations %d must be >= 0", iterations);
+  c->wiener_iters = iterations;
   return DCS_OK;
 }
 
@@ -514,7 +521,8 @@ static int check_clip(const char* fn, const dcs_ctx* ctx, const dcs_model* m, co
 
 // the workspace of a clip of L samples: nch STFT planes, nsrc x nch masked spectra, the score-informed net's input
 // channels; with `staged` also the device copies of host audio and stems.  keep (keep-channels mode of the DSD100
-// net): two STFT planes, one magnitude plane, nsrc x 2 spectra; staged: three audio planes (downmix, left, right)
+// net): two STFT planes, one magnitude plane, nsrc x 2 spectra; staged: three audio planes (downmix, left, right).
+// Two-channel stems with the Wiener post-filter on: its partial sums and covariances
 static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, bool staged, bool keep,
                           cudaStream_t st) {
   const int64_t plane = dcs_num_frames(L, p->hop) * dcs_padded_bins(p->N);
@@ -523,6 +531,8 @@ static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, i
   DCS_TRY(ctx->mag.ensure((size_t)m->nch * plane * sizeof(float), st));
   DCS_TRY(ctx->S.ensure((size_t)m->nsrc * nx * plane * sizeof(float2), st));
   if (m->arch == DCS_ARCH_BACH10_SCORE) DCS_TRY(ctx->net[NET_CHANS].ensure((size_t)m->sc.nch * plane * sizeof(float), st));
+  if (ctx->wiener_iters > 0 && m->nch * nx == 2)
+    DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, dcs_num_frames(L, p->hop), m->F), st));
   if (staged) {
     DCS_TRY(ctx->audio.ensure((size_t)(keep ? 3 : 1) * L * sizeof(float), st));
     DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * (keep ? 2 : 1) * L * sizeof(float), st));
@@ -533,7 +543,8 @@ static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, i
 // one clip, device to device: nch audio planes (audio_stride apart) -> nsrc x nch stem planes; d_filters: the
 // score filters that form the score-informed net's input channels.  d_mono (keep-channels mode, DSD100 net): the
 // downmix of the two audio planes; the network sees its magnitude, its masks are applied to the STFT of each
-// channel -> nsrc x 2 stem planes ordered (source, channel)
+// channel -> nsrc x 2 stem planes ordered (source, channel).  Two-channel stems (keep-channels, the stereo net) go
+// through the Wiener post-filter between the network and the iSTFT when dcs_set_wiener is above 0
 static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,
                          const float* d_filters, const float* d_mono, float scale_factor, int overlap, int patcher,
                          float* d_stems, int64_t stem_stride, cudaStream_t st) {
@@ -562,6 +573,8 @@ static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const fl
     in = chans;
   }
   DCS_TRY(run_network(ctx, m, in, plane, X, plane, nx, T, ldf, overlap, patcher, S, plane, st));
+  if (ctx->wiener_iters > 0 && nch * nx == 2)
+    DCS_TRY(launch_wiener(ctx, X, plane, S, plane, m->nsrc, T, ldf, m->F, ctx->wiener_iters, st));
   DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * nch * nx * plane, st));
   ProfScope ps(ctx, "istft_ola", st);
   return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc * nch * nx, T, ldf, plane, d_stems, L, stem_stride, st);
@@ -805,6 +818,18 @@ int dcs_separate_audio_keep_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, co
   }
   return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, mono, scale_factor, overlap, patcher, d_stems,
                        stem_stride, st);
+}
+
+// ------------------------------------------------------------------------------------ Wiener post-filter
+int dcs_wiener_stereo(dcs_ctx* ctx, const dcs_complex* d_X, int64_t x_plane, dcs_complex* d_S, int64_t src_stride, int nsrc,
+                      int64_t T, int64_t ldf, int F, int iterations, void* stream) {
+  DCS_REQUIRE(ctx && d_X && d_S, "dcs_wiener_stereo: NULL argument");
+  DCS_REQUIRE((uintptr_t)d_X % sizeof(float2) == 0 && (uintptr_t)d_S % sizeof(float2) == 0,
+              "dcs_wiener_stereo: spectra not 8-byte aligned");
+  DCS_TRY(wiener_check("dcs_wiener_stereo", nsrc, T, ldf, F, x_plane, src_stride, iterations));
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  return launch_wiener(ctx, (const float2*)d_X, x_plane, (float2*)d_S, src_stride, nsrc, T, ldf, F, iterations,
+                       (cudaStream_t)stream);
 }
 
 }  // extern "C"

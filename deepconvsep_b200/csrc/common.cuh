@@ -91,6 +91,8 @@ struct dcs_ctx {
   int64_t tap_cap = 0;
   uint8_t* pool_tap = nullptr;  // dcs_set_pool_tap: copy of the max-pool tie bits of the forward pass
   int64_t pool_tap_cap = 0;
+  int wiener_iters = 0;         // dcs_set_wiener: EM iterations of the stereo Wiener post-filter (0 = off)
+  dcs::DevBuf wiener;           // its partial sums, spatial covariances and mixture scale (wiener.cu)
 };
 
 struct dcs_stft {
@@ -270,5 +272,12 @@ int launch_pcm_decode_keep(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, float*
 int launch_downmix2(dcs_ctx* ctx, const float* d_audio, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st);
 int launch_pcm_encode_keep(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int64_t stem_stride, int16_t* d_out,
                            cudaStream_t st);
+
+// multichannel Wiener post-filter (wiener.cu): mixture channel c at X + c * x_plane, stem (j, c) at
+// S + (2 j + c) * src_stride, bins f < F filtered in place by `iterations` EM iterations
+int wiener_check(const char* fn, int nsrc, int64_t T, int64_t ldf, int F, int64_t x_plane, int64_t src_stride, int iterations);
+size_t wiener_workspace_bytes(int nsrc, int64_t T, int F);
+int launch_wiener(dcs_ctx* ctx, const float2* X, int64_t x_plane, float2* S, int64_t src_stride, int nsrc, int64_t T,
+                  int64_t ldf, int F, int iterations, cudaStream_t st);
 
 }  // namespace dcs

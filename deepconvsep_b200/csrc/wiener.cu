@@ -1,0 +1,253 @@
+// wiener.cu -- multichannel Wiener post-filter of stereo stems with EM re-estimation of each source's spatial
+// covariance (Duong, Vincent & Gribonval 2010; the filter the reference's util.py:633-719 `mwf` set out to be).
+//
+// Planes: mixture channel c at X + c * x_plane, stem (source j, channel c) at S + (2 j + c) * src_stride, each
+// complex[T][ldf]; bins f < F are filtered in place, pad bins are never touched.  Per iteration:
+//   v_j(t,f) = (|y_jL|^2 + |y_jR|^2) / 2
+//   R_j(f)   = sum_t y_j y_j^H / (eps s^2 + sum_t v_j)        eps = 2^-23, s = max(1, max|x| / 10)
+//   C(t,f)   = sum_j v_j R_j + sqrt(eps) s^2 I
+//   y_j      <- v_j R_j C^-1 x
+// C is near rank one wherever one source dominates or the channels nearly agree (cond ~ 1e6 at full scale), so
+// C, its adjugate and determinant and v R C^-1 x are fp64 in registers; the planes stay fp32 in HBM.
+//
+// One thread per bin walks a chunk of kWienerFrames frames; the grid is bin tiles x frame chunks.  The sums over
+// t are per-chunk fp64 partials reduced in chunk order: no atomics, the same bits on every run.
+#include "common.cuh"
+
+namespace dcs {
+namespace {
+
+constexpr int kWienerBins = 128;     // threads per block: consecutive bins, coalesced float2 rows
+constexpr int kWienerFrames = 128;   // frames per chunk: partials are 32 B per (source, bin) per 128 frames
+constexpr int kReduceThreads = 256;
+constexpr double kEps = 1.1920928955078125e-07;   // 2^-23 = FLT_EPSILON
+
+struct WienerArgs {
+  const float2* X; int64_t x_plane;
+  float2* S; int64_t src_stride;
+  int64_t T, ldf;
+  int F, nchunks, ntiles;
+  double* part;    // [nchunks][nsrc][4][F]: per-chunk sums of |yL|^2, |yR|^2, Re yL conj(yR), Im yL conj(yR)
+  double* Q;       // [nsrc][4][F]: the same summed over all chunks (chunk order)
+  double* pmax;    // [nchunks][ntiles]: per-block max of |x|^2 over both channels
+  double* scale;   // [1]: s
+};
+
+__device__ __forceinline__ void accumulate(double* q, float2 l, float2 r) {
+  const double a = l.x, b = l.y, c = r.x, d = r.y;
+  q[0] += fma(a, a, b * b);
+  q[1] += fma(c, c, d * d);
+  q[2] += fma(a, c, b * d);
+  q[3] += fma(b, c, -(a * d));
+}
+
+template <int NSRC>
+__device__ __forceinline__ void store_partials(const WienerArgs& a, const double (&acc)[NSRC][4], int f) {
+  double* p = a.part + (int64_t)blockIdx.y * NSRC * 4 * a.F + f;
+#pragma unroll
+  for (int j = 0; j < NSRC; ++j)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) p[(int64_t)(j * 4 + q) * a.F] = acc[j][q];
+}
+
+// the network's stems -> per-chunk partial sums, and the per-block max of |x|^2
+template <int NSRC>
+__global__ void __launch_bounds__(kWienerBins) wiener_init_kernel(const WienerArgs a) {
+  const int f = blockIdx.x * kWienerBins + threadIdx.x;
+  const int64_t t0 = (int64_t)blockIdx.y * kWienerFrames, t1 = min(a.T, t0 + kWienerFrames);
+  double mx = 0.0;
+  if (f < a.F) {
+    double acc[NSRC][4];
+#pragma unroll
+    for (int j = 0; j < NSRC; ++j)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[j][q] = 0.0;
+    for (int64_t t = t0; t < t1; ++t) {
+      const int64_t o = t * a.ldf + f;
+      const float2 xl = a.X[o], xr = a.X[a.x_plane + o];
+      mx = fmax(mx, fmax((double)xl.x * xl.x + (double)xl.y * xl.y, (double)xr.x * xr.x + (double)xr.y * xr.y));
+#pragma unroll
+      for (int j = 0; j < NSRC; ++j) accumulate(acc[j], a.S[(2 * j) * a.src_stride + o], a.S[(2 * j + 1) * a.src_stride + o]);
+    }
+    store_partials<NSRC>(a, acc, f);
+  }
+  __shared__ double wmax[kWienerBins / 32];
+#pragma unroll
+  for (int k = 16; k > 0; k >>= 1) mx = fmax(mx, __shfl_down_sync(0xffffffffu, mx, k));
+  if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = mx;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < kWienerBins / 32; ++w) mx = fmax(mx, wmax[w]);
+    a.pmax[(int64_t)blockIdx.y * a.ntiles + blockIdx.x] = mx;
+  }
+}
+
+// partials -> Q in chunk order, one thread per (source, quantity, bin); the extra last block: s from the maxima
+__global__ void __launch_bounds__(kReduceThreads) wiener_reduce_kernel(const WienerArgs a, int64_t n) {
+  if (blockIdx.x == gridDim.x - 1) {
+    __shared__ double wmax[kReduceThreads / 32];
+    double mx = 0.0;
+    for (int64_t i = threadIdx.x; i < (int64_t)a.nchunks * a.ntiles; i += kReduceThreads) mx = fmax(mx, a.pmax[i]);
+#pragma unroll
+    for (int k = 16; k > 0; k >>= 1) mx = fmax(mx, __shfl_down_sync(0xffffffffu, mx, k));
+    if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = mx;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int w = 1; w < kReduceThreads / 32; ++w) mx = fmax(mx, wmax[w]);
+      *a.scale = fmax(1.0, sqrt(mx) / 10.0);
+    }
+    return;
+  }
+  const int64_t e = (int64_t)blockIdx.x * kReduceThreads + threadIdx.x;
+  if (e >= n) return;
+  double sum = 0.0;
+#pragma unroll 8
+  for (int c = 0; c < a.nchunks; ++c) sum += a.part[(int64_t)c * n + e];
+  a.Q[e] = sum;
+}
+
+// one EM iteration in place; STATS: also the next iteration's partial sums of the stems it stores
+template <int NSRC, bool STATS>
+__global__ void __launch_bounds__(kWienerBins) wiener_em_kernel(const WienerArgs a) {
+  const int f = blockIdx.x * kWienerBins + threadIdx.x;
+  if (f >= a.F) return;
+  const int64_t t0 = (int64_t)blockIdx.y * kWienerFrames, t1 = min(a.T, t0 + kWienerFrames);
+  const double s2 = *a.scale * *a.scale, es2 = kEps * s2, ds2 = sqrt(kEps) * s2;
+  double r[NSRC][4];   // R_j(f): [0][0], [1][1], Re [0][1], Im [0][1]
+#pragma unroll
+  for (int j = 0; j < NSRC; ++j) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) r[j][q] = a.Q[(int64_t)(j * 4 + q) * a.F + f];
+    const double inv = 1.0 / (es2 + 0.5 * (r[j][0] + r[j][1]));
+#pragma unroll
+    for (int q = 0; q < 4; ++q) r[j][q] *= inv;
+  }
+  double acc[NSRC][4];
+#pragma unroll
+  for (int j = 0; j < NSRC; ++j)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) acc[j][q] = 0.0;
+  for (int64_t t = t0; t < t1; ++t) {
+    const int64_t o = t * a.ldf + f;
+    const float2 xl = a.X[o], xr = a.X[a.x_plane + o];
+    double v[NSRC];
+#pragma unroll
+    for (int j = 0; j < NSRC; ++j) {
+      const float2 l = a.S[(2 * j) * a.src_stride + o], rr = a.S[(2 * j + 1) * a.src_stride + o];
+      v[j] = 0.5 * (((double)l.x * l.x + (double)l.y * l.y) + ((double)rr.x * rr.x + (double)rr.y * rr.y));
+    }
+    // C = sum_j v_j R_j + delta s^2 I: [[c11, c12], [conj(c12), c22]].  The fma trees of the two channels mirror
+    // each other, so that equal channels (c11 = c22, Im c12 = 0) give bit-identical outputs
+    double c11 = 0.0, c22 = 0.0, c12r = 0.0, c12i = 0.0;
+#pragma unroll
+    for (int j = 0; j < NSRC; ++j) {
+      c11 = fma(v[j], r[j][0], c11);
+      c22 = fma(v[j], r[j][1], c22);
+      c12r = fma(v[j], r[j][2], c12r);
+      c12i = fma(v[j], r[j][3], c12i);
+    }
+    c11 += ds2;
+    c22 += ds2;
+    const double idet = 1.0 / fma(c11, c22, -fma(c12r, c12r, c12i * c12i));
+    // z = C^-1 x = adj(C) x / det
+    const double x1r = xl.x, x1i = xl.y, x2r = xr.x, x2i = xr.y;
+    const double z1r = fma(c22, x1r, -fma(c12r, x2r, -(c12i * x2i))) * idet;
+    const double z1i = fma(c22, x1i, -fma(c12r, x2i, c12i * x2r)) * idet;
+    const double z2r = fma(c11, x2r, -fma(c12r, x1r, c12i * x1i)) * idet;
+    const double z2i = fma(c11, x2i, -fma(c12r, x1i, -(c12i * x1r))) * idet;
+#pragma unroll
+    for (int j = 0; j < NSRC; ++j) {
+      // y_j = v_j R_j z
+      const double r0 = r[j][0], r1 = r[j][1], r2 = r[j][2], r3 = r[j][3];
+      const double ylr = v[j] * fma(r0, z1r, fma(r2, z2r, -(r3 * z2i))), yli = v[j] * fma(r0, z1i, fma(r2, z2i, r3 * z2r));
+      const double yrr = v[j] * fma(r1, z2r, fma(r2, z1r, r3 * z1i)), yri = v[j] * fma(r1, z2i, fma(r2, z1i, -(r3 * z1r)));
+      const float2 l = make_float2((float)ylr, (float)yli), rr = make_float2((float)yrr, (float)yri);
+      a.S[(2 * j) * a.src_stride + o] = l;
+      a.S[(2 * j + 1) * a.src_stride + o] = rr;
+      if (STATS) accumulate(acc[j], l, rr);
+    }
+  }
+  if (STATS) store_partials<NSRC>(a, acc, f);
+}
+
+template <int NSRC>
+int launch_wiener_n(dcs_ctx* ctx, const WienerArgs& a, int iterations, cudaStream_t st) {
+  const dim3 grid((unsigned)a.ntiles, (unsigned)a.nchunks);
+  const int64_t n = (int64_t)NSRC * 4 * a.F;
+  const unsigned rgrid = (unsigned)ceil_div64(n, kReduceThreads) + 1;
+  {
+    ProfScope ps(ctx, "wiener_init", st);
+    wiener_init_kernel<NSRC><<<grid, kWienerBins, 0, st>>>(a);
+    DCS_CHECK_LAUNCH();
+    ctx->launches++;
+    wiener_reduce_kernel<<<rgrid, kReduceThreads, 0, st>>>(a, n);
+    DCS_CHECK_LAUNCH();
+    ctx->launches++;
+  }
+  for (int k = 1; k <= iterations; ++k) {
+    ProfScope ps(ctx, "wiener_em", st);
+    if (k < iterations) {
+      wiener_em_kernel<NSRC, true><<<grid, kWienerBins, 0, st>>>(a);
+      DCS_CHECK_LAUNCH();
+      ctx->launches++;
+      wiener_reduce_kernel<<<rgrid, kReduceThreads, 0, st>>>(a, n);
+    } else {
+      wiener_em_kernel<NSRC, false><<<grid, kWienerBins, 0, st>>>(a);
+    }
+    DCS_CHECK_LAUNCH();
+    ctx->launches++;
+  }
+  return DCS_OK;
+}
+
+struct WienerLayout {
+  int nchunks, ntiles;
+  int64_t part, Q, pmax, total;   // offsets / size in doubles
+};
+
+WienerLayout wiener_layout(int nsrc, int64_t T, int F) {
+  WienerLayout l;
+  l.nchunks = (int)ceil_div64(T, kWienerFrames);
+  l.ntiles = (int)ceil_div64(F, kWienerBins);
+  const int64_t per = (int64_t)nsrc * 4 * F;
+  l.part = 0;
+  l.Q = (int64_t)l.nchunks * per;
+  l.pmax = l.Q + per;
+  l.total = l.pmax + (int64_t)l.nchunks * l.ntiles + 1;
+  return l;
+}
+
+}  // namespace
+
+int wiener_check(const char* fn, int nsrc, int64_t T, int64_t ldf, int F, int64_t x_plane, int64_t src_stride, int iterations) {
+  DCS_REQUIRE(iterations >= 0, "%s: iterations %d must be >= 0", fn, iterations);
+  DCS_REQUIRE(nsrc >= 1 && nsrc <= 4, "%s: nsrc %d not in [1, 4]", fn, nsrc);
+  DCS_REQUIRE(T > 0 && ceil_div64(T, kWienerFrames) <= 65535, "%s: %lld frames out of range", fn, (long long)T);
+  DCS_REQUIRE(F > 0 && ldf >= F, "%s: bins %d / row stride %lld", fn, F, (long long)ldf);
+  DCS_REQUIRE(x_plane >= T * ldf && src_stride >= T * ldf, "%s: plane strides %lld / %lld below T * ldf = %lld", fn,
+              (long long)x_plane, (long long)src_stride, (long long)(T * ldf));
+  return DCS_OK;
+}
+
+size_t wiener_workspace_bytes(int nsrc, int64_t T, int F) { return (size_t)wiener_layout(nsrc, T, F).total * sizeof(double); }
+
+int launch_wiener(dcs_ctx* ctx, const float2* X, int64_t x_plane, float2* S, int64_t src_stride, int nsrc, int64_t T,
+                  int64_t ldf, int F, int iterations, cudaStream_t st) {
+  if (iterations <= 0) return DCS_OK;
+  const WienerLayout l = wiener_layout(nsrc, T, F);
+  DCS_TRY(ctx->wiener.ensure((size_t)l.total * sizeof(double), st));
+  double* w = ctx->wiener.as<double>();
+  WienerArgs a;
+  a.X = X; a.x_plane = x_plane; a.S = S; a.src_stride = src_stride; a.T = T; a.ldf = ldf;
+  a.F = F; a.nchunks = l.nchunks; a.ntiles = l.ntiles;
+  a.part = w + l.part; a.Q = w + l.Q; a.pmax = w + l.pmax; a.scale = w + l.total - 1;
+  switch (nsrc) {
+    case 1: return launch_wiener_n<1>(ctx, a, iterations, st);
+    case 2: return launch_wiener_n<2>(ctx, a, iterations, st);
+    case 3: return launch_wiener_n<3>(ctx, a, iterations, st);
+    case 4: return launch_wiener_n<4>(ctx, a, iterations, st);
+  }
+  DCS_REQUIRE(false, "wiener: nsrc %d not in [1, 4]", nsrc);
+}
+
+}  // namespace dcs

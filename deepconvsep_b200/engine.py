@@ -46,6 +46,25 @@ def _stream_ptr(stream=None, device=None):
     return C.c_void_p(s.cuda_stream)
 
 
+def wiener_stereo(ctx, X, S, iterations, stream=None, num_bins=None):
+    """Multichannel Wiener post-filter with EM spatial covariances (dcs_wiener_stereo), in place on device spectra:
+    X torch complex64 cuda [2, T, ldf] (the mixture's channels), S [nsrc * 2, T, ldf] (the stems, planes ordered
+    (source, channel), nsrc <= 4).  Bins >= num_bins (default ldf) are left alone.  Returns S."""
+    import torch
+    if X.dim() != 3 or X.shape[0] != 2 or S.dim() != 3 or S.shape[0] % 2 or tuple(S.shape[1:]) != tuple(X.shape[1:]):
+        raise ValueError("wiener_stereo needs X [2, T, ldf] and S [nsrc * 2, T, ldf], got %r and %r"
+                         % (tuple(X.shape), tuple(S.shape)))
+    if X.dtype != torch.complex64 or S.dtype != torch.complex64 or not (X.is_cuda and S.is_cuda):
+        raise ValueError("wiener_stereo needs complex64 cuda tensors")
+    if X.stride(2) != 1 or X.stride(1) != X.shape[2] or S.stride(2) != 1 or S.stride(1) != S.shape[2]:
+        raise ValueError("wiener_stereo needs contiguous [T, ldf] planes")
+    T, ldf = int(X.shape[1]), int(X.shape[2])
+    F = ldf if num_bins is None else int(num_bins)
+    _lib.check(ctx.lib.dcs_wiener_stereo(ctx.handle, _ptr(X), X.stride(0), _ptr(S), S.stride(0), S.shape[0] // 2, T, ldf,
+                                         F, int(iterations), _stream_ptr(stream, ctx.device)))
+    return S
+
+
 class Context(object):
     """One dcs_ctx = one device + the workspace of one in-flight pipeline."""
 
@@ -64,6 +83,10 @@ class Context(object):
 
     def profile(self, enable):
         _lib.check(self.lib.dcs_profile(self.handle, 1 if enable else 0))
+
+    def set_wiener(self, iterations):
+        """EM iterations of the Wiener post-filter on the context's two-channel stems (dcs_set_wiener; 0 = off)"""
+        _lib.check(self.lib.dcs_set_wiener(self.handle, int(iterations)))
 
     def profile_read(self, max_n=4096):
         """[(stage name, milliseconds)] recorded since profiling was enabled (synchronises)."""
@@ -243,6 +266,13 @@ class Separator(object):
         self.sources = d["sources"]
         self.lib = self.ctx.lib
 
+    def _stereo_wiener(self, wiener, stereo):
+        """set the Wiener post-filter for the next call; it only exists for two-channel stems"""
+        if wiener and not stereo:
+            raise ValueError("wiener=%r: the Wiener post-filter needs two-channel stems (keep_channels=True on the "
+                             "DSD100 / hiphopss network, or the stereo / ILD network)" % (wiener,))
+        self.ctx.set_wiener(wiener)
+
     # ---- host buffers (numpy): H2D + pipeline + D2H inside the call ----
     def separate(self, audio, out=None):
         """audio: 1-D float array (any float dtype) -> float32 [nsrc, L].  `audio` / `out` may be
@@ -257,12 +287,15 @@ class Separator(object):
                                               _stream_ptr(None, self.ctx.device)))
         return out
 
-    def separate_pcm16(self, pcm, downmix=1, out=None, keep_channels=False):
+    def separate_pcm16(self, pcm, downmix=1, out=None, keep_channels=False, wiener=0):
         """int16 wav samples [L] or [L, channels] -> int16 [nsrc, L] (train_auto's wav contract).
         keep_channels=True (DSD100 / hiphopss net, stereo [L, 2] in): int16 [nsrc, L, 2] stereo stems, see
-        separate_keep_channels."""
+        separate_keep_channels; wiener: EM iterations of the Wiener post-filter on them (keep_channels only)."""
         if keep_channels:
-            return self.separate_pcm16_batch([pcm], outs=None if out is None else [out], keep_channels=True)[0]
+            return self.separate_pcm16_batch([pcm], outs=None if out is None else [out], keep_channels=True,
+                                             wiener=wiener)[0]
+        if wiener:
+            self._stereo_wiener(wiener, False)
         p = np.ascontiguousarray(pcm, dtype=np.int16)
         L = p.shape[0]
         ch = 1 if p.ndim == 1 else p.shape[1]
@@ -273,17 +306,20 @@ class Separator(object):
                                                     self.patcher, out.ctypes.data, L, _stream_ptr(None, self.ctx.device)))
         return out
 
-    def separate_pcm16_batch(self, clips, downmix=1, outs=None, keep_channels=False):
+    def separate_pcm16_batch(self, clips, downmix=1, outs=None, keep_channels=False, wiener=0):
         """Several clips through the context's multi-clip scheduler (dcs_separate_batch_pcm16_host): H2D of clip i+1,
         the kernels of clip i and D2H of clip i-1 overlap.  clips: list of int16 arrays [L] or [L, channels] (same
         channel count; pinned for real overlap) -> list of int16 [nsrc, L].  keep_channels=True: stereo clips
-        [L, 2] -> list of int16 [nsrc, L, 2] (dcs_separate_batch_pcm16_keep_channels_host)."""
+        [L, 2] -> list of int16 [nsrc, L, 2] (dcs_separate_batch_pcm16_keep_channels_host), with `wiener` EM iterations
+        of the Wiener post-filter on each clip's stems."""
+        if wiener and not keep_channels:
+            self._stereo_wiener(wiener, False)
         ps = [np.ascontiguousarray(c, dtype=np.int16) for c in clips]
         n = len(ps)
         if n == 0:
             return []
         if keep_channels:
-            return self._pcm16_batch_keep_channels(ps, outs)
+            return self._pcm16_batch_keep_channels(ps, outs, wiener)
         ch = 1 if ps[0].ndim == 1 else ps[0].shape[1]
         assert all((1 if p_.ndim == 1 else p_.shape[1]) == ch for p_ in ps), "all clips must have the same channel count"
         Ls = np.array([p_.shape[0] for p_ in ps], dtype=np.int64)
@@ -298,7 +334,7 @@ class Separator(object):
                                                           _stream_ptr(None, self.ctx.device)))
         return outs
 
-    def _pcm16_batch_keep_channels(self, ps, outs):
+    def _pcm16_batch_keep_channels(self, ps, outs, wiener=0):
         for p_ in ps:
             if p_.ndim != 2 or p_.shape[1] != 2:
                 raise ValueError("keep_channels needs stereo int16 clips [L, 2], got shape %r" % (p_.shape,))
@@ -309,6 +345,7 @@ class Separator(object):
         assert all(o.dtype == np.int16 and o.shape == (self.nsrc, int(L), 2) and o.flags.c_contiguous for o, L in zip(outs, Ls))
         pin = (C.c_void_p * n)(*[p_.ctypes.data for p_ in ps])
         pout = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
+        self._stereo_wiener(wiener, True)
         _lib.check(self.lib.dcs_separate_batch_pcm16_keep_channels_host(
             self.ctx.handle, self.model.handle, self.stft.handle, n, pin, Ls.ctypes.data, self.scale_factor, self.overlap,
             self.patcher, pout, Ls.ctypes.data, _stream_ptr(None, self.ctx.device)))
@@ -352,10 +389,11 @@ class Separator(object):
                                                      outd.stride(0), _stream_ptr(stream, self.ctx.device)))
         return outd.cpu().numpy() if host else outd
 
-    def separate_stereo(self, audio, out=None, stream=None):
+    def separate_stereo(self, audio, out=None, stream=None, wiener=0):
         """Stereo / ILD network (examples/dsd100_2ch_ILD/trainCNN_ILD_DSD100.py:299-327): audio float
         [L, 2] (numpy) or [2, L] (cuda tensor) -> `sep_audio` float32 [L, nsrc, 2] (numpy) or the device
-        planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> cuda tensor out)."""
+        planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> cuda tensor out).  wiener: EM iterations of
+        the multichannel Wiener post-filter (dcs_set_wiener) on the network's spectra, 0 = off."""
         import torch
         host = not hasattr(audio, "is_cuda")
         if host:
@@ -367,6 +405,7 @@ class Separator(object):
             assert x.dim() == 2 and x.shape[0] == 2 and x.dtype == torch.float32
         L = x.shape[1]
         outd = out if (out is not None and not host) else torch.empty((self.nsrc * 2, L), dtype=torch.float32, device=x.device)
+        self._stereo_wiener(wiener, True)
         _lib.check(self.lib.dcs_separate_audio_stereo(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), x.stride(0), L,
                                                       self.scale_factor, self.overlap, self.patcher, _ptr(outd), outd.stride(0),
                                                       _stream_ptr(stream, self.ctx.device)))
@@ -374,11 +413,12 @@ class Separator(object):
             return outd
         return np.ascontiguousarray(outd.cpu().numpy().reshape(self.nsrc, 2, L).transpose(2, 0, 1))
 
-    def separate_keep_channels(self, audio, out=None, stream=None):
+    def separate_keep_channels(self, audio, out=None, stream=None, wiener=0):
         """Stereo stems from the DSD100 / hiphopss network (dcs_separate_audio_keep_channels): the network sees the
         downmix (l + r) * 0.5, its soft masks are applied to each channel's STFT and inverted with that channel's
         phase.  audio float [L, 2] (numpy) or [2, L] (cuda tensor) -> float32 [L, nsrc, 2] (numpy, the layout of
-        separate_stereo) or the device planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out)."""
+        separate_stereo) or the device planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out).
+        wiener: EM iterations of the multichannel Wiener post-filter (dcs_set_wiener) on the masked spectra, 0 = off."""
         import torch
         host = not hasattr(audio, "is_cuda")
         if host:
@@ -391,6 +431,7 @@ class Separator(object):
             assert x.dim() == 2 and x.shape[0] == 2 and x.dtype == torch.float32
         L = x.shape[1]
         outd = out if (out is not None and not host) else torch.empty((self.nsrc * 2, L), dtype=torch.float32, device=x.device)
+        self._stereo_wiener(wiener, True)
         _lib.check(self.lib.dcs_separate_audio_keep_channels(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x),
                                                              x.stride(0), L, self.scale_factor, self.overlap, self.patcher,
                                                              _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
@@ -398,13 +439,17 @@ class Separator(object):
             return outd
         return np.ascontiguousarray(outd.cpu().numpy().reshape(self.nsrc, 2, L).transpose(2, 0, 1))
 
-    def separate_tapped(self, audio, filters=None, pool=False, keep_channels=False):
+    def separate_tapped(self, audio, filters=None, pool=False, keep_channels=False, wiener=0):
         """Parity-test entry: the same pipeline as separate() / separate_score() / separate_stereo() /
         separate_keep_channels() (keep_channels=True) with the spectrum tap on (dcs_set_spectrum_tap) -> (stems as
         that call returns them, masked spectra complex64 numpy [nplanes, T, F] -- the tensors the inverse STFT of THIS
         call consumed, (source, channel) planes for the stereo outputs).
-        pool=True (max-pool net): also the tie bits uint8 [T, WP, 32] of this call (dcs_set_pool_tap)."""
+        pool=True (max-pool net): also the tie bits uint8 [T, WP, 32] of this call (dcs_set_pool_tap).
+        wiener: EM iterations of the Wiener post-filter (two-channel stems only); the tap then holds the filtered spectra."""
         import torch
+        stereo = keep_channels or self.model.arch == "dsd_ild"
+        if wiener and not stereo:
+            self._stereo_wiener(wiener, False)
         a = np.asarray(audio)
         L = a.shape[0]
         T = self.stft.num_frames(L)
@@ -419,11 +464,11 @@ class Separator(object):
             _lib.check(self.lib.dcs_set_pool_tap(self.ctx.handle, _ptr(bits), bits.numel()))
         try:
             if keep_channels:
-                out = self.separate_keep_channels(a)
+                out = self.separate_keep_channels(a, wiener=wiener)
             elif self.model.arch == "bach10_score":
                 out = self.separate_score(a, filters)
             elif self.model.arch == "dsd_ild":
-                out = self.separate_stereo(a)
+                out = self.separate_stereo(a, wiener=wiener)
             else:
                 out = self.separate(a)
             torch.cuda.synchronize(self.stft.dev)

@@ -52,11 +52,22 @@ def check_keep_channels(family, audioObj=None, filein=""):
                          % (filein, 1 if audioObj.ndim == 1 else audioObj.shape[1]))
 
 
+def check_wiener(wiener, keep_channels):
+    """the Wiener post-filter works on two-channel stems: it needs keep_channels; raises ValueError otherwise"""
+    if wiener < 0:
+        raise ValueError("--wiener %d: the number of EM iterations cannot be negative" % wiener)
+    if wiener and not keep_channels:
+        raise ValueError("--wiener needs --keep-channels: the Wiener post-filter works on two-channel stems")
+
+
 def run(family, filein, outdir, model, scale_factor, time_context, overlap, batch_size, input_size, frame_size, hop,
-        out_name, window=None, device=0, slot=0, keep_channels=False):
+        out_name, window=None, device=0, slot=0, keep_channels=False, wiener=0):
     """wav in -> one int16 wav per source in `outdir`.  `batch_size` is accepted for signature
     compatibility; the CUDA path has no patch batches.  keep_channels (DSD100 / hiphopss, 2-channel wav): one
-    2-channel wav per source -- the soft masks of the downmix applied to each channel."""
+    2-channel wav per source -- the soft masks of the downmix applied to each channel; wiener: that many EM iterations
+    of the multichannel Wiener post-filter on them (keep_channels only)."""
+    check_wiener(wiener, keep_channels)
+    wkw = {"wiener": wiener} if wiener else {}
     d = dict(FAMILY_DEFAULTS[family])
     if window is not None:
         d["window"] = window
@@ -74,10 +85,10 @@ def run(family, filein, outdir, model, scale_factor, time_context, overlap, batc
         sep = get_separator(model, arch, frame_size, hop, d["window"], scale_factor, time_context, overlap, input_size,
                             device=device, slot=slot)
         if audioObj.dtype == np.int16:
-            stems16 = sep.separate_pcm16(audioObj, keep_channels=True)             # [nsrc, L, 2], int16 path on the GPU
+            stems16 = sep.separate_pcm16(audioObj, keep_channels=True, **wkw)      # [nsrc, L, 2], int16 path on the GPU
         else:
             maxv = np.finfo(audioObj.dtype).max if np.issubdtype(audioObj.dtype, np.floating) else np.iinfo(audioObj.dtype).max
-            stems = sep.separate_keep_channels(audioObj.astype('float') / maxv)    # [L, nsrc, 2]
+            stems = sep.separate_keep_channels(audioObj.astype('float') / maxv, **wkw)    # [L, nsrc, 2]
             stems16 = (stems.transpose(1, 0, 2).astype(np.float64) * np.iinfo(np.int16).max).astype('int16')
     elif isinstance(device, (list, tuple)):
         # one recording over several GPUs: hop- and patch-aligned segments with margins, one host thread per device,
@@ -108,11 +119,12 @@ def run(family, filein, outdir, model, scale_factor, time_context, overlap, batc
 
 
 # ---- command line shared by the separate_*.py scripts ------------------------------------------------------
-LONG_OPTS = ["ifile=", "odir=", "mfile=", "frame-size=", "window=", "devices=", "batch-clips=", "keep-channels"]
+LONG_OPTS = ["ifile=", "odir=", "mfile=", "frame-size=", "window=", "devices=", "batch-clips=", "keep-channels", "wiener="]
 EXTRA_USAGE = ("  optional: --frame-size N (STFT frame, feat_size = N/2+1)  --window hanning|blackmanharris|sinebell\n"
                "            --devices 0,1,...  --batch-clips K (clips in flight per device); with these, -i may be a directory of wavs\n"
                "            (one wav and several devices: the recording itself is cut into segments over the devices)\n"
-               "            --keep-channels (DSD100 / hiphopss, 2-channel wavs): 2-channel stems, the downmix's masks on each channel")
+               "            --keep-channels (DSD100 / hiphopss, 2-channel wavs): 2-channel stems, the downmix's masks on each channel\n"
+               "            --wiener K (with --keep-channels): K EM iterations of the multichannel Wiener post-filter on them")
 
 
 def parse_cli(argv, usage):
@@ -126,7 +138,7 @@ def parse_cli(argv, usage):
         print(EXTRA_USAGE)
         sys.exit(2)
     o = {"inputfile": None, "outdir": None, "model": None, "frame_size": None, "window": None, "devices": None, "batch_clips": 1,
-         "keep_channels": False}
+         "keep_channels": False, "wiener": 0}
     for opt, arg in opts:
         if opt == "-h":
             print(usage)
@@ -148,6 +160,8 @@ def parse_cli(argv, usage):
             o["batch_clips"] = max(1, int(arg))
         elif opt == "--keep-channels":
             o["keep_channels"] = True
+        elif opt == "--wiener":
+            o["wiener"] = int(arg)
     if o["inputfile"] is None or o["outdir"] is None or o["model"] is None:
         print(usage)
         sys.exit(2)
@@ -157,18 +171,26 @@ def parse_cli(argv, usage):
 def cli_main(argv, usage, train_auto_default, run_one, family=None):
     """`train_auto_default(inputfile, outdir, model)` = the script's literal reference call (no extra flag given);
     `run_one(filein, outdir, model, frame_size, window, device, slot, several_clips)` = the same with the overrides
-    (with --keep-channels also keep_channels=True; only the DSD100 / hiphopss script, family "dsd", takes it)."""
+    (with --keep-channels also keep_channels=True, and wiener=K with --wiener K; only the DSD100 / hiphopss script,
+    family "dsd", takes them)."""
     import sys
     o = parse_cli(argv, usage)
+    try:
+        check_wiener(o["wiener"], o["keep_channels"])
+    except ValueError as e:
+        sys.exit(str(e))
     if o["keep_channels"]:
         try:
             check_keep_channels(family)
         except ValueError as e:
             sys.exit(str(e))
         base = run_one
+        kw = {"keep_channels": True}
+        if o["wiener"]:
+            kw["wiener"] = o["wiener"]
 
         def run_one(*args):
-            return base(*args, keep_channels=True)
+            return base(*args, **kw)
     plain = o["frame_size"] is None and o["window"] is None and o["devices"] is None and o["batch_clips"] == 1 \
         and not os.path.isdir(o["inputfile"])
     if plain and o["keep_channels"]:

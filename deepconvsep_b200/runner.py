@@ -81,12 +81,18 @@ def _num_samples(path):
 
 
 def separate_dataset(family, testdir, outdir, model, scale_factor=0.3, time_context=30, rank=0, world_size=1, device=0,
-                     keep_channels=False, **overrides):
+                     keep_channels=False, wiener=0, **overrides):
     """keep_channels (family dsd): 2-channel stems in the same layout -- the soft masks of the downmix applied to each
     channel of the mixture (Separator.separate_keep_channels), so that a multichannel evaluation scores real stereo
-    images."""
+    images.  wiener (family dsd with keep_channels, or dsd_ild): that many EM iterations of the multichannel Wiener
+    post-filter on the stereo stems."""
     if keep_channels and family != "dsd":
         raise ValueError("--keep-channels is for --family dsd (the stereo / ILD net, dsd_ild, is stereo already)")
+    if wiener < 0:
+        raise ValueError("--wiener %d: the number of EM iterations cannot be negative" % wiener)
+    if wiener and not (keep_channels or family == "dsd_ild"):
+        raise ValueError("--wiener needs stereo stems: --family dsd --keep-channels, or --family dsd_ild")
+    wkw = {"wiener": wiener} if wiener else {}
     cfg = dict(TRAINER[family], **overrides)
     params = load_model(model) if isinstance(model, str) else model
     sep = Separator(params, arch=None if family == "ikala" else family, frame_size=cfg["frameSize"], hop=cfg["hopSize"],
@@ -104,7 +110,7 @@ def separate_dataset(family, testdir, outdir, model, scale_factor=0.3, time_cont
             assert audioObj.ndim == 2 and audioObj.shape[1] == 2, "%s needs 2-channel mixtures" % (
                 "--keep-channels" if keep_channels else "the stereo / ILD network")
             # [nsamples, nsrc, 2]
-            sep_audio = sep.separate_keep_channels(audioObj) if keep_channels else sep.separate_stereo(audioObj)
+            sep_audio = sep.separate_keep_channels(audioObj, **wkw) if keep_channels else sep.separate_stereo(audioObj, **wkw)
             for i, path in enumerate(outs):
                 os.makedirs(os.path.dirname(path), exist_ok=True)
                 util.writeAudioScipy(path, sep_audio[:, i, :].astype(np.float64), sampleRate, bitrate)
@@ -133,9 +139,16 @@ def main(argv=None):
     ap.add_argument("--scale-factor", type=float, default=0.3)
     ap.add_argument("--keep-channels", action="store_true",
                     help="--family dsd: 2-channel stems, the soft masks of the downmix applied to each channel")
+    ap.add_argument("--wiener", type=int, default=0, metavar="K",
+                    help="K EM iterations of the multichannel Wiener post-filter on the stereo stems "
+                         "(--family dsd --keep-channels, or --family dsd_ild)")
     args = ap.parse_args(argv)
     if args.keep_channels and args.family != "dsd":
         ap.error("--keep-channels is for --family dsd")
+    if args.wiener < 0:
+        ap.error("--wiener cannot be negative")
+    if args.wiener and not (args.keep_channels or args.family == "dsd_ild"):
+        ap.error("--wiener needs stereo stems: --family dsd --keep-channels, or --family dsd_ild")
     world, rank, local = (int(os.environ.get(k, d)) for k, d in (("WORLD_SIZE", "1"), ("RANK", "0"), ("LOCAL_RANK", "0")))
     if world > 1:
         import torch
@@ -146,7 +159,8 @@ def main(argv=None):
     import time
     t0 = time.time()
     secs, njobs = separate_dataset(args.family, args.db, args.out, args.model, args.scale_factor, rank=rank,
-                                   world_size=world, device=local, keep_channels=args.keep_channels)
+                                   world_size=world, device=local, keep_channels=args.keep_channels,
+                                   wiener=args.wiener)
     tot, ms, _ = reduce_stats(secs, (time.time() - t0) * 1e3)
     if rank == 0:
         print("separated %d files, %.1f audio-s in %.2f s (%.0f x real time) on %d GPU(s)" % (njobs, tot, ms / 1e3,

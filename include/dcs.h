@@ -84,6 +84,13 @@ int dcs_set_spectrum_tap(dcs_ctx* ctx, dcs_complex* d_S, int64_t capacity);
  * the window as ill-conditioned and require agreement elsewhere.  capacity in bytes; NULL = off. */
 int dcs_set_pool_tap(dcs_ctx* ctx, uint8_t* d_bits, int64_t capacity);
 
+/* Multichannel Wiener post-filter of two-channel stems (see dcs_wiener_stereo): while iterations > 0, the entry points
+ * that produce stereo stems -- dcs_separate_audio_keep_channels, dcs_separate_batch_pcm16_keep_channels_host and
+ * dcs_separate_audio_stereo -- run that many EM iterations on the network's spectra before the inverse STFT (the
+ * spectrum tap then holds the filtered spectra).  Single-channel entry points ignore the setting.  Default 0 (off:
+ * the network's spectra, bit for bit); negative values are refused. */
+int dcs_set_wiener(dcs_ctx* ctx, int iterations);
+
 /* per-stage device timing (CUDA events on the launching stream): enable, run, synchronise the
  * stream, then read.  dcs_profile_read writes up to max_n durations (ms) and the stage names
  * joined by '\n' into names_buf, clears the records and returns the number of records. */
@@ -239,6 +246,18 @@ int dcs_separate_batch_pcm16_keep_channels_host(dcs_ctx* ctx, dcs_model* model, 
                                                 const int16_t* const* h_pcm, const int64_t* num_samples,
                                                 float scale_factor, int overlap, int patcher, int16_t* const* h_out,
                                                 const int64_t* out_strides, void* stream);
+
+/* ---- multichannel Wiener filter with EM spatial covariances (Duong, Vincent & Gribonval 2010; util.py:633-719) -- */
+/* In place on caller-owned spectra, the plane layout of the stereo entry points: mixture channel c at d_X + c*x_plane,
+ * stem (source j, channel c) at d_S + (2j + c)*src_stride, each complex[T][ldf]; only bins f < F are read or written.
+ * With s = max(1, max|x| / 10) over the clip and eps = 2^-23, each iteration computes
+ *     v_j = (|y_jL|^2 + |y_jR|^2) / 2,   R_j(f) = sum_t y_j y_j^H / (eps s^2 + sum_t v_j),
+ *     C = sum_j v_j R_j + sqrt(eps) s^2 I,   y_j <- v_j R_j C^-1 x
+ * (2x2 algebra and the sums over t in fp64, fixed summation order: the same bits on every run).  Frames where every
+ * y_j is 0 stay 0.  nsrc in [1, 4]; iterations 0 returns without queuing work.  Every argument is checked before
+ * anything is queued.  The workspace grows to ~32 bytes per (source, bin) per 128 frames. */
+int dcs_wiener_stereo(dcs_ctx* ctx, const dcs_complex* d_X, int64_t x_plane, dcs_complex* d_S, int64_t src_stride,
+                      int nsrc, int64_t num_frames, int64_t ldf, int F, int iterations, void* stream);
 
 #ifdef __cplusplus
 }
