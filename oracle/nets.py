@@ -96,8 +96,10 @@ def infer_arch(params):
     """Infer (arch, F, time_context) from the shapes in a parameter list."""
     n = len(params)
     w1, w2, wfc = params[0].shape, params[3].shape, params[6].shape
+    # DSD nets: conv2 has kh2 = int(tc / 2) taps and leaves h2 = tc - kh2 + 1 rows, fc.W has 50 * h2 rows, so
+    # tc = h2 + kh2 - 1 (2 * kh2 is wrong for an odd time_context)
     if n == 15 and w1[0] == 50:
-        return "dsd", w1[3], 2 * w2[2]
+        return "dsd", w1[3], wfc[0] // 50 + w2[2] - 1
     if n == 13 and w1[0] == 30:
         # fc.W rows disambiguate the pool / no-pool iKala nets (SURVEY.md 0.7); F is not
         # recoverable from the parameters (conv1 is 30 wide) -> iKala default 513.
@@ -105,7 +107,7 @@ def infer_arch(params):
             if arch_dims(arch, 513, 30)["flat"] == wfc[0]:
                 return arch, 513, 30
     if n == 17 and w1[0] == 50 and w1[1] == 2:
-        return "dsd_ild", w1[3], 2 * w2[2]
+        return "dsd_ild", w1[3], wfc[0] // 50 + w2[2] - 1
     if n == 17 and w1[0] == 30:
         arch = "bach10_score" if w1[1] == 4 else "bach10"
         for F in (2049, 1025, 513):

@@ -83,3 +83,12 @@ def test_load_model_roundtrip_and_arch_inference(tmp_path):
     with open(fn, "wb") as f:
         pickle.dump([np.arange(4, dtype=np.float32)], f, protocol=2)
     assert models.load_model(fn)[0].tolist() == [0, 1, 2, 3]
+
+
+@pytest.mark.parametrize("arch", ["dsd", "dsd_ild"])
+@pytest.mark.parametrize("tc", [4, 17, 31, 64])
+def test_models_infer_arch_recovers_time_context(arch, tc):
+    """the DSD nets' time_context from the conv2 / fc.W shapes, odd values and both ends of the accepted 4..64"""
+    params = [np.zeros(s, dtype=np.float32) for s in nets.param_shapes(arch, 513, tc)]
+    assert models.infer_arch(params) == (arch, 513, tc)
+    assert nets.infer_arch(params) == (arch, 513, tc)

@@ -15,7 +15,10 @@ def ctx():
 
 @pytest.mark.parametrize("engine", [1, 0])
 @pytest.mark.parametrize("M,N,K,lda_extra", [(128, 64, 32, 0), (1, 1, 1, 0), (300, 50, 750, 0), (257, 128, 800, 4),
-                                             (1000, 150, 129, 3), (130, 2400, 128, 0), (4096, 50, 1025, 7)])
+                                             (1000, 150, 129, 3), (130, 2400, 128, 0), (4096, 50, 1025, 7),
+                                             # N <= 32 (the BN = 32 kernels of the 30-channel convolutions): A vector
+                                             # widths 2 / 1 with split K over 3 / 4 slices, a one-element K tail, width 4
+                                             (300, 30, 780, 2), (1000, 32, 1040, 1), (129, 17, 33, 0), (257, 30, 96, 0)])
 def test_gemm_matches_float64(ctx, engine, M, N, K, lda_extra):
     rng = np.random.default_rng(M * 7 + N * 3 + K)
     A = rng.standard_normal((M, K + lda_extra)).astype(np.float32)

@@ -69,7 +69,9 @@ def test_bach10_full_size():
 
 
 def test_models_share_a_context_safely():
-    """DSD100 and Bach10 alternating on ONE ctx: the zero-padded workspaces are re-zeroed when the layout changes."""
+    """DSD100 and Bach10 alternating on ONE ctx, at two time contexts and three overlaps of the DSD100 net and two
+    overlaps of Bach10: the zero-padded workspaces are re-zeroed when the layout changes (the layout signature leaves
+    the overlap out for the DSD nets), so every call gives the bits of its first round."""
     from deepconvsep_b200.engine import Context, Model, Stft
     from deepconvsep_b200 import _lib
     import ctypes as C
@@ -78,20 +80,24 @@ def test_models_share_a_context_safely():
     mix, _ = pipeline.synth_mixture(1.0, 3)
     outs = {}
     for rnd in range(2):
-        for arch, F, N, hop, win, ov in (("dsd", 257, 512, 256, np.hanning, 25), ("bach10", 257, 512, 256, dsp.blackmanharris, 25)):
-            params = nets.make_synthetic_params(arch, F, seed=4)
-            model = Model(ctx, params, arch=arch, feat_size=F)
+        for arch, F, N, hop, win, tc, ov in (("dsd", 257, 512, 256, np.hanning, 30, 25),
+                                             ("dsd", 257, 512, 256, np.hanning, 30, 0),
+                                             ("dsd", 257, 512, 256, np.hanning, 31, 26),
+                                             ("bach10", 257, 512, 256, dsp.blackmanharris, 30, 25),
+                                             ("bach10", 257, 512, 256, dsp.blackmanharris, 30, 28)):
+            params = nets.make_synthetic_params(arch, F, tc=tc, seed=4)
+            model = Model(ctx, params, arch=arch, feat_size=F, time_context=tc)
             st = Stft(ctx, N, hop, win(N))
             a = np.ascontiguousarray(mix, dtype=np.float32)
             out = np.empty((4, a.size), dtype=np.float32)
             _lib.check(lib.dcs_separate_host(ctx.handle, model.handle, st.handle, a.ctypes.data, a.size, C.c_float(0.3), ov, 0,
                                              out.ctypes.data, a.size, None))
             if rnd == 0:
-                outs[arch] = out
-                want = pipeline.separate(mix, params, arch, frameSize=N, hopSize=hop, window=win, overlap=ov)
-                assert max(rel(out[s].astype(np.float64), want[s]) for s in range(4)) < 5e-4
+                outs[arch, tc, ov] = out
+                want = pipeline.separate(mix, params, arch, frameSize=N, hopSize=hop, window=win, time_context=tc, overlap=ov)
+                assert max(rel(out[s].astype(np.float64), want[s]) for s in range(4)) < 5e-4, (arch, tc, ov)
             else:
-                assert np.array_equal(out, outs[arch])
+                assert np.array_equal(out, outs[arch, tc, ov]), (arch, tc, ov)
 
 
 def test_score_informed_bach10():

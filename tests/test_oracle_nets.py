@@ -74,6 +74,14 @@ def test_param_counts():
         assert nets.infer_arch(fake)[:2] == (arch, F)
 
 
+@pytest.mark.parametrize("arch", ["dsd", "dsd_ild"])
+@pytest.mark.parametrize("tc", [4, 17, 30, 31, 64])
+def test_infer_arch_recovers_time_context(arch, tc):
+    """conv2 has int(tc / 2) taps and leaves h2 = tc - int(tc / 2) + 1 rows: tc = h2 + kh2 - 1, odd tc included"""
+    shapes = nets.param_shapes(arch, 129, tc)
+    assert nets.infer_arch([np.zeros(s, dtype=np.float32) for s in shapes]) == (arch, 129, tc)
+
+
 def test_mask_rules_closed_form():
     """eps*rand cancels: 'dsd' rule -> 1/nsrc on all-zero bins, 'bach10' rule -> 0 there;
     elsewhere both equal p/sum(p) to float64 rounding."""
