@@ -7,7 +7,7 @@ import os
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libdcs.so")
 
-ARCH_IDS = {"dsd": 0, "ikala": 1, "ikala_nopool": 2, "bach10": 3, "bach10_score": 4, "dsd_ild": 5}
+ARCH_IDS = {"dsd": 0, "ikala": 1, "ikala_nopool": 2, "bach10": 3, "bach10_score": 4, "dsd_ild": 5, "bach10_score_1x1": 6}
 PATCHER_IDS = {"standalone": 0, "util": 1}
 
 

@@ -370,7 +370,9 @@ static int model_create_dsd(dcs_model* m, int nparams, const float* const* hp, c
 int dcs_model_create(dcs_ctx* ctx, int arch, int feat_size, int time_context, int nparams, const float* const* h_params,
                      const int64_t* shapes, const int* ndims, dcs_model** out) {
   DCS_REQUIRE(ctx && h_params && shapes && ndims && out, "dcs_model_create: NULL argument");
-  DCS_REQUIRE(feat_size >= 3 && ((feat_size - 1) & (feat_size - 2)) == 0, "feat_size %d is not 2^k+1", feat_size);
+  // the 1x1 score net also runs on spectra of other widths through dcs_separate_spec_channels
+  DCS_REQUIRE(feat_size >= 3 && (arch == DCS_ARCH_BACH10_SCORE_1X1 || ((feat_size - 1) & (feat_size - 2)) == 0),
+              "feat_size %d is not 2^k+1", feat_size);
   DCS_REQUIRE(time_context >= 4 && time_context <= 64, "time_context %d out of range", time_context);
   DCS_CUDA(cudaSetDevice(ctx->device));
   dcs_model* m = new dcs_model();
@@ -383,6 +385,7 @@ int dcs_model_create(dcs_ctx* ctx, int arch, int feat_size, int time_context, in
     case DCS_ARCH_IKALA_NOPOOL:
     case DCS_ARCH_BACH10:
     case DCS_ARCH_BACH10_SCORE: r = model_create_sconv(m, nparams, h_params, shapes, ndims); break;
+    case DCS_ARCH_BACH10_SCORE_1X1: r = model_create_s1x1(m, nparams, h_params, shapes, ndims); break;
     default:
       set_error("dcs_model_create: architecture %d has no CUDA path yet", arch);
       r = DCS_EINVAL;
@@ -492,17 +495,24 @@ static int run_network(dcs_ctx* ctx, const dcs_model* m, const float* in, int64_
   n.Tp = std::max<int64_t>(T, (n.P - 1) * n.step + m->tc);
   // the zero-padded slots are re-zeroed when the model changes; those of the 30-channel nets also when the overlap does
   n.sig = ((uint64_t)(m->arch + 1) << 48) ^ ((uint64_t)m->F << 24) ^ (uint64_t)(m->tc * 64 + (dsd ? 0 : overlap));
-  return dsd ? dsd_forward(ctx, m, n, st) : sconv_forward(ctx, m, n, st);
+  if (dsd) return dsd_forward(ctx, m, n, st);
+  return m->arch == DCS_ARCH_BACH10_SCORE_1X1 ? s1x1_forward(ctx, m, n, st) : sconv_forward(ctx, m, n, st);
 }
 
-// arch: the architecture an entry point serves, -1 for the single-channel nets
+static bool score_arch(int arch) { return arch == DCS_ARCH_BACH10_SCORE || arch == DCS_ARCH_BACH10_SCORE_1X1; }
+// input planes of the score-informed nets
+static int score_planes(const dcs_model* m) { return m->arch == DCS_ARCH_BACH10_SCORE_1X1 ? 4 : m->sc.nch; }
+
+// arch: the architecture an entry point serves (DCS_ARCH_BACH10_SCORE: both score-informed nets), -1 for the
+// single-channel nets
 static int check_model(const char* fn, const dcs_ctx* ctx, const dcs_model* m, int arch, int overlap, int patcher) {
   DCS_REQUIRE(ctx && m, "%s: NULL argument", fn);
-  const bool mono = m->arch != DCS_ARCH_DSD_ILD && m->arch != DCS_ARCH_BACH10_SCORE;
-  DCS_REQUIRE(arch < 0 ? mono : m->arch == arch, "%s does not serve architecture %d: use %s", fn, m->arch,
+  const bool mono = m->arch != DCS_ARCH_DSD_ILD && !score_arch(m->arch);
+  DCS_REQUIRE(arch < 0 ? mono : (arch == DCS_ARCH_BACH10_SCORE ? score_arch(m->arch) : m->arch == arch),
+              "%s does not serve architecture %d: use %s", fn, m->arch,
               m->arch == DCS_ARCH_DSD_ILD ? "dcs_separate_audio_stereo"
-              : m->arch == DCS_ARCH_BACH10_SCORE ? "dcs_separate_audio_score / dcs_separate_spec_channels"
-                                                 : "dcs_separate_audio / dcs_separate_spec");
+              : score_arch(m->arch)       ? "dcs_separate_audio_score / dcs_separate_spec_channels"
+                                          : "dcs_separate_audio / dcs_separate_spec");
   DCS_REQUIRE(overlap >= 0 && overlap < m->tc, "overlap %d must be in [0, time_context=%d)", overlap, m->tc);
   DCS_REQUIRE(patcher == DCS_PATCHER_STANDALONE || patcher == DCS_PATCHER_UTIL, "unknown patcher %d", patcher);
   return DCS_OK;
@@ -530,7 +540,7 @@ static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, i
   DCS_TRY(ctx->X.ensure((size_t)nx * plane * sizeof(float2), st));
   DCS_TRY(ctx->mag.ensure((size_t)m->nch * plane * sizeof(float), st));
   DCS_TRY(ctx->S.ensure((size_t)m->nsrc * nx * plane * sizeof(float2), st));
-  if (m->arch == DCS_ARCH_BACH10_SCORE) DCS_TRY(ctx->net[NET_CHANS].ensure((size_t)m->sc.nch * plane * sizeof(float), st));
+  if (score_arch(m->arch)) DCS_TRY(ctx->net[NET_CHANS].ensure((size_t)score_planes(m) * plane * sizeof(float), st));
   if (ctx->wiener_iters > 0 && m->nch * nx == 2)
     DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, dcs_num_frames(L, p->hop), m->F), st));
   if (staged) {
@@ -569,7 +579,7 @@ static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const fl
   if (d_filters) {
     float* chans = ctx->net[NET_CHANS].as<float>();
     ProfScope ps(ctx, "score_channels", st);
-    DCS_TRY(launch_channel_mul(ctx, mag, d_filters, chans, plane, m->sc.nch, st));
+    DCS_TRY(launch_channel_mul(ctx, mag, d_filters, chans, plane, score_planes(m), st));
     in = chans;
   }
   DCS_TRY(run_network(ctx, m, in, plane, X, plane, nx, T, ldf, overlap, patcher, S, plane, st));

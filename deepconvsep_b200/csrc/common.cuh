@@ -62,6 +62,7 @@ enum NetSlot {
   NET_SPLITK,                               // split-K partial sums of the tensor-core GEMM
   NET_XC_PTRS, NET_XC_PARTIAL,              // dcs_xcorr_lags
   NET_XTAB,                                 // DSD mask kernel's frame table
+  NET_ENC, NET_CODES, NET_DEC,              // 1x1 score net: encoder activations, ReLU gate codes, decoder chunk
   NET_SLOTS
 };
 
@@ -89,7 +90,7 @@ struct dcs_ctx {
   dcs::DevBuf pcm_in[2], pcm_out[2];
   float2* tap = nullptr;        // dcs_set_spectrum_tap: copy of the masked spectra the iSTFT consumed
   int64_t tap_cap = 0;
-  uint8_t* pool_tap = nullptr;  // dcs_set_pool_tap: copy of the max-pool tie bits of the forward pass
+  uint8_t* pool_tap = nullptr;  // dcs_set_pool_tap: copy of the routing decisions of the forward pass
   int64_t pool_tap_cap = 0;
   int wiener_iters = 0;         // dcs_set_wiener: EM iterations of the stereo Wiener post-filter (0 = off)
   dcs::DevBuf wiener;           // its partial sums, spatial covariances and mixture scale (wiener.cu)
@@ -143,18 +144,28 @@ struct dcs_sconv {   // strided-conv1 families: iKala (pool / no pool), Bach10
   dcs::TcWeight tW[8];                 // 0 conv1, 1 conv2, 2 fc, 3 convT2, 4.. decoder dense layers
   float *b1, *b2, *bfc, *bdec[4], *bout, *Wsc;
 };
+struct dcs_s1x1 {    // score-informed build_ca_1x1: six strided ReLU convolutions, a 1x1 conv, gated transposed convs
+  int W[7];             // W[0] = F, W[l] = width of conv l's output
+  int C[7], CP[7];      // channels and channel pitch of each activation (C[0] = 4 input planes)
+  dcs::TcWeight tF[7];  // forward: conv1..conv6 (index l), 1x1 conv (index 0; first 200 filters only)
+  dcs::TcWeight tI[7];  // InverseLayer(conv l) for l = 2..6
+  float *b[7], *c[7];   // bias before / after the ReLU (index 0: 1x1 conv)
+  float *bout, *Wsc;    // final bias 0..3; K3s filter banks of conv1
+};
 struct dcs_model {
   dcs_ctx* ctx;
   int arch, F, tc, nsrc;
   int nch = 1;    // audio channels of a clip; the stems are nsrc x nch planes (2: stereo / ILD net)
   dcs_dsd dsd;
   dcs_sconv sc;
+  dcs_s1x1 s1;
   std::vector<void*> dev;   // every device allocation of the model, tensor-core weights included
 };
 namespace dcs {
 // owned: a list the allocation is recorded in (a model's, which dcs_model_destroy frees)
 int upload(const std::vector<float>& h, float** d, std::vector<void*>* owned = nullptr);
 int model_create_sconv(dcs_model* m, int nparams, const float* const* hp, const int64_t* shp, const int* nd);
+int model_create_s1x1(dcs_model* m, int nparams, const float* const* hp, const int64_t* shp, const int* nd);
 bool shape_is(const int64_t* s, int nd, int want_nd, int64_t a, int64_t b = 1, int64_t c = 1, int64_t d = 1);
 
 // one call of the network stage (run_network, api.cu): the network's input planes [T][ldf] (plane c at
@@ -171,6 +182,7 @@ struct NetCall {
 };
 // the layer sequence of the 30-channel nets (DSD's: api.cu)
 int sconv_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaStream_t st);
+int s1x1_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaStream_t st);
 // (re)zero a workspace slot whenever what it holds changes layout: zero padding is relied upon
 int ensure_layout(dcs_ctx* ctx, NetSlot slot, size_t bytes, uint64_t sig, cudaStream_t st);
 }  // namespace dcs
@@ -209,7 +221,15 @@ struct GemmDesc {
   // non-zero input, so a tile skips the k-blocks outside [kc_unit*q_lo, kc_unit*(q_hi+1)).
   // kc_rows = 0 disables it.  (Pure optimisation: the skipped products are exact zeros.)
   int kc_rows, kc_unit, kc_pad, kc_n, kc_taps;
+  // epilogue of the rectifier-gated 1x1 score net, read only by launch_gemm_tc_epi (compile-time options):
+  //   EPI_POST: x = relu(x + bias) + bias2, and with `code` set the gate code 2*relu'(x + bias) in {0, 1, 2}
+  //             (1 at exactly 0, Theano's 0.5*(x + |x|)) is stored at code[m * N + n]
+  //   EPI_GATE: x *= 0.5 * gate[(m / g_inner) * g_so + ((m % g_inner) / g_inner2) * g_si + (m % g_inner2) * g_s2 + n];
+  //             where (m % g_inner2) * g_s2 + n >= g_lim (outside the gated layer's width) nothing is stored
+  const float* bias2; uint8_t* code;
+  const uint8_t* gate; int g_inner, g_inner2; int64_t g_so, g_si, g_s2, g_lim;
 };
+enum { EPI_POST = 1, EPI_GATE = 2 };
 // element offset of row m of C (without the column part)
 __host__ __device__ __forceinline__ int64_t gemm_c_row_offset(const GemmDesc& d, int m) {
   return (int64_t)(m / d.cm_inner) * d.c_so + (int64_t)((m % d.cm_inner) / d.cm_inner2) * d.c_si +
@@ -222,6 +242,8 @@ int launch_gemm(dcs_ctx* ctx, const GemmDesc& d, cudaStream_t st);
 int tc_weight_create(const float* B_rowmajor, int64_t ldb, int K, int N, TcWeight* out, std::vector<void*>* owned = nullptr);
 void tc_weight_destroy(TcWeight* w);
 int launch_gemm_tc(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStream_t st);
+// the same GEMM with the gated epilogue `epi` (EPI_POST | EPI_GATE); never split over K
+int launch_gemm_tc_epi(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, int epi, cudaStream_t st);
 
 struct DsdMaskArgs {
   const float* G;      // [P][3][tc][ldg]  decoder activations after the transposed conv2
@@ -253,6 +275,8 @@ struct SconvMaskArgs {
   float2* S;            // [nsrc][T][ldf]
   int64_t ldf, src_stride;
   int T, P, tc, overlap, F, J, WP;
+  // G holds patches p_base.. only; frames [t0, t1) are written (one decoder chunk; a whole clip: 0 and [0, T))
+  int p_base, t0, t1;
 };
 int launch_pool4(dcs_ctx* ctx, const float* H1, float* Hp, uint8_t* tie, int64_t rows, int J, int WP, cudaStream_t st);
 int launch_sconv_mask(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st);

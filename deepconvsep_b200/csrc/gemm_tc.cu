@@ -38,7 +38,7 @@ struct TcSmem {
 // (4 k-steps) therefore goes to a fresh accumulator that is added into an fp32 register sum
 // (round to nearest) once per stage; the two correction terms (2^-11 smaller, their truncation is
 // harmless) share one accumulator over the whole K range.
-template <int BN, int STAGES, int AVEC, bool SPLITK>
+template <int BN, int STAGES, int AVEC, bool SPLITK, int EPI = 0>
 __global__ void __launch_bounds__(TC_THREADS)
 gemm_tc_kernel(const GemmDesc d, const float* __restrict__ Bhi, const float* __restrict__ Blo, int Kp,
                int k_splits, float* __restrict__ partial, int ldp) {
@@ -205,6 +205,11 @@ gemm_tc_kernel(const GemmDesc d, const float* __restrict__ Bhi, const float* __r
     const int m = m0 + half * 64 + wq * 16 + (lane >> 2) + 8 * h;
     if (m >= d.M) continue;
     const int64_t roff = SPLITK ? 0 : gemm_c_row_offset(d, m);
+    int64_t groff = 0, gcol = 0;   // EPI_GATE: gate row offset and this row's column offset in the gated layer
+    if (EPI & EPI_GATE) {
+      groff = (int64_t)(m / d.g_inner) * d.g_so + (int64_t)((m % d.g_inner) / d.g_inner2) * d.g_si;
+      gcol = (int64_t)(m % d.g_inner2) * d.g_s2;
+    }
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
 #pragma unroll
@@ -212,7 +217,18 @@ gemm_tc_kernel(const GemmDesc d, const float* __restrict__ Bhi, const float* __r
         const int n = n0 + 8 * j + 2 * (lane & 3) + e;
         if (n >= d.N) continue;
         float x = sum[4 * j + 2 * h + e] + corr[4 * j + 2 * h + e];
-        if (SPLITK) {   // split-K: raw partial sums, reduced (+bias, activation) by splitk_reduce_kernel
+        if (EPI) {
+          if (EPI & EPI_POST) {
+            const float pre = x + __ldg(d.bias + n);
+            if (d.code) d.code[(int64_t)m * d.N + n] = pre > 0.f ? 2 : (pre == 0.f ? 1 : 0);
+            x = fmaxf(pre, 0.f) + __ldg(d.bias2 + n);
+          }
+          if (EPI & EPI_GATE) {
+            if (gcol + n >= d.g_lim) continue;
+            x *= 0.5f * (float)d.gate[groff + gcol + n];
+          }
+          d.C[roff + (int64_t)(n / d.n_seg) * d.n_ss + (n % d.n_seg)] = x;
+        } else if (SPLITK) {   // split-K: raw partial sums, reduced (+bias, activation) by splitk_reduce_kernel
           partial[((int64_t)blockIdx.z * d.M + m) * ldp + n] = x;
         } else {
           if (d.bias) x += __ldg(d.bias + n);
@@ -266,6 +282,18 @@ void tc_weight_destroy(TcWeight* w) {
   w->hi = w->lo = nullptr;
 }
 
+// the gated epilogues: one launch, no split K (its reduction kernel has the plain epilogue only)
+template <int BN, int STAGES, int AVEC, int EPI>
+static int launch_tc_epi(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStream_t st) {
+  using SM = TcSmem<BN, STAGES>;
+  DCS_TRY(ensure_smem_attr(gemm_tc_kernel<BN, STAGES, AVEC, false, EPI>, SM::TOTAL));
+  dim3 grid((unsigned)ceil_div64(d.M, TC_BM), (unsigned)ceil_div64(d.N, BN));
+  gemm_tc_kernel<BN, STAGES, AVEC, false, EPI><<<grid, TC_THREADS, SM::TOTAL, st>>>(d, w.hi, w.lo, w.Kp, 1, nullptr, 0);
+  DCS_CHECK_LAUNCH();
+  ctx->launches++;
+  return DCS_OK;
+}
+
 template <int BN, int STAGES, int AVEC>
 static int launch_tc(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStream_t st) {
   using SM = TcSmem<BN, STAGES>;
@@ -305,19 +333,22 @@ static int launch_tc(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStr
   return DCS_OK;
 }
 
-// `d.B` is ignored: the weight comes pre-transposed in `w`.
-int launch_gemm_tc(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStream_t st) {
-  if (d.M <= 0 || d.N <= 0) return DCS_OK;
-  DCS_REQUIRE(d.K == w.K && d.N == w.N, "tc gemm: weight is %dx%d, GEMM wants K=%d N=%d", w.K, w.N, d.K, d.N);
-  DCS_REQUIRE(ceil_div64(d.N, 64) <= 65535, "tc gemm: N=%d too large", d.N);
-  // vector width the A view allows: every row start and every segment must keep the alignment
-  int avec = 1;
+// vector width the A view allows: every row start and every segment must keep the alignment
+static int a_vector_width(const GemmDesc& d) {
   const bool one_seg = d.k_seg >= d.K;
   auto aligned = [&](int v) {
     return ((uintptr_t)d.A % (4 * v) == 0) && d.a_so % v == 0 && d.a_si % v == 0 && d.a_s2 % v == 0 &&
            (one_seg || (d.k_seg % KSTAGE == 0 && d.k_ss % v == 0));
   };
-  if (aligned(4)) avec = 4; else if (aligned(2)) avec = 2;
+  return aligned(4) ? 4 : (aligned(2) ? 2 : 1);
+}
+
+// `d.B` is ignored: the weight comes pre-transposed in `w`.
+int launch_gemm_tc(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStream_t st) {
+  if (d.M <= 0 || d.N <= 0) return DCS_OK;
+  DCS_REQUIRE(d.K == w.K && d.N == w.N, "tc gemm: weight is %dx%d, GEMM wants K=%d N=%d", w.K, w.N, d.K, d.N);
+  DCS_REQUIRE(ceil_div64(d.N, 64) <= 65535, "tc gemm: N=%d too large", d.N);
+  const int avec = a_vector_width(d);
   if (d.N <= 32) {   // the 30-channel convolutions of the iKala / Bach10 nets: half the weight traffic and MMA time
     if (avec == 4) return launch_tc<32, 4, 4>(ctx, d, w, st);
     if (avec == 2) return launch_tc<32, 4, 2>(ctx, d, w, st);
@@ -326,6 +357,20 @@ int launch_gemm_tc(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStrea
   if (avec == 4) return launch_tc<64, 4, 4>(ctx, d, w, st);
   if (avec == 2) return launch_tc<64, 4, 2>(ctx, d, w, st);
   return launch_tc<64, 4, 1>(ctx, d, w, st);
+}
+
+int launch_gemm_tc_epi(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, int epi, cudaStream_t st) {
+  if (d.M <= 0 || d.N <= 0) return DCS_OK;
+  DCS_REQUIRE(d.K == w.K && d.N == w.N, "tc gemm: weight is %dx%d, GEMM wants K=%d N=%d", w.K, w.N, d.K, d.N);
+  DCS_REQUIRE(ceil_div64(d.N, 64) <= 65535, "tc gemm: N=%d too large", d.N);
+  DCS_REQUIRE(!(epi & EPI_POST) || (d.bias && d.bias2), "tc gemm: EPI_POST needs both biases");
+  DCS_REQUIRE(!(epi & EPI_GATE) || (d.gate && d.g_inner > 0 && d.g_inner2 > 0), "tc gemm: EPI_GATE needs a gate view");
+  // float4 operand loads only: the gated layers lay their activations out for it (the scalar-load variant spills)
+  DCS_REQUIRE(a_vector_width(d) == 4, "tc gemm: the gated epilogues need a 16-byte aligned A view");
+  if (epi == EPI_POST) return launch_tc_epi<64, 4, 4, EPI_POST>(ctx, d, w, st);
+  if (epi == EPI_GATE) return launch_tc_epi<64, 4, 4, EPI_GATE>(ctx, d, w, st);
+  if (epi == (EPI_POST | EPI_GATE)) return launch_tc_epi<64, 4, 4, EPI_POST | EPI_GATE>(ctx, d, w, st);
+  DCS_REQUIRE(false, "tc gemm: unknown epilogue %d", epi);
 }
 
 }  // namespace dcs

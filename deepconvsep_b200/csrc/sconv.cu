@@ -36,7 +36,8 @@ __global__ void pool4_kernel(const float* __restrict__ H1, float* __restrict__ H
 
 constexpr int SC_TILE = 128;   // m values (threads) per CTA
 
-template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW>
+// CHUNK: as in sconv_mask_tc_kernel (G from patch a.p_base, frames [a.t0, a.t1))
+template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW, bool CHUNK = false>
 __global__ void __launch_bounds__(SC_TILE)
 sconv_mask_kernel(const SconvMaskArgs a) {
   constexpr int JT = SC_TILE + ND - 1;  // staged activation positions per tile
@@ -46,7 +47,8 @@ sconv_mask_kernel(const SconvMaskArgs a) {
   const int tid = threadIdx.x;
   // frames on gridDim.x (2^31-1 blocks: any clip length), bin tiles on gridDim.y (a handful)
   const int m0 = blockIdx.y * SC_TILE, m = m0 + tid;
-  const int t = blockIdx.x;
+  const int t = (CHUNK ? a.t0 : 0) + blockIdx.x;
+  const int p_base = CHUNK ? a.p_base : 0;
   const int step = a.tc - a.overlap;
   // weights: w[dd][f][r] = W1[f][KW-1 - r - STRIDE*dd] (0 where the tap index is negative)
   for (int i = tid; i < NW * ND * 32; i += SC_TILE) ws[i] = reinterpret_cast<const float4*>(a.W)[i];
@@ -70,12 +72,12 @@ sconv_mask_kernel(const SconvMaskArgs a) {
       const int j = m0 - (ND - 1) + jl;
       float v = 0.f;
       if (POOL == 0) {
-        if (j >= 0 && j < a.J) v = __ldg(a.G + ((((int64_t)k * NDEC + d) * a.tc + p) * a.J + j) * 32 + f);
+        if (j >= 0 && j < a.J) v = __ldg(a.G + ((((int64_t)(k - p_base) * NDEC + d) * a.tc + p) * a.J + j) * 32 + f);
       } else {
         const int jp = j / POOL;
         if (j >= 0 && jp < a.WP) {
           const uint8_t bits = a.tie[((int64_t)t * a.WP + jp) * 32 + f];
-          if ((bits >> (j - jp * POOL)) & 1) v = __ldg(a.G + ((((int64_t)k * NDEC + d) * a.tc + p) * a.WP + jp) * 32 + f);
+          if ((bits >> (j - jp * POOL)) & 1) v = __ldg(a.G + ((((int64_t)(k - p_base) * NDEC + d) * a.tc + p) * a.WP + jp) * 32 + f);
         }
       }
       gs[(d * JT + jl) * 33 + f] = v;
@@ -161,25 +163,27 @@ int launch_pool4(dcs_ctx* ctx, const float* H1, float* Hp, uint8_t* tie, int64_t
   return DCS_OK;
 }
 
-template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW>
+template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW, bool CHUNK = false>
 static int launch_sconv_t(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st) {
   constexpr int JT = SC_TILE + ND - 1;
   const size_t smem = (size_t)(NDEC * JT * 33 + 4) * sizeof(float) + NW * ND * 32 * sizeof(float4);
-  DCS_TRY(ensure_smem_attr(sconv_mask_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW>, (int)smem));
+  DCS_TRY(ensure_smem_attr(sconv_mask_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW, CHUNK>, (int)smem));
   const int mtot = (a.F + STRIDE - 1) / STRIDE;
-  dim3 grid((unsigned)a.T, (unsigned)ceil_div64(mtot, SC_TILE));
-  sconv_mask_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW><<<grid, SC_TILE, smem, st>>>(a);
+  dim3 grid((unsigned)(a.t1 - a.t0), (unsigned)ceil_div64(mtot, SC_TILE));
+  sconv_mask_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW, CHUNK><<<grid, SC_TILE, smem, st>>>(a);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;
 }
 
 int launch_sconv_mask(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st) {
-  if (a.T <= 0) return DCS_OK;
+  if (a.T <= 0 || a.t1 <= a.t0) return DCS_OK;
   const int step = a.tc - a.overlap;
   DCS_REQUIRE(step > 0 && (a.tc + step - 1) / step <= 64, "sconv_mask: bad time_context/overlap");
+  DCS_REQUIRE(a.t0 >= 0 && a.t1 <= a.T, "sconv_mask: frame range [%d, %d) outside [0, %d)", a.t0, a.t1, a.T);
   if (a.arch == DCS_ARCH_BACH10) return launch_sconv_t<4, 8, 4, 4, 1, 0, 1>(ctx, a, st);
   if (a.arch == DCS_ARCH_BACH10_SCORE) return launch_sconv_t<4, 8, 4, 1, 1, 0, 4>(ctx, a, st);
+  if (a.arch == DCS_ARCH_BACH10_SCORE_1X1) return launch_sconv_t<2, 3, 4, 1, 1, 0, 4, true>(ctx, a, st);
   if (a.arch == DCS_ARCH_IKALA) return launch_sconv_t<3, 10, 2, 2, 0, 4, 1>(ctx, a, st);
   if (a.arch == DCS_ARCH_IKALA_NOPOOL) return launch_sconv_t<3, 10, 2, 2, 0, 0, 1>(ctx, a, st);
   DCS_REQUIRE(false, "sconv_mask: architecture %d not supported", a.arch);

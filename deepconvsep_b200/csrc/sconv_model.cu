@@ -30,7 +30,8 @@ int model_create_sconv(dcs_model* m, int nparams, const float* const* hp, const 
     // 4 input channels; every InverseLayer(., conv1) returns 4 channels, the concat has 16 and only
     // channels 0..3 -- all from decoder 1 -- are used: decoders 2-4 are dead at inference
     // (trainCNNrwc.py:189,248-251; SURVEY.md 0.8)
-    c.nch = 4; c.sw1 = 4; c.pool = 0; c.kh2 = (2 * tc) / 3; c.kw2 = 1; c.ndec = 1; ndec_params = 4; c.rule = 1; m->nsrc = 4;
+    // The one-decoder variant (the default build_ca of trainCNNrwc_samp.py:195-235, 11 arrays) is decoder 1 alone
+    c.nch = 4; c.sw1 = 4; c.pool = 0; c.kh2 = (2 * tc) / 3; c.kw2 = 1; c.ndec = 1; ndec_params = nparams == 11 ? 1 : 4; c.rule = 1; m->nsrc = 4;
   } else {
     c.sw1 = 3; c.pool = m->arch == DCS_ARCH_IKALA ? 4 : 0; c.kh2 = 10; c.kw2 = 20; c.ndec = 2; c.rule = 0; m->nsrc = 2;
   }
@@ -46,7 +47,11 @@ int model_create_sconv(dcs_model* m, int nparams, const float* const* hp, const 
   const int64_t flat = (int64_t)C * h2 * w2, flatp = (int64_t)h2 * w2 * CP;
   if (!ndec_params) ndec_params = ndec;
   const int want = 8 + 2 * ndec_params + 1, nout = ndec_params * c.nch == 16 ? 16 : m->nsrc;
-  if (nparams != want) { set_error("architecture %d needs %d parameter arrays, got %d", m->arch, want, nparams); return DCS_EMODEL; }
+  if (nparams != want) {
+    set_error(m->arch == DCS_ARCH_BACH10_SCORE ? "architecture %d needs %d (or 11) parameter arrays, got %d" : "architecture %d needs %d parameter arrays, got %d",
+              m->arch, want, nparams);
+    return DCS_EMODEL;
+  }
   bool ok = shape_is(shp + 0, nd[0], 4, C, c.nch, 1, KW) && shape_is(shp + 4, nd[1], 1, C) && shape_is(shp + 8, nd[2], 1, C) &&
             shape_is(shp + 12, nd[3], 4, C, C, kh2, kw2) && shape_is(shp + 16, nd[4], 1, C) && shape_is(shp + 20, nd[5], 1, C) &&
             shape_is(shp + 24, nd[6], 2, flat, c.nfc) && shape_is(shp + 28, nd[7], 1, c.nfc) &&
@@ -194,6 +199,7 @@ int sconv_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaStream
   a.arch = m->arch; a.G = G; a.tie = tie; a.W = c.Wsc; a.bout = c.bout; a.X = n.X; a.S = n.S;
   a.ldf = ldf; a.src_stride = n.src_stride; a.T = (int)T; a.P = (int)P; a.tc = tc; a.overlap = n.overlap; a.F = m->F;
   a.J = J; a.WP = WP;
+  a.p_base = 0; a.t0 = 0; a.t1 = (int)T;
   ProfScope ps(ctx, "dec_convT1_mask_xfade", st);
   if (!ctx->debug_simt_gemm) {
     DCS_REQUIRE(sconv_mask_tc_supported(a), "sconv_forward: tensor-core mask kernel does not take this shape");

@@ -55,8 +55,8 @@ __device__ __forceinline__ void slot_range(int t, int tc, int step, int P, int& 
   k_lo = k_lo > 0 ? (k_lo + step - 1) / step : 0;
 }
 
-// activation chunk u of slot (t, k): item d, staged row jl, 16-byte channel chunk c4.  Un-pooled nets: G row
-// ((k*NDEC + d)*tc + p) at position j; max-pool net: InverseLayer(pool) -- position j receives G[j / POOL]
+// activation chunk u of slot (t, k): item d, staged row jl, 16-byte channel chunk c4 (k counts from G's first patch).
+// Un-pooled nets: G row ((k*NDEC + d)*tc + p) at position j; max-pool net: InverseLayer(pool) -- position j receives G[j / POOL]
 // where the forward pass had its window maximum (every tied position does), else 0.  Outside the axis: 0.
 template <int POOL>
 __device__ __forceinline__ float4 sconv_load(const SconvMaskArgs& a, int t, int k, int p, int d, int ndec, int j, int c4) {
@@ -80,7 +80,9 @@ __device__ __forceinline__ float4 sconv_load(const SconvMaskArgs& a, int t, int 
   return v;
 }
 
-template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW>
+// CHUNK: G holds patches a.p_base.. and the frames [a.t0, a.t1) are written (one decoder chunk of the 1x1 score net);
+// otherwise G holds every patch and all a.T frames are written
+template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW, bool CHUNK = false>
 __global__ void __launch_bounds__(ST_THREADS, 1)
 sconv_mask_tc_kernel(const SconvMaskArgs a, int frames_per_cta) {
   using TL = SconvTile<STRIDE, ND, NSRC, NDEC, NW>;
@@ -95,8 +97,9 @@ sconv_mask_tc_kernel(const SconvMaskArgs a, int frames_per_cta) {
   const int wg = warp >> 2, wq = warp & 3;
   const int m0 = blockIdx.x * OUT;
   const int j_start = m0 - (ND - 1);
-  const int t_begin = blockIdx.y * frames_per_cta;
-  const int t_end = min(a.T, t_begin + frames_per_cta);
+  const int t_begin = (CHUNK ? a.t0 : 0) + blockIdx.y * frames_per_cta;
+  const int t_end = min(CHUNK ? a.t1 : a.T, t_begin + frames_per_cta);
+  const int p_base = CHUNK ? a.p_base : 0;
   const int step = a.tc - a.overlap;
 
   // filter banks: B[c = o*32 + dd*STRIDE + r][f] = w[o][dd][f][r] (a.W: float4 [NW][ND][32], .xyzw = r), hi / lo planes
@@ -152,7 +155,7 @@ sconv_mask_tc_kernel(const SconvMaskArgs a, int frames_per_cta) {
 #pragma unroll
     for (int u = 0; u < CHUNKS; ++u) {
       const int idx = u * ST_THREADS + tid, c4 = idx & 7, jl = (idx >> 3) & (ST_ROWS - 1), d = idx >> 10;
-      ra[u] = sconv_load<POOL>(a, tt, kk, p, d, NDEC, j_start + jl, c4);
+      ra[u] = sconv_load<POOL>(a, tt, kk - p_base, p, d, NDEC, j_start + jl, c4);
     }
   };
   if (t < t_end) load_slot(t, k);
@@ -259,18 +262,19 @@ sconv_mask_tc_kernel(const SconvMaskArgs a, int frames_per_cta) {
   }
 }
 
-template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW>
+template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW, bool CHUNK = false>
 static int launch_sconv_tc_t(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st) {
   using TL = SconvTile<STRIDE, ND, NSRC, NDEC, NW>;
-  auto kern = sconv_mask_tc_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW>;
+  auto kern = sconv_mask_tc_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW, CHUNK>;
   DCS_TRY(ensure_smem_attr(kern, TL::SMEM));
   const int mtot = (a.F + STRIDE - 1) / STRIDE;
   const int mtiles = (mtot + TL::OUT - 1) / TL::OUT;
+  const int nt = a.t1 - a.t0;   // frames this launch writes
   int chunks = ctx->num_sms / mtiles;
   if (chunks < 1) chunks = 1;
-  if (chunks > a.T) chunks = a.T;
-  const int fpc = (a.T + chunks - 1) / chunks;
-  dim3 grid((unsigned)mtiles, (unsigned)((a.T + fpc - 1) / fpc));
+  if (chunks > nt) chunks = nt;
+  const int fpc = (nt + chunks - 1) / chunks;
+  dim3 grid((unsigned)mtiles, (unsigned)((nt + fpc - 1) / fpc));
   kern<<<grid, ST_THREADS, TL::SMEM, st>>>(a, fpc);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
@@ -279,15 +283,18 @@ static int launch_sconv_tc_t(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t 
 
 bool sconv_mask_tc_supported(const SconvMaskArgs& a) {
   const int step = a.tc - a.overlap;
-  return step > 0 && ((uintptr_t)a.G % 16 == 0) &&
-         (a.arch == DCS_ARCH_BACH10 || a.arch == DCS_ARCH_BACH10_SCORE || a.arch == DCS_ARCH_IKALA || a.arch == DCS_ARCH_IKALA_NOPOOL);
+  return step > 0 && ((uintptr_t)a.G % 16 == 0) && a.t0 >= 0 && a.t0 <= a.t1 && a.t1 <= a.T &&
+         (a.arch == DCS_ARCH_BACH10 || a.arch == DCS_ARCH_BACH10_SCORE || a.arch == DCS_ARCH_IKALA || a.arch == DCS_ARCH_IKALA_NOPOOL ||
+          a.arch == DCS_ARCH_BACH10_SCORE_1X1);
 }
 
 int launch_sconv_mask_tc(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st) {
-  if (a.T <= 0) return DCS_OK;
+  if (a.T <= 0 || a.t1 <= a.t0) return DCS_OK;
   DCS_REQUIRE(sconv_mask_tc_supported(a), "sconv_mask_tc: unsupported shape");
   if (a.arch == DCS_ARCH_BACH10) return launch_sconv_tc_t<4, 8, 4, 4, 1, 0, 1>(ctx, a, st);
   if (a.arch == DCS_ARCH_BACH10_SCORE) return launch_sconv_tc_t<4, 8, 4, 1, 1, 0, 4>(ctx, a, st);
+  // 1x1 score net: InverseLayer(conv1) of kernel (1,5) stride 2 -- 3 taps per output pair (score1x1.cu)
+  if (a.arch == DCS_ARCH_BACH10_SCORE_1X1) return launch_sconv_tc_t<2, 3, 4, 1, 1, 0, 4, true>(ctx, a, st);
   if (a.arch == DCS_ARCH_IKALA) return launch_sconv_tc_t<3, 10, 2, 2, 0, 4, 1>(ctx, a, st);
   return launch_sconv_tc_t<3, 10, 2, 2, 0, 0, 1>(ctx, a, st);
 }

@@ -7,7 +7,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .models import infer_arch, FAMILY_DEFAULTS
+from .models import infer_arch, check_1x1_geometry, gate_code_layout, FAMILY_DEFAULTS
 
 
 def get_window(window, n):
@@ -219,6 +219,8 @@ class Model(object):
         a = ia if arch is None else arch
         F = feat_size if (arch is not None and feat_size is not None) else iF
         self.arch, self.F, self.tc = a, int(F), int(time_context or itc)
+        if a == "bach10_score_1x1":
+            check_1x1_geometry(self.F, self.tc)
         arrs = [np.ascontiguousarray(p, dtype=np.float32) for p in params]
         n = len(arrs)
         ptrs = (C.c_void_p * n)(*[x.ctypes.data for x in arrs])
@@ -444,7 +446,8 @@ class Separator(object):
         separate_keep_channels() (keep_channels=True) with the spectrum tap on (dcs_set_spectrum_tap) -> (stems as
         that call returns them, masked spectra complex64 numpy [nplanes, T, F] -- the tensors the inverse STFT of THIS
         call consumed, (source, channel) planes for the stereo outputs).
-        pool=True (max-pool net): also the tie bits uint8 [T, WP, 32] of this call (dcs_set_pool_tap).
+        pool=True: also the routing decisions of this call (dcs_set_pool_tap) -- max-pool net: the tie bits uint8
+        [T, WP, 32]; 1x1 score net: the gate codes of conv1..conv6, a list of uint8 [rows, W, C] (gate_code_layout).
         wiener: EM iterations of the Wiener post-filter (two-channel stems only); the tap then holds the filtered spectra."""
         import torch
         stereo = keep_channels or self.model.arch == "dsd_ild"
@@ -458,14 +461,18 @@ class Separator(object):
         _lib.check(self.lib.dcs_set_spectrum_tap(self.ctx.handle, _ptr(tap), tap.numel()))
         bits = None
         if pool:
-            assert self.model.arch == "ikala", "only the max-pool network has routing decisions to tap"
-            WP = ((self.model.F - 30) // 3 + 1) // 4
-            bits = torch.zeros((T, WP, 32), dtype=torch.uint8, device=self.stft.dev)
+            assert self.model.arch in ("ikala", "bach10_score_1x1"), "only the max-pool and 1x1 score nets have routing decisions to tap"
+            if self.model.arch == "ikala":
+                WP = ((self.model.F - 30) // 3 + 1) // 4
+                bits = torch.zeros((T, WP, 32), dtype=torch.uint8, device=self.stft.dev)
+            else:
+                layout = gate_code_layout(self.model.F, self.model.tc, self._frames_spanned(T))
+                bits = torch.zeros(sum(r * w * c for r, w, c in layout), dtype=torch.uint8, device=self.stft.dev)
             _lib.check(self.lib.dcs_set_pool_tap(self.ctx.handle, _ptr(bits), bits.numel()))
         try:
             if keep_channels:
                 out = self.separate_keep_channels(a, wiener=wiener)
-            elif self.model.arch == "bach10_score":
+            elif self.model.arch in ("bach10_score", "bach10_score_1x1"):
                 out = self.separate_score(a, filters)
             elif self.model.arch == "dsd_ild":
                 out = self.separate_stereo(a, wiener=wiener)
@@ -476,7 +483,18 @@ class Separator(object):
             _lib.check(self.lib.dcs_set_spectrum_tap(self.ctx.handle, None, 0))
             _lib.check(self.lib.dcs_set_pool_tap(self.ctx.handle, None, 0))
         S = tap[:, :, :self.model.F].cpu().numpy()
+        if pool and self.model.arch == "bach10_score_1x1":
+            flat, codes = bits.cpu().numpy(), []
+            for r, w, c in gate_code_layout(self.model.F, self.model.tc, self._frames_spanned(T)):
+                codes.append(flat[:r * w * c].reshape(r, w, c))
+                flat = flat[r * w * c:]
+            return out, S, codes
         return (out, S, bits.cpu().numpy()) if pool else (out, S)
+
+    def _frames_spanned(self, T):
+        """Tp: the frames the patches of a T-frame clip span (dcs.h, dcs_set_pool_tap)"""
+        P, step = self.num_patches(T), self.model.tc - self.overlap
+        return max(T, (P - 1) * step + self.model.tc)
 
     def separate_spec(self, mag, X, stream=None):
         """scaled magnitude [T, ldf] + mixture STFT [T, ldf] -> masked spectra complex64 [nsrc, T, ldf]"""

@@ -16,7 +16,7 @@ import getopt
 import numpy as np
 import scipy.io.wavfile
 
-from ...models import load_model                       # noqa: F401
+from ...models import load_model, infer_arch           # noqa: F401
 from ...transform import sinebell, stft_norm, istft_norm, transformFFT  # noqa: F401
 from ...util import generate_overlapadd, overlapadd_multi  # noqa: F401  (util.py:220-327)
 from ...score import str2midi, getMidiNum, expandMidi, filterSpec, slicefft_slices, score_filters  # noqa: F401
@@ -48,7 +48,10 @@ def train_auto(filein, outdir, model, scale_factor=0.3, time_context=30, overlap
     key = (os.path.abspath(model), os.path.getmtime(model), scale_factor, time_context, overlap, input_size, frameSize, hopSize)
     if key not in _cache:
         _cache.clear()
-        _cache[key] = Separator(load_model(model), arch=FAMILY, frame_size=frameSize, hop=hopSize, window="blackmanharris",
+        params = load_model(model)
+        # build_ca (17 arrays; 11 for the one-decoder variant) or build_ca_1x1 (22 arrays): from the parameter list
+        family = infer_arch(params, input_size, time_context)[0]
+        _cache[key] = Separator(params, arch=family, frame_size=frameSize, hop=hopSize, window="blackmanharris",
                                 scale_factor=scale_factor, time_context=time_context, overlap=overlap, patcher="util",
                                 feat_size=input_size)
     stems = _cache[key].separate_score(audio, filters)

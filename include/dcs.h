@@ -44,8 +44,14 @@ enum {
   DCS_ARCH_IKALA = 1,        /* examples/ikala/separate_ikala.py:172-192 (max-pool) */
   DCS_ARCH_IKALA_NOPOOL = 2, /* examples/ikala/trainCNN.py:66-110 */
   DCS_ARCH_BACH10 = 3,       /* examples/bach10/separate_bach10.py:172-229 */
-  DCS_ARCH_BACH10_SCORE = 4, /* examples/bach10_scoreinformed/trainCNNrwc.py:134-193 */
-  DCS_ARCH_DSD_ILD = 5       /* examples/dsd100_2ch_ILD/trainCNN_ILD_DSD100.py:66-113 (stereo in, nsrc x 2 out) */
+  DCS_ARCH_BACH10_SCORE = 4, /* examples/bach10_scoreinformed/trainCNNrwc.py:134-193 (17 arrays); also the one-decoder
+                                build_ca of trainCNNrwc_samp.py:195-235 (11 arrays) */
+  DCS_ARCH_DSD_ILD = 5,      /* examples/dsd100_2ch_ILD/trainCNN_ILD_DSD100.py:66-113 (stereo in, nsrc x 2 out) */
+  DCS_ARCH_BACH10_SCORE_1X1 = 6 /* examples/bach10_scoreinformed/trainCNNrwc.py:66-132 (--function build_ca_1x1, 22 arrays):
+                                   six strided ReLU convolutions + a 1x1 conv, ReLU-gated InverseLayers.  Served by
+                                   dcs_separate_audio_score and dcs_separate_spec_channels only.  feat_size (>= 253) and
+                                   time_context (>= 19) are not in the weights; the trainer uses 2049 and 30.  feat_size
+                                   need not be 2^k+1 for dcs_separate_spec_channels */
 };
 
 /* patch generators */
@@ -77,11 +83,17 @@ int64_t dcs_launch_count(const dcs_ctx* ctx);
  * elements; the call fails if it is too small).  d_S = NULL switches it off.  These are the tensors
  * `overlapadd_multi(...)/scale * exp(j*phase)` of separate_dsd.py:301-304. */
 int dcs_set_spectrum_tap(dcs_ctx* ctx, dcs_complex* d_S, int64_t capacity);
-/* Same for the max-pool network (DCS_ARCH_IKALA): the tie bits of MaxPool2DLayer((1,4)) the un-pool
- * (InverseLayer(pool), separate_ikala.py:183,188) routes by -- uint8[T][WP][32], bit r set: position 4*jp+r
- * of the window equals its maximum, channel = last index (30 used), WP = ((F-30)/3+1)/4.  The routing is
- * a discrete decision of the reference's graph; the parity tests adopt the device's where float64 flags
- * the window as ill-conditioned and require agreement elsewhere.  capacity in bytes; NULL = off. */
+/* Same for the discrete routing decisions of the forward pass, which the InverseLayers of the decoder follow.
+ * The parity tests adopt the device's decisions where float64 flags them as ill-conditioned and require agreement
+ * elsewhere.  capacity in bytes; NULL = off.
+ *  - max-pool network (DCS_ARCH_IKALA): the tie bits of MaxPool2DLayer((1,4)) the un-pool (InverseLayer(pool),
+ *    separate_ikala.py:183,188) routes by -- uint8[T][WP][32], bit r set: position 4*jp+r of the window equals its
+ *    maximum, channel = last index (30 used), WP = ((F-30)/3+1)/4.
+ *  - 1x1 score net (DCS_ARCH_BACH10_SCORE_1X1): one gate code 2*relu'(pre) in {0, 1, 2} (1: pre-activation exactly 0,
+ *    where Theano's relu = 0.5*(x+|x|) has derivative 0.5) per encoder activation of conv1..conv6, the layers one after
+ *    the other, each uint8[rows][W_l][C_l] with W_0 = feat_size, W_l = (W_{l-1}-5)/2+1, C = 30, 50, 70, 100, 200, 200;
+ *    rows = Tp for conv1..conv4, Tp-9 for conv5, Tp-18 for conv6, where Tp = max(T, (P-1)*step + time_context) frames
+ *    are the ones the P patches span (row r of patch k is frame k*step + r). */
 int dcs_set_pool_tap(dcs_ctx* ctx, uint8_t* d_bits, int64_t capacity);
 
 /* Multichannel Wiener post-filter of two-channel stems (see dcs_wiener_stereo): while iterations > 0, the entry points
