@@ -131,6 +131,11 @@ int dcs_destroy(dcs_ctx* c) {
     if (c->ev_enc[i]) cudaEventDestroy(c->ev_enc[i]);
     if (c->ev_out[i]) cudaEventDestroy(c->ev_out[i]);
   }
+  if (c->ev_notes) {
+    cudaEventSynchronize(c->ev_notes);   // the last copy out of the pinned staging has completed
+    cudaEventDestroy(c->ev_notes);
+  }
+  if (c->notes_host) cudaFreeHost(c->notes_host);
   if (c->s_h2d) cudaStreamDestroy(c->s_h2d);
   if (c->s_d2h) cudaStreamDestroy(c->s_d2h);
   delete c;
@@ -556,8 +561,8 @@ static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, i
 // channel -> nsrc x 2 stem planes ordered (source, channel).  Two-channel stems (keep-channels, the stereo net) go
 // through the Wiener post-filter between the network and the iSTFT when dcs_set_wiener is above 0
 static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,
-                         const float* d_filters, const float* d_mono, float scale_factor, int overlap, int patcher,
-                         float* d_stems, int64_t stem_stride, cudaStream_t st) {
+                         const float* d_filters, const NoteTable* notes, const float* d_mono, float scale_factor,
+                         int overlap, int patcher, float* d_stems, int64_t stem_stride, cudaStream_t st) {
   const bool keep = d_mono != nullptr;
   DCS_TRY(size_workspace(ctx, m, p, L, false, keep, st));
   const int nch = m->nch, nx = keep ? 2 : 1;
@@ -576,10 +581,13 @@ static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const fl
     }
   }
   const float* in = mag;
-  if (d_filters) {
+  if (d_filters || notes) {
     float* chans = ctx->net[NET_CHANS].as<float>();
     ProfScope ps(ctx, "score_channels", st);
-    DCS_TRY(launch_channel_mul(ctx, mag, d_filters, chans, plane, score_planes(m), st));
+    if (notes)   // the filters rasterised from the note table, times mag: no filter plane in memory
+      DCS_TRY(launch_score_notes(ctx, *notes, mag, chans, ldf, plane, st));
+    else
+      DCS_TRY(launch_channel_mul(ctx, mag, d_filters, chans, plane, score_planes(m), st));
     in = chans;
   }
   DCS_TRY(run_network(ctx, m, in, plane, X, plane, nx, T, ldf, overlap, patcher, S, plane, st));
@@ -617,8 +625,39 @@ int dcs_separate_audio_score(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const floa
                      overlap, patcher));
   DCS_REQUIRE(d_filters, "dcs_separate_audio_score: NULL filters");
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return separate_clip(ctx, m, p, d_audio, L, L, d_filters, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
-                       (cudaStream_t)stream);
+  return separate_clip(ctx, m, p, d_audio, L, L, d_filters, nullptr, nullptr, scale_factor, overlap, patcher, d_stems,
+                       stem_stride, (cudaStream_t)stream);
+}
+
+int dcs_score_filters(dcs_ctx* ctx, const double* h_melody, int ninst, int nnotes, int ncols, int64_t start, int64_t T, int F,
+                      const float* d_mag, int64_t ldf, float* d_out, int64_t plane, void* stream) {
+  DCS_REQUIRE(ctx && d_out, "dcs_score_filters: NULL argument");
+  std::vector<int32_t> tab;
+  NoteTable nt;
+  DCS_TRY(notes_compact("dcs_score_filters", h_melody, ninst, nnotes, ncols, start, T, F, &tab, &nt));
+  DCS_REQUIRE(ldf >= F && ldf < ((int64_t)1 << 31) && plane >= T * ldf, "dcs_score_filters: bad shape (ldf %lld, plane %lld)",
+              (long long)ldf, (long long)plane);
+  cudaStream_t st = (cudaStream_t)stream;
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  DCS_TRY(notes_stage(ctx, tab, &nt, st));
+  ProfScope ps(ctx, "score_filters", st);
+  return launch_score_notes(ctx, nt, d_mag, d_out, ldf, plane, st);
+}
+
+int dcs_separate_audio_notes(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t L, const double* h_melody,
+                             int nnotes, int ncols, int64_t frame0, float scale_factor, int overlap, int patcher, float* d_stems,
+                             int64_t stem_stride, void* stream) {
+  DCS_TRY(check_clip("dcs_separate_audio_notes", ctx, m, p, DCS_ARCH_BACH10_SCORE, d_audio, d_stems, L, L, stem_stride,
+                     overlap, patcher));
+  std::vector<int32_t> tab;
+  NoteTable nt;
+  DCS_TRY(notes_compact("dcs_separate_audio_notes", h_melody, score_planes(m), nnotes, ncols, frame0,
+                        dcs_num_frames(L, p->hop), m->F, &tab, &nt));
+  cudaStream_t st = (cudaStream_t)stream;
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  DCS_TRY(notes_stage(ctx, tab, &nt, st));
+  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, &nt, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
+                       st);
 }
 
 int dcs_gemm_f32(dcs_ctx* ctx, int engine, const float* d_A, int64_t lda, const float* h_B, int64_t ldb,
@@ -664,8 +703,8 @@ int dcs_separate_audio_stereo(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const flo
   DCS_TRY(check_clip("dcs_separate_audio_stereo", ctx, m, p, DCS_ARCH_DSD_ILD, d_audio, d_stems, L, audio_stride, stem_stride,
                      overlap, patcher));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
-                       (cudaStream_t)stream);
+  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher, d_stems,
+                       stem_stride, (cudaStream_t)stream);
 }
 
 int dcs_xcorr_lags(dcs_ctx* ctx, const float* const* h_a, const float* const* h_b, int npairs, int64_t num_samples, int flen,
@@ -679,8 +718,8 @@ int dcs_separate_audio(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_a
                        int overlap, int patcher, float* d_stems, int64_t stem_stride, void* stream) {
   DCS_TRY(check_clip("dcs_separate_audio", ctx, m, p, -1, d_audio, d_stems, L, L, stem_stride, overlap, patcher));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
-                       (cudaStream_t)stream);
+  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher, d_stems,
+                       stem_stride, (cudaStream_t)stream);
 }
 
 int dcs_separate_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* h_audio, int64_t L, float scale_factor,
@@ -690,7 +729,8 @@ int dcs_separate_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* h_au
   DCS_CUDA(cudaSetDevice(ctx->device));
   DCS_TRY(size_workspace(ctx, m, p, L, true, false, st));
   DCS_CUDA(cudaMemcpyAsync(ctx->audio.p, h_audio, (size_t)L * sizeof(float), cudaMemcpyHostToDevice, st));
-  DCS_TRY(separate_clip(ctx, m, p, ctx->audio.as<float>(), L, L, nullptr, nullptr, scale_factor, overlap, patcher, ctx->stems.as<float>(), L, st));
+  DCS_TRY(separate_clip(ctx, m, p, ctx->audio.as<float>(), L, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher,
+                        ctx->stems.as<float>(), L, st));
   DCS_CUDA(cudaMemcpy2DAsync(h_stems, (size_t)stem_stride * sizeof(float), ctx->stems.p, (size_t)L * sizeof(float),
                              (size_t)L * sizeof(float), m->nsrc, cudaMemcpyDeviceToHost, st));
   DCS_CUDA(cudaStreamSynchronize(st));
@@ -734,11 +774,13 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, c
     if (keep) {
       DCS_TRY(launch_pcm_decode_keep(ctx, ctx->pcm_in[b].as<int16_t>(), L, audio, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
-      DCS_TRY(separate_clip(ctx, m, p, audio + L, L, L, nullptr, audio, scale_factor, overlap, patcher, stems, L, st));
+      DCS_TRY(separate_clip(ctx, m, p, audio + L, L, L, nullptr, nullptr, audio, scale_factor, overlap, patcher, stems, L,
+                            st));
     } else {
       DCS_TRY(launch_pcm_decode(ctx, ctx->pcm_in[b].as<int16_t>(), L, channels, downmix, audio, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
-      DCS_TRY(separate_clip(ctx, m, p, audio, L, L, nullptr, nullptr, scale_factor, overlap, patcher, stems, L, st));
+      DCS_TRY(separate_clip(ctx, m, p, audio, L, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher, stems, L,
+                            st));
     }
     if (i >= 2) DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_out[b], 0));     // D2H of clip i-2 has drained the output staging
     if (keep)
@@ -826,7 +868,7 @@ int dcs_separate_audio_keep_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, co
     ProfScope ps(ctx, "downmix", st);
     DCS_TRY(launch_downmix2(ctx, d_audio, audio_stride, L, mono, st));
   }
-  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, mono, scale_factor, overlap, patcher, d_stems,
+  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, nullptr, mono, scale_factor, overlap, patcher, d_stems,
                        stem_stride, st);
 }
 

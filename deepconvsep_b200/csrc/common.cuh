@@ -63,6 +63,7 @@ enum NetSlot {
   NET_XC_PTRS, NET_XC_PARTIAL,              // dcs_xcorr_lags
   NET_XTAB,                                 // DSD mask kernel's frame table
   NET_ENC, NET_CODES, NET_DEC,              // 1x1 score net: encoder activations, ReLU gate codes, decoder chunk
+  NET_NOTES,                                // compacted note table of the score-informed nets (score_notes.cu)
   NET_SLOTS
 };
 
@@ -94,6 +95,9 @@ struct dcs_ctx {
   int64_t pool_tap_cap = 0;
   int wiener_iters = 0;         // dcs_set_wiener: EM iterations of the stereo Wiener post-filter (0 = off)
   dcs::DevBuf wiener;           // its partial sums, spatial covariances and mixture scale (wiener.cu)
+  int32_t* notes_host = nullptr;      // pinned staging of the compacted note table (its device copy: net[NET_NOTES])
+  size_t notes_host_cap = 0;
+  cudaEvent_t ev_notes = nullptr;     // the copy out of notes_host; guards its reuse
 };
 
 struct dcs_stft {
@@ -283,6 +287,23 @@ int launch_sconv_mask(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st);
 bool sconv_mask_tc_supported(const SconvMaskArgs& a);
 int launch_sconv_mask_tc(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st);   // wgmma (sconv_tc.cu)
 int launch_channel_mul(dcs_ctx* ctx, const float* mag, const float* filt, float* out, int64_t plane, int nch, cudaStream_t st);
+
+// the note table of the score-informed nets (score_notes.cu), compacted for the frame window [start, start + T):
+// int32 words, frame_ptr[T + 1] at 0 (CSR of the notes sounding in each frame), note indices at `entries`,
+// (instrument, first range, range count) per note at `recs`, (lo, hi) bin pairs at `ranges`
+struct NoteTable {
+  const int32_t* d;   // device copy
+  int ninst, F;
+  int64_t T, entries, recs, ranges, size;
+};
+// validates the whole table (DCS_EINVAL, nothing queued) and compacts it
+int notes_compact(const char* fn, const double* h_melody, int ninst, int nnotes, int ncols, int64_t start, int64_t T, int F,
+                  std::vector<int32_t>* tab, NoteTable* nt);
+// pinned staging -> net[NET_NOTES] on `st`; sets nt->d
+int notes_stage(dcs_ctx* ctx, const std::vector<int32_t>& tab, NoteTable* nt, cudaStream_t st);
+// out + j * plane: filter j [T][ldf] (mag == NULL) or filter j * mag (mag [T][ldf]); pad columns F..ldf-1 = 0
+int launch_score_notes(dcs_ctx* ctx, const NoteTable& nt, const float* mag, float* out, int64_t ldf, int64_t plane,
+                       cudaStream_t st);
 
 int launch_xcorr_lags(dcs_ctx* ctx, const float* const* h_a, const float* const* h_b, int npairs, int64_t L, int flen,
                       double* h_out, cudaStream_t st);

@@ -65,6 +65,42 @@ def wiener_stereo(ctx, X, S, iterations, stream=None, num_bins=None):
     return S
 
 
+def check_melody(melody, ninst=None):
+    """The note table (deepconvsep_b200.score.score_melody) as the library takes it: float64 C-contiguous
+    [ninst, nnotes, ncols], ninst in 1..4 (`ninst` when given), ncols >= 3.  The rows themselves are checked by the
+    library before it queues anything (include/dcs.h, dcs_score_filters)."""
+    m = np.ascontiguousarray(melody, dtype=np.float64)
+    if m.ndim != 3:
+        raise ValueError("melody must be [ninst, nnotes, ncols], got shape %r" % (m.shape,))
+    if not 1 <= m.shape[0] <= 4 or (ninst is not None and m.shape[0] != ninst):
+        raise ValueError("melody has %d instruments, %s" % (m.shape[0], "the model takes %d" % ninst if ninst else "1 to 4 allowed"))
+    if m.shape[2] < 3:
+        raise ValueError("melody rows have %d columns, at least 3 (first frame, last frame, MIDI number)" % m.shape[2])
+    return m
+
+
+def score_filters(ctx, melody, T, F, start=0, mag=None, ldf=None, stream=None):
+    """filterSpec(mag, melody, start, start + T) rasterised on the device (dcs_score_filters) -> torch float32 cuda
+    [ninst, T, ldf], pad columns 0.  mag None: the normalised filters; mag (torch float32 cuda [T, ldf]): the filters
+    times mag.  ldf defaults to mag's row length, else F rounded up to 8."""
+    import torch
+    m = check_melody(melody)
+    T, F, start = int(T), int(F), int(start)
+    if T < 1 or F < 1 or start < 0:
+        raise ValueError("score_filters: T %d and F %d must be >= 1, start %d >= 0" % (T, F, start))
+    if mag is not None:
+        if not (mag.is_cuda and mag.dtype == torch.float32 and mag.dim() == 2 and mag.shape[0] == T and mag.is_contiguous()):
+            raise ValueError("mag must be a contiguous float32 cuda tensor [T, ldf]")
+        ldf = mag.shape[1] if ldf is None else ldf
+        if mag.shape[1] != ldf:
+            raise ValueError("mag has rows of %d, ldf is %d" % (mag.shape[1], ldf))
+    ldf = int(ldf if ldf is not None else (F + 7) // 8 * 8)
+    out = torch.empty((m.shape[0], T, ldf), dtype=torch.float32, device=torch.device("cuda", ctx.device))
+    _lib.check(ctx.lib.dcs_score_filters(ctx.handle, m.ctypes.data, m.shape[0], m.shape[1], m.shape[2], start, T, F,
+                                         _ptr(mag), ldf, _ptr(out), T * ldf, _stream_ptr(stream, ctx.device)))
+    return out
+
+
 class Context(object):
     """One dcs_ctx = one device + the workspace of one in-flight pipeline."""
 
@@ -391,6 +427,27 @@ class Separator(object):
                                                      outd.stride(0), _stream_ptr(stream, self.ctx.device)))
         return outd.cpu().numpy() if host else outd
 
+    def separate_notes(self, audio, melody, frame0=0, out=None, stream=None):
+        """separate_score with the filters rasterised on the device from the note table (dcs_separate_audio_notes):
+        audio float [L] (numpy or cuda tensor) + melody float64 [4, nnotes, ncols] (deepconvsep_b200.score.score_melody)
+        -> stems float32 [4, L] (same kind as `audio`), the bits of separate_score(audio, filterSpec(..., frame0,
+        frame0 + T)).  frame0: the table frame of the clip's first STFT frame (a segment of a longer recording)."""
+        import torch
+        if self.model.arch not in ("bach10_score", "bach10_score_1x1"):
+            raise ValueError("separate_notes needs a score-informed network, this one is %r" % self.model.arch)
+        if int(frame0) < 0:
+            raise ValueError("frame0 %d must be >= 0" % frame0)
+        m = check_melody(melody, 4)
+        host = not hasattr(audio, "is_cuda")
+        x = torch.as_tensor(np.ascontiguousarray(audio, dtype=np.float32), device=self.stft.dev) if host else audio
+        L = x.numel()
+        outd = out if (out is not None and not host) else torch.empty((self.nsrc, L), dtype=torch.float32, device=x.device)
+        _lib.check(self.lib.dcs_separate_audio_notes(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), L,
+                                                     m.ctypes.data, m.shape[1], m.shape[2], int(frame0), self.scale_factor,
+                                                     self.overlap, self.patcher, _ptr(outd), outd.stride(0),
+                                                     _stream_ptr(stream, self.ctx.device)))
+        return outd.cpu().numpy() if host else outd
+
     def separate_stereo(self, audio, out=None, stream=None, wiener=0):
         """Stereo / ILD network (examples/dsd100_2ch_ILD/trainCNN_ILD_DSD100.py:299-327): audio float
         [L, 2] (numpy) or [2, L] (cuda tensor) -> `sep_audio` float32 [L, nsrc, 2] (numpy) or the device
@@ -441,14 +498,15 @@ class Separator(object):
             return outd
         return np.ascontiguousarray(outd.cpu().numpy().reshape(self.nsrc, 2, L).transpose(2, 0, 1))
 
-    def separate_tapped(self, audio, filters=None, pool=False, keep_channels=False, wiener=0):
+    def separate_tapped(self, audio, filters=None, pool=False, keep_channels=False, wiener=0, melody=None, frame0=0):
         """Parity-test entry: the same pipeline as separate() / separate_score() / separate_stereo() /
         separate_keep_channels() (keep_channels=True) with the spectrum tap on (dcs_set_spectrum_tap) -> (stems as
         that call returns them, masked spectra complex64 numpy [nplanes, T, F] -- the tensors the inverse STFT of THIS
         call consumed, (source, channel) planes for the stereo outputs).
         pool=True: also the routing decisions of this call (dcs_set_pool_tap) -- max-pool net: the tie bits uint8
         [T, WP, 32]; 1x1 score net: the gate codes of conv1..conv6, a list of uint8 [rows, W, C] (gate_code_layout).
-        wiener: EM iterations of the Wiener post-filter (two-channel stems only); the tap then holds the filtered spectra."""
+        wiener: EM iterations of the Wiener post-filter (two-channel stems only); the tap then holds the filtered spectra.
+        melody (score-informed nets): the note table instead of `filters`, through separate_notes(audio, melody, frame0)."""
         import torch
         stereo = keep_channels or self.model.arch == "dsd_ild"
         if wiener and not stereo:
@@ -472,6 +530,8 @@ class Separator(object):
         try:
             if keep_channels:
                 out = self.separate_keep_channels(a, wiener=wiener)
+            elif melody is not None:
+                out = self.separate_notes(a, melody, frame0=frame0)
             elif self.model.arch in ("bach10_score", "bach10_score_1x1"):
                 out = self.separate_score(a, filters)
             elif self.model.arch == "dsd_ild":

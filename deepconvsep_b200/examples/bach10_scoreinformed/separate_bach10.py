@@ -19,7 +19,7 @@ import scipy.io.wavfile
 from ...models import load_model, infer_arch           # noqa: F401
 from ...transform import sinebell, stft_norm, istft_norm, transformFFT  # noqa: F401
 from ...util import generate_overlapadd, overlapadd_multi  # noqa: F401  (util.py:220-327)
-from ...score import str2midi, getMidiNum, expandMidi, filterSpec, slicefft_slices, score_filters  # noqa: F401
+from ...score import str2midi, getMidiNum, expandMidi, filterSpec, slicefft_slices, score_filters, score_melody  # noqa: F401
 from ...engine import Separator
 from .. import _common
 
@@ -43,8 +43,9 @@ def train_auto(filein, outdir, model, scale_factor=0.3, time_context=30, overlap
         return None
     audio = _common.decode(audioObj, "bach10")
     nframes = int(np.ceil(len(audio) / np.double(hopSize))) + 2
-    filters = score_filters(os.path.dirname(os.path.abspath(filein)), SOURCES_MIDI, nframes, input_size, frameSize=frameSize,
-                            hopSize=hopSize, sampleRate=sampleRate)
+    # the note table; the filters are rasterised from it on the GPU
+    melody = score_melody(os.path.dirname(os.path.abspath(filein)), SOURCES_MIDI, nframes, frameSize=frameSize,
+                          hopSize=hopSize, sampleRate=sampleRate)
     key = (os.path.abspath(model), os.path.getmtime(model), scale_factor, time_context, overlap, input_size, frameSize, hopSize)
     if key not in _cache:
         _cache.clear()
@@ -54,7 +55,7 @@ def train_auto(filein, outdir, model, scale_factor=0.3, time_context=30, overlap
         _cache[key] = Separator(params, arch=family, frame_size=frameSize, hop=hopSize, window="blackmanharris",
                                 scale_factor=scale_factor, time_context=time_context, overlap=overlap, patcher="util",
                                 feat_size=input_size)
-    stems = _cache[key].separate_score(audio, filters)
+    stems = _cache[key].separate_notes(audio, melody)
     maxn = np.iinfo(np.int16).max
     _, filename = os.path.split(filein)
     paths = []

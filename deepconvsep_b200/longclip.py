@@ -48,7 +48,7 @@ def plan_segments(num_samples, parts, frame_size, hop, time_context, overlap):
     """Cut [0, num_samples) into at most `parts` segments.  Each Segment holds the sample range to feed the pipeline
     (in_start:in_stop), the range of the result that is kept (out_start:out_stop, absolute sample indices) and the
     index of the whole-clip STFT frame its first frame corresponds to (a multiple of step; score filters are sliced
-    from there).
+    from there, a note table is rasterised from there).
 
     Left bound.  With s0 = frame0 * hop the sub-clip's frame t' is the clip's frame frame0 + t' once
     t' >= q = ceil(N/2 / hop) (no front padding inside the frame); the first patch made of such frames starts at
@@ -102,13 +102,14 @@ def _geometry(sep):
     return sep.frame_size, sep.hop, sep.model.tc, sep.overlap
 
 
-def _run(sep, sub, filt):
-    """One segment through a Separator (or a callable (sub, filt) -> array with the sample axis last)."""
+def _run(sep, sub, filt, melody=None, frame0=0):
+    """One segment through a Separator (or a callable (sub, filt) -> array with the sample axis last; with a note
+    table: (sub, melody, frame0)).  The note table goes to the device whole: each segment rasterises its own frames."""
     if not hasattr(sep, "model"):
-        return np.asarray(sep(sub, filt))
+        return np.asarray(sep(sub, melody, frame0) if melody is not None else sep(sub, filt))
     arch = sep.model.arch
     if arch == "bach10_score":
-        return sep.separate_score(sub, filt)
+        return sep.separate_notes(sub, melody, frame0=frame0) if melody is not None else sep.separate_score(sub, filt)
     if arch == "dsd_ild":
         return np.ascontiguousarray(sep.separate_stereo(sub).transpose(1, 2, 0))     # [L, nsrc, 2] -> [nsrc, 2, L]
     return sep.separate(sub)
@@ -123,14 +124,25 @@ def _slice_filters(filters, sg, hop):
     return f
 
 
-def separate_long(separators, audio, parts=None, filters=None, geometry=None):
+def _check_score_inputs(filters, melody):
+    if filters is not None and melody is not None:
+        raise ValueError("pass the score as filters= or as melody=, not both")
+    if melody is not None:
+        from .engine import check_melody
+        return check_melody(melody)
+    return None
+
+
+def separate_long(separators, audio, parts=None, filters=None, geometry=None, melody=None):
     """audio float [L] (stereo / ILD network: [L, 2]) -> what the Separator's own call returns for the whole clip
     (float32 [nsrc, L]; stereo: [L, nsrc, 2]).  `separators`: one Separator or a list (one per GPU, or several
     contexts of one GPU); segment i runs on separators[i % len], one host thread per separator (the C-ABI calls
     release the GIL).  parts defaults to len(separators).  filters: score filters [4, T, F] of the whole clip
-    (score-informed network).  geometry=(frame_size, hop, time_context, overlap) is needed only when the
+    (score-informed network), sliced per segment on the host; or melody: its note table [4, nnotes, ncols]
+    (score.score_melody), which each segment rasterises on the device from its first frame on.  geometry=(frame_size, hop, time_context, overlap) is needed only when the
     separators are plain callables (tests)."""
     seps = list(separators) if isinstance(separators, (list, tuple)) else [separators]
+    melody = _check_score_inputs(filters, melody)
     N, H, tc, ov = geometry if geometry is not None else _geometry(seps[0])
     a = np.asarray(audio)
     L = a.shape[0]
@@ -142,7 +154,7 @@ def separate_long(separators, audio, parts=None, filters=None, geometry=None):
         try:
             for i in range(w, len(segs), len(seps)):
                 sg = segs[i]
-                pieces[i] = _run(seps[w], a[sg.in_start:sg.in_stop], _slice_filters(filters, sg, H))
+                pieces[i] = _run(seps[w], a[sg.in_start:sg.in_stop], _slice_filters(filters, sg, H), melody, sg.frame0)
         except BaseException as e:          # surfaced in the caller's thread
             errors.append(e)
 
@@ -163,12 +175,13 @@ def separate_long(separators, audio, parts=None, filters=None, geometry=None):
     return out
 
 
-def separate_long_distributed(separator, audio, filters=None, geometry=None, group=None):
-    """The same over the ranks of an initialised process group (one process per GPU, every rank holds the clip):
+def separate_long_distributed(separator, audio, filters=None, geometry=None, group=None, melody=None):
+    """The same (filters= or melody=) over the ranks of an initialised process group (one process per GPU, every rank holds the clip):
     rank r separates segments r, r + world, ...; the kept parts are gathered to rank 0 (sharding.gather_stems,
     the path's only exchange, off the data path) which returns the stitched stems; other ranks return None."""
     import torch.distributed as dist
     from .sharding import gather_stems
+    melody = _check_score_inputs(filters, melody)
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     N, H, tc, ov = geometry if geometry is not None else _geometry(separator)
     a = np.asarray(audio)
@@ -177,7 +190,7 @@ def separate_long_distributed(separator, audio, filters=None, geometry=None, gro
     mine = []
     for i in range(rank, len(segs), world):
         sg = segs[i]
-        p = _run(separator, a[sg.in_start:sg.in_stop], _slice_filters(filters, sg, H))
+        p = _run(separator, a[sg.in_start:sg.in_stop], _slice_filters(filters, sg, H), melody, sg.frame0)
         mine.append((i, np.ascontiguousarray(p[..., sg.out_start - sg.in_start:sg.out_stop - sg.in_start])))
     gathered = gather_stems(mine, world, rank, group=group)
     if rank != 0:

@@ -7,6 +7,7 @@ training process; here the model stays resident on the GPU and the songs are sha
 GPUs of a box (one process per GPU, `torchrun`), with no collective on the data path.
 
     python -m deepconvsep_b200.runner --family dsd --db <DSD100/Mixtures> --out <dir> --model model.pkl
+    python -m deepconvsep_b200.runner --family bach10_score --db <Bach10> --out <dir> --model model.pkl
     torchrun --nproc-per-node 8 -m deepconvsep_b200.runner --family dsd --db ... --out ... --model ...
 """
 import argparse
@@ -16,6 +17,7 @@ import numpy as np
 from . import util
 from .engine import Separator
 from .models import load_model, FAMILY_DEFAULTS
+from .score import score_melody
 from .sharding import shard_clips, reduce_stats
 
 # trainer settings: (frameSize, hop, window, overlap) -- dsd100/trainCNN.py:431,399; ikala/trainCNN.py:382;
@@ -27,7 +29,16 @@ TRAINER = {
     # stereo / ILD trainer: transformFFT(frameSize=1024, hopSize=512, window=hanning), overlap 25
     # (dsd100_2ch_ILD/trainCNN_ILD_DSD100.py:487, 438-441)
     "dsd_ild": dict(frameSize=1024, hopSize=512, window="hanning", overlap=25),
+    # score-informed Bach10: transformFFT(4096, 512, blackmanharris), overlap 25 (trainCNNrwc.py:585-587,653); the
+    # network (build_ca, 17 or 11 arrays, or build_ca_1x1, 22 arrays) is inferred from the parameter list
+    "bach10_score": dict(frameSize=4096, hopSize=512, window="blackmanharris", overlap=25),
 }
+# scale_factor_test of the score-informed trainer (trainCNNrwc.py:600-603,672); the other trainers separate with 0.3
+DEFAULT_SCALE = {"bach10_score": 0.2}
+# the score-informed trainer's sources (spelling of the reference) and their score files <instrument>_b.txt
+# (trainCNNrwc.py:361-362)
+SCORE_SOURCES = ["bassoon", "clarinet", "saxphone", "violin"]
+SCORE_MIDI = ["bassoon_b", "clarinet_b", "saxophone_b", "violin_b"]
 
 
 def list_jobs(family, testdir, outdir):
@@ -56,6 +67,13 @@ def list_jobs(family, testdir, outdir):
                 if f.startswith('.'):
                     continue
                 jobs.append((os.path.join(d, f, "mixture.wav"), [os.path.join(outdir, sub, f, s + ".wav") for s in src]))
+    elif family == "bach10_score":
+        # piece directories whose name starts with a digit, the four source wavs inside, stems <out>/<piece>-<source>.wav
+        # (trainCNNrwc.py:357-416,646-647); the job's input is the piece directory
+        for f in sorted(os.listdir(testdir)):
+            d = os.path.join(testdir, f)
+            if os.path.isdir(d) and f[0].isdigit():
+                jobs.append((d, [os.path.join(outdir, f + "-" + s + ".wav") for s in SCORE_SOURCES]))
     elif family == "ikala":
         for f in sorted(os.listdir(testdir)):
             if f.endswith(".wav"):
@@ -80,9 +98,29 @@ def _num_samples(path):
         return int(os.path.getsize(path))
 
 
-def separate_dataset(family, testdir, outdir, model, scale_factor=0.3, time_context=30, rank=0, world_size=1, device=0,
+def _piece_sources(piece):
+    name = os.path.basename(os.path.normpath(piece))
+    return [os.path.join(piece, name + "-" + s + ".wav") for s in SCORE_SOURCES]
+
+
+def read_piece(piece):
+    """A Bach10 piece directory -> (mixture float64 [L] = the float sum of its four source wavs, sampleRate, bit depth)
+    (trainCNNrwc.py:367-378)."""
+    audio = None
+    for path in _piece_sources(piece):
+        audioObj, sampleRate, bitrate = util.readAudioScipy(path)
+        assert sampleRate == 44100, "Sample rate needs to be 44100"
+        audio = audioObj if audio is None else audio + audioObj
+    return audio, sampleRate, bitrate
+
+
+def separate_dataset(family, testdir, outdir, model, scale_factor=None, time_context=30, rank=0, world_size=1, device=0,
                      keep_channels=False, wiener=0, **overrides):
-    """keep_channels (family dsd): 2-channel stems in the same layout -- the soft masks of the downmix applied to each
+    """scale_factor: None = the family's trainer value (0.2 for bach10_score, else 0.3).
+    bach10_score: every piece directory of `testdir` (name starting with a digit): the mixture is the sum of its four
+    source wavs, the note table comes from its <instrument>_b.txt scores (40 s window, 20 harmonics, +-50 cents,
+    440 Hz) and the filters are rasterised from it on the GPU (Separator.separate_notes).
+    keep_channels (family dsd): 2-channel stems in the same layout -- the soft masks of the downmix applied to each
     channel of the mixture (Separator.separate_keep_channels), so that a multichannel evaluation scores real stereo
     images.  wiener (family dsd with keep_channels, or dsd_ild): that many EM iterations of the multichannel Wiener
     post-filter on the stereo stems."""
@@ -94,16 +132,32 @@ def separate_dataset(family, testdir, outdir, model, scale_factor=0.3, time_cont
         raise ValueError("--wiener needs stereo stems: --family dsd --keep-channels, or --family dsd_ild")
     wkw = {"wiener": wiener} if wiener else {}
     cfg = dict(TRAINER[family], **overrides)
+    if scale_factor is None:
+        scale_factor = DEFAULT_SCALE.get(family, 0.3)
     params = load_model(model) if isinstance(model, str) else model
-    sep = Separator(params, arch=None if family == "ikala" else family, frame_size=cfg["frameSize"], hop=cfg["hopSize"],
-                    window=cfg["window"], scale_factor=scale_factor, time_context=time_context, overlap=cfg["overlap"],
-                    patcher="util", device=device, feat_size=cfg["frameSize"] // 2 + 1)
+    sep = Separator(params, arch=None if family in ("ikala", "bach10_score") else family, frame_size=cfg["frameSize"],
+                    hop=cfg["hopSize"], window=cfg["window"], scale_factor=scale_factor, time_context=time_context,
+                    overlap=cfg["overlap"], patcher="util", device=device, feat_size=cfg["frameSize"] // 2 + 1)
+    if family == "bach10_score" and sep.model.arch not in ("bach10_score", "bach10_score_1x1"):
+        raise ValueError("--family bach10_score needs a score-informed network, %s holds a %r network" % (
+            model if isinstance(model, str) else "the parameter list", sep.model.arch))
     jobs = list_jobs(family, testdir, outdir)
-    sizes = [_num_samples(j[0]) for j in jobs]
+    sizes = [_num_samples(_piece_sources(j[0])[0] if family == "bach10_score" else j[0]) for j in jobs]
     seconds = 0.0
     # longest first: the workspace buffers only grow, so the first song sizes them once for the whole shard
     for idx in sorted(shard_clips(sizes, world_size, rank), key=lambda i: (-sizes[i], i)):
         wav, outs = jobs[idx]
+        if family == "bach10_score":
+            audio, sampleRate, bitrate = read_piece(wav)
+            nframes = int(np.ceil(len(audio) / np.double(cfg["hopSize"]))) + 2
+            melody = score_melody(wav, SCORE_MIDI, nframes, frameSize=cfg["frameSize"], hopSize=cfg["hopSize"],
+                                  sampleRate=sampleRate)
+            stems = sep.separate_notes(audio, melody)
+            for i, path in enumerate(outs):
+                os.makedirs(os.path.dirname(path), exist_ok=True)
+                util.writeAudioScipy(path, stems[i].astype(np.float64), sampleRate, bitrate)
+            seconds += len(audio) / float(sampleRate)
+            continue
         audioObj, sampleRate, bitrate = util.readAudioScipy(wav)
         assert sampleRate == 44100, "Sample rate needs to be 44100"
         if family == "dsd_ild" or keep_channels:             # both channels in, stereo stems out
@@ -136,7 +190,8 @@ def main(argv=None):
     ap.add_argument("--db", required=True)
     ap.add_argument("--out", required=True)
     ap.add_argument("--model", required=True)
-    ap.add_argument("--scale-factor", type=float, default=0.3)
+    ap.add_argument("--scale-factor", type=float, default=None,
+                    help="magnitude scale of the network input (default: 0.2 for --family bach10_score, else 0.3)")
     ap.add_argument("--keep-channels", action="store_true",
                     help="--family dsd: 2-channel stems, the soft masks of the downmix applied to each channel")
     ap.add_argument("--wiener", type=int, default=0, metavar="K",

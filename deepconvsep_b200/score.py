@@ -179,10 +179,11 @@ def filterSpec(mag, notes, start, stop, dtype=np.float32):
     return mask
 
 
-def score_filters(score_dir, instruments, nframes, feat_size, frameSize=4096, hopSize=512, sampleRate=44100,
-                  nharmonics=20, interval=50, tuning_freq=440, duration=40.0):
-    """The four normalised filter planes [ninst, nframes, F] the network input is built from
-    (trainCNNrwc.py:364-391: getMidiNum -> expandMidi(..., 0.2, 0.2, nframes, 0.5) -> filterSpec)."""
+def score_melody(score_dir, instruments, nframes, frameSize=4096, hopSize=512, sampleRate=44100, nharmonics=20,
+                 interval=50, tuning_freq=440, duration=40.0):
+    """The note table `melody` float64 [ninst, nnotes, 2*nharmonics+3] the filters are rasterised from
+    (trainCNNrwc.py:364-382: getMidiNum -> expandMidi(..., 0.2, 0.2, nframes, 0.5)); zero rows pad the
+    instruments with fewer notes.  The input of Separator.separate_notes / engine.score_filters."""
     nelem = 1
     for inst in instruments:
         nelem = max(nelem, getMidiNum(inst, score_dir, 0, duration))
@@ -192,5 +193,14 @@ def score_filters(score_dir, instruments, nframes, feat_size, frameSize=4096, ho
                          0.2, 0.2, nframes, 0.5)
         if tmp is not None:
             melody[i, :tmp.shape[0], :] = tmp
+    return melody
+
+
+def score_filters(score_dir, instruments, nframes, feat_size, frameSize=4096, hopSize=512, sampleRate=44100,
+                  nharmonics=20, interval=50, tuning_freq=440, duration=40.0):
+    """The four normalised filter planes [ninst, nframes, F] the network input is built from
+    (trainCNNrwc.py:364-391: filterSpec of score_melody)."""
+    melody = score_melody(score_dir, instruments, nframes, frameSize=frameSize, hopSize=hopSize, sampleRate=sampleRate,
+                          nharmonics=nharmonics, interval=interval, tuning_freq=tuning_freq, duration=duration)
     mask = filterSpec(np.zeros((nframes, feat_size), dtype=np.float32), melody, 0, nframes)
     return np.ascontiguousarray(mask.reshape(nframes, len(instruments), feat_size).transpose(1, 0, 2))

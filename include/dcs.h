@@ -176,6 +176,34 @@ int dcs_separate_audio_score(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, con
                              int64_t num_samples, const float* d_filters, float scale_factor, int overlap,
                              int patcher, float* d_stems, int64_t stem_stride, void* stream);
 
+/* Score filters from the note table, rasterised on the device (filterSpec(mag, melody, start, start + T),
+ * dataset.py:839-862, bit for bit).  h_melody: the reference's `melody` as it is, HOST float64
+ * [ninst][nnotes][ncols] (ninst 1..4, ncols >= 3): per row the first frame n0, the last frame n1 (exclusive), the
+ * MIDI number, then (ncols-3)/2 (lo, hi) bin pairs.  A row sounds when its MIDI number is > 0 (NaN, the '?' note, is
+ * not) and max(0, min(n1, stop) - max(n0, start)) > 0 in double; it covers frames int(max(n0, start)) - start ..
+ * int(min(n1, stop)) - start (exclusive; int = C truncation) and the bins int(lo) .. int(hi) (exclusive) of every pair
+ * with hi > 0.  Bins of sounding notes are 1, the others float(1e-18); filter_j = v_j / (((v_0 + v_1) + v_2) + v_3)
+ * in fp32 with IEEE division.  Frame t of the output is frame start + t of the whole-clip filters.
+ * Every row with a MIDI number > 0, whatever the window, is checked before anything is queued, and the call fails
+ * with DCS_EINVAL where numpy would wrap or raise: a non-finite frame or bin, or a non-empty bin range reaching below
+ * 0 or above F.
+ * d_mag NULL (filters mode): d_out + j * plane = filter_j [T][ldf]; d_mag float[T][ldf] (channels mode): filter_j * mag.
+ * Pad columns F..ldf-1 are written as 0.  The compacted table goes through a pinned staging buffer of the ctx (an
+ * event guards its reuse) into a ctx workspace buffer; the stream is not synchronised. */
+int dcs_score_filters(dcs_ctx* ctx, const double* h_melody, int ninst, int nnotes, int ncols, int64_t start,
+                      int64_t num_frames, int F, const float* d_mag, int64_t ldf, float* d_out, int64_t plane,
+                      void* stream);
+/* dcs_separate_audio_score with the filter planes replaced by the note table (the model's 4 input planes = 4
+ * instruments, h_melody [4][nnotes][ncols] as in dcs_score_filters): the filters are rasterised times the scaled
+ * magnitude straight into the network's input channels, so no filter plane is read or written.  The clip's first STFT
+ * frame is table frame frame0 (0 for a whole clip; a segment of a longer recording starting at sample frame0 * hop
+ * passes frame0).  Same stems, spectrum tap and launch count as dcs_separate_audio_score on
+ * filterSpec(..., frame0, frame0 + T); the table is validated with the other arguments before anything is queued. */
+int dcs_separate_audio_notes(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const float* d_audio,
+                             int64_t num_samples, const double* h_melody, int nnotes, int ncols, int64_t frame0,
+                             float scale_factor, int overlap, int patcher, float* d_stems, int64_t stem_stride,
+                             void* stream);
+
 /* ---- building block: the dense layer / im2col-free convolution GEMM ------------------------ */
 /* d_C[M][ldc] = act(d_A[M][lda] * h_B[K][ldb] (+ h_bias[N])), fp32 in / fp32 out.  The weight is a
  * HOST array (it is transposed, padded and split for the tensor cores on the fly -- the models
