@@ -4,6 +4,7 @@
 stand-alone scripts (examples/dsd100/separate_dsd.py:239-313).  torch is used only as a
 device-memory / stream container; numpy arrays go through the *_host entry points."""
 import ctypes as C
+from functools import partial
 import numpy as np
 
 from . import _lib
@@ -63,6 +64,43 @@ def wiener_stereo(ctx, X, S, iterations, stream=None, num_bins=None):
     _lib.check(ctx.lib.dcs_wiener_stereo(ctx.handle, _ptr(X), X.stride(0), _ptr(S), S.stride(0), S.shape[0] // 2, T, ldf,
                                          F, int(iterations), _stream_ptr(stream, ctx.device)))
     return S
+
+
+def check_stereo_options(family, keep_channels=False, wiener=0):
+    """The rule for the options of two-channel stems, by network family (the keys of models.FAMILY_DEFAULTS, which
+    are also the Separator's architecture names): keep_channels (the soft masks of the downmix applied to each
+    channel) exists for the DSD100 / hiphopss network "dsd" only; wiener (EM iterations of the multichannel Wiener
+    post-filter) cannot be negative and needs two-channel stems: keep_channels, or the stereo / ILD network
+    "dsd_ild".  Raises ValueError with the reason otherwise."""
+    if keep_channels and family != "dsd":
+        raise ValueError("--keep-channels: only the DSD100 / hiphopss network (family dsd) keeps the stereo channels, "
+                         "not %s" % (family,))
+    if wiener < 0:
+        raise ValueError("--wiener %d: the number of EM iterations cannot be negative" % wiener)
+    if wiener and not (keep_channels or family == "dsd_ild"):
+        raise ValueError("--wiener needs --keep-channels (family dsd) or the stereo / ILD network (family dsd_ild): "
+                         "the Wiener post-filter works on two-channel stems")
+
+
+def clip_call(sep, filters=None, melody=None, frame0=0, keep_channels=False, wiener=0):
+    """The call that separates a whole clip with Separator `sep`'s network and these inputs, as a function of the
+    audio: sep.separate_keep_channels (keep_channels=True), sep.separate_notes (the note table melody, from table frame
+    frame0), sep.separate_score (a score-informed net and its score filters), sep.separate_stereo (the stereo / ILD
+    net) or sep.separate.  wiener: EM iterations of the Wiener post-filter, passed to the two-channel calls and refused
+    for the others here, before anything runs.  Only sep.model.arch and the method picked are used, so stand-ins with
+    just those work too."""
+    if keep_channels:
+        return partial(sep.separate_keep_channels, wiener=wiener)
+    if melody is not None:
+        run = partial(sep.separate_notes, melody=melody, frame0=frame0)
+    elif sep.model.arch in ("bach10_score", "bach10_score_1x1"):
+        run = partial(sep.separate_score, filters=filters)
+    elif sep.model.arch == "dsd_ild":
+        return partial(sep.separate_stereo, wiener=wiener)
+    else:
+        run = sep.separate
+    check_stereo_options(sep.model.arch, wiener=wiener)
+    return run
 
 
 def check_melody(melody, ninst=None):
@@ -304,13 +342,6 @@ class Separator(object):
         self.sources = d["sources"]
         self.lib = self.ctx.lib
 
-    def _stereo_wiener(self, wiener, stereo):
-        """set the Wiener post-filter for the next call; it only exists for two-channel stems"""
-        if wiener and not stereo:
-            raise ValueError("wiener=%r: the Wiener post-filter needs two-channel stems (keep_channels=True on the "
-                             "DSD100 / hiphopss network, or the stereo / ILD network)" % (wiener,))
-        self.ctx.set_wiener(wiener)
-
     # ---- host buffers (numpy): H2D + pipeline + D2H inside the call ----
     def separate(self, audio, out=None):
         """audio: 1-D float array (any float dtype) -> float32 [nsrc, L].  `audio` / `out` may be
@@ -332,8 +363,7 @@ class Separator(object):
         if keep_channels:
             return self.separate_pcm16_batch([pcm], outs=None if out is None else [out], keep_channels=True,
                                              wiener=wiener)[0]
-        if wiener:
-            self._stereo_wiener(wiener, False)
+        check_stereo_options(self.model.arch, wiener=wiener)
         p = np.ascontiguousarray(pcm, dtype=np.int16)
         L = p.shape[0]
         ch = 1 if p.ndim == 1 else p.shape[1]
@@ -350,43 +380,35 @@ class Separator(object):
         channel count; pinned for real overlap) -> list of int16 [nsrc, L].  keep_channels=True: stereo clips
         [L, 2] -> list of int16 [nsrc, L, 2] (dcs_separate_batch_pcm16_keep_channels_host), with `wiener` EM iterations
         of the Wiener post-filter on each clip's stems."""
-        if wiener and not keep_channels:
-            self._stereo_wiener(wiener, False)
+        if not keep_channels:
+            check_stereo_options(self.model.arch, wiener=wiener)
         ps = [np.ascontiguousarray(c, dtype=np.int16) for c in clips]
-        n = len(ps)
-        if n == 0:
+        if not ps:
             return []
         if keep_channels:
-            return self._pcm16_batch_keep_channels(ps, outs, wiener)
+            for p_ in ps:
+                if p_.ndim != 2 or p_.shape[1] != 2:
+                    raise ValueError("keep_channels needs stereo int16 clips [L, 2], got shape %r" % (p_.shape,))
+            self.ctx.set_wiener(wiener)
+            return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_keep_channels_host, ps, outs, (2,), ())
         ch = 1 if ps[0].ndim == 1 else ps[0].shape[1]
         assert all((1 if p_.ndim == 1 else p_.shape[1]) == ch for p_ in ps), "all clips must have the same channel count"
-        Ls = np.array([p_.shape[0] for p_ in ps], dtype=np.int64)
-        if outs is None:
-            outs = [np.empty((self.nsrc, int(L)), dtype=np.int16) for L in Ls]
-        assert all(o.dtype == np.int16 and o.shape == (self.nsrc, int(L)) and o.flags.c_contiguous for o, L in zip(outs, Ls))
-        pin = (C.c_void_p * n)(*[p_.ctypes.data for p_ in ps])
-        pout = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
-        _lib.check(self.lib.dcs_separate_batch_pcm16_host(self.ctx.handle, self.model.handle, self.stft.handle, n, pin,
-                                                          Ls.ctypes.data, ch, int(downmix if ch > 1 else 0), self.scale_factor,
-                                                          self.overlap, self.patcher, pout, Ls.ctypes.data,
-                                                          _stream_ptr(None, self.ctx.device)))
-        return outs
+        return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_host, ps, outs, (), (ch, int(downmix if ch > 1 else 0)))
 
-    def _pcm16_batch_keep_channels(self, ps, outs, wiener=0):
-        for p_ in ps:
-            if p_.ndim != 2 or p_.shape[1] != 2:
-                raise ValueError("keep_channels needs stereo int16 clips [L, 2], got shape %r" % (p_.shape,))
+    def _pcm16_batch(self, entry, ps, outs, channels, args):
+        """int16 clips ps through the multi-clip entry point `entry` -> outs, int16 [nsrc, L, *channels] each (made
+        when None).  args: the entry's arguments between the clip lengths and scale_factor."""
         n = len(ps)
         Ls = np.array([p_.shape[0] for p_ in ps], dtype=np.int64)
         if outs is None:
-            outs = [np.empty((self.nsrc, int(L), 2), dtype=np.int16) for L in Ls]
-        assert all(o.dtype == np.int16 and o.shape == (self.nsrc, int(L), 2) and o.flags.c_contiguous for o, L in zip(outs, Ls))
+            outs = [np.empty((self.nsrc, int(L)) + channels, dtype=np.int16) for L in Ls]
+        assert all(o.dtype == np.int16 and o.shape == (self.nsrc, int(L)) + channels and o.flags.c_contiguous
+                   for o, L in zip(outs, Ls))
         pin = (C.c_void_p * n)(*[p_.ctypes.data for p_ in ps])
         pout = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
-        self._stereo_wiener(wiener, True)
-        _lib.check(self.lib.dcs_separate_batch_pcm16_keep_channels_host(
-            self.ctx.handle, self.model.handle, self.stft.handle, n, pin, Ls.ctypes.data, self.scale_factor, self.overlap,
-            self.patcher, pout, Ls.ctypes.data, _stream_ptr(None, self.ctx.device)))
+        _lib.check(entry(self.ctx.handle, self.model.handle, self.stft.handle, n, pin, Ls.ctypes.data, *args,
+                         self.scale_factor, self.overlap, self.patcher, pout, Ls.ctypes.data,
+                         _stream_ptr(None, self.ctx.device)))
         return outs
 
     # ---- device buffers (torch tensors) ----
@@ -407,45 +429,42 @@ class Separator(object):
         device) -> stems float32 [4, L] (same kind as `audio`).  The four input channels are formed on the device."""
         import torch
         host = not hasattr(audio, "is_cuda")
-        x = torch.as_tensor(np.ascontiguousarray(audio, dtype=np.float32), device=self.stft.dev) if host else audio
-        L = x.numel()
-        T = self.stft.num_frames(L)
+        T = self.stft.num_frames(np.size(audio) if host else audio.numel())
         if hasattr(filters, "is_cuda"):      # already on the device, padded rows: [4, T, ldf] float32
             fd = filters
             assert fd.is_cuda and fd.dtype == torch.float32 and fd.is_contiguous() and tuple(fd.shape) == (4, T, self.stft.ldf)
         else:
+            dev = self.stft.dev if host else audio.device
             f = np.asarray(filters, dtype=np.float32)
             assert f.shape == (4, T, self.model.F), (f.shape, (4, T, self.model.F))
-            fd = torch.zeros((4, T, self.stft.ldf), dtype=torch.float32, device=x.device)
-            fd[:, :, :self.model.F] = torch.as_tensor(f, device=x.device)
-        if out is None or host:
-            outd = torch.empty((self.nsrc, L), dtype=torch.float32, device=x.device)
-        else:
-            outd = out
-        _lib.check(self.lib.dcs_separate_audio_score(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), L,
-                                                     _ptr(fd), self.scale_factor, self.overlap, self.patcher, _ptr(outd),
-                                                     outd.stride(0), _stream_ptr(stream, self.ctx.device)))
-        return outd.cpu().numpy() if host else outd
+            fd = torch.zeros((4, T, self.stft.ldf), dtype=torch.float32, device=dev)
+            fd[:, :, :self.model.F] = torch.as_tensor(f, device=dev)
+        return self._score_clip(self.lib.dcs_separate_audio_score, audio, (_ptr(fd),), out, stream)
 
     def separate_notes(self, audio, melody, frame0=0, out=None, stream=None):
         """separate_score with the filters rasterised on the device from the note table (dcs_separate_audio_notes):
         audio float [L] (numpy or cuda tensor) + melody float64 [4, nnotes, ncols] (deepconvsep_b200.score.score_melody)
         -> stems float32 [4, L] (same kind as `audio`), the bits of separate_score(audio, filterSpec(..., frame0,
         frame0 + T)).  frame0: the table frame of the clip's first STFT frame (a segment of a longer recording)."""
-        import torch
         if self.model.arch not in ("bach10_score", "bach10_score_1x1"):
             raise ValueError("separate_notes needs a score-informed network, this one is %r" % self.model.arch)
         if int(frame0) < 0:
             raise ValueError("frame0 %d must be >= 0" % frame0)
         m = check_melody(melody, 4)
+        return self._score_clip(self.lib.dcs_separate_audio_notes, audio, (m.ctypes.data, m.shape[1], m.shape[2], int(frame0)),
+                                out, stream)
+
+    def _score_clip(self, entry, audio, args, out, stream):
+        """audio float [L] (numpy, or a cuda tensor) through the score-informed clip entry point `entry` -> stems
+        float32 [nsrc, L], numpy for numpy audio.  args: the entry's arguments between the clip length and
+        scale_factor."""
+        import torch
         host = not hasattr(audio, "is_cuda")
         x = torch.as_tensor(np.ascontiguousarray(audio, dtype=np.float32), device=self.stft.dev) if host else audio
         L = x.numel()
         outd = out if (out is not None and not host) else torch.empty((self.nsrc, L), dtype=torch.float32, device=x.device)
-        _lib.check(self.lib.dcs_separate_audio_notes(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), L,
-                                                     m.ctypes.data, m.shape[1], m.shape[2], int(frame0), self.scale_factor,
-                                                     self.overlap, self.patcher, _ptr(outd), outd.stride(0),
-                                                     _stream_ptr(stream, self.ctx.device)))
+        _lib.check(entry(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), L, *args, self.scale_factor,
+                         self.overlap, self.patcher, _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
         return outd.cpu().numpy() if host else outd
 
     def separate_stereo(self, audio, out=None, stream=None, wiener=0):
@@ -453,24 +472,7 @@ class Separator(object):
         [L, 2] (numpy) or [2, L] (cuda tensor) -> `sep_audio` float32 [L, nsrc, 2] (numpy) or the device
         planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> cuda tensor out).  wiener: EM iterations of
         the multichannel Wiener post-filter (dcs_set_wiener) on the network's spectra, 0 = off."""
-        import torch
-        host = not hasattr(audio, "is_cuda")
-        if host:
-            a = np.asarray(audio, dtype=np.float32)
-            assert a.ndim == 2 and a.shape[1] == 2, a.shape
-            x = torch.as_tensor(np.ascontiguousarray(a.T), device=self.stft.dev)
-        else:
-            x = audio.contiguous()
-            assert x.dim() == 2 and x.shape[0] == 2 and x.dtype == torch.float32
-        L = x.shape[1]
-        outd = out if (out is not None and not host) else torch.empty((self.nsrc * 2, L), dtype=torch.float32, device=x.device)
-        self._stereo_wiener(wiener, True)
-        _lib.check(self.lib.dcs_separate_audio_stereo(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), x.stride(0), L,
-                                                      self.scale_factor, self.overlap, self.patcher, _ptr(outd), outd.stride(0),
-                                                      _stream_ptr(stream, self.ctx.device)))
-        if not host:
-            return outd
-        return np.ascontiguousarray(outd.cpu().numpy().reshape(self.nsrc, 2, L).transpose(2, 0, 1))
+        return self._two_channel_clip(self.lib.dcs_separate_audio_stereo, audio, out, stream, wiener)
 
     def separate_keep_channels(self, audio, out=None, stream=None, wiener=0):
         """Stereo stems from the DSD100 / hiphopss network (dcs_separate_audio_keep_channels): the network sees the
@@ -478,39 +480,42 @@ class Separator(object):
         phase.  audio float [L, 2] (numpy) or [2, L] (cuda tensor) -> float32 [L, nsrc, 2] (numpy, the layout of
         separate_stereo) or the device planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out).
         wiener: EM iterations of the multichannel Wiener post-filter (dcs_set_wiener) on the masked spectra, 0 = off."""
+        return self._two_channel_clip(self.lib.dcs_separate_audio_keep_channels, audio, out, stream, wiener)
+
+    def _two_channel_clip(self, entry, audio, out, stream, wiener):
+        """audio float [L, 2] (numpy) or [2, L] (cuda tensor) through the two-channel clip entry point `entry`, with
+        `wiener` EM iterations of the Wiener post-filter -> float32 [L, nsrc, 2] (numpy) or the device planes
+        [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out)."""
         import torch
         host = not hasattr(audio, "is_cuda")
         if host:
             a = np.asarray(audio, dtype=np.float32)
             if a.ndim != 2 or a.shape[1] != 2:
-                raise ValueError("keep-channels separation needs stereo audio [L, 2], got shape %r" % (a.shape,))
+                raise ValueError("two-channel separation needs stereo audio [L, 2], got shape %r" % (a.shape,))
             x = torch.as_tensor(np.ascontiguousarray(a.T), device=self.stft.dev)
         else:
             x = audio.contiguous()
             assert x.dim() == 2 and x.shape[0] == 2 and x.dtype == torch.float32
         L = x.shape[1]
         outd = out if (out is not None and not host) else torch.empty((self.nsrc * 2, L), dtype=torch.float32, device=x.device)
-        self._stereo_wiener(wiener, True)
-        _lib.check(self.lib.dcs_separate_audio_keep_channels(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x),
-                                                             x.stride(0), L, self.scale_factor, self.overlap, self.patcher,
-                                                             _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
+        self.ctx.set_wiener(wiener)
+        _lib.check(entry(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), x.stride(0), L, self.scale_factor,
+                         self.overlap, self.patcher, _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
         if not host:
             return outd
         return np.ascontiguousarray(outd.cpu().numpy().reshape(self.nsrc, 2, L).transpose(2, 0, 1))
 
     def separate_tapped(self, audio, filters=None, pool=False, keep_channels=False, wiener=0, melody=None, frame0=0):
-        """Parity-test entry: the same pipeline as separate() / separate_score() / separate_stereo() /
-        separate_keep_channels() (keep_channels=True) with the spectrum tap on (dcs_set_spectrum_tap) -> (stems as
-        that call returns them, masked spectra complex64 numpy [nplanes, T, F] -- the tensors the inverse STFT of THIS
-        call consumed, (source, channel) planes for the stereo outputs).
+        """Parity-test entry: the whole-clip call clip_call() picks for these inputs (separate() / separate_score() /
+        separate_notes() / separate_stereo() / separate_keep_channels()) with the spectrum tap on
+        (dcs_set_spectrum_tap) -> (stems as that call returns them, masked spectra complex64 numpy [nplanes, T, F] --
+        the tensors the inverse STFT of THIS call consumed, (source, channel) planes for the stereo outputs).
         pool=True: also the routing decisions of this call (dcs_set_pool_tap) -- max-pool net: the tie bits uint8
         [T, WP, 32]; 1x1 score net: the gate codes of conv1..conv6, a list of uint8 [rows, W, C] (gate_code_layout).
         wiener: EM iterations of the Wiener post-filter (two-channel stems only); the tap then holds the filtered spectra.
         melody (score-informed nets): the note table instead of `filters`, through separate_notes(audio, melody, frame0)."""
         import torch
-        stereo = keep_channels or self.model.arch == "dsd_ild"
-        if wiener and not stereo:
-            self._stereo_wiener(wiener, False)
+        run = clip_call(self, filters, melody, frame0, keep_channels, wiener)
         a = np.asarray(audio)
         L = a.shape[0]
         T = self.stft.num_frames(L)
@@ -528,16 +533,7 @@ class Separator(object):
                 bits = torch.zeros(sum(r * w * c for r, w, c in layout), dtype=torch.uint8, device=self.stft.dev)
             _lib.check(self.lib.dcs_set_pool_tap(self.ctx.handle, _ptr(bits), bits.numel()))
         try:
-            if keep_channels:
-                out = self.separate_keep_channels(a, wiener=wiener)
-            elif melody is not None:
-                out = self.separate_notes(a, melody, frame0=frame0)
-            elif self.model.arch in ("bach10_score", "bach10_score_1x1"):
-                out = self.separate_score(a, filters)
-            elif self.model.arch == "dsd_ild":
-                out = self.separate_stereo(a, wiener=wiener)
-            else:
-                out = self.separate(a)
+            out = run(a)
             torch.cuda.synchronize(self.stft.dev)
         finally:
             _lib.check(self.lib.dcs_set_spectrum_tap(self.ctx.handle, None, 0))

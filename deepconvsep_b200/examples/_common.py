@@ -5,7 +5,7 @@ import threading
 import numpy as np
 import scipy.io.wavfile
 
-from ..engine import Separator
+from ..engine import Separator, check_stereo_options
 from ..models import load_model, FAMILY_DEFAULTS
 
 _cache = {}
@@ -42,44 +42,26 @@ def decode(audioObj, family):
     return a if a.ndim == 1 else a[:, 0]
 
 
-def check_keep_channels(family, audioObj=None, filein=""):
-    """keep_channels (stereo stems from the masks of the downmix) exists for the DSD100 / hiphopss network and 2-channel
-    recordings only: raises ValueError with the reason otherwise."""
-    if family != "dsd":
-        raise ValueError("--keep-channels: only the DSD100 / hiphopss network keeps the stereo channels, not %s" % family)
-    if audioObj is not None and (audioObj.ndim != 2 or audioObj.shape[1] != 2):
-        raise ValueError("--keep-channels needs a 2-channel recording; %s has %d channel(s)"
-                         % (filein, 1 if audioObj.ndim == 1 else audioObj.shape[1]))
-
-
-def check_wiener(wiener, keep_channels):
-    """the Wiener post-filter works on two-channel stems: it needs keep_channels; raises ValueError otherwise"""
-    if wiener < 0:
-        raise ValueError("--wiener %d: the number of EM iterations cannot be negative" % wiener)
-    if wiener and not keep_channels:
-        raise ValueError("--wiener needs --keep-channels: the Wiener post-filter works on two-channel stems")
-
-
 def run(family, filein, outdir, model, scale_factor, time_context, overlap, batch_size, input_size, frame_size, hop,
         out_name, window=None, device=0, slot=0, keep_channels=False, wiener=0):
     """wav in -> one int16 wav per source in `outdir`.  `batch_size` is accepted for signature
     compatibility; the CUDA path has no patch batches.  keep_channels (DSD100 / hiphopss, 2-channel wav): one
     2-channel wav per source -- the soft masks of the downmix applied to each channel; wiener: that many EM iterations
     of the multichannel Wiener post-filter on them (keep_channels only)."""
-    check_wiener(wiener, keep_channels)
+    check_stereo_options(family, keep_channels, wiener)
     wkw = {"wiener": wiener} if wiener else {}
     d = dict(FAMILY_DEFAULTS[family])
     if window is not None:
         d["window"] = window
-    if keep_channels:
-        check_keep_channels(family)
     sampleRate, audioObj = scipy.io.wavfile.read(filein)
     if sampleRate != 44100:
         print("Sample rate is not 44100")        # separate_dsd.py:313
         return None
     arch = None if family in ("ikala",) else family
     if keep_channels:
-        check_keep_channels(family, audioObj, filein)
+        if audioObj.ndim != 2 or audioObj.shape[1] != 2:
+            raise ValueError("--keep-channels needs a 2-channel recording; %s has %d channel(s)"
+                             % (filein, 1 if audioObj.ndim == 1 else audioObj.shape[1]))
         if isinstance(device, (list, tuple)):
             raise ValueError("--keep-channels separates each recording on one device; give several files for several devices")
         sep = get_separator(model, arch, frame_size, hop, d["window"], scale_factor, time_context, overlap, input_size,
@@ -176,14 +158,10 @@ def cli_main(argv, usage, train_auto_default, run_one, family=None):
     import sys
     o = parse_cli(argv, usage)
     try:
-        check_wiener(o["wiener"], o["keep_channels"])
+        check_stereo_options(family, o["keep_channels"], o["wiener"])
     except ValueError as e:
         sys.exit(str(e))
     if o["keep_channels"]:
-        try:
-            check_keep_channels(family)
-        except ValueError as e:
-            sys.exit(str(e))
         base = run_one
         kw = {"keep_channels": True}
         if o["wiener"]:

@@ -102,17 +102,22 @@ def _geometry(sep):
     return sep.frame_size, sep.hop, sep.model.tc, sep.overlap
 
 
+def _sample_axis(sep, stems, last):
+    """The stereo / ILD network's stems [L, nsrc, 2] with the sample axis moved last (last=True: the layout the
+    segments are stitched in) or back to the front; the other networks' stems are sample-last already."""
+    if not (hasattr(sep, "model") and sep.model.arch == "dsd_ild"):
+        return stems
+    return np.ascontiguousarray(np.moveaxis(stems, 0, -1) if last else np.moveaxis(stems, -1, 0))
+
+
 def _run(sep, sub, filt, melody=None, frame0=0):
-    """One segment through a Separator (or a callable (sub, filt) -> array with the sample axis last; with a note
-    table: (sub, melody, frame0)).  The note table goes to the device whole: each segment rasterises its own frames."""
+    """One segment through a Separator's whole-clip call (engine.clip_call), or through a callable (sub, filt) ->
+    array with the sample axis last (with a note table: (sub, melody, frame0)).  The note table goes to the device
+    whole: each segment rasterises its own frames."""
     if not hasattr(sep, "model"):
         return np.asarray(sep(sub, melody, frame0) if melody is not None else sep(sub, filt))
-    arch = sep.model.arch
-    if arch == "bach10_score":
-        return sep.separate_notes(sub, melody, frame0=frame0) if melody is not None else sep.separate_score(sub, filt)
-    if arch == "dsd_ild":
-        return np.ascontiguousarray(sep.separate_stereo(sub).transpose(1, 2, 0))     # [L, nsrc, 2] -> [nsrc, 2, L]
-    return sep.separate(sub)
+    from .engine import clip_call
+    return _sample_axis(sep, clip_call(sep, filt, melody, frame0)(sub), last=True)
 
 
 def _slice_filters(filters, sg, hop):
@@ -124,7 +129,12 @@ def _slice_filters(filters, sg, hop):
     return f
 
 
-def _check_score_inputs(filters, melody):
+def _check_inputs(seps, filters, melody):
+    """The refusals made before any segment runs -> the note table as the library takes it, or None."""
+    for sep in seps:
+        if hasattr(sep, "model") and sep.model.arch == "bach10_score_1x1":
+            raise ValueError("long clips are not built for the score-informed build_ca_1x1 network (bach10_score_1x1): "
+                             "its segments have never been checked against the whole clip; separate the whole clip")
     if filters is not None and melody is not None:
         raise ValueError("pass the score as filters= or as melody=, not both")
     if melody is not None:
@@ -142,7 +152,7 @@ def separate_long(separators, audio, parts=None, filters=None, geometry=None, me
     (score.score_melody), which each segment rasterises on the device from its first frame on.  geometry=(frame_size, hop, time_context, overlap) is needed only when the
     separators are plain callables (tests)."""
     seps = list(separators) if isinstance(separators, (list, tuple)) else [separators]
-    melody = _check_score_inputs(filters, melody)
+    melody = _check_inputs(seps, filters, melody)
     N, H, tc, ov = geometry if geometry is not None else _geometry(seps[0])
     a = np.asarray(audio)
     L = a.shape[0]
@@ -169,10 +179,7 @@ def separate_long(separators, audio, parts=None, filters=None, geometry=None, me
             t.join()
     if errors:
         raise errors[0]
-    out = stitch(segs, pieces, L, dtype=pieces[0].dtype)
-    if hasattr(seps[0], "model") and seps[0].model.arch == "dsd_ild":
-        out = np.ascontiguousarray(out.transpose(2, 0, 1))
-    return out
+    return _sample_axis(seps[0], stitch(segs, pieces, L, dtype=pieces[0].dtype), last=False)
 
 
 def separate_long_distributed(separator, audio, filters=None, geometry=None, group=None, melody=None):
@@ -181,7 +188,7 @@ def separate_long_distributed(separator, audio, filters=None, geometry=None, gro
     the path's only exchange, off the data path) which returns the stitched stems; other ranks return None."""
     import torch.distributed as dist
     from .sharding import gather_stems
-    melody = _check_score_inputs(filters, melody)
+    melody = _check_inputs([separator], filters, melody)
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     N, H, tc, ov = geometry if geometry is not None else _geometry(separator)
     a = np.asarray(audio)
@@ -200,6 +207,4 @@ def separate_long_distributed(separator, audio, filters=None, geometry=None, gro
     out = np.zeros(first.shape[:-1] + (L,), dtype=first.dtype)
     for i, sg in enumerate(segs):
         out[..., sg.out_start:sg.out_stop] = kept[i]
-    if hasattr(separator, "model") and separator.model.arch == "dsd_ild":
-        out = np.ascontiguousarray(out.transpose(2, 0, 1))
-    return out
+    return _sample_axis(separator, out, last=False)

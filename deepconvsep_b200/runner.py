@@ -15,7 +15,7 @@ import os
 import numpy as np
 
 from . import util
-from .engine import Separator
+from .engine import Separator, check_stereo_options
 from .models import load_model, FAMILY_DEFAULTS
 from .score import score_melody
 from .sharding import shard_clips, reduce_stats
@@ -114,6 +114,13 @@ def read_piece(piece):
     return audio, sampleRate, bitrate
 
 
+def _write_stems(paths, stems, sampleRate, bitrate):
+    """stems[i] (float [nsamples] or [nsamples, 2]) -> the wav paths[i] at the input's bit depth."""
+    for path, stem in zip(paths, stems):
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        util.writeAudioScipy(path, stem.astype(np.float64), sampleRate, bitrate)
+
+
 def separate_dataset(family, testdir, outdir, model, scale_factor=None, time_context=30, rank=0, world_size=1, device=0,
                      keep_channels=False, wiener=0, **overrides):
     """scale_factor: None = the family's trainer value (0.2 for bach10_score, else 0.3).
@@ -124,12 +131,7 @@ def separate_dataset(family, testdir, outdir, model, scale_factor=None, time_con
     channel of the mixture (Separator.separate_keep_channels), so that a multichannel evaluation scores real stereo
     images.  wiener (family dsd with keep_channels, or dsd_ild): that many EM iterations of the multichannel Wiener
     post-filter on the stereo stems."""
-    if keep_channels and family != "dsd":
-        raise ValueError("--keep-channels is for --family dsd (the stereo / ILD net, dsd_ild, is stereo already)")
-    if wiener < 0:
-        raise ValueError("--wiener %d: the number of EM iterations cannot be negative" % wiener)
-    if wiener and not (keep_channels or family == "dsd_ild"):
-        raise ValueError("--wiener needs stereo stems: --family dsd --keep-channels, or --family dsd_ild")
+    check_stereo_options(family, keep_channels, wiener)
     wkw = {"wiener": wiener} if wiener else {}
     cfg = dict(TRAINER[family], **overrides)
     if scale_factor is None:
@@ -153,33 +155,19 @@ def separate_dataset(family, testdir, outdir, model, scale_factor=None, time_con
             melody = score_melody(wav, SCORE_MIDI, nframes, frameSize=cfg["frameSize"], hopSize=cfg["hopSize"],
                                   sampleRate=sampleRate)
             stems = sep.separate_notes(audio, melody)
-            for i, path in enumerate(outs):
-                os.makedirs(os.path.dirname(path), exist_ok=True)
-                util.writeAudioScipy(path, stems[i].astype(np.float64), sampleRate, bitrate)
-            seconds += len(audio) / float(sampleRate)
-            continue
-        audioObj, sampleRate, bitrate = util.readAudioScipy(wav)
-        assert sampleRate == 44100, "Sample rate needs to be 44100"
-        if family == "dsd_ild" or keep_channels:             # both channels in, stereo stems out
-            assert audioObj.ndim == 2 and audioObj.shape[1] == 2, "%s needs 2-channel mixtures" % (
-                "--keep-channels" if keep_channels else "the stereo / ILD network")
-            # [nsamples, nsrc, 2]
-            sep_audio = sep.separate_keep_channels(audioObj, **wkw) if keep_channels else sep.separate_stereo(audioObj, **wkw)
-            for i, path in enumerate(outs):
-                os.makedirs(os.path.dirname(path), exist_ok=True)
-                util.writeAudioScipy(path, sep_audio[:, i, :].astype(np.float64), sampleRate, bitrate)
-            seconds += audioObj.shape[0] / float(sampleRate)
-            continue
-        if audioObj.ndim == 1:
-            audio = audioObj
-        elif family == "ikala":
-            audio = audioObj[:, 0] + audioObj[:, 1]          # ikala/trainCNN.py:255
         else:
-            audio = (audioObj[:, 0] + audioObj[:, 1]) / 2    # dsd100/trainCNN.py:304
-        stems = sep.separate(audio)
-        for i, path in enumerate(outs):
-            os.makedirs(os.path.dirname(path), exist_ok=True)
-            util.writeAudioScipy(path, stems[i].astype(np.float64), sampleRate, bitrate)
+            audio, sampleRate, bitrate = util.readAudioScipy(wav)
+            assert sampleRate == 44100, "Sample rate needs to be 44100"
+            if family == "dsd_ild" or keep_channels:             # both channels in, stereo stems out
+                assert audio.ndim == 2 and audio.shape[1] == 2, "%s needs 2-channel mixtures" % (
+                    "--keep-channels" if keep_channels else "the stereo / ILD network")
+                stereo = sep.separate_keep_channels(audio, **wkw) if keep_channels else sep.separate_stereo(audio, **wkw)
+                stems = stereo.transpose(1, 0, 2)                  # [nsamples, nsrc, 2] -> [nsrc, nsamples, 2]
+            else:
+                if audio.ndim > 1:                                  # ikala/trainCNN.py:255, dsd100/trainCNN.py:304
+                    audio = audio[:, 0] + audio[:, 1] if family == "ikala" else (audio[:, 0] + audio[:, 1]) / 2
+                stems = sep.separate(audio)
+        _write_stems(outs, stems, sampleRate, bitrate)
         seconds += len(audio) / float(sampleRate)
     return seconds, len(jobs)
 
@@ -198,12 +186,10 @@ def main(argv=None):
                     help="K EM iterations of the multichannel Wiener post-filter on the stereo stems "
                          "(--family dsd --keep-channels, or --family dsd_ild)")
     args = ap.parse_args(argv)
-    if args.keep_channels and args.family != "dsd":
-        ap.error("--keep-channels is for --family dsd")
-    if args.wiener < 0:
-        ap.error("--wiener cannot be negative")
-    if args.wiener and not (args.keep_channels or args.family == "dsd_ild"):
-        ap.error("--wiener needs stereo stems: --family dsd --keep-channels, or --family dsd_ild")
+    try:
+        check_stereo_options(args.family, args.keep_channels, args.wiener)
+    except ValueError as e:
+        ap.error(str(e))
     world, rank, local = (int(os.environ.get(k, d)) for k, d in (("WORLD_SIZE", "1"), ("RANK", "0"), ("LOCAL_RANK", "0")))
     if world > 1:
         import torch

@@ -168,6 +168,35 @@ def test_cli_splits_one_recording_over_the_listed_devices(tmp_path, monkeypatch)
         assert sr == 44100 and np.array_equal(got, want)
 
 
+def test_the_1x1_score_net_is_refused_before_any_segment_runs():
+    """long clips are not built for the score-informed build_ca_1x1 network: with either kind of score, on one host or
+    over ranks, a separator of that network is refused before any segment is separated"""
+    from types import SimpleNamespace
+    picked = []
+
+    class FakeSeparator(object):
+        def __init__(self):
+            self.model = SimpleNamespace(arch="bach10_score_1x1", tc=30)
+            self.frame_size, self.hop, self.overlap = 4096, 512, 25
+
+        def separate_score(self, sub, filters):
+            picked.append("score")
+            return np.zeros((4, len(sub)), dtype=np.float32)
+
+        def separate_notes(self, sub, melody, frame0=0):
+            picked.append("notes")
+            return np.zeros((4, len(sub)), dtype=np.float32)
+
+    L = 44100 * 20
+    T = -(-L // 512) + 2
+    for score in ({"filters": np.zeros((4, T, 2049), dtype=np.float32)}, {"melody": np.zeros((4, 1, 43))}):
+        with pytest.raises(ValueError, match="build_ca_1x1"):
+            longclip.separate_long([FakeSeparator(), FakeSeparator()], np.zeros(L), parts=2, **score)
+        with pytest.raises(ValueError, match="build_ca_1x1"):
+            longclip.separate_long_distributed(FakeSeparator(), np.zeros(L), **score)
+    assert picked == []
+
+
 def _toy_engine(N, H, tc, ov, patcher):
     """The pipeline's time structure with a toy network: every output frame of a patch depends on ALL frames of the
     patch (so one contaminated frame spoils the whole patch), two sources, the real patchers / cross-fade / STFTs."""
