@@ -51,6 +51,7 @@ _SIGS = {
     "dcs_separate_audio_stereo": (C.c_int, [_p, _p, _p, _p, _i64, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
     "dcs_xcorr_lags": (C.c_int, [_p, _p, _p, C.c_int, _i64, C.c_int, _p, _p]),
     "dcs_gemm_f32": (C.c_int, [_p, C.c_int, _p, _i64, _p, _i64, _p, _p, _i64, C.c_int, C.c_int, C.c_int, C.c_int, _p]),
+    "dcs_gemm_view_f32": (C.c_int, [_p, C.c_int, C.c_int, _p, _p, _p]),
     "dcs_separate_audio": (C.c_int, [_p, _p, _p, _p, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
     "dcs_separate_host": (C.c_int, [_p, _p, _p, _p, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
     "dcs_separate_batch_pcm16_host": (C.c_int, [_p, _p, _p, C.c_int, _p, _p, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _p, _p, _p]),
@@ -60,6 +61,27 @@ _SIGS = {
     "dcs_separate_batch_pcm16_keep_channels_host": (C.c_int, [_p, _p, _p, C.c_int, _p, _p, C.c_float, C.c_int, C.c_int,
                                                               _p, _p, _p]),
 }
+
+
+
+class GemmView(C.Structure):
+    """dcs_gemm_view (include/dcs.h): the operand view of dcs_gemm_view_f32, field for field."""
+    _fields_ = [("A", _p), ("B", _p), ("bias", _p), ("C", _p),
+                ("M", C.c_int), ("N", C.c_int), ("K", C.c_int),
+                ("a_valid_rows", C.c_int),
+                ("m_inner", C.c_int), ("a_so", _i64), ("a_si", _i64),
+                ("m_inner2", C.c_int), ("a_s2", _i64),
+                ("k_seg", C.c_int), ("k_ss", _i64),
+                ("ldb", _i64),
+                ("cm_inner", C.c_int), ("c_so", _i64), ("c_si", _i64),
+                ("cm_inner2", C.c_int), ("c_s2", _i64),
+                ("n_seg", C.c_int), ("n_ss", _i64), ("c_col0", _i64),
+                ("relu", C.c_int),
+                ("kc_rows", C.c_int), ("kc_unit", C.c_int), ("kc_pad", C.c_int), ("kc_n", C.c_int), ("kc_taps", C.c_int),
+                ("bias2", _p), ("code", _p),
+                ("gate", _p), ("g_inner", C.c_int), ("g_inner2", C.c_int),
+                ("g_so", _i64), ("g_si", _i64), ("g_s2", _i64), ("g_lim", _i64)]
+
 
 _lib = None
 

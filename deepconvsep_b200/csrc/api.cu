@@ -660,42 +660,63 @@ int dcs_separate_audio_notes(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const floa
                        st);
 }
 
-int dcs_gemm_f32(dcs_ctx* ctx, int engine, const float* d_A, int64_t lda, const float* h_B, int64_t ldb,
-                 const float* h_bias, float* d_C, int64_t ldc, int M, int N, int K, int relu, void* stream) {
-  DCS_REQUIRE(ctx && d_A && h_B && d_C && M > 0 && N > 0 && K > 0, "dcs_gemm_f32: bad argument");
-  DCS_REQUIRE(lda >= 1 && ldb >= N && ldc >= N, "dcs_gemm_f32: leading dimension too small");  // lda < K: overlapping rows
-  cudaStream_t st = (cudaStream_t)stream;
-  DCS_CUDA(cudaSetDevice(ctx->device));
-  float* d_bias = nullptr;
+// one GEMM on view g with the host weight h_B[K][g.ldb]: uploaded for the FFMA kernel (engine 0) or transposed and
+// split for the tensor cores (engine 1, with the epilogue epi); the stream is synchronised before the weight is freed
+static int gemm_host_weight(const char* fn, dcs_ctx* ctx, int engine, int epi, GemmDesc g, const float* h_B, cudaStream_t st) {
   float* d_B = nullptr;
   TcWeight w;
-  int r = DCS_OK;
-  if (h_bias) {
-    std::vector<float> hb(h_bias, h_bias + N);
-    r = upload(hb, &d_bias);
-  }
-  GemmDesc g = gemm_plain(d_A, lda, nullptr, N, d_bias, d_C, ldc, M, N, K, relu);
-  if (r == DCS_OK) {
-    if (engine == 1) {
-      r = tc_weight_create(h_B, ldb, K, N, &w);
-      if (r == DCS_OK) r = launch_gemm_tc(ctx, g, w, st);
-    } else {
-      std::vector<float> hB((size_t)K * N);
-      for (int k = 0; k < K; ++k) memcpy(&hB[(size_t)k * N], h_B + (size_t)k * ldb, (size_t)N * sizeof(float));
-      r = upload(hB, &d_B);
-      g.B = d_B;
-      if (r == DCS_OK) r = launch_gemm(ctx, g, st);
-    }
+  int r;
+  if (engine == 1) {
+    r = tc_weight_create(h_B, g.ldb, g.K, g.N, &w);
+    if (r == DCS_OK) r = epi ? launch_gemm_tc_epi(ctx, g, w, epi, st) : launch_gemm_tc(ctx, g, w, st);
+  } else {
+    std::vector<float> hB((size_t)g.K * g.N);
+    for (int k = 0; k < g.K; ++k) memcpy(&hB[(size_t)k * g.N], h_B + (size_t)k * g.ldb, (size_t)g.N * sizeof(float));
+    r = upload(hB, &d_B);
+    g.B = d_B; g.ldb = g.N;
+    if (r == DCS_OK) r = launch_gemm(ctx, g, st);
   }
   cudaError_t e = cudaStreamSynchronize(st);
   tc_weight_destroy(&w);
   if (d_B) cudaFree(d_B);
-  if (d_bias) cudaFree(d_bias);
   if (r == DCS_OK && e != cudaSuccess) {
-    set_error("dcs_gemm_f32: %s", cudaGetErrorString(e));
+    set_error("%s: %s", fn, cudaGetErrorString(e));
     return DCS_ECUDA;
   }
   return r;
+}
+
+int dcs_gemm_f32(dcs_ctx* ctx, int engine, const float* d_A, int64_t lda, const float* h_B, int64_t ldb,
+                 const float* h_bias, float* d_C, int64_t ldc, int M, int N, int K, int relu, void* stream) {
+  DCS_REQUIRE(ctx && d_A && h_B && d_C && M > 0 && N > 0 && K > 0, "dcs_gemm_f32: bad argument");
+  DCS_REQUIRE(lda >= 1 && ldb >= N && ldc >= N, "dcs_gemm_f32: leading dimension too small");  // lda < K: overlapping rows
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  float* d_bias = nullptr;
+  if (h_bias) DCS_TRY(upload(std::vector<float>(h_bias, h_bias + N), &d_bias));
+  const GemmDesc g = gemm_plain(d_A, lda, nullptr, ldb, d_bias, d_C, ldc, M, N, K, relu);
+  const int r = gemm_host_weight("dcs_gemm_f32", ctx, engine, 0, g, h_B, (cudaStream_t)stream);
+  if (d_bias) cudaFree(d_bias);
+  return r;
+}
+
+static_assert(sizeof(dcs_gemm_view) == sizeof(GemmDesc) && offsetof(dcs_gemm_view, ldb) == offsetof(GemmDesc, ldb) &&
+                  offsetof(dcs_gemm_view, kc_rows) == offsetof(GemmDesc, kc_rows) &&
+                  offsetof(dcs_gemm_view, g_lim) == offsetof(GemmDesc, g_lim),
+              "dcs_gemm_view must mirror GemmDesc");
+
+int dcs_gemm_view_f32(dcs_ctx* ctx, int engine, int epi, const dcs_gemm_view* view, const float* h_B, void* stream) {
+  DCS_REQUIRE(ctx && view && h_B && view->A && view->C, "dcs_gemm_view_f32: NULL argument");
+  DCS_REQUIRE(engine == 0 || engine == 1, "dcs_gemm_view_f32: unknown engine %d", engine);
+  DCS_REQUIRE(epi >= 0 && epi <= (EPI_POST | EPI_GATE) && (epi == 0 || engine == 1),
+              "dcs_gemm_view_f32: epilogue %d needs engine 1", epi);
+  GemmDesc g;
+  memcpy(&g, view, sizeof g);
+  DCS_REQUIRE(g.M > 0 && g.N > 0 && g.K > 0 && g.ldb >= g.N, "dcs_gemm_view_f32: bad shape");
+  DCS_REQUIRE(g.m_inner > 0 && g.m_inner2 > 0 && g.k_seg > 0 && g.cm_inner > 0 && g.cm_inner2 > 0 && g.n_seg > 0 &&
+                  (g.kc_rows == 0 || (g.kc_rows > 0 && g.kc_unit > 0 && g.kc_taps > 0)),
+              "dcs_gemm_view_f32: bad view");
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  return gemm_host_weight("dcs_gemm_view_f32", ctx, engine, epi, g, h_B, (cudaStream_t)stream);
 }
 
 int dcs_separate_audio_stereo(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,

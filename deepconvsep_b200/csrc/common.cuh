@@ -233,7 +233,12 @@ struct GemmDesc {
   const float* bias2; uint8_t* code;
   const uint8_t* gate; int g_inner, g_inner2; int64_t g_so, g_si, g_s2, g_lim;
 };
-enum { EPI_POST = 1, EPI_GATE = 2 };
+enum { EPI_POST = DCS_GEMM_EPI_POST, EPI_GATE = DCS_GEMM_EPI_GATE };
+// every C offset of the view is >= 0: the epilogues store without a lower bound check.  All layers build their views
+// from non-negative strides; each launcher refuses a view that breaks this.
+inline bool gemm_c_view_ok(const GemmDesc& d) {
+  return d.c_so >= 0 && d.c_si >= 0 && d.c_s2 >= 0 && d.n_ss >= 0 && d.c_col0 >= 0;
+}
 // element offset of row m of C (without the column part)
 __host__ __device__ __forceinline__ int64_t gemm_c_row_offset(const GemmDesc& d, int m) {
   return (int64_t)(m / d.cm_inner) * d.c_so + (int64_t)((m % d.cm_inner) / d.cm_inner2) * d.c_si +

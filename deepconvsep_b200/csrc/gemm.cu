@@ -85,7 +85,6 @@ gemm_f32_kernel(const GemmDesc d) {
     const int m = m0 + ty * TM + i;
     if (m >= d.M) continue;
     const int64_t roff = gemm_c_row_offset(d, m);
-    if (roff < 0) continue;
 #pragma unroll
     for (int j = 0; j < TN; ++j) {
       const int n = n0 + tx * TN + j;
@@ -117,6 +116,7 @@ GemmDesc gemm_plain(const float* A, int64_t lda, const float* B, int64_t ldb, co
 int launch_gemm(dcs_ctx* ctx, const GemmDesc& d, cudaStream_t st) {
   if (d.M <= 0 || d.N <= 0) return DCS_OK;
   DCS_REQUIRE(d.K > 0 && d.m_inner > 0 && d.m_inner2 > 0 && d.k_seg > 0 && d.cm_inner > 0 && d.cm_inner2 > 0 && d.n_seg > 0, "bad GEMM descriptor");
+  DCS_REQUIRE(gemm_c_view_ok(d), "GEMM: negative C stride or column offset");
   dim3 grid((unsigned)ceil_div64(d.N, BN), (unsigned)ceil_div64(d.M, BM));
   DCS_REQUIRE(grid.y <= 65535u * 16u, "GEMM M=%d too large", d.M);
   if (grid.y > 65535u) {

@@ -348,6 +348,7 @@ int launch_gemm_tc(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStrea
   if (d.M <= 0 || d.N <= 0) return DCS_OK;
   DCS_REQUIRE(d.K == w.K && d.N == w.N, "tc gemm: weight is %dx%d, GEMM wants K=%d N=%d", w.K, w.N, d.K, d.N);
   DCS_REQUIRE(ceil_div64(d.N, 64) <= 65535, "tc gemm: N=%d too large", d.N);
+  DCS_REQUIRE(gemm_c_view_ok(d), "tc gemm: negative C stride or column offset");
   const int avec = a_vector_width(d);
   if (d.N <= 32) {   // the 30-channel convolutions of the iKala / Bach10 nets: half the weight traffic and MMA time
     if (avec == 4) return launch_tc<32, 4, 4>(ctx, d, w, st);
@@ -363,6 +364,7 @@ int launch_gemm_tc_epi(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, int e
   if (d.M <= 0 || d.N <= 0) return DCS_OK;
   DCS_REQUIRE(d.K == w.K && d.N == w.N, "tc gemm: weight is %dx%d, GEMM wants K=%d N=%d", w.K, w.N, d.K, d.N);
   DCS_REQUIRE(ceil_div64(d.N, 64) <= 65535, "tc gemm: N=%d too large", d.N);
+  DCS_REQUIRE(gemm_c_view_ok(d), "tc gemm: negative C stride or column offset");
   DCS_REQUIRE(!(epi & EPI_POST) || (d.bias && d.bias2), "tc gemm: EPI_POST needs both biases");
   DCS_REQUIRE(!(epi & EPI_GATE) || (d.gate && d.g_inner > 0 && d.g_inner2 > 0), "tc gemm: EPI_GATE needs a gate view");
   // float4 operand loads only: the gated layers lay their activations out for it (the scalar-load variant spills)

@@ -213,6 +213,43 @@ int dcs_separate_audio_notes(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, con
 int dcs_gemm_f32(dcs_ctx* ctx, int engine, const float* d_A, int64_t lda, const float* h_B, int64_t ldb,
                  const float* h_bias, float* d_C, int64_t ldc, int M, int N, int K, int relu, void* stream);
 
+/* Bring-up and test entry: the same GEMM on an arbitrary operand view -- the descriptor through which every layer of
+ * every network reaches the kernels, field for field.  Its layout follows DCS_VERSION and may change with it.
+ *   A row m      = (m / m_inner) * a_so + ((m % m_inner) / m_inner2) * a_si + (m % m_inner2) * a_s2; rows
+ *                  >= a_valid_rows read as zeros
+ *   A column k   = (k / k_seg) * k_ss + (k % k_seg)
+ *   C row m      = the same three-level form with cm_inner, c_so, c_si, cm_inner2, c_s2; every stride and c_col0
+ *                  must be >= 0
+ *   C column n   = c_col0 + (n / n_seg) * n_ss + (n % n_seg)
+ *   kc_*         K clipping of a transposed convolution on a zero-padded A (kc_rows = 0: off): rows are grouped by
+ *                  u = m / kc_rows, and K block kc_unit * q (tap q) is skipped where kc_pad <= u + q < kc_pad + kc_n
+ *                  fails.  The skipped products must be zeros of A.
+ *   epi          0: C = act(A B + bias), relu selects the ReLU;  DCS_GEMM_EPI_POST: x = relu(AB + bias) + bias2 and,
+ *                  with `code`, code[m * N + n] = 2 relu'(AB + bias) in {0, 1 (exactly 0), 2};  DCS_GEMM_EPI_GATE:
+ *                  x *= 0.5 * gate[(m / g_inner) * g_so + ((m % g_inner) / g_inner2) * g_si + (m % g_inner2) * g_s2 + n],
+ *                  and nothing is stored where (m % g_inner2) * g_s2 + n >= g_lim.
+ * Pointers are device memory except `B`, which is ignored: the weight is the HOST array h_B[K][ldb], uploaded (engine 0,
+ * the FFMA kernel) or transposed and split for the tensor cores (engine 1) on every call.  The epilogues need engine
+ * 1 and a 16-byte aligned A view.  Synchronises the stream before returning. */
+typedef struct {
+  const float* A; const float* B; const float* bias; float* C;
+  int M, N, K;
+  int a_valid_rows;
+  int m_inner; int64_t a_so, a_si;
+  int m_inner2; int64_t a_s2;
+  int k_seg; int64_t k_ss;
+  int64_t ldb;
+  int cm_inner; int64_t c_so, c_si;
+  int cm_inner2; int64_t c_s2;
+  int n_seg; int64_t n_ss, c_col0;
+  int relu;
+  int kc_rows, kc_unit, kc_pad, kc_n, kc_taps;
+  const float* bias2; uint8_t* code;
+  const uint8_t* gate; int g_inner, g_inner2; int64_t g_so, g_si, g_s2, g_lim;
+} dcs_gemm_view;
+enum { DCS_GEMM_EPI_POST = 1, DCS_GEMM_EPI_GATE = 2 };
+int dcs_gemm_view_f32(dcs_ctx* ctx, int engine, int epi, const dcs_gemm_view* view, const float* h_B, void* stream);
+
 /* ---- stereo / ILD variant (examples/dsd100_2ch_ILD/trainCNN_ILD_DSD100.py:299-327) ------------ */
 /* d_audio float[2][audio_stride] (left, right; first num_samples valid) ->
  * d_stems float[nsrc*2][stem_stride], plane (s*2 + j) = source s, channel j (`sep_audio[:, s, j]`).
