@@ -52,6 +52,8 @@ _SIGS = {
     "dcs_xcorr_lags": (C.c_int, [_p, _p, _p, C.c_int, _i64, C.c_int, _p, _p]),
     "dcs_gemm_f32": (C.c_int, [_p, C.c_int, _p, _i64, _p, _i64, _p, _p, _i64, C.c_int, C.c_int, C.c_int, C.c_int, _p]),
     "dcs_gemm_view_f32": (C.c_int, [_p, C.c_int, C.c_int, _p, _p, _p]),
+    "dcs_dsd_mask_f32": (C.c_int, [_p, C.c_int, _p, _p]),
+    "dcs_sconv_mask_f32": (C.c_int, [_p, C.c_int, _p, _p]),
     "dcs_separate_audio": (C.c_int, [_p, _p, _p, _p, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
     "dcs_separate_host": (C.c_int, [_p, _p, _p, _p, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
     "dcs_separate_batch_pcm16_host": (C.c_int, [_p, _p, _p, C.c_int, _p, _p, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, _p, _p, _p]),
@@ -81,6 +83,22 @@ class GemmView(C.Structure):
                 ("bias2", _p), ("code", _p),
                 ("gate", _p), ("g_inner", C.c_int), ("g_inner2", C.c_int),
                 ("g_so", _i64), ("g_si", _i64), ("g_s2", _i64), ("g_lim", _i64)]
+
+
+class DsdMaskView(C.Structure):
+    """dcs_dsd_mask_view (include/dcs.h): the arguments of dcs_dsd_mask_f32, field for field."""
+    _fields_ = [("G", _p), ("ldg", C.c_int), ("W1t", _p), ("ldw", C.c_int), ("bout", _p), ("X", _p), ("S", _p),
+                ("ldf", _i64), ("src_stride", _i64),
+                ("T", C.c_int), ("P", C.c_int), ("tc", C.c_int), ("overlap", C.c_int), ("F", C.c_int),
+                ("ndec", C.c_int), ("nx", C.c_int), ("x_plane", _i64)]
+
+
+class SconvMaskView(C.Structure):
+    """dcs_sconv_mask_view (include/dcs.h): the arguments of dcs_sconv_mask_f32, field for field."""
+    _fields_ = [("arch", C.c_int), ("G", _p), ("tie", _p), ("W", _p), ("bout", _p), ("X", _p), ("S", _p),
+                ("ldf", _i64), ("src_stride", _i64),
+                ("T", C.c_int), ("P", C.c_int), ("tc", C.c_int), ("overlap", C.c_int), ("F", C.c_int), ("J", C.c_int),
+                ("WP", C.c_int), ("p_base", C.c_int), ("t0", C.c_int), ("t1", C.c_int)]
 
 
 _lib = None

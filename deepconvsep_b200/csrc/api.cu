@@ -719,6 +719,84 @@ int dcs_gemm_view_f32(dcs_ctx* ctx, int engine, int epi, const dcs_gemm_view* vi
   return gemm_host_weight("dcs_gemm_view_f32", ctx, engine, epi, g, h_B, (cudaStream_t)stream);
 }
 
+static_assert(sizeof(dcs_dsd_mask_view) == sizeof(DsdMaskArgs) && offsetof(dcs_dsd_mask_view, ldw) == offsetof(DsdMaskArgs, ldw) &&
+                  offsetof(dcs_dsd_mask_view, X) == offsetof(DsdMaskArgs, X) &&
+                  offsetof(dcs_dsd_mask_view, src_stride) == offsetof(DsdMaskArgs, src_stride) &&
+                  offsetof(dcs_dsd_mask_view, F) == offsetof(DsdMaskArgs, F) && offsetof(dcs_dsd_mask_view, nx) == offsetof(DsdMaskArgs, nx) &&
+                  offsetof(dcs_dsd_mask_view, x_plane) == offsetof(DsdMaskArgs, x_plane),
+              "dcs_dsd_mask_view must mirror DsdMaskArgs");
+static_assert(sizeof(dcs_sconv_mask_view) == sizeof(SconvMaskArgs) && offsetof(dcs_sconv_mask_view, G) == offsetof(SconvMaskArgs, G) &&
+                  offsetof(dcs_sconv_mask_view, S) == offsetof(SconvMaskArgs, S) &&
+                  offsetof(dcs_sconv_mask_view, src_stride) == offsetof(SconvMaskArgs, src_stride) &&
+                  offsetof(dcs_sconv_mask_view, WP) == offsetof(SconvMaskArgs, WP) &&
+                  offsetof(dcs_sconv_mask_view, t1) == offsetof(SconvMaskArgs, t1),
+              "dcs_sconv_mask_view must mirror SconvMaskArgs");
+
+// one mask launch, then the stream is synchronised
+static int sync_after(const char* fn, int r, cudaStream_t st) {
+  const cudaError_t e = cudaStreamSynchronize(st);
+  if (r == DCS_OK && e != cudaSuccess) {
+    set_error("%s: %s", fn, cudaGetErrorString(e));
+    return DCS_ECUDA;
+  }
+  return r;
+}
+
+int dcs_dsd_mask_f32(dcs_ctx* ctx, int engine, const dcs_dsd_mask_view* view, void* stream) {
+  DCS_REQUIRE(ctx && view && view->G && view->W1t && view->bout && view->X && view->S, "dcs_dsd_mask_f32: NULL argument");
+  DCS_REQUIRE(engine == 0 || engine == 1, "dcs_dsd_mask_f32: unknown engine %d", engine);
+  DsdMaskArgs a;
+  memcpy(&a, view, sizeof a);
+  const int64_t plane = (int64_t)a.T * a.ldf;
+  DCS_REQUIRE(a.T > 0 && a.P > 0 && a.tc > a.overlap && a.overlap >= 0 && a.F >= 2 && a.ldf >= a.F && a.ldw >= a.F && a.ldg >= 50,
+              "dcs_dsd_mask_f32: bad shape");
+  DCS_REQUIRE((a.ndec == 3 || a.ndec == 4) && (a.nx == 1 || (a.nx == 2 && a.ndec == 3)),
+              "dcs_dsd_mask_f32: ndec %d with nx %d (nx = 2 needs ndec = 3)", a.ndec, a.nx);
+  DCS_REQUIRE(a.src_stride >= plane && (a.nx == 1 || a.x_plane >= plane), "dcs_dsd_mask_f32: planes overlap");
+  DCS_REQUIRE((uintptr_t)a.X % 8 == 0 && (uintptr_t)a.S % 8 == 0, "dcs_dsd_mask_f32: misaligned X or S");
+  DCS_REQUIRE(engine == 1 || a.nx == 1, "dcs_dsd_mask_f32: engine 0 applies the masks to one channel per call (nx = 1)");
+  DCS_REQUIRE(engine == 0 || dsd_mask_tc_supported(a),
+              "dcs_dsd_mask_f32: engine 1 takes at most 6 patches per frame, ldg >= 52 with ldg %% 4 == 0 and a 16-byte aligned G");
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  return sync_after("dcs_dsd_mask_f32", engine == 1 ? launch_dsd_mask_tc(ctx, a, st) : launch_dsd_mask(ctx, a, st), st);
+}
+
+int dcs_sconv_mask_f32(dcs_ctx* ctx, int engine, const dcs_sconv_mask_view* view, void* stream) {
+  DCS_REQUIRE(ctx && view && view->G && view->W && view->bout && view->X && view->S, "dcs_sconv_mask_f32: NULL argument");
+  DCS_REQUIRE(engine == 0 || engine == 1, "dcs_sconv_mask_f32: unknown engine %d", engine);
+  SconvMaskArgs a;
+  memcpy(&a, view, sizeof a);
+  int KW, stride;
+  switch (a.arch) {
+    case DCS_ARCH_BACH10:
+    case DCS_ARCH_BACH10_SCORE: KW = 30; stride = 4; break;
+    case DCS_ARCH_BACH10_SCORE_1X1: KW = 5; stride = 2; break;
+    case DCS_ARCH_IKALA:
+    case DCS_ARCH_IKALA_NOPOOL: KW = 30; stride = 3; break;
+    default: DCS_REQUIRE(false, "dcs_sconv_mask_f32: architecture %d has no strided conv1", a.arch);
+  }
+  const bool pooled = a.arch == DCS_ARCH_IKALA, chunked = a.arch == DCS_ARCH_BACH10_SCORE_1X1;
+  const int step = a.tc - a.overlap;
+  DCS_REQUIRE(a.T > 0 && a.P > 0 && step > 0 && a.overlap >= 0 && a.F >= KW && a.ldf >= a.F && a.src_stride >= (int64_t)a.T * a.ldf,
+              "dcs_sconv_mask_f32: bad shape");
+  DCS_REQUIRE(a.J == (a.F - KW) / stride + 1 && a.WP == (pooled ? a.J / 4 : a.J), "dcs_sconv_mask_f32: J %d / WP %d do not match F %d",
+              a.J, a.WP, a.F);
+  DCS_REQUIRE(pooled == (a.tie != nullptr), "dcs_sconv_mask_f32: tie bits go with the max-pool net only");
+  DCS_REQUIRE(0 <= a.t0 && a.t0 < a.t1 && a.t1 <= a.T && a.p_base >= 0 && (chunked || (a.p_base == 0 && a.t0 == 0 && a.t1 == a.T)),
+              "dcs_sconv_mask_f32: frames [%d, %d) from patch %d", a.t0, a.t1, a.p_base);
+  // the first patch covering frame t0 must be in G
+  DCS_REQUIRE(a.t0 - a.tc + 1 <= 0 || (a.t0 - a.tc + 1 + step - 1) / step >= a.p_base, "dcs_sconv_mask_f32: G starts after frame %d's patches",
+              a.t0);
+  DCS_REQUIRE(engine == 0 || ((uintptr_t)a.tie % 4 == 0 && sconv_mask_tc_supported(a)),
+              "dcs_sconv_mask_f32: engine 1 needs a 16-byte aligned G and a 4-byte aligned tie");
+  DCS_REQUIRE(engine == 1 || (a.tc + step - 1) / step <= 64, "dcs_sconv_mask_f32: engine 0 takes at most 64 patches per frame");
+  DCS_REQUIRE((uintptr_t)a.W % 16 == 0 && (uintptr_t)a.X % 8 == 0 && (uintptr_t)a.S % 8 == 0, "dcs_sconv_mask_f32: misaligned W, X or S");
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  return sync_after("dcs_sconv_mask_f32", engine == 1 ? launch_sconv_mask_tc(ctx, a, st) : launch_sconv_mask(ctx, a, st), st);
+}
+
 int dcs_separate_audio_stereo(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,
                               float scale_factor, int overlap, int patcher, float* d_stems, int64_t stem_stride, void* stream) {
   DCS_TRY(check_clip("dcs_separate_audio_stereo", ctx, m, p, DCS_ARCH_DSD_ILD, d_audio, d_stems, L, audio_stride, stem_stride,

@@ -270,6 +270,9 @@ struct DsdMaskArgs {
                        //    downmix's masks; tensor-core kernel only)
   int64_t x_plane;
 };
+// every mask kernel takes a total of the rectified sources at or below this as "all sources zero" (the rule's 1/nsrc or
+// 0): the reciprocal of a subnormal total overflows, and the masks would be inf * 0 = NaN.  dsd_tc.cu tests the same value.
+constexpr float MASK_TOT_MIN = 1.2e-38f;
 int launch_dsd_mask(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st);
 bool dsd_mask_tc_supported(const DsdMaskArgs& a);
 int launch_dsd_mask_tc(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st);   // wgmma (dsd_tc.cu)

@@ -33,9 +33,9 @@ dsd_mask_kernel(const DsdMaskArgs a, int frames_per_cta) {
   const int tid = threadIdx.x;
   int b = -1;
   if (tid < MASK_TILE) {
-    const int bb = blockIdx.x * MASK_TILE + tid;
+    const int bb = blockIdx.y * MASK_TILE + tid;
     if (bb < a.F - 1) b = bb;
-  } else if (tid == MASK_TILE && blockIdx.x == 0) {
+  } else if (tid == MASK_TILE && blockIdx.y == 0) {
     b = a.F - 1;
   }
   const bool bok = b >= 0;
@@ -46,7 +46,7 @@ dsd_mask_kernel(const DsdMaskArgs a, int frames_per_cta) {
   const int step = a.tc - a.overlap;
   const float inv_ov1 = a.overlap > 1 ? 1.0f / (float)(a.overlap - 1) : 0.f;
 
-  const int t0 = blockIdx.y * frames_per_cta;
+  const int t0 = blockIdx.x * frames_per_cta;
   for (int f = 0; f < frames_per_cta; ++f) {
     const int t = t0 + f;
     if (t >= a.T) break;
@@ -91,7 +91,7 @@ dsd_mask_kernel(const DsdMaskArgs a, int frames_per_cta) {
           const float p2 = fmaxf(y[2] + bo2, 0.f), p3 = fmaxf(y[NDEC == 4 ? 3 : 1] + bo3, 0.f);
           const float tot = (p0 + p1) + (p2 + p3);
           float m0, m1, m2, m3;
-          if (tot > 0.f) {
+          if (tot > MASK_TOT_MIN) {
             const float r = 1.0f / tot;
             m0 = p0 * r; m1 = p1 * r; m2 = p2 * r; m3 = p3 * r;
           } else if (NDEC == 3) {  // eps*rand cancels: every source gets 1/4 (separate_dsd.py:258-266)
@@ -127,7 +127,8 @@ int launch_dsd_mask(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st) {
   if (a.T <= 0) return DCS_OK;
   DCS_REQUIRE(a.tc > a.overlap && a.overlap >= 0, "time_context %d must exceed overlap %d", a.tc, a.overlap);
   const int fpc = 16;
-  dim3 grid((unsigned)ceil_div64(a.F - 1, MASK_TILE), (unsigned)ceil_div64(a.T, fpc));
+  // frames on gridDim.x (2^31-1 blocks: any clip length), bin tiles on gridDim.y (a handful)
+  dim3 grid((unsigned)ceil_div64(a.T, fpc), (unsigned)ceil_div64(a.F - 1, MASK_TILE));
   if (a.ndec == 4) dsd_mask_kernel<50, 4><<<grid, MASK_THREADS, 0, st>>>(a, fpc);
   else dsd_mask_kernel<50, 3><<<grid, MASK_THREADS, 0, st>>>(a, fpc);
   DCS_CHECK_LAUNCH();

@@ -118,7 +118,7 @@ sconv_mask_kernel(const SconvMaskArgs a) {
         pv[o] = fmaxf(acc[o][r] + a.bout[o], 0.f);
         tot += pv[o];
       }
-      const bool pos = tot > 0.f;
+      const bool pos = tot > MASK_TOT_MIN;
       const float rr = pos ? __fdividef(up, tot) : 0.f;
       const float q = (pos || RULE == 1) ? 0.f : up / (float)NSRC;
 #pragma unroll

@@ -239,7 +239,7 @@ sconv_mask_tc_kernel(const SconvMaskArgs a, int frames_per_cta) {
           pv[o] = fmaxf(y + bo[o], 0.f);
           tot += pv[o];
         }
-        const bool pos = tot > 0.f;
+        const bool pos = tot > MASK_TOT_MIN;
         const float rr = pos ? __fdividef(up, tot) : 0.f;
         const float q = (pos || RULE == 1) ? 0.f : up / (float)NSRC;
 #pragma unroll

@@ -250,6 +250,68 @@ typedef struct {
 enum { DCS_GEMM_EPI_POST = 1, DCS_GEMM_EPI_GATE = 2 };
 int dcs_gemm_view_f32(dcs_ctx* ctx, int engine, int epi, const dcs_gemm_view* view, const float* h_B, void* stream);
 
+/* Bring-up and test entries: the fused last stage of the networks -- InverseLayer(conv1) + output bias + ReLU + soft
+ * ratio mask + sequential patch cross-fade + times the mixture STFT -- on one argument set, field for field the one
+ * the layer sequence passes to the kernels.  Layouts follow DCS_VERSION and may change with it.  Every pointer is
+ * device memory, weights included, in the kernels' own layouts.  engine 1: the wgmma kernel; engine 0: its FFMA twin.
+ * Every argument is checked before anything is queued; a shape the chosen engine does not take is DCS_EINVAL with
+ * nothing launched (there is no switch to the other engine).  Synchronises the stream before returning.
+ *
+ * DSD100 / hiphopss (ndec 3) and stereo / ILD (ndec 4, one call per input channel):
+ *   G     [P][ndec][tc][ldg]  decoder activations after InverseLayer(conv2); columns 0..49 are the 50 conv1 filters
+ *   W1t   [50][ldw]           W1t[c][b] = conv1.W[c, ch, 0, F-1-b] for bins b < F
+ *   bout  [4]                 output biases (ndec 3: source 4 is decoder 2 with bias 4; all-zero bins get 1/4 each;
+ *                             ndec 4: one decoder per source, all-zero bins get 0)
+ *   X     complex [nx][T][ldf], channel c at X + c * x_plane;  S complex, source s / channel c at S + (s*nx + c) * src_stride
+ *   patch k covers frames [k*(tc-overlap), k*(tc-overlap) + tc); frames no patch covers get S = 0.
+ *   engine 1 takes at most 6 patches per frame, ldg >= 52 with ldg % 4 == 0 and a 16-byte aligned G; nx = 2 (the
+ *   masks of one mixture applied to two channels) needs ndec 3.  engine 0 takes nx = 1 only.
+ *   Pad elements read: engine 1 multiplies G columns 50..51 by zero W1t rows, so they must be finite.  No other pad
+ *   element (G columns >= 52, W1t columns >= F, X / S columns >= F) is read.
+ */
+typedef struct {
+  const float* G; int ldg;
+  const float* W1t; int ldw;
+  const float* bout;
+  const dcs_complex* X;
+  dcs_complex* S;
+  int64_t ldf, src_stride;
+  int T, P, tc, overlap, F;
+  int ndec, nx;
+  int64_t x_plane;
+} dcs_dsd_mask_view;
+int dcs_dsd_mask_f32(dcs_ctx* ctx, int engine, const dcs_dsd_mask_view* view, void* stream);
+
+/* The strided-conv1 networks (K3s): arch DCS_ARCH_BACH10, _BACH10_SCORE, _BACH10_SCORE_1X1, _IKALA, _IKALA_NOPOOL.
+ * conv1 has KW taps at stride STRIDE over frequency (Bach10 nets 30 / 4, iKala 30 / 3, build_ca_1x1 5 / 2); J = (F-KW) /
+ * STRIDE + 1 windows, WP = J / 4 pooled windows (DCS_ARCH_IKALA) or J; ND = ceil(KW / STRIDE).
+ *   G     [P'][ndec][tc][WP][32] decoder activations, 30 channels of 32 (ndec: Bach10 4, iKala 2, score-informed 1);
+ *         G holds patches p_base.. (P' = P - p_base)
+ *   tie   [T][WP][32] (DCS_ARCH_IKALA only, else NULL): bit r of frame t, window jp, channel f set where position
+ *         4*jp + r held the window maximum in the forward pass; InverseLayer(pool) routes the value to every set bit
+ *   W     float4 [NW][ND][32]: W[o][dd][f][r] = conv1.W[f][o][0][KW-1-r-STRIDE*dd], one bank per source o for the
+ *         score-informed nets (NW = 4), one bank otherwise (NW = 1)
+ *   bout  [nsrc];  X complex [T][ldf];  S complex [nsrc][T][ldf], source s at S + s * src_stride
+ *   frames [t0, t1) are written (build_ca_1x1 decodes in chunks; every other arch needs p_base = 0, t0 = 0, t1 = T);
+ *   frames no patch covers get S = 0.  engine 1 needs a 16-byte aligned G and a 4-byte aligned tie.
+ *   Pad elements read: both engines multiply the filter-bank entries whose tap index KW-1-r-STRIDE*dd is negative
+ *   (r < STRIDE), and engine 1 multiplies G channels 30..31 by W channels 30..31: those weights must be zero and the
+ *   activations finite.  No other pad element (components r >= STRIDE of W, X / S columns >= F) is read.
+ */
+typedef struct {
+  int arch;
+  const float* G;
+  const uint8_t* tie;
+  const float* W;
+  const float* bout;
+  const dcs_complex* X;
+  dcs_complex* S;
+  int64_t ldf, src_stride;
+  int T, P, tc, overlap, F, J, WP;
+  int p_base, t0, t1;
+} dcs_sconv_mask_view;
+int dcs_sconv_mask_f32(dcs_ctx* ctx, int engine, const dcs_sconv_mask_view* view, void* stream);
+
 /* ---- stereo / ILD variant (examples/dsd100_2ch_ILD/trainCNN_ILD_DSD100.py:299-327) ------------ */
 /* d_audio float[2][audio_stride] (left, right; first num_samples valid) ->
  * d_stems float[nsrc*2][stem_stride], plane (s*2 + j) = source s, channel j (`sep_audio[:, s, j]`).
