@@ -9,6 +9,8 @@ LIB_PATH = os.path.join(HERE, "libdcs.so")
 
 ARCH_IDS = {"dsd": 0, "ikala": 1, "ikala_nopool": 2, "bach10": 3, "bach10_score": 4, "dsd_ild": 5, "bach10_score_1x1": 6}
 PATCHER_IDS = {"standalone": 0, "util": 1}
+# frames per chunk of the Wiener post-filter's sums over time (DCS_WIENER_CHUNK_FRAMES, include/dcs.h)
+WIENER_CHUNK_FRAMES = 128
 
 
 class DcsError(RuntimeError):
@@ -28,6 +30,8 @@ _SIGS = {
     "dcs_set_pool_tap": (C.c_int, [_p, _p, _i64]),
     "dcs_set_wiener": (C.c_int, [_p, C.c_int]),
     "dcs_wiener_stereo": (C.c_int, [_p, _p, _i64, _p, _i64, C.c_int, _i64, _i64, C.c_int, C.c_int, _p]),
+    "dcs_set_wiener_radius": (C.c_int, [_p, C.c_int]),
+    "dcs_wiener_stereo_windowed": (C.c_int, [_p, _p, _i64, _p, _i64, C.c_int, _i64, _i64, C.c_int, C.c_int, C.c_int, _p]),
     "dcs_profile": (C.c_int, [_p, C.c_int]),
     "dcs_profile_read": (C.c_int, [_p, C.c_char_p, C.c_int, _p, C.c_int]),
     "dcs_stft_plan": (C.c_int, [_p, C.c_int, C.c_int, _p, _p, C.POINTER(_p)]),

@@ -163,6 +163,13 @@ int dcs_set_wiener(dcs_ctx* c, int iterations) {
   return DCS_OK;
 }
 
+int dcs_set_wiener_radius(dcs_ctx* c, int radius) {
+  DCS_REQUIRE(c != nullptr, "dcs_set_wiener_radius: NULL ctx");
+  DCS_REQUIRE(radius >= 0, "dcs_set_wiener_radius: radius %d must be >= 0", radius);
+  c->wiener_radius = radius;
+  return DCS_OK;
+}
+
 int dcs_set_pool_tap(dcs_ctx* c, uint8_t* d_bits, int64_t capacity) {
   DCS_REQUIRE(c != nullptr && capacity >= 0, "dcs_set_pool_tap: bad argument");
   c->pool_tap = d_bits;
@@ -547,7 +554,7 @@ static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, i
   DCS_TRY(ctx->S.ensure((size_t)m->nsrc * nx * plane * sizeof(float2), st));
   if (score_arch(m->arch)) DCS_TRY(ctx->net[NET_CHANS].ensure((size_t)score_planes(m) * plane * sizeof(float), st));
   if (ctx->wiener_iters > 0 && m->nch * nx == 2)
-    DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, dcs_num_frames(L, p->hop), m->F), st));
+    DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, dcs_num_frames(L, p->hop), m->F, ctx->wiener_radius), st));
   if (staged) {
     DCS_TRY(ctx->audio.ensure((size_t)(keep ? 3 : 1) * L * sizeof(float), st));
     DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * (keep ? 2 : 1) * L * sizeof(float), st));
@@ -559,7 +566,8 @@ static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, i
 // score filters that form the score-informed net's input channels.  d_mono (keep-channels mode, DSD100 net): the
 // downmix of the two audio planes; the network sees its magnitude, its masks are applied to the STFT of each
 // channel -> nsrc x 2 stem planes ordered (source, channel).  Two-channel stems (keep-channels, the stereo net) go
-// through the Wiener post-filter between the network and the iSTFT when dcs_set_wiener is above 0
+// through the Wiener post-filter between the network and the iSTFT when dcs_set_wiener is above 0, with the covariance
+// window of dcs_set_wiener_radius
 static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,
                          const float* d_filters, const NoteTable* notes, const float* d_mono, float scale_factor,
                          int overlap, int patcher, float* d_stems, int64_t stem_stride, cudaStream_t st) {
@@ -592,7 +600,7 @@ static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const fl
   }
   DCS_TRY(run_network(ctx, m, in, plane, X, plane, nx, T, ldf, overlap, patcher, S, plane, st));
   if (ctx->wiener_iters > 0 && nch * nx == 2)
-    DCS_TRY(launch_wiener(ctx, X, plane, S, plane, m->nsrc, T, ldf, m->F, ctx->wiener_iters, st));
+    DCS_TRY(launch_wiener(ctx, X, plane, S, plane, m->nsrc, T, ldf, m->F, ctx->wiener_iters, ctx->wiener_radius, st));
   DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * nch * nx * plane, st));
   ProfScope ps(ctx, "istft_ola", st);
   return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc * nch * nx, T, ldf, plane, d_stems, L, stem_stride, st);
@@ -972,15 +980,25 @@ int dcs_separate_audio_keep_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, co
 }
 
 // ------------------------------------------------------------------------------------ Wiener post-filter
+static int wiener_stereo(const char* fn, dcs_ctx* ctx, const dcs_complex* d_X, int64_t x_plane, dcs_complex* d_S,
+                         int64_t src_stride, int nsrc, int64_t T, int64_t ldf, int F, int iterations, int radius, void* stream) {
+  DCS_REQUIRE(ctx && d_X && d_S, "%s: NULL argument", fn);
+  DCS_REQUIRE((uintptr_t)d_X % sizeof(float2) == 0 && (uintptr_t)d_S % sizeof(float2) == 0, "%s: spectra not 8-byte aligned", fn);
+  DCS_TRY(wiener_check(fn, nsrc, T, ldf, F, x_plane, src_stride, iterations, radius));
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  return launch_wiener(ctx, (const float2*)d_X, x_plane, (float2*)d_S, src_stride, nsrc, T, ldf, F, iterations, radius,
+                       (cudaStream_t)stream);
+}
+
 int dcs_wiener_stereo(dcs_ctx* ctx, const dcs_complex* d_X, int64_t x_plane, dcs_complex* d_S, int64_t src_stride, int nsrc,
                       int64_t T, int64_t ldf, int F, int iterations, void* stream) {
-  DCS_REQUIRE(ctx && d_X && d_S, "dcs_wiener_stereo: NULL argument");
-  DCS_REQUIRE((uintptr_t)d_X % sizeof(float2) == 0 && (uintptr_t)d_S % sizeof(float2) == 0,
-              "dcs_wiener_stereo: spectra not 8-byte aligned");
-  DCS_TRY(wiener_check("dcs_wiener_stereo", nsrc, T, ldf, F, x_plane, src_stride, iterations));
-  DCS_CUDA(cudaSetDevice(ctx->device));
-  return launch_wiener(ctx, (const float2*)d_X, x_plane, (float2*)d_S, src_stride, nsrc, T, ldf, F, iterations,
-                       (cudaStream_t)stream);
+  return wiener_stereo("dcs_wiener_stereo", ctx, d_X, x_plane, d_S, src_stride, nsrc, T, ldf, F, iterations, 0, stream);
+}
+
+int dcs_wiener_stereo_windowed(dcs_ctx* ctx, const dcs_complex* d_X, int64_t x_plane, dcs_complex* d_S, int64_t src_stride,
+                               int nsrc, int64_t T, int64_t ldf, int F, int iterations, int radius, void* stream) {
+  return wiener_stereo("dcs_wiener_stereo_windowed", ctx, d_X, x_plane, d_S, src_stride, nsrc, T, ldf, F, iterations, radius,
+                       stream);
 }
 
 }  // extern "C"

@@ -94,6 +94,7 @@ struct dcs_ctx {
   uint8_t* pool_tap = nullptr;  // dcs_set_pool_tap: copy of the routing decisions of the forward pass
   int64_t pool_tap_cap = 0;
   int wiener_iters = 0;         // dcs_set_wiener: EM iterations of the stereo Wiener post-filter (0 = off)
+  int wiener_radius = 0;        // dcs_set_wiener_radius: its covariance window in chunks to either side (0 = whole clip)
   dcs::DevBuf wiener;           // its partial sums, spatial covariances and mixture scale (wiener.cu)
   int32_t* notes_host = nullptr;      // pinned staging of the compacted note table (its device copy: net[NET_NOTES])
   size_t notes_host_cap = 0;
@@ -327,10 +328,12 @@ int launch_pcm_encode_keep(dcs_ctx* ctx, const float* d_stems, int64_t L, int ns
                            cudaStream_t st);
 
 // multichannel Wiener post-filter (wiener.cu): mixture channel c at X + c * x_plane, stem (j, c) at
-// S + (2 j + c) * src_stride, bins f < F filtered in place by `iterations` EM iterations
-int wiener_check(const char* fn, int nsrc, int64_t T, int64_t ldf, int F, int64_t x_plane, int64_t src_stride, int iterations);
-size_t wiener_workspace_bytes(int nsrc, int64_t T, int F);
+// S + (2 j + c) * src_stride, bins f < F filtered in place by `iterations` EM iterations; radius: the covariance window
+// in chunks of DCS_WIENER_CHUNK_FRAMES frames to either side (0 = the whole clip)
+int wiener_check(const char* fn, int nsrc, int64_t T, int64_t ldf, int F, int64_t x_plane, int64_t src_stride, int iterations,
+                 int radius);
+size_t wiener_workspace_bytes(int nsrc, int64_t T, int F, int radius);
 int launch_wiener(dcs_ctx* ctx, const float2* X, int64_t x_plane, float2* S, int64_t src_stride, int nsrc, int64_t T,
-                  int64_t ldf, int F, int iterations, cudaStream_t st);
+                  int64_t ldf, int F, int iterations, int radius, cudaStream_t st);
 
 }  // namespace dcs

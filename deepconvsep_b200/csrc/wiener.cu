@@ -12,13 +12,17 @@
 //
 // One thread per bin walks a chunk of kWienerFrames frames; the grid is bin tiles x frame chunks.  The sums over
 // t are per-chunk fp64 partials reduced in chunk order: no atomics, the same bits on every run.
+//
+// Sliding window (radius W >= 1): chunk c takes R_j(f; c) and s_c from the chunks max(0, c-W) .. min(n-1, c+W)
+// instead of the whole clip.  Each chunk's window sum is formed directly from the partials, in ascending chunk order,
+// so a chunk's R is the same bits in any segment that holds its window, and W >= n-1 gives the whole-clip bits.
 #include "common.cuh"
 
 namespace dcs {
 namespace {
 
 constexpr int kWienerBins = 128;     // threads per block: consecutive bins, coalesced float2 rows
-constexpr int kWienerFrames = 128;   // frames per chunk: partials are 32 B per (source, bin) per 128 frames
+constexpr int kWienerFrames = DCS_WIENER_CHUNK_FRAMES;   // frames per chunk: partials are 32 B per (source, bin) per 128 frames
 constexpr int kReduceThreads = 256;
 constexpr double kEps = 1.1920928955078125e-07;   // 2^-23 = FLT_EPSILON
 
@@ -28,9 +32,11 @@ struct WienerArgs {
   int64_t T, ldf;
   int F, nchunks, ntiles;
   double* part;    // [nchunks][nsrc][4][F]: per-chunk sums of |yL|^2, |yR|^2, Re yL conj(yR), Im yL conj(yR)
-  double* Q;       // [nsrc][4][F]: the same summed over all chunks (chunk order)
+  double* Q;       // [nsrc][4][F]: the same summed over all chunks (chunk order); windowed: [nchunks][nsrc][4][F]
   double* pmax;    // [nchunks][ntiles]: per-block max of |x|^2 over both channels
-  double* scale;   // [1]: s
+  double* scale;   // [1]: s; windowed: [nchunks]: s_c
+  int64_t q_stride;   // doubles between the Q of consecutive chunks: 0 (one Q for the clip) or nsrc * 4 * F
+  int s_stride;       // the same for the scale: 0 or 1
 };
 
 __device__ __forceinline__ void accumulate(double* q, float2 l, float2 r) {
@@ -106,18 +112,50 @@ __global__ void __launch_bounds__(kReduceThreads) wiener_reduce_kernel(const Wie
   a.Q[e] = sum;
 }
 
-// one EM iteration in place; STATS: also the next iteration's partial sums of the stems it stores
+// partials -> the Q of chunk c = blockIdx.y over its window c-W .. c+W (clipped to the clip), summed directly in
+// ascending chunk order, one thread per (source, quantity, bin); the extra last block of each row: s_c from the
+// maxima of the window's chunks.  radius <= nchunks - 1 (the host clips it; a larger radius is the same window)
+__global__ void __launch_bounds__(kReduceThreads) wiener_reduce_window_kernel(const WienerArgs a, int64_t n, int radius) {
+  const int c = blockIdx.y;
+  const int c0 = max(0, c - radius), c1 = min(a.nchunks - 1, c + radius);
+  if (blockIdx.x == gridDim.x - 1) {
+    __shared__ double wmax[kReduceThreads / 32];
+    double mx = 0.0;
+    for (int64_t i = (int64_t)c0 * a.ntiles + threadIdx.x; i < (int64_t)(c1 + 1) * a.ntiles; i += kReduceThreads)
+      mx = fmax(mx, a.pmax[i]);
+#pragma unroll
+    for (int k = 16; k > 0; k >>= 1) mx = fmax(mx, __shfl_down_sync(0xffffffffu, mx, k));
+    if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = mx;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int w = 1; w < kReduceThreads / 32; ++w) mx = fmax(mx, wmax[w]);
+      a.scale[c] = fmax(1.0, sqrt(mx) / 10.0);
+    }
+    return;
+  }
+  const int64_t e = (int64_t)blockIdx.x * kReduceThreads + threadIdx.x;
+  if (e >= n) return;
+  double sum = 0.0;
+#pragma unroll 8
+  for (int k = c0; k <= c1; ++k) sum += a.part[(int64_t)k * n + e];
+  a.Q[(int64_t)c * n + e] = sum;
+}
+
+// one EM iteration in place; STATS: also the next iteration's partial sums of the stems it stores.  Chunk
+// blockIdx.y reads its Q and scale at q_stride / s_stride (0: the clip's)
 template <int NSRC, bool STATS>
 __global__ void __launch_bounds__(kWienerBins) wiener_em_kernel(const WienerArgs a) {
   const int f = blockIdx.x * kWienerBins + threadIdx.x;
   if (f >= a.F) return;
   const int64_t t0 = (int64_t)blockIdx.y * kWienerFrames, t1 = min(a.T, t0 + kWienerFrames);
-  const double s2 = *a.scale * *a.scale, es2 = kEps * s2, ds2 = sqrt(kEps) * s2;
+  const double* Q = a.Q + (int64_t)blockIdx.y * a.q_stride;
+  const double s = a.scale[(int64_t)blockIdx.y * a.s_stride];
+  const double s2 = s * s, es2 = kEps * s2, ds2 = sqrt(kEps) * s2;
   double r[NSRC][4];   // R_j(f): [0][0], [1][1], Re [0][1], Im [0][1]
 #pragma unroll
   for (int j = 0; j < NSRC; ++j) {
 #pragma unroll
-    for (int q = 0; q < 4; ++q) r[j][q] = a.Q[(int64_t)(j * 4 + q) * a.F + f];
+    for (int q = 0; q < 4; ++q) r[j][q] = Q[(int64_t)(j * 4 + q) * a.F + f];
     const double inv = 1.0 / (es2 + 0.5 * (r[j][0] + r[j][1]));
 #pragma unroll
     for (int q = 0; q < 4; ++q) r[j][q] *= inv;
@@ -170,17 +208,25 @@ __global__ void __launch_bounds__(kWienerBins) wiener_em_kernel(const WienerArgs
   if (STATS) store_partials<NSRC>(a, acc, f);
 }
 
+// partials -> Q and scale: over the whole clip (radius 0) or over each chunk's window
+void launch_reduce(const WienerArgs& a, int64_t n, int radius, cudaStream_t st) {
+  const unsigned rgrid = (unsigned)ceil_div64(n, kReduceThreads) + 1;
+  if (radius == 0)
+    wiener_reduce_kernel<<<rgrid, kReduceThreads, 0, st>>>(a, n);
+  else
+    wiener_reduce_window_kernel<<<dim3(rgrid, (unsigned)a.nchunks), kReduceThreads, 0, st>>>(a, n, min(radius, a.nchunks - 1));
+}
+
 template <int NSRC>
-int launch_wiener_n(dcs_ctx* ctx, const WienerArgs& a, int iterations, cudaStream_t st) {
+int launch_wiener_n(dcs_ctx* ctx, const WienerArgs& a, int iterations, int radius, cudaStream_t st) {
   const dim3 grid((unsigned)a.ntiles, (unsigned)a.nchunks);
   const int64_t n = (int64_t)NSRC * 4 * a.F;
-  const unsigned rgrid = (unsigned)ceil_div64(n, kReduceThreads) + 1;
   {
     ProfScope ps(ctx, "wiener_init", st);
     wiener_init_kernel<NSRC><<<grid, kWienerBins, 0, st>>>(a);
     DCS_CHECK_LAUNCH();
     ctx->launches++;
-    wiener_reduce_kernel<<<rgrid, kReduceThreads, 0, st>>>(a, n);
+    launch_reduce(a, n, radius, st);
     DCS_CHECK_LAUNCH();
     ctx->launches++;
   }
@@ -190,7 +236,7 @@ int launch_wiener_n(dcs_ctx* ctx, const WienerArgs& a, int iterations, cudaStrea
       wiener_em_kernel<NSRC, true><<<grid, kWienerBins, 0, st>>>(a);
       DCS_CHECK_LAUNCH();
       ctx->launches++;
-      wiener_reduce_kernel<<<rgrid, kReduceThreads, 0, st>>>(a, n);
+      launch_reduce(a, n, radius, st);
     } else {
       wiener_em_kernel<NSRC, false><<<grid, kWienerBins, 0, st>>>(a);
     }
@@ -202,25 +248,29 @@ int launch_wiener_n(dcs_ctx* ctx, const WienerArgs& a, int iterations, cudaStrea
 
 struct WienerLayout {
   int nchunks, ntiles;
-  int64_t part, Q, pmax, total;   // offsets / size in doubles
+  int64_t part, Q, pmax, scale, total;   // offsets / size in doubles
 };
 
-WienerLayout wiener_layout(int nsrc, int64_t T, int F) {
+// radius >= 1: one Q and one scale per chunk
+WienerLayout wiener_layout(int nsrc, int64_t T, int F, int radius) {
   WienerLayout l;
   l.nchunks = (int)ceil_div64(T, kWienerFrames);
   l.ntiles = (int)ceil_div64(F, kWienerBins);
-  const int64_t per = (int64_t)nsrc * 4 * F;
+  const int64_t per = (int64_t)nsrc * 4 * F, nq = radius > 0 ? l.nchunks : 1;
   l.part = 0;
   l.Q = (int64_t)l.nchunks * per;
-  l.pmax = l.Q + per;
-  l.total = l.pmax + (int64_t)l.nchunks * l.ntiles + 1;
+  l.pmax = l.Q + nq * per;
+  l.scale = l.pmax + (int64_t)l.nchunks * l.ntiles;
+  l.total = l.scale + nq;
   return l;
 }
 
 }  // namespace
 
-int wiener_check(const char* fn, int nsrc, int64_t T, int64_t ldf, int F, int64_t x_plane, int64_t src_stride, int iterations) {
+int wiener_check(const char* fn, int nsrc, int64_t T, int64_t ldf, int F, int64_t x_plane, int64_t src_stride, int iterations,
+                 int radius) {
   DCS_REQUIRE(iterations >= 0, "%s: iterations %d must be >= 0", fn, iterations);
+  DCS_REQUIRE(radius >= 0, "%s: radius %d must be >= 0", fn, radius);
   DCS_REQUIRE(nsrc >= 1 && nsrc <= 4, "%s: nsrc %d not in [1, 4]", fn, nsrc);
   DCS_REQUIRE(T > 0 && ceil_div64(T, kWienerFrames) <= 65535, "%s: %lld frames out of range", fn, (long long)T);
   DCS_REQUIRE(F > 0 && ldf >= F, "%s: bins %d / row stride %lld", fn, F, (long long)ldf);
@@ -229,23 +279,27 @@ int wiener_check(const char* fn, int nsrc, int64_t T, int64_t ldf, int F, int64_
   return DCS_OK;
 }
 
-size_t wiener_workspace_bytes(int nsrc, int64_t T, int F) { return (size_t)wiener_layout(nsrc, T, F).total * sizeof(double); }
+size_t wiener_workspace_bytes(int nsrc, int64_t T, int F, int radius) {
+  return (size_t)wiener_layout(nsrc, T, F, radius).total * sizeof(double);
+}
 
 int launch_wiener(dcs_ctx* ctx, const float2* X, int64_t x_plane, float2* S, int64_t src_stride, int nsrc, int64_t T,
-                  int64_t ldf, int F, int iterations, cudaStream_t st) {
+                  int64_t ldf, int F, int iterations, int radius, cudaStream_t st) {
   if (iterations <= 0) return DCS_OK;
-  const WienerLayout l = wiener_layout(nsrc, T, F);
+  const WienerLayout l = wiener_layout(nsrc, T, F, radius);
   DCS_TRY(ctx->wiener.ensure((size_t)l.total * sizeof(double), st));
   double* w = ctx->wiener.as<double>();
   WienerArgs a;
   a.X = X; a.x_plane = x_plane; a.S = S; a.src_stride = src_stride; a.T = T; a.ldf = ldf;
   a.F = F; a.nchunks = l.nchunks; a.ntiles = l.ntiles;
-  a.part = w + l.part; a.Q = w + l.Q; a.pmax = w + l.pmax; a.scale = w + l.total - 1;
+  a.part = w + l.part; a.Q = w + l.Q; a.pmax = w + l.pmax; a.scale = w + l.scale;
+  a.q_stride = radius > 0 ? (int64_t)nsrc * 4 * F : 0;
+  a.s_stride = radius > 0 ? 1 : 0;
   switch (nsrc) {
-    case 1: return launch_wiener_n<1>(ctx, a, iterations, st);
-    case 2: return launch_wiener_n<2>(ctx, a, iterations, st);
-    case 3: return launch_wiener_n<3>(ctx, a, iterations, st);
-    case 4: return launch_wiener_n<4>(ctx, a, iterations, st);
+    case 1: return launch_wiener_n<1>(ctx, a, iterations, radius, st);
+    case 2: return launch_wiener_n<2>(ctx, a, iterations, radius, st);
+    case 3: return launch_wiener_n<3>(ctx, a, iterations, radius, st);
+    case 4: return launch_wiener_n<4>(ctx, a, iterations, radius, st);
   }
   DCS_REQUIRE(false, "wiener: nsrc %d not in [1, 4]", nsrc);
 }

@@ -47,10 +47,12 @@ def _stream_ptr(stream=None, device=None):
     return C.c_void_p(s.cuda_stream)
 
 
-def wiener_stereo(ctx, X, S, iterations, stream=None, num_bins=None):
-    """Multichannel Wiener post-filter with EM spatial covariances (dcs_wiener_stereo), in place on device spectra:
-    X torch complex64 cuda [2, T, ldf] (the mixture's channels), S [nsrc * 2, T, ldf] (the stems, planes ordered
-    (source, channel), nsrc <= 4).  Bins >= num_bins (default ldf) are left alone.  Returns S."""
+def wiener_stereo(ctx, X, S, iterations, stream=None, num_bins=None, radius=0):
+    """Multichannel Wiener post-filter with EM spatial covariances (dcs_wiener_stereo_windowed), in place on device
+    spectra: X torch complex64 cuda [2, T, ldf] (the mixture's channels), S [nsrc * 2, T, ldf] (the stems, planes
+    ordered (source, channel), nsrc <= 4).  Bins >= num_bins (default ldf) are left alone.  radius: 0 = one spatial
+    covariance per source for the whole clip; W >= 1 = per chunk of _lib.WIENER_CHUNK_FRAMES frames, from the chunks
+    within W of it.  Returns S."""
     import torch
     if X.dim() != 3 or X.shape[0] != 2 or S.dim() != 3 or S.shape[0] % 2 or tuple(S.shape[1:]) != tuple(X.shape[1:]):
         raise ValueError("wiener_stereo needs X [2, T, ldf] and S [nsrc * 2, T, ldf], got %r and %r"
@@ -61,17 +63,18 @@ def wiener_stereo(ctx, X, S, iterations, stream=None, num_bins=None):
         raise ValueError("wiener_stereo needs contiguous [T, ldf] planes")
     T, ldf = int(X.shape[1]), int(X.shape[2])
     F = ldf if num_bins is None else int(num_bins)
-    _lib.check(ctx.lib.dcs_wiener_stereo(ctx.handle, _ptr(X), X.stride(0), _ptr(S), S.stride(0), S.shape[0] // 2, T, ldf,
-                                         F, int(iterations), _stream_ptr(stream, ctx.device)))
+    _lib.check(ctx.lib.dcs_wiener_stereo_windowed(ctx.handle, _ptr(X), X.stride(0), _ptr(S), S.stride(0), S.shape[0] // 2, T,
+                                                  ldf, F, int(iterations), int(radius), _stream_ptr(stream, ctx.device)))
     return S
 
 
-def check_stereo_options(family, keep_channels=False, wiener=0):
+def check_stereo_options(family, keep_channels=False, wiener=0, wiener_radius=0):
     """The rule for the options of two-channel stems, by network family (the keys of models.FAMILY_DEFAULTS, which
     are also the Separator's architecture names): keep_channels (the soft masks of the downmix applied to each
     channel) exists for the DSD100 / hiphopss network "dsd" only; wiener (EM iterations of the multichannel Wiener
     post-filter) cannot be negative and needs two-channel stems: keep_channels, or the stereo / ILD network
-    "dsd_ild".  Raises ValueError with the reason otherwise."""
+    "dsd_ild"; wiener_radius (the filter's covariance window in chunks to either side, 0 = the whole clip) cannot be
+    negative and needs wiener > 0.  Raises ValueError with the reason otherwise."""
     if keep_channels and family != "dsd":
         raise ValueError("--keep-channels: only the DSD100 / hiphopss network (family dsd) keeps the stereo channels, "
                          "not %s" % (family,))
@@ -80,26 +83,36 @@ def check_stereo_options(family, keep_channels=False, wiener=0):
     if wiener and not (keep_channels or family == "dsd_ild"):
         raise ValueError("--wiener needs --keep-channels (family dsd) or the stereo / ILD network (family dsd_ild): "
                          "the Wiener post-filter works on two-channel stems")
+    check_wiener_radius(wiener, wiener_radius)
 
 
-def clip_call(sep, filters=None, melody=None, frame0=0, keep_channels=False, wiener=0):
+def check_wiener_radius(wiener, wiener_radius):
+    """The wiener_radius half of check_stereo_options, for the calls whose network and layout are already fixed."""
+    if wiener_radius < 0:
+        raise ValueError("--wiener-radius %d: the covariance window cannot be negative" % wiener_radius)
+    if wiener_radius and not wiener:
+        raise ValueError("--wiener-radius needs --wiener K > 0: it is the window of the Wiener post-filter's covariances")
+
+
+def clip_call(sep, filters=None, melody=None, frame0=0, keep_channels=False, wiener=0, wiener_radius=0):
     """The call that separates a whole clip with Separator `sep`'s network and these inputs, as a function of the
     audio: sep.separate_keep_channels (keep_channels=True), sep.separate_notes (the note table melody, from table frame
     frame0), sep.separate_score (a score-informed net and its score filters), sep.separate_stereo (the stereo / ILD
-    net) or sep.separate.  wiener: EM iterations of the Wiener post-filter, passed to the two-channel calls and refused
-    for the others here, before anything runs.  Only sep.model.arch and the method picked are used, so stand-ins with
-    just those work too."""
+    net) or sep.separate.  wiener: EM iterations of the Wiener post-filter, and wiener_radius its covariance window
+    (passed only when set), given to the two-channel calls and refused for the others here, before anything runs.
+    Only sep.model.arch and the method picked are used, so stand-ins with just those work too."""
+    rkw = {"wiener_radius": wiener_radius} if wiener_radius else {}
     if keep_channels:
-        return partial(sep.separate_keep_channels, wiener=wiener)
+        return partial(sep.separate_keep_channels, wiener=wiener, **rkw)
     if melody is not None:
         run = partial(sep.separate_notes, melody=melody, frame0=frame0)
     elif sep.model.arch in ("bach10_score", "bach10_score_1x1"):
         run = partial(sep.separate_score, filters=filters)
     elif sep.model.arch == "dsd_ild":
-        return partial(sep.separate_stereo, wiener=wiener)
+        return partial(sep.separate_stereo, wiener=wiener, **rkw)
     else:
         run = sep.separate
-    check_stereo_options(sep.model.arch, wiener=wiener)
+    check_stereo_options(sep.model.arch, wiener=wiener, wiener_radius=wiener_radius)
     return run
 
 
@@ -161,6 +174,11 @@ class Context(object):
     def set_wiener(self, iterations):
         """EM iterations of the Wiener post-filter on the context's two-channel stems (dcs_set_wiener; 0 = off)"""
         _lib.check(self.lib.dcs_set_wiener(self.handle, int(iterations)))
+
+    def set_wiener_radius(self, radius):
+        """covariance window of that filter in chunks of _lib.WIENER_CHUNK_FRAMES frames to either side
+        (dcs_set_wiener_radius; 0 = the whole clip)"""
+        _lib.check(self.lib.dcs_set_wiener_radius(self.handle, int(radius)))
 
     def profile_read(self, max_n=4096):
         """[(stage name, milliseconds)] recorded since profiling was enabled (synchronises)."""
@@ -356,14 +374,15 @@ class Separator(object):
                                               _stream_ptr(None, self.ctx.device)))
         return out
 
-    def separate_pcm16(self, pcm, downmix=1, out=None, keep_channels=False, wiener=0):
+    def separate_pcm16(self, pcm, downmix=1, out=None, keep_channels=False, wiener=0, wiener_radius=0):
         """int16 wav samples [L] or [L, channels] -> int16 [nsrc, L] (train_auto's wav contract).
         keep_channels=True (DSD100 / hiphopss net, stereo [L, 2] in): int16 [nsrc, L, 2] stereo stems, see
-        separate_keep_channels; wiener: EM iterations of the Wiener post-filter on them (keep_channels only)."""
+        separate_keep_channels; wiener: EM iterations of the Wiener post-filter on them and wiener_radius its
+        covariance window (keep_channels only)."""
         if keep_channels:
             return self.separate_pcm16_batch([pcm], outs=None if out is None else [out], keep_channels=True,
-                                             wiener=wiener)[0]
-        check_stereo_options(self.model.arch, wiener=wiener)
+                                             wiener=wiener, wiener_radius=wiener_radius)[0]
+        check_stereo_options(self.model.arch, wiener=wiener, wiener_radius=wiener_radius)
         p = np.ascontiguousarray(pcm, dtype=np.int16)
         L = p.shape[0]
         ch = 1 if p.ndim == 1 else p.shape[1]
@@ -374,14 +393,14 @@ class Separator(object):
                                                     self.patcher, out.ctypes.data, L, _stream_ptr(None, self.ctx.device)))
         return out
 
-    def separate_pcm16_batch(self, clips, downmix=1, outs=None, keep_channels=False, wiener=0):
+    def separate_pcm16_batch(self, clips, downmix=1, outs=None, keep_channels=False, wiener=0, wiener_radius=0):
         """Several clips through the context's multi-clip scheduler (dcs_separate_batch_pcm16_host): H2D of clip i+1,
         the kernels of clip i and D2H of clip i-1 overlap.  clips: list of int16 arrays [L] or [L, channels] (same
         channel count; pinned for real overlap) -> list of int16 [nsrc, L].  keep_channels=True: stereo clips
         [L, 2] -> list of int16 [nsrc, L, 2] (dcs_separate_batch_pcm16_keep_channels_host), with `wiener` EM iterations
-        of the Wiener post-filter on each clip's stems."""
+        of the Wiener post-filter on each clip's stems, over covariance windows of `wiener_radius` chunks."""
         if not keep_channels:
-            check_stereo_options(self.model.arch, wiener=wiener)
+            check_stereo_options(self.model.arch, wiener=wiener, wiener_radius=wiener_radius)
         ps = [np.ascontiguousarray(c, dtype=np.int16) for c in clips]
         if not ps:
             return []
@@ -389,7 +408,9 @@ class Separator(object):
             for p_ in ps:
                 if p_.ndim != 2 or p_.shape[1] != 2:
                     raise ValueError("keep_channels needs stereo int16 clips [L, 2], got shape %r" % (p_.shape,))
+            check_wiener_radius(wiener, wiener_radius)
             self.ctx.set_wiener(wiener)
+            self.ctx.set_wiener_radius(wiener_radius)
             return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_keep_channels_host, ps, outs, (2,), ())
         ch = 1 if ps[0].ndim == 1 else ps[0].shape[1]
         assert all((1 if p_.ndim == 1 else p_.shape[1]) == ch for p_ in ps), "all clips must have the same channel count"
@@ -467,26 +488,29 @@ class Separator(object):
                          self.overlap, self.patcher, _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
         return outd.cpu().numpy() if host else outd
 
-    def separate_stereo(self, audio, out=None, stream=None, wiener=0):
+    def separate_stereo(self, audio, out=None, stream=None, wiener=0, wiener_radius=0):
         """Stereo / ILD network (examples/dsd100_2ch_ILD/trainCNN_ILD_DSD100.py:299-327): audio float
         [L, 2] (numpy) or [2, L] (cuda tensor) -> `sep_audio` float32 [L, nsrc, 2] (numpy) or the device
         planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> cuda tensor out).  wiener: EM iterations of
-        the multichannel Wiener post-filter (dcs_set_wiener) on the network's spectra, 0 = off."""
-        return self._two_channel_clip(self.lib.dcs_separate_audio_stereo, audio, out, stream, wiener)
+        the multichannel Wiener post-filter (dcs_set_wiener) on the network's spectra, 0 = off; wiener_radius: its
+        covariance window in chunks to either side (dcs_set_wiener_radius), 0 = the whole clip."""
+        return self._two_channel_clip(self.lib.dcs_separate_audio_stereo, audio, out, stream, wiener, wiener_radius)
 
-    def separate_keep_channels(self, audio, out=None, stream=None, wiener=0):
+    def separate_keep_channels(self, audio, out=None, stream=None, wiener=0, wiener_radius=0):
         """Stereo stems from the DSD100 / hiphopss network (dcs_separate_audio_keep_channels): the network sees the
         downmix (l + r) * 0.5, its soft masks are applied to each channel's STFT and inverted with that channel's
         phase.  audio float [L, 2] (numpy) or [2, L] (cuda tensor) -> float32 [L, nsrc, 2] (numpy, the layout of
         separate_stereo) or the device planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out).
-        wiener: EM iterations of the multichannel Wiener post-filter (dcs_set_wiener) on the masked spectra, 0 = off."""
-        return self._two_channel_clip(self.lib.dcs_separate_audio_keep_channels, audio, out, stream, wiener)
+        wiener: EM iterations of the multichannel Wiener post-filter (dcs_set_wiener) on the masked spectra, 0 = off;
+        wiener_radius: its covariance window in chunks to either side (dcs_set_wiener_radius), 0 = the whole clip."""
+        return self._two_channel_clip(self.lib.dcs_separate_audio_keep_channels, audio, out, stream, wiener, wiener_radius)
 
-    def _two_channel_clip(self, entry, audio, out, stream, wiener):
+    def _two_channel_clip(self, entry, audio, out, stream, wiener, wiener_radius):
         """audio float [L, 2] (numpy) or [2, L] (cuda tensor) through the two-channel clip entry point `entry`, with
-        `wiener` EM iterations of the Wiener post-filter -> float32 [L, nsrc, 2] (numpy) or the device planes
-        [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out)."""
+        `wiener` EM iterations of the Wiener post-filter over covariance windows of `wiener_radius` chunks -> float32
+        [L, nsrc, 2] (numpy) or the device planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out)."""
         import torch
+        check_wiener_radius(wiener, wiener_radius)
         host = not hasattr(audio, "is_cuda")
         if host:
             a = np.asarray(audio, dtype=np.float32)
@@ -499,23 +523,26 @@ class Separator(object):
         L = x.shape[1]
         outd = out if (out is not None and not host) else torch.empty((self.nsrc * 2, L), dtype=torch.float32, device=x.device)
         self.ctx.set_wiener(wiener)
+        self.ctx.set_wiener_radius(wiener_radius)
         _lib.check(entry(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), x.stride(0), L, self.scale_factor,
                          self.overlap, self.patcher, _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
         if not host:
             return outd
         return np.ascontiguousarray(outd.cpu().numpy().reshape(self.nsrc, 2, L).transpose(2, 0, 1))
 
-    def separate_tapped(self, audio, filters=None, pool=False, keep_channels=False, wiener=0, melody=None, frame0=0):
+    def separate_tapped(self, audio, filters=None, pool=False, keep_channels=False, wiener=0, melody=None, frame0=0,
+                        wiener_radius=0):
         """Parity-test entry: the whole-clip call clip_call() picks for these inputs (separate() / separate_score() /
         separate_notes() / separate_stereo() / separate_keep_channels()) with the spectrum tap on
         (dcs_set_spectrum_tap) -> (stems as that call returns them, masked spectra complex64 numpy [nplanes, T, F] --
         the tensors the inverse STFT of THIS call consumed, (source, channel) planes for the stereo outputs).
         pool=True: also the routing decisions of this call (dcs_set_pool_tap) -- max-pool net: the tie bits uint8
         [T, WP, 32]; 1x1 score net: the gate codes of conv1..conv6, a list of uint8 [rows, W, C] (gate_code_layout).
-        wiener: EM iterations of the Wiener post-filter (two-channel stems only); the tap then holds the filtered spectra.
+        wiener: EM iterations of the Wiener post-filter (two-channel stems only), wiener_radius its covariance window;
+        the tap then holds the filtered spectra.
         melody (score-informed nets): the note table instead of `filters`, through separate_notes(audio, melody, frame0)."""
         import torch
-        run = clip_call(self, filters, melody, frame0, keep_channels, wiener)
+        run = clip_call(self, filters, melody, frame0, keep_channels, wiener, wiener_radius)
         a = np.asarray(audio)
         L = a.shape[0]
         T = self.stft.num_frames(L)

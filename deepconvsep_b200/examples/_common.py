@@ -43,13 +43,17 @@ def decode(audioObj, family):
 
 
 def run(family, filein, outdir, model, scale_factor, time_context, overlap, batch_size, input_size, frame_size, hop,
-        out_name, window=None, device=0, slot=0, keep_channels=False, wiener=0):
+        out_name, window=None, device=0, slot=0, keep_channels=False, wiener=0, wiener_radius=0):
     """wav in -> one int16 wav per source in `outdir`.  `batch_size` is accepted for signature
     compatibility; the CUDA path has no patch batches.  keep_channels (DSD100 / hiphopss, 2-channel wav): one
     2-channel wav per source -- the soft masks of the downmix applied to each channel; wiener: that many EM iterations
-    of the multichannel Wiener post-filter on them (keep_channels only)."""
-    check_stereo_options(family, keep_channels, wiener)
+    of the multichannel Wiener post-filter on them (keep_channels only), wiener_radius: its covariance window in chunks
+    to either side (0 = the whole clip).  A device list cuts the recording into segments over the devices; with
+    keep_channels and wiener that needs wiener_radius >= 1."""
+    check_stereo_options(family, keep_channels, wiener, wiener_radius)
     wkw = {"wiener": wiener} if wiener else {}
+    if wiener_radius:
+        wkw["wiener_radius"] = wiener_radius
     d = dict(FAMILY_DEFAULTS[family])
     if window is not None:
         d["window"] = window
@@ -62,14 +66,22 @@ def run(family, filein, outdir, model, scale_factor, time_context, overlap, batc
         if audioObj.ndim != 2 or audioObj.shape[1] != 2:
             raise ValueError("--keep-channels needs a 2-channel recording; %s has %d channel(s)"
                              % (filein, 1 if audioObj.ndim == 1 else audioObj.shape[1]))
+        maxv = np.finfo(audioObj.dtype).max if np.issubdtype(audioObj.dtype, np.floating) else np.iinfo(audioObj.dtype).max
         if isinstance(device, (list, tuple)):
-            raise ValueError("--keep-channels separates each recording on one device; give several files for several devices")
-        sep = get_separator(model, arch, frame_size, hop, d["window"], scale_factor, time_context, overlap, input_size,
-                            device=device, slot=slot)
-        if audioObj.dtype == np.int16:
+            # one stereo recording over several GPUs: segments on the chunk grid of the Wiener filter's windows
+            from .. import longclip
+            seps = [get_separator(model, arch, frame_size, hop, d["window"], scale_factor, time_context, overlap, input_size,
+                                  device=dev, slot=slot) for dev in device]
+            sep = seps[0]
+            stems = longclip.separate_long(seps, audioObj.astype('float') / maxv, keep_channels=True, **wkw)
+            stems16 = (stems.transpose(1, 0, 2).astype(np.float64) * np.iinfo(np.int16).max).astype('int16')
+        elif audioObj.dtype == np.int16:
+            sep = get_separator(model, arch, frame_size, hop, d["window"], scale_factor, time_context, overlap, input_size,
+                                device=device, slot=slot)
             stems16 = sep.separate_pcm16(audioObj, keep_channels=True, **wkw)      # [nsrc, L, 2], int16 path on the GPU
         else:
-            maxv = np.finfo(audioObj.dtype).max if np.issubdtype(audioObj.dtype, np.floating) else np.iinfo(audioObj.dtype).max
+            sep = get_separator(model, arch, frame_size, hop, d["window"], scale_factor, time_context, overlap, input_size,
+                                device=device, slot=slot)
             stems = sep.separate_keep_channels(audioObj.astype('float') / maxv, **wkw)    # [L, nsrc, 2]
             stems16 = (stems.transpose(1, 0, 2).astype(np.float64) * np.iinfo(np.int16).max).astype('int16')
     elif isinstance(device, (list, tuple)):
@@ -101,12 +113,15 @@ def run(family, filein, outdir, model, scale_factor, time_context, overlap, batc
 
 
 # ---- command line shared by the separate_*.py scripts ------------------------------------------------------
-LONG_OPTS = ["ifile=", "odir=", "mfile=", "frame-size=", "window=", "devices=", "batch-clips=", "keep-channels", "wiener="]
+LONG_OPTS = ["ifile=", "odir=", "mfile=", "frame-size=", "window=", "devices=", "batch-clips=", "keep-channels", "wiener=",
+             "wiener-radius="]
 EXTRA_USAGE = ("  optional: --frame-size N (STFT frame, feat_size = N/2+1)  --window hanning|blackmanharris|sinebell\n"
                "            --devices 0,1,...  --batch-clips K (clips in flight per device); with these, -i may be a directory of wavs\n"
                "            (one wav and several devices: the recording itself is cut into segments over the devices)\n"
                "            --keep-channels (DSD100 / hiphopss, 2-channel wavs): 2-channel stems, the downmix's masks on each channel\n"
-               "            --wiener K (with --keep-channels): K EM iterations of the multichannel Wiener post-filter on them")
+               "            --wiener K (with --keep-channels): K EM iterations of the multichannel Wiener post-filter on them\n"
+               "            --wiener-radius R (with --wiener): covariances over a window of R chunks of 128 frames to either\n"
+               "            side instead of the whole clip; needed to cut one recording over several devices with --wiener")
 
 
 def parse_cli(argv, usage):
@@ -120,7 +135,7 @@ def parse_cli(argv, usage):
         print(EXTRA_USAGE)
         sys.exit(2)
     o = {"inputfile": None, "outdir": None, "model": None, "frame_size": None, "window": None, "devices": None, "batch_clips": 1,
-         "keep_channels": False, "wiener": 0}
+         "keep_channels": False, "wiener": 0, "wiener_radius": 0}
     for opt, arg in opts:
         if opt == "-h":
             print(usage)
@@ -144,6 +159,8 @@ def parse_cli(argv, usage):
             o["keep_channels"] = True
         elif opt == "--wiener":
             o["wiener"] = int(arg)
+        elif opt == "--wiener-radius":
+            o["wiener_radius"] = int(arg)
     if o["inputfile"] is None or o["outdir"] is None or o["model"] is None:
         print(usage)
         sys.exit(2)
@@ -153,19 +170,25 @@ def parse_cli(argv, usage):
 def cli_main(argv, usage, train_auto_default, run_one, family=None):
     """`train_auto_default(inputfile, outdir, model)` = the script's literal reference call (no extra flag given);
     `run_one(filein, outdir, model, frame_size, window, device, slot, several_clips)` = the same with the overrides
-    (with --keep-channels also keep_channels=True, and wiener=K with --wiener K; only the DSD100 / hiphopss script,
-    family "dsd", takes them)."""
+    (with --keep-channels also keep_channels=True, wiener=K with --wiener K and wiener_radius=R with --wiener-radius R;
+    only the DSD100 / hiphopss script, family "dsd", takes them)."""
     import sys
     o = parse_cli(argv, usage)
     try:
-        check_stereo_options(family, o["keep_channels"], o["wiener"])
+        check_stereo_options(family, o["keep_channels"], o["wiener"], o["wiener_radius"])
     except ValueError as e:
         sys.exit(str(e))
+    one_over_devices = not os.path.isdir(o["inputfile"]) and len(o["devices"] or []) > 1
+    if o["wiener"] and not o["wiener_radius"] and one_over_devices:
+        sys.exit("--wiener %d over several devices needs --wiener-radius R >= 1: the recording is cut into segments, and "
+                 "whole-clip covariances (wiener_radius 0) need the whole recording in one" % o["wiener"])
     if o["keep_channels"]:
         base = run_one
         kw = {"keep_channels": True}
         if o["wiener"]:
             kw["wiener"] = o["wiener"]
+        if o["wiener_radius"]:
+            kw["wiener_radius"] = o["wiener_radius"]
 
         def run_one(*args):
             return base(*args, **kw)

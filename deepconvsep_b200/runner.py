@@ -122,7 +122,7 @@ def _write_stems(paths, stems, sampleRate, bitrate):
 
 
 def separate_dataset(family, testdir, outdir, model, scale_factor=None, time_context=30, rank=0, world_size=1, device=0,
-                     keep_channels=False, wiener=0, **overrides):
+                     keep_channels=False, wiener=0, wiener_radius=0, **overrides):
     """scale_factor: None = the family's trainer value (0.2 for bach10_score, else 0.3).
     bach10_score: every piece directory of `testdir` (name starting with a digit): the mixture is the sum of its four
     source wavs, the note table comes from its <instrument>_b.txt scores (40 s window, 20 harmonics, +-50 cents,
@@ -130,9 +130,12 @@ def separate_dataset(family, testdir, outdir, model, scale_factor=None, time_con
     keep_channels (family dsd): 2-channel stems in the same layout -- the soft masks of the downmix applied to each
     channel of the mixture (Separator.separate_keep_channels), so that a multichannel evaluation scores real stereo
     images.  wiener (family dsd with keep_channels, or dsd_ild): that many EM iterations of the multichannel Wiener
-    post-filter on the stereo stems."""
-    check_stereo_options(family, keep_channels, wiener)
+    post-filter on the stereo stems; wiener_radius: its covariance window in chunks of 128 frames to either side
+    (0 = the whole song)."""
+    check_stereo_options(family, keep_channels, wiener, wiener_radius)
     wkw = {"wiener": wiener} if wiener else {}
+    if wiener_radius:
+        wkw["wiener_radius"] = wiener_radius
     cfg = dict(TRAINER[family], **overrides)
     if scale_factor is None:
         scale_factor = DEFAULT_SCALE.get(family, 0.3)
@@ -185,9 +188,12 @@ def main(argv=None):
     ap.add_argument("--wiener", type=int, default=0, metavar="K",
                     help="K EM iterations of the multichannel Wiener post-filter on the stereo stems "
                          "(--family dsd --keep-channels, or --family dsd_ild)")
+    ap.add_argument("--wiener-radius", type=int, default=0, metavar="R",
+                    help="with --wiener: spatial covariances over a sliding window of R chunks of 128 frames to either "
+                         "side (default 0: one per song)")
     args = ap.parse_args(argv)
     try:
-        check_stereo_options(args.family, args.keep_channels, args.wiener)
+        check_stereo_options(args.family, args.keep_channels, args.wiener, args.wiener_radius)
     except ValueError as e:
         ap.error(str(e))
     world, rank, local = (int(os.environ.get(k, d)) for k, d in (("WORLD_SIZE", "1"), ("RANK", "0"), ("LOCAL_RANK", "0")))
@@ -201,7 +207,7 @@ def main(argv=None):
     t0 = time.time()
     secs, njobs = separate_dataset(args.family, args.db, args.out, args.model, args.scale_factor, rank=rank,
                                    world_size=world, device=local, keep_channels=args.keep_channels,
-                                   wiener=args.wiener)
+                                   wiener=args.wiener, wiener_radius=args.wiener_radius)
     tot, ms, _ = reduce_stats(secs, (time.time() - t0) * 1e3)
     if rank == 0:
         print("separated %d files, %.1f audio-s in %.2f s (%.0f x real time) on %d GPU(s)" % (njobs, tot, ms / 1e3,

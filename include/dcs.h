@@ -30,6 +30,9 @@ extern "C" {
 
 #define DCS_VERSION 100
 
+/* frames per chunk of the Wiener post-filter's sums over time (dcs_wiener_stereo_windowed) */
+#define DCS_WIENER_CHUNK_FRAMES 128
+
 enum {
   DCS_OK = 0,
   DCS_EINVAL = -1,   /* bad argument / unsupported shape */
@@ -102,6 +105,10 @@ int dcs_set_pool_tap(dcs_ctx* ctx, uint8_t* d_bits, int64_t capacity);
  * spectrum tap then holds the filtered spectra).  Single-channel entry points ignore the setting.  Default 0 (off:
  * the network's spectra, bit for bit); negative values are refused. */
 int dcs_set_wiener(dcs_ctx* ctx, int iterations);
+/* The covariance window of that filter on the same entry points (see dcs_wiener_stereo_windowed): 0 (the default) =
+ * one R_j(f) and one scale for the whole clip, bit for bit the filter without this setting; radius >= 1 = per chunk
+ * of DCS_WIENER_CHUNK_FRAMES frames, from the chunks within `radius` of it.  Negative values are refused. */
+int dcs_set_wiener_radius(dcs_ctx* ctx, int radius);
 
 /* per-stage device timing (CUDA events on the launching stream): enable, run, synchronise the
  * stream, then read.  dcs_profile_read writes up to max_n durations (ms) and the stage names
@@ -397,6 +404,19 @@ int dcs_separate_batch_pcm16_keep_channels_host(dcs_ctx* ctx, dcs_model* model, 
  * anything is queued.  The workspace grows to ~32 bytes per (source, bin) per 128 frames. */
 int dcs_wiener_stereo(dcs_ctx* ctx, const dcs_complex* d_X, int64_t x_plane, dcs_complex* d_S, int64_t src_stride,
                       int nsrc, int64_t num_frames, int64_t ldf, int F, int iterations, void* stream);
+/* The same with a sliding-window spatial covariance.  Chunk k is frames [128k, min(T, 128k + 128)) (128 =
+ * DCS_WIENER_CHUNK_FRAMES), n chunks in all.  radius 0 is dcs_wiener_stereo, bit for bit.  radius W >= 1: chunk c's
+ * window is chunks max(0, c-W) .. min(n-1, c+W), and for every frame of chunk c
+ *     s_c = max(1, max|x| / 10) over the window's frames (both channels, bins < F),
+ *     R_j(f; c) = sum_{t in window} y_j y_j^H / (eps s_c^2 + sum_{t in window} v_j),
+ *     C = sum_j v_j R_j(f; c) + sqrt(eps) s_c^2 I,   y_j <- v_j R_j(f; c) C^-1 x.
+ * Per-chunk sums run in frame order and each window adds them directly in ascending chunk order, so a chunk's filter
+ * depends only on the frames within K*W chunks of it (K = iterations) and W >= n-1 gives the bits of radius 0.
+ * Same launch count (2 * iterations + 1).  The workspace grows by one R and one scale per chunk (~32 bytes per
+ * (source, bin) per chunk more).  A negative radius is refused with the other arguments before anything is queued. */
+int dcs_wiener_stereo_windowed(dcs_ctx* ctx, const dcs_complex* d_X, int64_t x_plane, dcs_complex* d_S,
+                               int64_t src_stride, int nsrc, int64_t num_frames, int64_t ldf, int F, int iterations,
+                               int radius, void* stream);
 
 #ifdef __cplusplus
 }
