@@ -256,6 +256,7 @@ int dcs_stft_plan_destroy(dcs_stft* p) {
 int dcs_stft_forward(dcs_stft* p, const float* d_audio, int64_t L, dcs_complex* d_X, float* d_mag, float mag_scale,
                      int64_t ldf, void* stream) {
   DCS_REQUIRE(p && d_audio && L > 0, "dcs_stft_forward: bad argument");
+  DCS_REQUIRE((uintptr_t)d_X % 8 == 0, "dcs_stft_forward: d_X not 8-byte aligned");
   DCS_CUDA(cudaSetDevice(p->ctx->device));
   return launch_stft(p, d_audio, L, (float2*)d_X, d_mag, nullptr, mag_scale, ldf, (cudaStream_t)stream);
 }
@@ -270,6 +271,14 @@ int dcs_stft_forward_polar(dcs_stft* p, const float* d_audio, int64_t L, float* 
 int dcs_istft(dcs_stft* p, const dcs_complex* d_S, int nsrc, int64_t T, int64_t ldf, int64_t src_stride, float* d_out,
               int64_t Lout, int64_t out_stride, void* stream) {
   DCS_REQUIRE(p && d_S && d_out && T > 0, "dcs_istft: bad argument");
+  DCS_REQUIRE(ldf >= p->N / 2 + 1, "dcs_istft: ldf %lld < F %d", (long long)ldf, p->N / 2 + 1);
+  DCS_REQUIRE(src_stride >= 0 && out_stride >= 0, "dcs_istft: negative stride");
+  // sources must not share spectrum rows (reads past a row) nor output samples (CTAs of two sources race)
+  DCS_REQUIRE(nsrc <= 1 || src_stride >= T * ldf, "dcs_istft: src_stride %lld < num_frames * ldf %lld",
+              (long long)src_stride, (long long)(T * ldf));
+  DCS_REQUIRE(nsrc <= 1 || out_stride >= Lout, "dcs_istft: out_stride %lld < num_out %lld", (long long)out_stride,
+              (long long)Lout);
+  DCS_REQUIRE((uintptr_t)d_S % 8 == 0, "dcs_istft: d_S not 8-byte aligned");
   DCS_CUDA(cudaSetDevice(p->ctx->device));
   return launch_istft(p, (const float2*)d_S, nullptr, nullptr, 1.f, nsrc, T, ldf, src_stride, d_out, Lout, out_stride,
                       (cudaStream_t)stream);
@@ -278,6 +287,7 @@ int dcs_istft(dcs_stft* p, const dcs_complex* d_S, int nsrc, int64_t T, int64_t 
 int dcs_istft_polar(dcs_stft* p, dcs_ctx* ctx, const float* d_mag, const float* d_phase, float mag_scale, int64_t T,
                     int64_t ldf, float* d_out, int64_t Lout, void* stream) {
   DCS_REQUIRE(p && d_mag && d_phase && d_out && T > 0, "dcs_istft_polar: bad argument");
+  DCS_REQUIRE(ldf >= p->N / 2 + 1, "dcs_istft_polar: ldf %lld < F %d", (long long)ldf, p->N / 2 + 1);
   DCS_CUDA(cudaSetDevice(p->ctx->device));
   (void)ctx;
   return launch_istft(p, nullptr, d_mag, d_phase, mag_scale * sqrtf((float)p->N), 1, T, ldf, 0, d_out, Lout, Lout,

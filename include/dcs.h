@@ -130,7 +130,8 @@ int64_t dcs_padded_bins(int frame_size);
 
 /* stft_norm (+ the |X|*scale/sqrt(N) of compute_file, transform.py:243-245, fused):
  * d_audio float[L] -> d_X complex[T][ldf] (may be NULL) and d_mag float[T][ldf] (may be NULL),
- * d_mag = mag_scale * |X| / sqrt(N).  Pad columns F..ldf-1 are written as zeros. */
+ * d_mag = mag_scale * |X| / sqrt(N).  Pad columns F..ldf-1 are written as zeros; F <= ldf <= F + 16.
+ * d_X must be 8-byte aligned (DCS_EINVAL otherwise).  The imaginary parts of the DC and Nyquist bins are +0. */
 int dcs_stft_forward(dcs_stft* plan, const float* d_audio, int64_t num_samples, dcs_complex* d_X,
                      float* d_mag, float mag_scale, int64_t ldf, void* stream);
 /* same analysis, polar output: d_mag = mag_scale*|X|/sqrt(N), d_phase = angle(X)  (compute_file
@@ -140,10 +141,15 @@ int dcs_stft_forward_polar(dcs_stft* plan, const float* d_audio, int64_t num_sam
 /* istft_norm for nsrc spectrograms d_S complex[nsrc][T][ldf] (source stride src_stride elements)
  * -> d_out float[nsrc][out_stride], the first num_out samples of each (= data[:L],
  * separate_dsd.py:305-306; num_out <= (T-1)*hop + N - N/2).  Imaginary parts of the DC and
- * Nyquist bins are ignored like np.fft.irfft does. */
+ * Nyquist bins are ignored like np.fft.irfft does: they are never read into the result, so they
+ * may hold anything, NaN included; so may the pad columns F..ldf-1 and the gaps between sources.
+ * Refused with DCS_EINVAL before anything is queued: ldf < N/2 + 1, a negative stride, d_S not
+ * 8-byte aligned, and with nsrc > 1 src_stride < T*ldf or out_stride < num_out (sources that
+ * share spectrum rows or output samples). */
 int dcs_istft(dcs_stft* plan, const dcs_complex* d_S, int nsrc, int64_t num_frames, int64_t ldf,
               int64_t src_stride, float* d_out, int64_t num_out, int64_t out_stride, void* stream);
-/* compute_inverse (transform.py:271-273): X = mag_scale*sqrt(N)*mag*exp(j*phase) -> istft_norm */
+/* compute_inverse (transform.py:271-273): X = mag_scale*sqrt(N)*mag*exp(j*phase) -> istft_norm;
+ * ldf < N/2 + 1 is DCS_EINVAL */
 int dcs_istft_polar(dcs_stft* plan, dcs_ctx* ctx, const float* d_mag, const float* d_phase,
                     float mag_scale, int64_t num_frames, int64_t ldf, float* d_out, int64_t num_out,
                     void* stream);
