@@ -6,10 +6,10 @@
 // cross-check.
 //
 // GEMM view (D = A * B^T, fp32-accurate 3xTF32):
-//   M = frequency bins  (128 per tile, one 64-row half per warpgroup)
+//   M = frequency bins  (128 per tile, one 64-row half per consumer warpgroup)
 //   N = (frame, patch slot, decoder) per group: 8 x 6 x 3 = 144 columns (DSD100), 4 x 6 x 4 = 96 (stereo net)
 //   K = conv1 filters (50, padded to 56 = 7 k-steps; two 32-wide swizzled planes)
-//   A = W1t tile [128 bins][K]  (weights; split hi/lo into shared memory once per tile and CTA)
+//   A = W1t tile [128 bins][K]  (weights; split hi/lo into shared memory by each consumer for its half, once per tile)
 //   B = G rows   [N][K]         (decoder activations of the patches covering the group's frames,
 //                                gathered from the patch-major G; empty slots are zero rows)
 // The B rows are ordered so that each thread's accumulator fragment holds every value its outputs
@@ -17,12 +17,20 @@
 // from the wgmma registers.
 //
 // Persistent CTAs, one per SM, each over a contiguous range of (tile, group) work items in tile-major
-// order.  B is double-buffered.  Per item, after one barrier: each warpgroup issues the 21 k8 products
-// (the 14 small correction products first, then the 7 main ones, so the truncating accumulation sees
-// only 7 large addends) on stage s as two commit groups, columns of slots 0-2 and of slots 3-5; while
-// they run, every thread issues this item's X loads, splits and stores the prefetched B rows of the next
-// item into stage s^1 and issues the global loads of the item after that; then it runs the mask
-// epilogue from registers, slots 0-2 as soon as the first commit group has landed.
+// order, with three warpgroups:
+//   - the producer (warpgroup 2) loads the B rows of item w + 1 while it splits and stores those of item w
+//     into one of two stages, stages the group's fade-table entries in a ring of four, and arrives on the
+//     stage's `full` mbarrier;
+//   - consumers 0 and 1 each issue the 21 k8 products of their 64 bins as one m64n144k8 (m64n96k8) chain --
+//     the 14 small correction products first, then the 7 main ones, so the truncating accumulation sees
+//     only 7 large addends -- release the stage on its `empty` mbarrier once they are complete, and run
+//     the mask epilogue from registers.  Two named barriers alternate the issue: consumer 1 issues item w
+//     while consumer 0 runs its epilogue of item w, and consumer 0 issues item w + 1 while consumer 1 runs
+//     its epilogue of item w, so one consumer's epilogue runs under the other's products.
+// F = 128 m + 1 (the nets' N / 2 + 1): the tiles cover bins [0, F - 1) and the Nyquist bin, which would
+// take a 128-bin tile of its own, is computed by the producer from the fp32 rows it has loaded: an FMA
+// chain over each thread's 4 k-values and a fixed xor tree over the 16 threads of a row, then the same
+// epilogue arithmetic (mask_slot), for item (tile, g) with tile = g mod m.
 #include "common.cuh"
 #include "tc.cuh"
 
@@ -34,14 +42,21 @@ constexpr int MT_BINS = 128;             // bins per tile
 constexpr int MT_SLOTS = 6;              // patch slots per frame
 constexpr int MT_C1 = 50;
 constexpr int MT_KSTEPS = 7;             // ceil(50 / 8)
-constexpr int MT_THREADS = 256;          // two warpgroups
+constexpr int MT_CONSUMERS = 256;        // warpgroups 0 and 1: one 64-bin half of the tile each
+constexpr int MT_PRODUCER = 128;         // warpgroup 2: B rows (and the Nyquist bin)
+constexpr int MT_THREADS = MT_CONSUMERS + MT_PRODUCER;
 constexpr int MT_A_SUB = MT_BINS * ROW_BYTES;      // 16 KB: [128][32] fp32
 constexpr int MT_A_BYTES = 4 * MT_A_SUB;           // hi k0-31, hi k32-63, lo k0-31, lo k32-63
+// named barriers
+constexpr int MT_BAR_TURN1 = 1;          // consumer 1 may issue item w: consumer 0 has issued it
+constexpr int MT_BAR_TURN0 = 2;          // consumer 0 may issue item w + 1: consumer 1 has issued item w
+constexpr int MT_BAR_PROD = 3;           // the producer's Nyquist dot products are in shared memory
+constexpr int MT_BAR_A = 4;              // + consumer: its A half of a new tile is stored
 
 // NDEC = 3: the DSD100 / hiphopss net (4th output = decoder 2 with its own bias, all-zero bins get 1/4 each,
-//           separate_dsd.py:228,258-266), 8 frames per group, 144 columns (two m64n72k8 halves);
+//           separate_dsd.py:228,258-266), 8 frames per group, 144 columns (m64n144k8);
 // NDEC = 4: the stereo / ILD net, one launch per input channel (one decoder per source, all-zero bins get 0,
-//           trainCNN_ILD_DSD100.py:99-106,183-186), 4 frames per group, 96 columns (two m64n48k8 halves).
+//           trainCNN_ILD_DSD100.py:99-106,183-186), 4 frames per group, 96 columns (m64n96k8).
 // NX: mixture channels the cross-faded masks are applied to -- 1, or 2 with NDEC = 3 (stereo stems from the masks of
 //     the downmix: the same m times each channel's X; GEMM, gather and cross-fade run once).
 // Value v = slot * NDEC + decoder.  Fragment (tc.cuh): d[4j + 2i + e] = D[16w + l/4 + 8i][8j + 2(l%4) + e].
@@ -51,27 +66,34 @@ template <int NDEC>
 struct MaskTile {
   static constexpr int FRAMES = NDEC == 3 ? 8 : 4;
   static constexpr int COLS = FRAMES * MT_SLOTS * NDEC;         // 144 or 96
-  static constexpr int HCOLS = COLS / 2;                        // columns of slots 0-2 (and of slots 3-5)
   static constexpr int TFRAMES = NDEC == 3 ? 2 : 1;             // frames per thread
   static constexpr int B_SUB = COLS * ROW_BYTES;
   static constexpr int B_BYTES = 4 * B_SUB;                     // one stage: the same four planes as A
-  static constexpr int B_CHUNKS = COLS * 16 / MT_THREADS;       // 16-byte pieces of B per thread and group: 9 or 6
-  static constexpr int SMEM = MT_A_BYTES + 2 * B_BYTES + 1024;  // + alignment slack
-  __device__ static int col_frame(int c) { return NDEC == 3 ? (c & 7) : (c & 7) >> 1; }
-  __device__ static int col_value(int c) { return NDEC == 3 ? c >> 3 : 2 * (c >> 3) + (c & 1); }
+  static constexpr int B_CHUNKS = COLS * 16 / MT_PRODUCER;      // 16-byte pieces of B per producer thread and group: 18 or 12
+  static constexpr int HCHUNKS = B_CHUNKS / 2;                  // loaded and stored in two halves
+  static constexpr int NYQ_BYTES = 2 * COLS * 4;                // two buffers of the Nyquist bin's GEMM values
+  static constexpr int XF = FRAMES * MT_SLOTS;                  // fade-table entries of a group
+  static constexpr int XF_BYTES = 4 * XF * 16;                  // a ring of four groups' entries
+  static constexpr int SMEM = MT_A_BYTES + 2 * B_BYTES + NYQ_BYTES + XF_BYTES + 1024;   // + alignment slack
+  __host__ __device__ static constexpr int col_frame(int c) { return NDEC == 3 ? (c & 7) : (c & 7) >> 1; }
+  __host__ __device__ static constexpr int col_value(int c) { return NDEC == 3 ? c >> 3 : 2 * (c >> 3) + (c & 1); }
+  // the column of (frame f, value v), the inverse of col_frame / col_value
+  __host__ __device__ static constexpr int col(int f, int v) { return NDEC == 3 ? 8 * v + f : 8 * (v >> 1) + 2 * f + (v & 1); }
   // frame of the thread's e-th frame (lane = l)
   __device__ static int thread_frame(int lane, int e) { return NDEC == 3 ? 2 * (lane & 3) + e : lane & 3; }
-  // accumulator register of (row half i, thread frame e, value v) in the fragment of the column half holding v
+  // accumulator register of (row half i, thread frame e, value v)
   __host__ __device__ static constexpr int acc(int i, int e, int v) { return NDEC == 3 ? 4 * v + 2 * i + e : 4 * (v >> 1) + 2 * i + (v & 1); }
 };
 
-// A tile: thread = bin row (threads 0..127), W1t is [c][bin] so the reads are coalesced over bins
-__device__ __forceinline__ void mask_load_a(const DsdMaskArgs& a, int tile, int tid, uint8_t* sA) {
-  if (tid >= MT_BINS) return;
-  const int b = tile * MT_BINS + tid;
+// one consumer warpgroup's 64 rows of the A tile: thread = (bin row, k half); W1t is [c][bin], so the reads are
+// coalesced over bins
+__device__ __forceinline__ void mask_load_a(const DsdMaskArgs& a, int tile, int wg, int wtid, uint8_t* sA) {
+  const int r = wg * 64 + (wtid & 63), kh = wtid >> 6;
+  const int b = tile * MT_BINS + r;
   const bool ok = b < a.F;
 #pragma unroll
-  for (int c4 = 0; c4 < 16; ++c4) {
+  for (int c8 = 0; c8 < 8; ++c8) {
+    const int c4 = 8 * kh + c8;
     float e[4], hi[4], lo[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -79,25 +101,26 @@ __device__ __forceinline__ void mask_load_a(const DsdMaskArgs& a, int tile, int 
       e[i] = (ok && c < MT_C1) ? __ldg(a.W1t + (int64_t)c * a.ldw + b) : 0.f;
       split_tf32(e[i], hi[i], lo[i]);
     }
-    const uint32_t off = (c4 >> 3) * MT_A_SUB + tile_off(tid, c4 & 7);
+    const uint32_t off = kh * MT_A_SUB + tile_off(r, c8);
     *reinterpret_cast<float4*>(sA + off) = make_float4(hi[0], hi[1], hi[2], hi[3]);
     *reinterpret_cast<float4*>(sA + 2 * MT_A_SUB + off) = make_float4(lo[0], lo[1], lo[2], lo[3]);
   }
 }
 
-// B rows of group g: row r = GEMM column (MaskTile::col_frame / col_value), 16 float4 per row (columns
-// 52..63 are zero).  The patch in slot j of frame t is k_lo(t) + j; an empty slot is a zero row.
-template <int NDEC>
-__device__ __forceinline__ void mask_load_b(const DsdMaskArgs& a, int g, int tid, float4 (&rb)[MaskTile<NDEC>::B_CHUNKS]) {
+// B rows of group g, chunks [I0, I0 + HCHUNKS) of producer thread ptid: row r = GEMM column (MaskTile::col_frame /
+// col_value), 16 float4 per row (columns 52..63 are zero).  The patch in slot j of frame t is k_lo(t) + j; an empty
+// slot is a zero row.
+template <int NDEC, int I0>
+__device__ __forceinline__ void mask_load_b(const DsdMaskArgs& a, int g, int ptid, float4 (&rb)[MaskTile<NDEC>::HCHUNKS]) {
   using MT = MaskTile<NDEC>;
   const int step = a.tc - a.overlap;
-  // chunk i covers row 16 i + tid / 16: the frame (row % 8 decides it) is the same for all of a thread's chunks
-  const int t = g * MT::FRAMES + MT::col_frame(tid >> 4), c4 = tid & 15;
+  // chunk i covers row 8 i + ptid / 16: the frame (row % 8 decides it) is the same for all of a thread's chunks
+  const int t = g * MT::FRAMES + MT::col_frame(ptid >> 4), c4 = ptid & 15;
   int k_lo = t - a.tc + 1;
   k_lo = k_lo > 0 ? (k_lo + step - 1) / step : 0;
 #pragma unroll
-  for (int i = 0; i < MT::B_CHUNKS; ++i) {
-    const int v = MT::col_value(16 * i + (tid >> 4)), j = v / NDEC, d = v - j * NDEC;
+  for (int i = 0; i < MT::HCHUNKS; ++i) {
+    const int v = MT::col_value(8 * (I0 + i) + (ptid >> 4)), j = v / NDEC, d = v - j * NDEC;
     const int k = k_lo + j;
     rb[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (c4 < 13 && t < a.T && k < a.P && k * step <= t) {
@@ -107,13 +130,13 @@ __device__ __forceinline__ void mask_load_b(const DsdMaskArgs& a, int g, int tid
   }
 }
 
-// the prefetched B rows, split into hi/lo planes, into one stage
-template <int NDEC>
-__device__ __forceinline__ void mask_store_b(uint8_t* sB, int tid, const float4 (&rb)[MaskTile<NDEC>::B_CHUNKS]) {
+// chunks [I0, I0 + HCHUNKS) of the loaded B rows, split into hi/lo planes, into one stage
+template <int NDEC, int I0>
+__device__ __forceinline__ void mask_store_b(uint8_t* sB, int ptid, const float4 (&rb)[MaskTile<NDEC>::HCHUNKS]) {
   using MT = MaskTile<NDEC>;
 #pragma unroll
-  for (int i = 0; i < MT::B_CHUNKS; ++i) {
-    const int idx = i * MT_THREADS + tid, r = idx >> 4, c4 = idx & 15;
+  for (int i = 0; i < MT::HCHUNKS; ++i) {
+    const int idx = (I0 + i) * MT_PRODUCER + ptid, r = idx >> 4, c4 = idx & 15;
     float h[4], l[4];
     split_tf32(rb[i].x, h[0], l[0]); split_tf32(rb[i].y, h[1], l[1]);
     split_tf32(rb[i].z, h[2], l[2]); split_tf32(rb[i].w, h[3], l[3]);
@@ -123,72 +146,197 @@ __device__ __forceinline__ void mask_store_b(uint8_t* sB, int tid, const float4 
   }
 }
 
+// the Nyquist bin's GEMM value of every column of chunks [I0, I0 + HCHUNKS) from the loaded fp32 B rows: each thread
+// an FMA chain over its 4 of the 50 k-values (wn = W1t[k][F - 1]), then a fixed xor tree over the 16 threads of the row
+template <int NDEC, int I0>
+__device__ __forceinline__ void mask_nyquist_dots(const float4 (&rb)[MaskTile<NDEC>::HCHUNKS], const float (&wn)[4], int ptid,
+                                                  float* nyq) {
+  using MT = MaskTile<NDEC>;
+  const int c4 = ptid & 15;
+#pragma unroll
+  for (int i = 0; i < MT::HCHUNKS; ++i) {
+    float d = rb[i].x * wn[0];
+    d = fmaf(rb[i].y, wn[1], d);
+    if (c4 < 12) {   // k = 50, 51 of the last chunk are padding
+      d = fmaf(rb[i].z, wn[2], d);
+      d = fmaf(rb[i].w, wn[3], d);
+    }
+    d += __shfl_xor_sync(0xffffffffu, d, 8);
+    d += __shfl_xor_sync(0xffffffffu, d, 4);
+    d += __shfl_xor_sync(0xffffffffu, d, 2);
+    d += __shfl_xor_sync(0xffffffffu, d, 1);
+    if (c4 == 0) nyq[8 * (I0 + i) + (ptid >> 4)] = d;
+  }
+}
+
+// one patch slot of the cross-fade: bias + ReLU + soft ratio mask, then mm <- down * mm + up * mask with
+// c = (up, down, up/4, -) of (frame, slot) (dsd_xfade_table_kernel).  y3 is the 4th source's GEMM value (DSD100:
+// decoder 2 again, separate_dsd.py:228).  The tensor-core bins and the Nyquist bin share it.
+template <int NDEC>
+__device__ __forceinline__ void mask_slot(const float4 c, float y0, float y1, float y2, float y3, float bo0, float bo1, float bo2,
+                                          float bo3, bool first, float (&mm)[4]) {
+  const float p0 = fmaxf(y0 + bo0, 0.f);
+  const float p1 = fmaxf(y1 + bo1, 0.f);
+  const float p2 = fmaxf(y2 + bo2, 0.f);
+  const float p3 = fmaxf(y3 + bo3, 0.f);
+  const float tot = (p0 + p1) + (p2 + p3);
+  const bool pos = tot > MASK_TOT_MIN;
+  float rc;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rc) : "f"(tot));
+  const float r = pos ? c.x * rc : 0.f;             // up * mask = p * (up / tot)
+  const float q = (pos || NDEC == 4) ? 0.f : c.z;   // all-zero bin: 1/4 each (DSD100 rule); 0 (ILD rule)
+  mm[0] = fmaf(c.y, first ? 0.f : mm[0], fmaf(p0, r, q));
+  mm[1] = fmaf(c.y, first ? 0.f : mm[1], fmaf(p1, r, q));
+  mm[2] = fmaf(c.y, first ? 0.f : mm[2], fmaf(p2, r, q));
+  mm[3] = fmaf(c.y, first ? 0.f : mm[3], fmaf(p3, r, q));
+}
+
+// the Nyquist bin of frame t from the producer's dot products of its group (f = frame in the group, xf = the group's
+// fade-table entries)
+template <int NDEC, int NX>
+__device__ __forceinline__ void mask_nyquist_epilogue(const DsdMaskArgs& a, const float4* xf, int t, int f, const float* nyq,
+                                                      float bo0, float bo1, float bo2, float bo3) {
+  using MT = MaskTile<NDEC>;
+  if (t >= a.T) return;
+  float mm[4];
+#pragma unroll
+  for (int j = 0; j < MT_SLOTS; ++j) {
+    const float4 c = xf[f * MT_SLOTS + j];
+    mask_slot<NDEC>(c, nyq[MT::col(f, NDEC * j + 0)], nyq[MT::col(f, NDEC * j + 1)], nyq[MT::col(f, NDEC * j + 2)],
+                    nyq[MT::col(f, NDEC * j + (NDEC == 3 ? 1 : 3))], bo0, bo1, bo2, bo3, j == 0, mm);
+  }
+  const int bin = a.F - 1;
+#pragma unroll
+  for (int c = 0; c < NX; ++c) {
+    const float2 xx = a.X[c * a.x_plane + (int64_t)t * a.ldf + bin];
+    const int64_t o = (int64_t)t * a.ldf + bin + c * a.src_stride;
+    a.S[o] = make_float2(mm[0] * xx.x, mm[0] * xx.y);
+    a.S[o + NX * a.src_stride] = make_float2(mm[1] * xx.x, mm[1] * xx.y);
+    a.S[o + 2 * NX * a.src_stride] = make_float2(mm[2] * xx.x, mm[2] * xx.y);
+    a.S[o + 3 * NX * a.src_stride] = make_float2(mm[3] * xx.x, mm[3] * xx.y);
+  }
+}
+
+// nyq_tiles > 0: the tiles cover bins [0, F - 1) and item (tile, g) with tile == g % nyq_tiles also computes bin F - 1
+// of group g on the producer; 0: the tiles cover all F bins.
 template <int NDEC, int NX>
 __global__ void __launch_bounds__(MT_THREADS, 1)
-dsd_mask_tc_kernel(const DsdMaskArgs a, const float4* __restrict__ xtab, int num_groups, int num_items) {
+dsd_mask_tc_kernel(const DsdMaskArgs a, const float4* __restrict__ xtab, int num_groups, int num_items, int nyq_tiles) {
   using MT = MaskTile<NDEC>;
   constexpr int FRAMES = MT::FRAMES, TF = MT::TFRAMES;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
+  __shared__ uint64_t full_bar[2], empty_bar[2];
   uint8_t* smem = align1024(smem_raw);
   uint8_t* sA = smem;
   uint8_t* sB = smem + MT_A_BYTES;   // two stages of MT::B_BYTES
+  float* sNyq = reinterpret_cast<float*>(sB + 2 * MT::B_BYTES);   // two buffers of MT::COLS
+  float4* sXf = reinterpret_cast<float4*>(sNyq + 2 * MT::COLS);   // fade-table entries of item w at (w - w_begin) % 4
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int wg = warp >> 2, wq = warp & 3;
   // work items w = tile * num_groups + group; this CTA's share [w_begin, w_end) differs from the others' by at most one
   const int w_begin = (int)((int64_t)blockIdx.x * num_items / gridDim.x);
   const int w_end = (int)((int64_t)(blockIdx.x + 1) * num_items / gridDim.x);
-  const int row0 = wg * 64 + wq * 16 + (lane >> 2);   // tile rows row0 and row0 + 8 are this thread's bins
   const float bo0 = __ldg(a.bout + 0), bo1 = __ldg(a.bout + 1), bo2 = __ldg(a.bout + 2), bo3 = __ldg(a.bout + 3);
-
-  float4 rb[MT::B_CHUNKS];
-  if (w_begin < w_end) {
-    mask_load_b<NDEC>(a, w_begin % num_groups, tid, rb);
-    mask_store_b<NDEC>(sB, tid, rb);
-    fence_proxy_async();
-    if (w_begin + 1 < w_end) mask_load_b<NDEC>(a, (w_begin + 1) % num_groups, tid, rb);
-  }
-  int tile = -1;
-  for (int w = w_begin, s = 0; w < w_end; ++w, s ^= 1) {
-    const int g = w % num_groups;
-    // publishes stage s; every warpgroup has waited for its MMAs of item w - 1, so stage s^1 and A are free
-    __syncthreads();
-    if (w / num_groups != tile) {
-      tile = w / num_groups;
-      mask_load_a(a, tile, tid, sA);
-      fence_proxy_async();
-      __syncthreads();
+  if (tid == 0) {
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(&full_bar[s], MT_PRODUCER);        // every producer thread, after its stores
+      mbar_init(&empty_bar[s], MT_CONSUMERS / 32); // every consumer warp, once its products on the stage are complete
     }
+    fence_barrier_init();
+  }
+  __syncthreads();
 
-    // ---- MMAs: warpgroup wg computes bins [64 wg, 64 wg + 64) x MT::COLS columns, as two commit groups:
-    //      columns [0, HCOLS) hold slots 0-2, [HCOLS, COLS) slots 3-5
-    float acc[2][MT::HCOLS / 2];
-    {
-      const uint32_t a_hi = smem_u32(sA) + wg * 64 * ROW_BYTES, a_lo = a_hi + 2 * MT_A_SUB;
-      wgmma_fence();
+  if (wg == 2) {
+    // ---- producer: B rows of item w into stage (w - w_begin) % 2 once the consumers have released it
+    const int ptid = tid - MT_CONSUMERS;
+    float wn[4];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const uint32_t b_hi = smem_u32(sB + s * MT::B_BYTES) + h * (MT::HCOLS / 8) * SBO, b_lo = b_hi + 2 * MT::B_SUB;
-#pragma unroll
-        for (int j = 0; j < MT_KSTEPS; ++j) {
-          const uint32_t ao = (j >> 2) * MT_A_SUB + KSTEP_BYTES * (j & 3), bo = (j >> 2) * MT::B_SUB + KSTEP_BYTES * (j & 3);
-          wgmma_tf32<MT::HCOLS>(acc[h], make_desc(a_lo + ao), make_desc(b_hi + bo), j != 0);
-        }
-#pragma unroll
-        for (int j = 0; j < MT_KSTEPS; ++j) {
-          const uint32_t ao = (j >> 2) * MT_A_SUB + KSTEP_BYTES * (j & 3), bo = (j >> 2) * MT::B_SUB + KSTEP_BYTES * (j & 3);
-          wgmma_tf32<MT::HCOLS>(acc[h], make_desc(a_hi + ao), make_desc(b_lo + bo), 1);
-        }
-#pragma unroll
-        for (int j = 0; j < MT_KSTEPS; ++j) {
-          const uint32_t ao = (j >> 2) * MT_A_SUB + KSTEP_BYTES * (j & 3), bo = (j >> 2) * MT::B_SUB + KSTEP_BYTES * (j & 3);
-          wgmma_tf32<MT::HCOLS>(acc[h], make_desc(a_hi + ao), make_desc(b_hi + bo), 1);
-        }
-        wgmma_commit();
+    for (int i = 0; i < 4; ++i) {
+      const int c = 4 * (ptid & 15) + i;
+      wn[i] = (nyq_tiles > 0 && c < MT_C1) ? __ldg(a.W1t + (int64_t)c * a.ldw + a.F - 1) : 0.f;
+    }
+    // item w + 1's loads are in flight while item w is stored and while the producer waits for the next stage
+    constexpr int H = MT::HCHUNKS;
+    float4 r0[H], r1[H], xf = make_float4(0.f, 0.f, 0.f, 0.f);
+    const bool xf_thread = ptid < MT::XF;
+    if (w_begin < w_end) {
+      mask_load_b<NDEC, 0>(a, w_begin % num_groups, ptid, r0);
+      mask_load_b<NDEC, H>(a, w_begin % num_groups, ptid, r1);
+      if (xf_thread) xf = __ldg(xtab + (int64_t)(w_begin % num_groups) * MT::XF + ptid);
+    }
+    int nb = 0;
+    for (int w = w_begin, it = 0; w < w_end; ++w, ++it) {
+      const int s = it & 1, g = w % num_groups, gn = (w + 1) % num_groups;
+      const bool nyq_item = nyq_tiles > 0 && w / num_groups == g % nyq_tiles;
+      float* nq = sNyq + nb * MT::COLS;   // buffer nb was last read before the previous Nyquist item's barrier
+      if (it >= 2) mbar_wait_relaxed(&empty_bar[s], ((it >> 1) - 1) & 1);
+      mask_store_b<NDEC, 0>(sB + s * MT::B_BYTES, ptid, r0);
+      if (nyq_item) mask_nyquist_dots<NDEC, 0>(r0, wn, ptid, nq);
+      if (w + 1 < w_end) mask_load_b<NDEC, 0>(a, gn, ptid, r0);
+      mask_store_b<NDEC, H>(sB + s * MT::B_BYTES, ptid, r1);
+      if (nyq_item) mask_nyquist_dots<NDEC, H>(r1, wn, ptid, nq);
+      if (w + 1 < w_end) mask_load_b<NDEC, H>(a, gn, ptid, r1);
+      // the consumers' epilogue of item w - 4, the last reader of this ring slot, precedes their release of item w - 2
+      if (xf_thread) sXf[(it & 3) * MT::XF + ptid] = xf;
+      if (xf_thread && w + 1 < w_end) xf = __ldg(xtab + (int64_t)gn * MT::XF + ptid);
+      fence_proxy_async();
+      mbar_arrive(&full_bar[s]);
+      if (nyq_item) {
+        nb ^= 1;
+        bar_sync(MT_BAR_PROD, MT_PRODUCER);
+        if (ptid < FRAMES) mask_nyquist_epilogue<NDEC, NX>(a, sXf + (it & 3) * MT::XF, g * FRAMES + ptid, ptid, nq, bo0, bo1, bo2, bo3);
       }
     }
+    return;
+  }
 
-    // ---- while they run: this item's X (of every channel), B of item w + 1 into stage s^1, global loads of item w + 2
+  // ---- consumers, phase-shifted by half an item: consumer 1 issues its products of item w while consumer 0 runs
+  //      the epilogue of item w, and consumer 0 issues item w + 1 while consumer 1 runs the epilogue of item w
+  const int row0 = wg * 64 + wq * 16 + (lane >> 2);   // tile rows row0 and row0 + 8 are this thread's bins
+  int tile = -1;
+  for (int w = w_begin, it = 0; w < w_end; ++w, ++it) {
+    const int s = it & 1, g = w % num_groups;
+    if (w / num_groups != tile) {
+      // this warpgroup's products of the previous item are complete: its A half is free
+      tile = w / num_groups;
+      mask_load_a(a, tile, wg, tid & 127, sA);
+      fence_proxy_async();
+      bar_sync(MT_BAR_A + wg, 128);
+    }
+    mbar_wait(&full_bar[s], (it >> 1) & 1);
+    if (wg == 1) bar_sync(MT_BAR_TURN1, MT_CONSUMERS);
+    else if (it > 0) bar_sync(MT_BAR_TURN0, MT_CONSUMERS);
+
+    // ---- MMAs: bins [64 wg, 64 wg + 64) x MT::COLS columns, the 14 small correction products first, then the 7
+    //      main ones, so the truncating accumulation sees only 7 large addends
+    float acc[MT::COLS / 2];
+    {
+      const uint32_t a_hi = smem_u32(sA) + wg * 64 * ROW_BYTES, a_lo = a_hi + 2 * MT_A_SUB;
+      const uint32_t b_hi = smem_u32(sB + s * MT::B_BYTES), b_lo = b_hi + 2 * MT::B_SUB;
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < MT_KSTEPS; ++j) {
+        const uint32_t ao = (j >> 2) * MT_A_SUB + KSTEP_BYTES * (j & 3), bo = (j >> 2) * MT::B_SUB + KSTEP_BYTES * (j & 3);
+        wgmma_tf32<MT::COLS>(acc, make_desc(a_lo + ao), make_desc(b_hi + bo), j != 0);
+      }
+#pragma unroll
+      for (int j = 0; j < MT_KSTEPS; ++j) {
+        const uint32_t ao = (j >> 2) * MT_A_SUB + KSTEP_BYTES * (j & 3), bo = (j >> 2) * MT::B_SUB + KSTEP_BYTES * (j & 3);
+        wgmma_tf32<MT::COLS>(acc, make_desc(a_hi + ao), make_desc(b_lo + bo), 1);
+      }
+#pragma unroll
+      for (int j = 0; j < MT_KSTEPS; ++j) {
+        const uint32_t ao = (j >> 2) * MT_A_SUB + KSTEP_BYTES * (j & 3), bo = (j >> 2) * MT::B_SUB + KSTEP_BYTES * (j & 3);
+        wgmma_tf32<MT::COLS>(acc, make_desc(a_hi + ao), make_desc(b_hi + bo), 1);
+      }
+      wgmma_commit();
+    }
+    if (wg == 0) bar_arrive(MT_BAR_TURN1, MT_CONSUMERS);
+    else if (w + 1 < w_end) bar_arrive(MT_BAR_TURN0, MT_CONSUMERS);
+
+    // ---- while they run: this item's X (of every channel)
     int bin[2];
     bool bok[2];
 #pragma unroll
@@ -206,50 +354,22 @@ dsd_mask_tc_kernel(const DsdMaskArgs a, const float4* __restrict__ xtab, int num
         for (int i = 0; i < 2; ++i)
           x[c][e][i] = (bok[i] && t < a.T) ? a.X[c * a.x_plane + (int64_t)t * a.ldf + bin[i]] : make_float2(0.f, 0.f);
       }
-    if (w + 1 < w_end) {
-      mask_store_b<NDEC>(sB + (s ^ 1) * MT::B_BYTES, tid, rb);
-      fence_proxy_async();
-    }
-    if (w + 2 < w_end) mask_load_b<NDEC>(a, (w + 2) % num_groups, tid, rb);
+    wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    if (lane == 0) mbar_arrive(&empty_bar[s]);
 
-    // ---- epilogue per (bin, frame): bias + ReLU + ratio mask + sequential cross-fade + .X; slots 0-2 run
-    //      while the MMAs of slots 3-5 are still in flight
+    // ---- epilogue per (bin, frame): bias + ReLU + ratio mask + sequential cross-fade + .X
     float m[TF][2][4];   // cross-faded masks of the 4 sources
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      if (h == 0) {
-        wgmma_wait<1>();
-        wgmma_fence_acc(acc[0]);
-      } else {
-        wgmma_wait<0>();
-        wgmma_fence_acc(acc[1]);
-      }
+    for (int e = 0; e < TF; ++e) {
+      const float4* xf = sXf + (it & 3) * MT::XF + MT::thread_frame(lane, e) * MT_SLOTS;   // the frame's (up, down, up/4, -)
 #pragma unroll
-      for (int e = 0; e < TF; ++e) {
-        const int t = g * FRAMES + MT::thread_frame(lane, e);
+      for (int i = 0; i < 2; ++i) {
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-#pragma unroll
-          for (int jj = 0; jj < MT_SLOTS / 2; ++jj) {
-            const int j = h * (MT_SLOTS / 2) + jj;
-            // (up, down, up/4, -) of (frame, slot) (dsd_xfade_table_kernel): m <- down*m + up*mask
-            const float4 c = __ldg(xtab + (int64_t)t * MT_SLOTS + j);
-            const float p0 = fmaxf(acc[h][MT::acc(i, e, NDEC * jj + 0)] + bo0, 0.f);
-            const float p1 = fmaxf(acc[h][MT::acc(i, e, NDEC * jj + 1)] + bo1, 0.f);
-            const float p2 = fmaxf(acc[h][MT::acc(i, e, NDEC * jj + 2)] + bo2, 0.f);
-            const float p3 = fmaxf(acc[h][MT::acc(i, e, NDEC * jj + (NDEC == 3 ? 1 : 3))] + bo3, 0.f);   // DSD100: decoder 2 again (separate_dsd.py:228)
-            const float tot = (p0 + p1) + (p2 + p3);
-            const bool pos = tot > 1.2e-38f;
-            float rc;
-            asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(rc) : "f"(tot));
-            const float r = pos ? c.x * rc : 0.f;             // up * mask = p * (up / tot)
-            const float q = (pos || NDEC == 4) ? 0.f : c.z;   // all-zero bin: 1/4 each (DSD100 rule); 0 (ILD rule)
-            float* mm = m[e][i];
-            mm[0] = fmaf(c.y, j == 0 ? 0.f : mm[0], fmaf(p0, r, q));
-            mm[1] = fmaf(c.y, j == 0 ? 0.f : mm[1], fmaf(p1, r, q));
-            mm[2] = fmaf(c.y, j == 0 ? 0.f : mm[2], fmaf(p2, r, q));
-            mm[3] = fmaf(c.y, j == 0 ? 0.f : mm[3], fmaf(p3, r, q));
-          }
+        for (int j = 0; j < MT_SLOTS; ++j) {
+          const float4 c = xf[j];
+          mask_slot<NDEC>(c, acc[MT::acc(i, e, NDEC * j + 0)], acc[MT::acc(i, e, NDEC * j + 1)], acc[MT::acc(i, e, NDEC * j + 2)],
+                          acc[MT::acc(i, e, NDEC * j + (NDEC == 3 ? 1 : 3))], bo0, bo1, bo2, bo3, j == 0, m[e][i]);
         }
       }
     }
@@ -303,12 +423,14 @@ bool dsd_mask_tc_supported(const DsdMaskArgs& a) {
          ((uintptr_t)a.G % 16 == 0);
 }
 
-// all F bins; the last 128-bin tile holds only the Nyquist bin (F = 2^k + 1)
+// F = 128 m + 1 (the DSD nets' F = N / 2 + 1) with m >= 1: m tiles, and the producer computes the Nyquist bin, which
+// would otherwise take a tile of its own; any other F: ceil(F / 128) tiles
 template <int NDEC, int NX>
 static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st) {
   using MT = MaskTile<NDEC>;
   DCS_TRY(ensure_smem_attr(dsd_mask_tc_kernel<NDEC, NX>, MT::SMEM));
-  const int m_tiles = (a.F + MT_BINS - 1) / MT_BINS;
+  const bool nyq = a.F > MT_BINS && (a.F - 1) % MT_BINS == 0;
+  const int m_tiles = nyq ? (a.F - 1) / MT_BINS : (a.F + MT_BINS - 1) / MT_BINS;
   const int num_groups = (a.T + MT::FRAMES - 1) / MT::FRAMES;
   const int num_items = m_tiles * num_groups;
   const int ctas = std::min(ctx->num_sms, num_items);
@@ -318,7 +440,7 @@ static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t
   dsd_xfade_table_kernel<<<(unsigned)ceil_div64((int64_t)Tpad * MT_SLOTS, 256), 256, 0, st>>>(xtab, a.T, Tpad, a.P, a.tc, a.overlap);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
-  dsd_mask_tc_kernel<NDEC, NX><<<(unsigned)ctas, MT_THREADS, MT::SMEM, st>>>(a, xtab, num_groups, num_items);
+  dsd_mask_tc_kernel<NDEC, NX><<<(unsigned)ctas, MT_THREADS, MT::SMEM, st>>>(a, xtab, num_groups, num_items, nyq ? m_tiles : 0);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;
