@@ -488,12 +488,18 @@ static int dsd_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaS
       continue;
     }
     for (int c = 0; c < n.nx; ++c) {   // ch + c: the channel (nch and n.nx are never both 2)
-      a.X = n.X + (ch + c) * n.x_plane; a.S = n.S + (ch + c) * n.src_stride; a.src_stride = nplanes * n.src_stride; a.nx = 1;
+      a.src_stride = nplanes * n.src_stride; a.nx = 1;
+      float* M = nullptr;   // masks mode: plane (s * nch + ch), the layout of the spectra
+      if (n.M) {
+        a.X = nullptr; a.S = nullptr; M = n.M + (ch + c) * n.src_stride;
+      } else {
+        a.X = n.X + (ch + c) * n.x_plane; a.S = n.S + (ch + c) * n.src_stride;
+      }
       if (tc_path) {
         DCS_REQUIRE(dsd_mask_tc_supported(a), "dsd_forward: tensor-core mask kernel does not take this shape");
-        DCS_TRY(launch_dsd_mask_tc(ctx, a, st));
+        DCS_TRY(launch_dsd_mask_tc(ctx, a, st, M));
       } else {
-        DCS_TRY(launch_dsd_mask(ctx, a, st));
+        DCS_TRY(launch_dsd_mask(ctx, a, st, M));
       }
     }
   }
@@ -502,17 +508,24 @@ static int dsd_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaS
 
 // the network stage of every entry point: the input planes (plane stride in_plane) and the mixture STFT
 // (channel stride x_plane) -> masked spectra, nsrc x nch planes of stride src_stride; nx = 2 (DSD100 net only): the
-// masks applied to two mixture channels, nsrc x 2 planes (source, channel)
+// masks applied to two mixture channels, nsrc x 2 planes (source, channel).  M (masks mode, nx = 1): the blended masks
+// instead, float planes ordered like the spectra, bins < F of each frame written; X and S are not used
 static int run_network(dcs_ctx* ctx, const dcs_model* m, const float* in, int64_t in_plane, const float2* X, int64_t x_plane,
-                       int nx, int64_t T, int64_t ldf, int overlap, int patcher, float2* S, int64_t src_stride, cudaStream_t st) {
+                       int nx, int64_t T, int64_t ldf, int overlap, int patcher, float2* S, int64_t src_stride, cudaStream_t st,
+                       float* M = nullptr) {
   const bool dsd = m->arch == DCS_ARCH_DSD || m->arch == DCS_ARCH_DSD_ILD;
   NetCall n;
   n.P = dcs_num_patches(T, m->tc, overlap, patcher);
-  if (n.P == 0) {  // clip shorter than one patch: nothing is predicted, every stem is silence
-    for (int s = 0; s < m->nsrc * m->nch * nx; ++s) DCS_CUDA(cudaMemsetAsync(S + s * src_stride, 0, (size_t)T * ldf * sizeof(float2), st));
+  if (n.P == 0) {  // clip shorter than one patch: nothing is predicted, every stem is silence (every mask 0)
+    for (int s = 0; s < m->nsrc * m->nch * nx; ++s) {
+      if (M)
+        DCS_CUDA(cudaMemset2DAsync(M + s * src_stride, (size_t)ldf * sizeof(float), 0, (size_t)m->F * sizeof(float), (size_t)T, st));
+      else
+        DCS_CUDA(cudaMemsetAsync(S + s * src_stride, 0, (size_t)T * ldf * sizeof(float2), st));
+    }
     return DCS_OK;
   }
-  n.in = in; n.in_plane = in_plane; n.X = X; n.x_plane = x_plane; n.nx = nx; n.S = S; n.src_stride = src_stride;
+  n.in = in; n.in_plane = in_plane; n.X = X; n.x_plane = x_plane; n.nx = nx; n.S = S; n.src_stride = src_stride; n.M = M;
   n.T = T; n.ldf = ldf; n.overlap = overlap; n.step = m->tc - overlap;
   n.Tp = std::max<int64_t>(T, (n.P - 1) * n.step + m->tc);
   // the zero-padded slots are re-zeroed when the model changes; those of the 30-channel nets also when the overlap does
@@ -554,16 +567,17 @@ static int check_clip(const char* fn, const dcs_ctx* ctx, const dcs_model* m, co
 // the workspace of a clip of L samples: nch STFT planes, nsrc x nch masked spectra, the score-informed net's input
 // channels; with `staged` also the device copies of host audio and stems.  keep (keep-channels mode of the DSD100
 // net): two STFT planes, one magnitude plane, nsrc x 2 spectra; staged: three audio planes (downmix, left, right).
-// Two-channel stems with the Wiener post-filter on: its partial sums and covariances
+// Two-channel stems with the Wiener post-filter on: its partial sums and covariances.  masks (masks-output mode): the
+// magnitude planes and the network's buffers only -- no mixture STFT, no spectra, no Wiener workspace
 static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, bool staged, bool keep,
-                          cudaStream_t st) {
+                          cudaStream_t st, bool masks = false) {
   const int64_t plane = dcs_num_frames(L, p->hop) * dcs_padded_bins(p->N);
   const int nx = keep ? 2 : m->nch;   // mixture STFT planes = stem planes per source
-  DCS_TRY(ctx->X.ensure((size_t)nx * plane * sizeof(float2), st));
+  if (!masks) DCS_TRY(ctx->X.ensure((size_t)nx * plane * sizeof(float2), st));
   DCS_TRY(ctx->mag.ensure((size_t)m->nch * plane * sizeof(float), st));
-  DCS_TRY(ctx->S.ensure((size_t)m->nsrc * nx * plane * sizeof(float2), st));
+  if (!masks) DCS_TRY(ctx->S.ensure((size_t)m->nsrc * nx * plane * sizeof(float2), st));
   if (score_arch(m->arch)) DCS_TRY(ctx->net[NET_CHANS].ensure((size_t)score_planes(m) * plane * sizeof(float), st));
-  if (ctx->wiener_iters > 0 && m->nch * nx == 2)
+  if (!masks && ctx->wiener_iters > 0 && m->nch * nx == 2)
     DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, dcs_num_frames(L, p->hop), m->F, ctx->wiener_radius), st));
   if (staged) {
     DCS_TRY(ctx->audio.ensure((size_t)(keep ? 3 : 1) * L * sizeof(float), st));
@@ -577,19 +591,24 @@ static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, i
 // downmix of the two audio planes; the network sees its magnitude, its masks are applied to the STFT of each
 // channel -> nsrc x 2 stem planes ordered (source, channel).  Two-channel stems (keep-channels, the stereo net) go
 // through the Wiener post-filter between the network and the iSTFT when dcs_set_wiener is above 0, with the covariance
-// window of dcs_set_wiener_radius
+// window of dcs_set_wiener_radius.  masks (masks-output mode, not with d_mono): d_stems receives the network's blended
+// masks instead, float planes [T][ldf] stem_stride apart in the order of the stems; the STFT writes the magnitude only
+// and there is no Wiener pass, spectrum tap or iSTFT
 static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,
                          const float* d_filters, const NoteTable* notes, const float* d_mono, float scale_factor,
-                         int overlap, int patcher, float* d_stems, int64_t stem_stride, cudaStream_t st) {
+                         int overlap, int patcher, float* d_stems, int64_t stem_stride, cudaStream_t st, bool masks = false) {
   const bool keep = d_mono != nullptr;
-  DCS_TRY(size_workspace(ctx, m, p, L, false, keep, st));
+  DCS_TRY(size_workspace(ctx, m, p, L, false, keep, st, masks));
   const int nch = m->nch, nx = keep ? 2 : 1;
   const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
-  float2 *X = ctx->X.as<float2>(), *S = ctx->S.as<float2>();
+  float2 *X = masks ? nullptr : ctx->X.as<float2>(), *S = masks ? nullptr : ctx->S.as<float2>();
   float* mag = ctx->mag.as<float>();
   {
     ProfScope ps(ctx, "stft_fwd", st);   // compute_transform: one STFT per channel (transform.py:105-119)
-    if (keep) {
+    if (masks) {
+      for (int ch = 0; ch < nch; ++ch)
+        DCS_TRY(launch_stft(p, d_audio + ch * audio_stride, L, nullptr, mag + ch * plane, nullptr, scale_factor, ldf, st));
+    } else if (keep) {
       DCS_TRY(launch_stft(p, d_mono, L, nullptr, mag, nullptr, scale_factor, ldf, st));
       for (int c = 0; c < 2; ++c)
         DCS_TRY(launch_stft(p, d_audio + c * audio_stride, L, X + c * plane, nullptr, nullptr, scale_factor, ldf, st));
@@ -608,6 +627,7 @@ static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const fl
       DCS_TRY(launch_channel_mul(ctx, mag, d_filters, chans, plane, score_planes(m), st));
     in = chans;
   }
+  if (masks) return run_network(ctx, m, in, plane, nullptr, 0, 1, T, ldf, overlap, patcher, nullptr, stem_stride, st, d_stems);
   DCS_TRY(run_network(ctx, m, in, plane, X, plane, nx, T, ldf, overlap, patcher, S, plane, st));
   if (ctx->wiener_iters > 0 && nch * nx == 2)
     DCS_TRY(launch_wiener(ctx, X, plane, S, plane, m->nsrc, T, ldf, m->F, ctx->wiener_iters, ctx->wiener_radius, st));
@@ -987,6 +1007,51 @@ int dcs_separate_audio_keep_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, co
   }
   return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, nullptr, mono, scale_factor, overlap, patcher, d_stems,
                        stem_stride, st);
+}
+
+// ------------------------------------------------------------------------------------ masks output
+// the checks of a masks entry point beyond check_clip's: the caller's planes hold T x ldf floats each
+static int check_masks(const char* fn, const dcs_stft* p, int64_t L, const float* d_masks, int64_t m_stride) {
+  const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N);
+  DCS_REQUIRE(m_stride >= T * ldf, "%s: m_stride %lld < num_frames * ldf %lld", fn, (long long)m_stride, (long long)(T * ldf));
+  DCS_REQUIRE((uintptr_t)d_masks % sizeof(float) == 0, "%s: d_masks not 4-byte aligned", fn);
+  return DCS_OK;
+}
+
+int dcs_separate_masks(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,
+                       float scale_factor, int overlap, int patcher, float* d_masks, int64_t m_stride, void* stream) {
+  const int arch = m && m->arch == DCS_ARCH_DSD_ILD ? DCS_ARCH_DSD_ILD : -1;   // the single-channel nets or the stereo net
+  DCS_TRY(check_clip("dcs_separate_masks", ctx, m, p, arch, d_audio, d_masks, L, audio_stride, L, overlap, patcher));
+  DCS_TRY(check_masks("dcs_separate_masks", p, L, d_masks, m_stride));
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher, d_masks,
+                       m_stride, (cudaStream_t)stream, true);
+}
+
+int dcs_separate_masks_score(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t L, const float* d_filters,
+                             float scale_factor, int overlap, int patcher, float* d_masks, int64_t m_stride, void* stream) {
+  DCS_TRY(check_clip("dcs_separate_masks_score", ctx, m, p, DCS_ARCH_BACH10_SCORE, d_audio, d_masks, L, L, L, overlap, patcher));
+  DCS_REQUIRE(d_filters, "dcs_separate_masks_score: NULL filters");
+  DCS_TRY(check_masks("dcs_separate_masks_score", p, L, d_masks, m_stride));
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  return separate_clip(ctx, m, p, d_audio, L, L, d_filters, nullptr, nullptr, scale_factor, overlap, patcher, d_masks, m_stride,
+                       (cudaStream_t)stream, true);
+}
+
+int dcs_separate_masks_notes(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t L, const double* h_melody,
+                             int nnotes, int ncols, int64_t frame0, float scale_factor, int overlap, int patcher, float* d_masks,
+                             int64_t m_stride, void* stream) {
+  DCS_TRY(check_clip("dcs_separate_masks_notes", ctx, m, p, DCS_ARCH_BACH10_SCORE, d_audio, d_masks, L, L, L, overlap, patcher));
+  DCS_TRY(check_masks("dcs_separate_masks_notes", p, L, d_masks, m_stride));
+  std::vector<int32_t> tab;
+  NoteTable nt;
+  DCS_TRY(notes_compact("dcs_separate_masks_notes", h_melody, score_planes(m), nnotes, ncols, frame0,
+                        dcs_num_frames(L, p->hop), m->F, &tab, &nt));
+  cudaStream_t st = (cudaStream_t)stream;
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  DCS_TRY(notes_stage(ctx, tab, &nt, st));
+  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, &nt, nullptr, scale_factor, overlap, patcher, d_masks, m_stride, st,
+                       true);
 }
 
 // ------------------------------------------------------------------------------------ Wiener post-filter

@@ -180,6 +180,7 @@ struct NetCall {
   const float2* X; int64_t x_plane;
   int nx;           // mixture channels the masks apply to (2: DSD100 net in keep-channels mode, planes (s * 2 + c))
   float2* S; int64_t src_stride;
+  float* M;         // masks mode (non-NULL): the blended masks, float plane p at M + p * src_stride; X and S unused
   int64_t T, ldf;
   int64_t P, Tp;    // patches (> 0) and the frames they span
   int overlap, step;
@@ -274,9 +275,12 @@ struct DsdMaskArgs {
 // every mask kernel takes a total of the rectified sources at or below this as "all sources zero" (the rule's 1/nsrc or
 // 0): the reciprocal of a subnormal total overflows, and the masks would be inf * 0 = NaN.  dsd_tc.cu tests the same value.
 constexpr float MASK_TOT_MIN = 1.2e-38f;
-int launch_dsd_mask(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st);
+// Every mask launcher has a masks-output mode: with M set, the blended masks -- the fp32 values the other mode multiplies
+// by X -- are stored instead, float plane of source s at M + s * src_stride (bins < F of each frame); X and S are not
+// read or written (nx must be 1).
+int launch_dsd_mask(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st, float* M = nullptr);
 bool dsd_mask_tc_supported(const DsdMaskArgs& a);
-int launch_dsd_mask_tc(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st);   // wgmma (dsd_tc.cu)
+int launch_dsd_mask_tc(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st, float* M = nullptr);   // wgmma (dsd_tc.cu)
 // strided-conv1 families (iKala / Bach10): K3s arguments
 struct SconvMaskArgs {
   int arch;
@@ -292,9 +296,9 @@ struct SconvMaskArgs {
   int p_base, t0, t1;
 };
 int launch_pool4(dcs_ctx* ctx, const float* H1, float* Hp, uint8_t* tie, int64_t rows, int J, int WP, cudaStream_t st);
-int launch_sconv_mask(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st);
+int launch_sconv_mask(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st, float* M = nullptr);
 bool sconv_mask_tc_supported(const SconvMaskArgs& a);
-int launch_sconv_mask_tc(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st);   // wgmma (sconv_tc.cu)
+int launch_sconv_mask_tc(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st, float* M = nullptr);   // wgmma (sconv_tc.cu)
 int launch_channel_mul(dcs_ctx* ctx, const float* mag, const float* filt, float* out, int64_t plane, int nch, cudaStream_t st);
 
 // the note table of the score-informed nets (score_notes.cu), compacted for the frame window [start, start + T):

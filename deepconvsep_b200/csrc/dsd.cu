@@ -25,9 +25,10 @@ constexpr int MASK_TILE = 256;
 constexpr int MASK_THREADS = MASK_TILE + 32;
 constexpr int MASK_MAXP = 6;
 
-template <int C1, int NDEC>
+// MASKS: the blended masks themselves to M (source s at M + s * src_stride); X and S are not touched
+template <int C1, int NDEC, bool MASKS = false>
 __global__ void __launch_bounds__(MASK_THREADS)
-dsd_mask_kernel(const DsdMaskArgs a, int frames_per_cta) {
+dsd_mask_kernel(const DsdMaskArgs a, float* __restrict__ M, int frames_per_cta) {
   constexpr int PITCH = (C1 + 3) / 4 * 4;
   __shared__ __align__(16) float gs[MASK_MAXP][NDEC][PITCH];
   const int tid = threadIdx.x;
@@ -112,7 +113,13 @@ dsd_mask_kernel(const DsdMaskArgs a, int frames_per_cta) {
         }
       }
     }
-    if (bok) {
+    if (MASKS && bok) {
+      const int64_t o = (int64_t)t * a.ldf + b;
+      M[o] = acc0;
+      M[o + a.src_stride] = acc1;
+      M[o + 2 * a.src_stride] = acc2;
+      M[o + 3 * a.src_stride] = acc3;
+    } else if (bok) {
       const int64_t o = (int64_t)t * a.ldf + b;
       const float2 x = a.X[o];
       a.S[o] = make_float2(acc0 * x.x, acc0 * x.y);
@@ -123,14 +130,16 @@ dsd_mask_kernel(const DsdMaskArgs a, int frames_per_cta) {
   }
 }
 
-int launch_dsd_mask(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st) {
+int launch_dsd_mask(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st, float* M) {
   if (a.T <= 0) return DCS_OK;
   DCS_REQUIRE(a.tc > a.overlap && a.overlap >= 0, "time_context %d must exceed overlap %d", a.tc, a.overlap);
   const int fpc = 16;
   // frames on gridDim.x (2^31-1 blocks: any clip length), bin tiles on gridDim.y (a handful)
   dim3 grid((unsigned)ceil_div64(a.T, fpc), (unsigned)ceil_div64(a.F - 1, MASK_TILE));
-  if (a.ndec == 4) dsd_mask_kernel<50, 4><<<grid, MASK_THREADS, 0, st>>>(a, fpc);
-  else dsd_mask_kernel<50, 3><<<grid, MASK_THREADS, 0, st>>>(a, fpc);
+  if (M && a.ndec == 4) dsd_mask_kernel<50, 4, true><<<grid, MASK_THREADS, 0, st>>>(a, M, fpc);
+  else if (M) dsd_mask_kernel<50, 3, true><<<grid, MASK_THREADS, 0, st>>>(a, M, fpc);
+  else if (a.ndec == 4) dsd_mask_kernel<50, 4><<<grid, MASK_THREADS, 0, st>>>(a, nullptr, fpc);
+  else dsd_mask_kernel<50, 3><<<grid, MASK_THREADS, 0, st>>>(a, nullptr, fpc);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;

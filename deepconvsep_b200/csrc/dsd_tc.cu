@@ -192,9 +192,9 @@ __device__ __forceinline__ void mask_slot(const float4 c, float y0, float y1, fl
 }
 
 // the Nyquist bin of frame t from the producer's dot products of its group (f = frame in the group, xf = the group's
-// fade-table entries)
-template <int NDEC, int NX>
-__device__ __forceinline__ void mask_nyquist_epilogue(const DsdMaskArgs& a, const float4* xf, int t, int f, const float* nyq,
+// fade-table entries); MASKS: the masks themselves to M (source s at M + s * src_stride), no X read
+template <int NDEC, int NX, bool MASKS>
+__device__ __forceinline__ void mask_nyquist_epilogue(const DsdMaskArgs& a, float* M, const float4* xf, int t, int f, const float* nyq,
                                                       float bo0, float bo1, float bo2, float bo3) {
   using MT = MaskTile<NDEC>;
   if (t >= a.T) return;
@@ -206,22 +206,32 @@ __device__ __forceinline__ void mask_nyquist_epilogue(const DsdMaskArgs& a, cons
                     nyq[MT::col(f, NDEC * j + (NDEC == 3 ? 1 : 3))], bo0, bo1, bo2, bo3, j == 0, mm);
   }
   const int bin = a.F - 1;
+  if constexpr (MASKS) {
+    const int64_t o = (int64_t)t * a.ldf + bin;
 #pragma unroll
-  for (int c = 0; c < NX; ++c) {
-    const float2 xx = a.X[c * a.x_plane + (int64_t)t * a.ldf + bin];
-    const int64_t o = (int64_t)t * a.ldf + bin + c * a.src_stride;
-    a.S[o] = make_float2(mm[0] * xx.x, mm[0] * xx.y);
-    a.S[o + NX * a.src_stride] = make_float2(mm[1] * xx.x, mm[1] * xx.y);
-    a.S[o + 2 * NX * a.src_stride] = make_float2(mm[2] * xx.x, mm[2] * xx.y);
-    a.S[o + 3 * NX * a.src_stride] = make_float2(mm[3] * xx.x, mm[3] * xx.y);
+    for (int s = 0; s < 4; ++s) M[o + s * a.src_stride] = mm[s];
+  } else {
+#pragma unroll
+    for (int c = 0; c < NX; ++c) {
+      const float2 xx = a.X[c * a.x_plane + (int64_t)t * a.ldf + bin];
+      const int64_t o = (int64_t)t * a.ldf + bin + c * a.src_stride;
+      a.S[o] = make_float2(mm[0] * xx.x, mm[0] * xx.y);
+      a.S[o + NX * a.src_stride] = make_float2(mm[1] * xx.x, mm[1] * xx.y);
+      a.S[o + 2 * NX * a.src_stride] = make_float2(mm[2] * xx.x, mm[2] * xx.y);
+      a.S[o + 3 * NX * a.src_stride] = make_float2(mm[3] * xx.x, mm[3] * xx.y);
+    }
   }
 }
 
 // nyq_tiles > 0: the tiles cover bins [0, F - 1) and item (tile, g) with tile == g % nyq_tiles also computes bin F - 1
 // of group g on the producer; 0: the tiles cover all F bins.
-template <int NDEC, int NX>
+// MASKS (NX = 1): the cross-faded masks themselves -- the fp32 values the other mode multiplies by X -- go to M,
+// source s at M + s * src_stride; X and S are not touched.
+template <int NDEC, int NX, bool MASKS>
 __global__ void __launch_bounds__(MT_THREADS, 1)
-dsd_mask_tc_kernel(const DsdMaskArgs a, const float4* __restrict__ xtab, int num_groups, int num_items, int nyq_tiles) {
+dsd_mask_tc_kernel(const DsdMaskArgs a, float* __restrict__ M, const float4* __restrict__ xtab, int num_groups, int num_items,
+                   int nyq_tiles) {
+  static_assert(!MASKS || NX == 1, "the masks do not depend on the mixture channel");
   using MT = MaskTile<NDEC>;
   constexpr int FRAMES = MT::FRAMES, TF = MT::TFRAMES;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -286,7 +296,8 @@ dsd_mask_tc_kernel(const DsdMaskArgs a, const float4* __restrict__ xtab, int num
       if (nyq_item) {
         nb ^= 1;
         bar_sync(MT_BAR_PROD, MT_PRODUCER);
-        if (ptid < FRAMES) mask_nyquist_epilogue<NDEC, NX>(a, sXf + (it & 3) * MT::XF, g * FRAMES + ptid, ptid, nq, bo0, bo1, bo2, bo3);
+        if (ptid < FRAMES)
+          mask_nyquist_epilogue<NDEC, NX, MASKS>(a, M, sXf + (it & 3) * MT::XF, g * FRAMES + ptid, ptid, nq, bo0, bo1, bo2, bo3);
       }
     }
     return;
@@ -345,15 +356,17 @@ dsd_mask_tc_kernel(const DsdMaskArgs a, const float4* __restrict__ xtab, int num
       bok[i] = bin[i] < a.F;
     }
     float2 x[NX][TF][2];
+    if constexpr (!MASKS) {
 #pragma unroll
-    for (int c = 0; c < NX; ++c)
+      for (int c = 0; c < NX; ++c)
 #pragma unroll
-      for (int e = 0; e < TF; ++e) {
-        const int t = g * FRAMES + MT::thread_frame(lane, e);
+        for (int e = 0; e < TF; ++e) {
+          const int t = g * FRAMES + MT::thread_frame(lane, e);
 #pragma unroll
-        for (int i = 0; i < 2; ++i)
-          x[c][e][i] = (bok[i] && t < a.T) ? a.X[c * a.x_plane + (int64_t)t * a.ldf + bin[i]] : make_float2(0.f, 0.f);
-      }
+          for (int i = 0; i < 2; ++i)
+            x[c][e][i] = (bok[i] && t < a.T) ? a.X[c * a.x_plane + (int64_t)t * a.ldf + bin[i]] : make_float2(0.f, 0.f);
+        }
+    }
     wgmma_wait<0>();
     wgmma_fence_acc(acc);
     if (lane == 0) mbar_arrive(&empty_bar[s]);
@@ -373,25 +386,39 @@ dsd_mask_tc_kernel(const DsdMaskArgs a, const float4* __restrict__ xtab, int num
         }
       }
     }
-    // source s, channel c at S + (s * NX + c) * src_stride
-#pragma unroll
-    for (int c = 0; c < NX; ++c)
+    if constexpr (MASKS) {   // source s at M + s * src_stride
 #pragma unroll
       for (int e = 0; e < TF; ++e) {
         const int t = g * FRAMES + MT::thread_frame(lane, e);
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
           if (bok[i] && t < a.T) {
-            const float2 xx = x[c][e][i];
-            const float* mm = m[e][i];
-            const int64_t o = (int64_t)t * a.ldf + bin[i] + c * a.src_stride;
-            a.S[o] = make_float2(mm[0] * xx.x, mm[0] * xx.y);
-            a.S[o + NX * a.src_stride] = make_float2(mm[1] * xx.x, mm[1] * xx.y);
-            a.S[o + 2 * NX * a.src_stride] = make_float2(mm[2] * xx.x, mm[2] * xx.y);
-            a.S[o + 3 * NX * a.src_stride] = make_float2(mm[3] * xx.x, mm[3] * xx.y);
+            const int64_t o = (int64_t)t * a.ldf + bin[i];
+#pragma unroll
+            for (int s = 0; s < 4; ++s) M[o + s * a.src_stride] = m[e][i][s];
           }
         }
       }
+    } else {   // source s, channel c at S + (s * NX + c) * src_stride
+#pragma unroll
+      for (int c = 0; c < NX; ++c)
+#pragma unroll
+        for (int e = 0; e < TF; ++e) {
+          const int t = g * FRAMES + MT::thread_frame(lane, e);
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            if (bok[i] && t < a.T) {
+              const float2 xx = x[c][e][i];
+              const float* mm = m[e][i];
+              const int64_t o = (int64_t)t * a.ldf + bin[i] + c * a.src_stride;
+              a.S[o] = make_float2(mm[0] * xx.x, mm[0] * xx.y);
+              a.S[o + NX * a.src_stride] = make_float2(mm[1] * xx.x, mm[1] * xx.y);
+              a.S[o + 2 * NX * a.src_stride] = make_float2(mm[2] * xx.x, mm[2] * xx.y);
+              a.S[o + 3 * NX * a.src_stride] = make_float2(mm[3] * xx.x, mm[3] * xx.y);
+            }
+          }
+        }
+    }
   }
 }
 
@@ -425,10 +452,10 @@ bool dsd_mask_tc_supported(const DsdMaskArgs& a) {
 
 // F = 128 m + 1 (the DSD nets' F = N / 2 + 1) with m >= 1: m tiles, and the producer computes the Nyquist bin, which
 // would otherwise take a tile of its own; any other F: ceil(F / 128) tiles
-template <int NDEC, int NX>
-static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st) {
+template <int NDEC, int NX, bool MASKS = false>
+static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, float* M, cudaStream_t st) {
   using MT = MaskTile<NDEC>;
-  DCS_TRY(ensure_smem_attr(dsd_mask_tc_kernel<NDEC, NX>, MT::SMEM));
+  DCS_TRY(ensure_smem_attr(dsd_mask_tc_kernel<NDEC, NX, MASKS>, MT::SMEM));
   const bool nyq = a.F > MT_BINS && (a.F - 1) % MT_BINS == 0;
   const int m_tiles = nyq ? (a.F - 1) / MT_BINS : (a.F + MT_BINS - 1) / MT_BINS;
   const int num_groups = (a.T + MT::FRAMES - 1) / MT::FRAMES;
@@ -440,17 +467,22 @@ static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t
   dsd_xfade_table_kernel<<<(unsigned)ceil_div64((int64_t)Tpad * MT_SLOTS, 256), 256, 0, st>>>(xtab, a.T, Tpad, a.P, a.tc, a.overlap);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
-  dsd_mask_tc_kernel<NDEC, NX><<<(unsigned)ctas, MT_THREADS, MT::SMEM, st>>>(a, xtab, num_groups, num_items, nyq ? m_tiles : 0);
+  dsd_mask_tc_kernel<NDEC, NX, MASKS><<<(unsigned)ctas, MT_THREADS, MT::SMEM, st>>>(a, M, xtab, num_groups, num_items,
+                                                                                   nyq ? m_tiles : 0);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;
 }
 
-int launch_dsd_mask_tc(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st) {
+int launch_dsd_mask_tc(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st, float* M) {
   if (a.T <= 0) return DCS_OK;
   DCS_REQUIRE(dsd_mask_tc_supported(a), "dsd_mask_tc: unsupported shape");
-  if (a.ndec == 4) return launch_dsd_mask_tc_t<4, 1>(ctx, a, st);
-  return a.nx == 2 ? launch_dsd_mask_tc_t<3, 2>(ctx, a, st) : launch_dsd_mask_tc_t<3, 1>(ctx, a, st);
+  if (M) {
+    DCS_REQUIRE(a.nx == 1, "dsd_mask_tc: the masks are written once, not per mixture channel (nx = 1)");
+    return a.ndec == 4 ? launch_dsd_mask_tc_t<4, 1, true>(ctx, a, M, st) : launch_dsd_mask_tc_t<3, 1, true>(ctx, a, M, st);
+  }
+  if (a.ndec == 4) return launch_dsd_mask_tc_t<4, 1>(ctx, a, nullptr, st);
+  return a.nx == 2 ? launch_dsd_mask_tc_t<3, 2>(ctx, a, nullptr, st) : launch_dsd_mask_tc_t<3, 1>(ctx, a, nullptr, st);
 }
 
 }  // namespace dcs

@@ -36,10 +36,11 @@ __global__ void pool4_kernel(const float* __restrict__ H1, float* __restrict__ H
 
 constexpr int SC_TILE = 128;   // m values (threads) per CTA
 
-// CHUNK: as in sconv_mask_tc_kernel (G from patch a.p_base, frames [a.t0, a.t1))
-template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW, bool CHUNK = false>
+// CHUNK: as in sconv_mask_tc_kernel (G from patch a.p_base, frames [a.t0, a.t1)); MASKS: the blended masks to M
+// (source s at M + s * src_stride), X and S untouched
+template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW, bool CHUNK = false, bool MASKS = false>
 __global__ void __launch_bounds__(SC_TILE)
-sconv_mask_kernel(const SconvMaskArgs a) {
+sconv_mask_kernel(const SconvMaskArgs a, float* __restrict__ M) {
   constexpr int JT = SC_TILE + ND - 1;  // staged activation positions per tile
   extern __shared__ __align__(16) float sm[];
   float* gs = sm;                                   // [NDEC][JT][33]
@@ -128,7 +129,11 @@ sconv_mask_kernel(const SconvMaskArgs a) {
 #pragma unroll
   for (int r = 0; r < STRIDE; ++r) {
     const int b = STRIDE * m + r;
-    if (b < a.F) {
+    if (MASKS && b < a.F) {
+      const int64_t o = (int64_t)t * a.ldf + b;
+#pragma unroll
+      for (int s = 0; s < NSRC; ++s) M[o + s * a.src_stride] = macc[s][r];
+    } else if (b < a.F) {
       const int64_t o = (int64_t)t * a.ldf + b;
       const float2 x = a.X[o];
 #pragma unroll
@@ -164,28 +169,30 @@ int launch_pool4(dcs_ctx* ctx, const float* H1, float* Hp, uint8_t* tie, int64_t
 }
 
 template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW, bool CHUNK = false>
-static int launch_sconv_t(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st) {
+static int launch_sconv_t(dcs_ctx* ctx, const SconvMaskArgs& a, float* M, cudaStream_t st) {
   constexpr int JT = SC_TILE + ND - 1;
   const size_t smem = (size_t)(NDEC * JT * 33 + 4) * sizeof(float) + NW * ND * 32 * sizeof(float4);
-  DCS_TRY(ensure_smem_attr(sconv_mask_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW, CHUNK>, (int)smem));
+  auto kern = M ? sconv_mask_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW, CHUNK, true>
+                : sconv_mask_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW, CHUNK, false>;
+  DCS_TRY(ensure_smem_attr(kern, (int)smem));
   const int mtot = (a.F + STRIDE - 1) / STRIDE;
   dim3 grid((unsigned)(a.t1 - a.t0), (unsigned)ceil_div64(mtot, SC_TILE));
-  sconv_mask_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW, CHUNK><<<grid, SC_TILE, smem, st>>>(a);
+  kern<<<grid, SC_TILE, smem, st>>>(a, M);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;
 }
 
-int launch_sconv_mask(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st) {
+int launch_sconv_mask(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st, float* M) {
   if (a.T <= 0 || a.t1 <= a.t0) return DCS_OK;
   const int step = a.tc - a.overlap;
   DCS_REQUIRE(step > 0 && (a.tc + step - 1) / step <= 64, "sconv_mask: bad time_context/overlap");
   DCS_REQUIRE(a.t0 >= 0 && a.t1 <= a.T, "sconv_mask: frame range [%d, %d) outside [0, %d)", a.t0, a.t1, a.T);
-  if (a.arch == DCS_ARCH_BACH10) return launch_sconv_t<4, 8, 4, 4, 1, 0, 1>(ctx, a, st);
-  if (a.arch == DCS_ARCH_BACH10_SCORE) return launch_sconv_t<4, 8, 4, 1, 1, 0, 4>(ctx, a, st);
-  if (a.arch == DCS_ARCH_BACH10_SCORE_1X1) return launch_sconv_t<2, 3, 4, 1, 1, 0, 4, true>(ctx, a, st);
-  if (a.arch == DCS_ARCH_IKALA) return launch_sconv_t<3, 10, 2, 2, 0, 4, 1>(ctx, a, st);
-  if (a.arch == DCS_ARCH_IKALA_NOPOOL) return launch_sconv_t<3, 10, 2, 2, 0, 0, 1>(ctx, a, st);
+  if (a.arch == DCS_ARCH_BACH10) return launch_sconv_t<4, 8, 4, 4, 1, 0, 1>(ctx, a, M, st);
+  if (a.arch == DCS_ARCH_BACH10_SCORE) return launch_sconv_t<4, 8, 4, 1, 1, 0, 4>(ctx, a, M, st);
+  if (a.arch == DCS_ARCH_BACH10_SCORE_1X1) return launch_sconv_t<2, 3, 4, 1, 1, 0, 4, true>(ctx, a, M, st);
+  if (a.arch == DCS_ARCH_IKALA) return launch_sconv_t<3, 10, 2, 2, 0, 4, 1>(ctx, a, M, st);
+  if (a.arch == DCS_ARCH_IKALA_NOPOOL) return launch_sconv_t<3, 10, 2, 2, 0, 0, 1>(ctx, a, M, st);
   DCS_REQUIRE(false, "sconv_mask: architecture %d not supported", a.arch);
 }
 

@@ -203,9 +203,9 @@ int sconv_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaStream
   ProfScope ps(ctx, "dec_convT1_mask_xfade", st);
   if (!ctx->debug_simt_gemm) {
     DCS_REQUIRE(sconv_mask_tc_supported(a), "sconv_forward: tensor-core mask kernel does not take this shape");
-    return launch_sconv_mask_tc(ctx, a, st);
+    return launch_sconv_mask_tc(ctx, a, st, n.M);
   }
-  return launch_sconv_mask(ctx, a, st);    // FFMA twin: cross-check (DCS_DEBUG_SIMT_GEMM=1)
+  return launch_sconv_mask(ctx, a, st, n.M);    // FFMA twin: cross-check (DCS_DEBUG_SIMT_GEMM=1)
 }
 
 }  // namespace dcs

@@ -81,10 +81,11 @@ __device__ __forceinline__ float4 sconv_load(const SconvMaskArgs& a, int t, int 
 }
 
 // CHUNK: G holds patches a.p_base.. and the frames [a.t0, a.t1) are written (one decoder chunk of the 1x1 score net);
-// otherwise G holds every patch and all a.T frames are written
-template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW, bool CHUNK = false>
+// otherwise G holds every patch and all a.T frames are written.  MASKS: the blended masks themselves go to M (source s at
+// M + s * src_stride); X and S are not touched
+template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW, bool CHUNK = false, bool MASKS = false>
 __global__ void __launch_bounds__(ST_THREADS, 1)
-sconv_mask_tc_kernel(const SconvMaskArgs a, int frames_per_cta) {
+sconv_mask_tc_kernel(const SconvMaskArgs a, float* __restrict__ M, int frames_per_cta) {
   using TL = SconvTile<STRIDE, ND, NSRC, NDEC, NW>;
   constexpr int OUT = TL::OUT, NB = TL::NB, ITEMS = TL::ITEMS, CHUNKS = TL::CHUNKS;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -134,7 +135,10 @@ sconv_mask_tc_kernel(const SconvMaskArgs a, int frames_per_cta) {
       const int b = STRIDE * m + r;
       if ((r & 1) == half && b < a.F)
 #pragma unroll
-        for (int s = 0; s < NSRC; ++s) a.S[(int64_t)tt * a.ldf + b + s * a.src_stride] = make_float2(0.f, 0.f);
+        for (int s = 0; s < NSRC; ++s) {
+          if (MASKS) M[(int64_t)tt * a.ldf + b + s * a.src_stride] = 0.f;
+          else a.S[(int64_t)tt * a.ldf + b + s * a.src_stride] = make_float2(0.f, 0.f);
+        }
     }
   };
   // first slot at or after frame tt: (tt, k_lo .. k_hi), or tt = t_end
@@ -250,7 +254,11 @@ sconv_mask_tc_kernel(const SconvMaskArgs a, int frames_per_cta) {
 #pragma unroll
       for (int r = 0; r < STRIDE; ++r) {
         const int b = STRIDE * m + r;
-        if ((r & 1) == half && b < a.F) {
+        if (MASKS && (r & 1) == half && b < a.F) {
+          const int64_t o = (int64_t)t * a.ldf + b;
+#pragma unroll
+          for (int s = 0; s < NSRC; ++s) M[o + s * a.src_stride] = macc[s][r];
+        } else if ((r & 1) == half && b < a.F) {
           const int64_t o = (int64_t)t * a.ldf + b;
           const float2 x = a.X[o];
 #pragma unroll
@@ -263,9 +271,10 @@ sconv_mask_tc_kernel(const SconvMaskArgs a, int frames_per_cta) {
 }
 
 template <int STRIDE, int ND, int NSRC, int NDEC, int RULE, int POOL, int NW, bool CHUNK = false>
-static int launch_sconv_tc_t(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st) {
+static int launch_sconv_tc_t(dcs_ctx* ctx, const SconvMaskArgs& a, float* M, cudaStream_t st) {
   using TL = SconvTile<STRIDE, ND, NSRC, NDEC, NW>;
-  auto kern = sconv_mask_tc_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW, CHUNK>;
+  auto kern = M ? sconv_mask_tc_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW, CHUNK, true>
+                : sconv_mask_tc_kernel<STRIDE, ND, NSRC, NDEC, RULE, POOL, NW, CHUNK, false>;
   DCS_TRY(ensure_smem_attr(kern, TL::SMEM));
   const int mtot = (a.F + STRIDE - 1) / STRIDE;
   const int mtiles = (mtot + TL::OUT - 1) / TL::OUT;
@@ -275,7 +284,7 @@ static int launch_sconv_tc_t(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t 
   if (chunks > nt) chunks = nt;
   const int fpc = (nt + chunks - 1) / chunks;
   dim3 grid((unsigned)mtiles, (unsigned)((nt + fpc - 1) / fpc));
-  kern<<<grid, ST_THREADS, TL::SMEM, st>>>(a, fpc);
+  kern<<<grid, ST_THREADS, TL::SMEM, st>>>(a, M, fpc);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;
@@ -288,15 +297,15 @@ bool sconv_mask_tc_supported(const SconvMaskArgs& a) {
           a.arch == DCS_ARCH_BACH10_SCORE_1X1);
 }
 
-int launch_sconv_mask_tc(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st) {
+int launch_sconv_mask_tc(dcs_ctx* ctx, const SconvMaskArgs& a, cudaStream_t st, float* M) {
   if (a.T <= 0 || a.t1 <= a.t0) return DCS_OK;
   DCS_REQUIRE(sconv_mask_tc_supported(a), "sconv_mask_tc: unsupported shape");
-  if (a.arch == DCS_ARCH_BACH10) return launch_sconv_tc_t<4, 8, 4, 4, 1, 0, 1>(ctx, a, st);
-  if (a.arch == DCS_ARCH_BACH10_SCORE) return launch_sconv_tc_t<4, 8, 4, 1, 1, 0, 4>(ctx, a, st);
+  if (a.arch == DCS_ARCH_BACH10) return launch_sconv_tc_t<4, 8, 4, 4, 1, 0, 1>(ctx, a, M, st);
+  if (a.arch == DCS_ARCH_BACH10_SCORE) return launch_sconv_tc_t<4, 8, 4, 1, 1, 0, 4>(ctx, a, M, st);
   // 1x1 score net: InverseLayer(conv1) of kernel (1,5) stride 2 -- 3 taps per output pair (score1x1.cu)
-  if (a.arch == DCS_ARCH_BACH10_SCORE_1X1) return launch_sconv_tc_t<2, 3, 4, 1, 1, 0, 4, true>(ctx, a, st);
-  if (a.arch == DCS_ARCH_IKALA) return launch_sconv_tc_t<3, 10, 2, 2, 0, 4, 1>(ctx, a, st);
-  return launch_sconv_tc_t<3, 10, 2, 2, 0, 0, 1>(ctx, a, st);
+  if (a.arch == DCS_ARCH_BACH10_SCORE_1X1) return launch_sconv_tc_t<2, 3, 4, 1, 1, 0, 4, true>(ctx, a, M, st);
+  if (a.arch == DCS_ARCH_IKALA) return launch_sconv_tc_t<3, 10, 2, 2, 0, 4, 1>(ctx, a, M, st);
+  return launch_sconv_tc_t<3, 10, 2, 2, 0, 0, 1>(ctx, a, M, st);
 }
 
 }  // namespace dcs

@@ -238,9 +238,9 @@ int s1x1_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaStream_
     ProfScope ps(ctx, "dec_convT1_mask_xfade", st);
     if (!ctx->debug_simt_gemm) {   // the product path
       DCS_REQUIRE(sconv_mask_tc_supported(a), "s1x1_forward: tensor-core mask kernel does not take this shape");
-      DCS_TRY(launch_sconv_mask_tc(ctx, a, st));
+      DCS_TRY(launch_sconv_mask_tc(ctx, a, st, n.M));
     } else {
-      DCS_TRY(launch_sconv_mask(ctx, a, st));   // FFMA twin: cross-check (DCS_DEBUG_SIMT_GEMM=1)
+      DCS_TRY(launch_sconv_mask(ctx, a, st, n.M));   // FFMA twin: cross-check (DCS_DEBUG_SIMT_GEMM=1)
     }
   }
   return DCS_OK;

@@ -530,6 +530,72 @@ class Separator(object):
             return outd
         return np.ascontiguousarray(outd.cpu().numpy().reshape(self.nsrc, 2, L).transpose(2, 0, 1))
 
+    def separate_masks(self, audio, filters=None, melody=None, frame0=0, out=None, stream=None):
+        """The network's blended soft masks, from a pipeline that stops before the inverse STFT (dcs_separate_masks*):
+        the fp32 values the stems calls multiply by the mixture STFT, so Stft.inverse(X * masks) gives the stems.
+        audio as the stems call of this network takes it -- float [L] (single-channel nets), [L, 2] numpy or [2, L] cuda
+        tensor (stereo / ILD net); score-informed nets also need the score filters `filters` (as separate_score) or the
+        note table `melody` from table frame `frame0` (as separate_notes).  numpy in -> float32 [nsrc, T, F] ([nsrc, 2,
+        T, F] for the stereo net); cuda tensor in -> the device planes [nplanes, T, ldf] (or into `out`, whose rows must be
+        contiguous; its pad columns and the gaps between planes are not written), planes ordered (source, channel)."""
+        import torch
+        arch = self.model.arch
+        score = arch in ("bach10_score", "bach10_score_1x1")
+        if melody is not None and not score:
+            raise ValueError("separate_notes needs a score-informed network, this one is %r" % arch)
+        if filters is not None and not score:
+            raise ValueError("separate_score needs a score-informed network, this one is %r" % arch)
+        if score and (filters is None) == (melody is None):
+            raise ValueError("the score-informed network %r needs either the score filters or the note table" % arch)
+        if int(frame0) < 0:
+            raise ValueError("frame0 %d must be >= 0" % frame0)
+        host = not hasattr(audio, "is_cuda")
+        stereo = arch == "dsd_ild"
+        if host:
+            a = np.asarray(audio, dtype=np.float32)
+            if stereo and (a.ndim != 2 or a.shape[1] != 2):
+                raise ValueError("the stereo network needs stereo audio [L, 2], got shape %r" % (a.shape,))
+            if not stereo and a.ndim != 1:
+                raise ValueError("this network needs mono audio [L], got shape %r" % (a.shape,))
+            x = torch.as_tensor(np.ascontiguousarray(a.T if stereo else a), device=self.stft.dev)
+        else:
+            x = audio.contiguous()
+            assert x.dtype == torch.float32 and x.dim() == (2 if stereo else 1) and (not stereo or x.shape[0] == 2)
+        L = x.shape[-1]
+        T, ldf, nplanes = self.stft.num_frames(L), self.stft.ldf, self.nsrc * (2 if stereo else 1)
+        if out is not None and not host:
+            assert out.is_cuda and out.dtype == torch.float32 and out.dim() == 3 and tuple(out.shape[1:]) == (T, ldf)
+            assert out.shape[0] == nplanes and out.stride(2) == 1 and out.stride(1) == ldf
+            outd = out
+        else:
+            outd = torch.empty((nplanes, T, ldf), dtype=torch.float32, device=x.device)
+        tail = (self.scale_factor, self.overlap, self.patcher, _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device))
+        h, m, p = self.ctx.handle, self.model.handle, self.stft.handle
+        if melody is not None:
+            mel = check_melody(melody, 4)
+            _lib.check(self.lib.dcs_separate_masks_notes(h, m, p, _ptr(x), L, mel.ctypes.data, mel.shape[1], mel.shape[2],
+                                                         int(frame0), *tail))
+        elif filters is not None:
+            if hasattr(filters, "is_cuda"):
+                fd = filters
+                assert fd.is_cuda and fd.dtype == torch.float32 and fd.is_contiguous() and tuple(fd.shape) == (4, T, ldf)
+            else:
+                f = np.asarray(filters, dtype=np.float32)
+                assert f.shape == (4, T, self.model.F), (f.shape, (4, T, self.model.F))
+                fd = torch.zeros((4, T, ldf), dtype=torch.float32, device=x.device)
+                fd[:, :, :self.model.F] = torch.as_tensor(f, device=x.device)
+            _lib.check(self.lib.dcs_separate_masks_score(h, m, p, _ptr(x), L, _ptr(fd), *tail))
+        else:
+            _lib.check(self.lib.dcs_separate_masks(h, m, p, _ptr(x), x.stride(0) if stereo else L, L, *tail))
+        if not host:
+            return outd
+        M = outd[:, :, :self.model.F].cpu().numpy()
+        M = M.reshape(self.nsrc, 2, T, self.model.F) if stereo else M
+        if out is not None:
+            out[...] = M
+            return out
+        return M
+
     def separate_tapped(self, audio, filters=None, pool=False, keep_channels=False, wiener=0, melody=None, frame0=0,
                         wiener_radius=0):
         """Parity-test entry: the whole-clip call clip_call() picks for these inputs (separate() / separate_score() /

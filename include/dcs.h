@@ -399,6 +399,37 @@ int dcs_separate_batch_pcm16_keep_channels_host(dcs_ctx* ctx, dcs_model* model, 
                                                 float scale_factor, int overlap, int patcher, int16_t* const* h_out,
                                                 const int64_t* out_strides, void* stream);
 
+/* ---- masks output: the network's blended soft masks, from a pipeline that stops before the iSTFT ----------------- */
+/* The soft masks M_s[t, f] every separation entry point computes and multiplies by the mixture STFT: the ratio masks of
+ * each patch, cross-faded over the patches (overlapadd_multi, separate_dsd.py:139-169) -- the same fp32 values, bit for
+ * bit, that the stems path multiplies by X, so  iSTFT(X * M_s)  (dcs_stft_forward, the product componentwise in fp32,
+ * dcs_istft) is the stem of the matching dcs_separate_audio* call.  The masks of a downmix (l + r) * 0.5f applied to
+ * each channel's STFT are the keep-channels mode.  Each entry point mirrors the stems call named beside it, with the same
+ * checks, and writes d_masks float[nplanes][T][ldf], T = dcs_num_frames(num_samples, hop), ldf = dcs_padded_bins(N),
+ * planes m_stride (>= T * ldf) apart: nplanes = nsrc, or nsrc x 2 ordered (source, channel) for the stereo / ILD net.
+ * Only bins f < F of each frame are written: the pad columns F..ldf-1 and the gaps between planes keep their contents.
+ *  - The forward STFT writes the magnitude only; there is no Wiener pass (dcs_set_wiener is ignored), no spectrum tap
+ *    and no inverse STFT, and the workspace holds neither the mixture STFT nor the masked spectra.
+ *  - The routing tap (dcs_set_pool_tap) is honoured as by the stems calls.
+ *  - A clip shorter than one patch gives all-zero masks.
+ *  - Refused with DCS_EINVAL before anything is queued: an architecture the entry point does not serve, a NULL pointer,
+ *    a plan whose N/2+1 is not the model's F, m_stride < T * ldf, a misaligned d_masks, and what the mirrored stems call
+ *    refuses (lengths, strides, overlap, patcher, the note table). */
+/* dcs_separate_audio (single-channel nets: d_audio float[L], audio_stride >= L) and dcs_separate_audio_stereo (stereo /
+ * ILD net: d_audio float[2][audio_stride]) */
+int dcs_separate_masks(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const float* d_audio, int64_t audio_stride,
+                       int64_t num_samples, float scale_factor, int overlap, int patcher, float* d_masks,
+                       int64_t m_stride, void* stream);
+/* dcs_separate_audio_score: the score-informed nets with the filter planes d_filters float[4][T][ldf] */
+int dcs_separate_masks_score(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const float* d_audio,
+                             int64_t num_samples, const float* d_filters, float scale_factor, int overlap,
+                             int patcher, float* d_masks, int64_t m_stride, void* stream);
+/* dcs_separate_audio_notes: the score-informed nets with the note table h_melody (HOST) from table frame frame0 */
+int dcs_separate_masks_notes(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const float* d_audio,
+                             int64_t num_samples, const double* h_melody, int nnotes, int ncols, int64_t frame0,
+                             float scale_factor, int overlap, int patcher, float* d_masks, int64_t m_stride,
+                             void* stream);
+
 /* ---- multichannel Wiener filter with EM spatial covariances (Duong, Vincent & Gribonval 2010; util.py:633-719) -- */
 /* In place on caller-owned spectra, the plane layout of the stereo entry points: mixture channel c at d_X + c*x_plane,
  * stem (source j, channel c) at d_S + (2j + c)*src_stride, each complex[T][ldf]; only bins f < F are read or written.
