@@ -57,6 +57,9 @@ _SIGS = {
     "dcs_separate_masks_score": (C.c_int, [_p, _p, _p, _p, _i64, _p, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
     "dcs_separate_masks_notes": (C.c_int, [_p, _p, _p, _p, _i64, _p, C.c_int, C.c_int, _i64, C.c_float, C.c_int, C.c_int,
                                            _p, _i64, _p]),
+    "dcs_istft_masked": (C.c_int, [_p, _p, C.c_int, _i64, _p, C.c_int, _i64, _i64, _i64, _p, _i64, _i64, _p]),
+    "dcs_apply_masks": (C.c_int, [_p, _p, _p, C.c_int, _i64, _i64, _p, C.c_int, _i64, _p, _i64, _p]),
+    "dcs_separate_audio_channels": (C.c_int, [_p, _p, _p, _p, C.c_int, _i64, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
     "dcs_xcorr_lags": (C.c_int, [_p, _p, _p, C.c_int, _i64, C.c_int, _p, _p]),
     "dcs_gemm_f32": (C.c_int, [_p, C.c_int, _p, _i64, _p, _i64, _p, _p, _i64, C.c_int, C.c_int, C.c_int, C.c_int, _p]),
     "dcs_gemm_view_f32": (C.c_int, [_p, C.c_int, C.c_int, _p, _p, _p]),

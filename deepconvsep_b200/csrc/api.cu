@@ -88,7 +88,7 @@ using namespace dcs;
 
 // every device buffer of a context's workspace
 template <class Ctx, class F> static void for_each_buffer(Ctx* c, F f) {
-  for (auto* b : {&c->audio, &c->X, &c->mag, &c->S, &c->stems, &c->pcm_in[0], &c->pcm_in[1], &c->pcm_out[0], &c->pcm_out[1], &c->wiener}) f(*b);
+  for (auto* b : {&c->audio, &c->X, &c->mag, &c->S, &c->stems, &c->pcm_in[0], &c->pcm_in[1], &c->pcm_out[0], &c->pcm_out[1], &c->wiener, &c->masks}) f(*b);
   for (auto& b : c->net) f(b);
 }
 
@@ -568,10 +568,17 @@ static int check_clip(const char* fn, const dcs_ctx* ctx, const dcs_model* m, co
 // channels; with `staged` also the device copies of host audio and stems.  keep (keep-channels mode of the DSD100
 // net): two STFT planes, one magnitude plane, nsrc x 2 spectra; staged: three audio planes (downmix, left, right).
 // Two-channel stems with the Wiener post-filter on: its partial sums and covariances.  masks (masks-output mode): the
-// magnitude planes and the network's buffers only -- no mixture STFT, no spectra, no Wiener workspace
+// magnitude planes and the network's buffers only -- no mixture STFT, no spectra, no Wiener workspace.  channels (with
+// masks: the downmix's masks applied to any number of channels): also the downmix, the nsrc mask planes and ONE mixture
+// STFT plane, whatever the channel count
 static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, bool staged, bool keep,
-                          cudaStream_t st, bool masks = false) {
+                          cudaStream_t st, bool masks = false, bool channels = false) {
   const int64_t plane = dcs_num_frames(L, p->hop) * dcs_padded_bins(p->N);
+  if (channels) {
+    DCS_TRY(ctx->audio.ensure((size_t)L * sizeof(float), st));
+    DCS_TRY(ctx->X.ensure((size_t)plane * sizeof(float2), st));
+    DCS_TRY(ctx->masks.ensure((size_t)m->nsrc * plane * sizeof(float), st));
+  }
   const int nx = keep ? 2 : m->nch;   // mixture STFT planes = stem planes per source
   if (!masks) DCS_TRY(ctx->X.ensure((size_t)nx * plane * sizeof(float2), st));
   DCS_TRY(ctx->mag.ensure((size_t)m->nch * plane * sizeof(float), st));
@@ -1052,6 +1059,94 @@ int dcs_separate_masks_notes(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const floa
   DCS_TRY(notes_stage(ctx, tab, &nt, st));
   return separate_clip(ctx, m, p, d_audio, L, L, nullptr, &nt, nullptr, scale_factor, overlap, patcher, d_masks, m_stride, st,
                        true);
+}
+
+// ------------------------------------------------------------------------------------ masks applied to C channels
+// what dcs_istft_masked refuses; fn names the entry point
+static int check_istft_masked(const char* fn, const dcs_stft* p, const void* d_X, int nx, int64_t x_plane, const void* d_M,
+                              int nsrc, int64_t m_stride, int64_t T, int64_t ldf, const void* d_out, int64_t Lout,
+                              int64_t out_stride) {
+  DCS_REQUIRE(p && d_X && d_M && d_out, "%s: NULL argument", fn);
+  DCS_REQUIRE(T > 0, "%s: num_frames %lld must be > 0", fn, (long long)T);
+  DCS_REQUIRE(nx >= 1 && nx <= 16, "%s: nx %d not in [1, 16]", fn, nx);
+  DCS_REQUIRE(nsrc >= 1, "%s: nsrc %d must be >= 1", fn, nsrc);
+  DCS_REQUIRE(ldf >= p->N / 2 + 1, "%s: ldf %lld < F %d", fn, (long long)ldf, p->N / 2 + 1);
+  DCS_REQUIRE(x_plane >= 0 && m_stride >= 0 && out_stride >= 0, "%s: negative stride", fn);
+  DCS_REQUIRE(nx <= 1 || x_plane >= T * ldf, "%s: x_plane %lld < num_frames * ldf %lld", fn, (long long)x_plane, (long long)(T * ldf));
+  DCS_REQUIRE(nsrc <= 1 || m_stride >= T * ldf, "%s: m_stride %lld < num_frames * ldf %lld", fn, (long long)m_stride,
+              (long long)(T * ldf));
+  DCS_REQUIRE(nsrc * nx <= 1 || out_stride >= Lout, "%s: out_stride %lld < num_out %lld", fn, (long long)out_stride, (long long)Lout);
+  DCS_REQUIRE(Lout <= (T - 1) * p->hop + p->N - p->N / 2, "%s: num_out %lld exceeds the istft length", fn, (long long)Lout);
+  DCS_REQUIRE((uintptr_t)d_X % 8 == 0, "%s: d_X not 8-byte aligned", fn);
+  DCS_REQUIRE((uintptr_t)d_M % sizeof(float) == 0, "%s: d_M not 4-byte aligned", fn);
+  return DCS_OK;
+}
+
+int dcs_istft_masked(dcs_stft* p, const dcs_complex* d_X, int nx, int64_t x_plane, const float* d_M, int nsrc, int64_t m_stride,
+                     int64_t T, int64_t ldf, float* d_out, int64_t Lout, int64_t out_stride, void* stream) {
+  DCS_TRY(check_istft_masked("dcs_istft_masked", p, d_X, nx, x_plane, d_M, nsrc, m_stride, T, ldf, d_out, Lout, out_stride));
+  DCS_CUDA(cudaSetDevice(p->ctx->device));
+  return launch_istft(p, (const float2*)d_X, nullptr, nullptr, 1.f, nsrc, T, ldf, x_plane, d_out, Lout, out_stride,
+                      (cudaStream_t)stream, d_M, m_stride, nx);
+}
+
+// what dcs_apply_masks checks beyond the plan: nx channels of L samples, nsrc mask planes of the clip's T x ldf
+static int check_apply_masks(const char* fn, const dcs_ctx* ctx, const dcs_stft* p, const float* d_audio, int nx,
+                             int64_t audio_stride, int64_t L, const float* d_masks, int nsrc, int64_t m_stride,
+                             const float* d_stems, int64_t stem_stride) {
+  DCS_REQUIRE(ctx && p && d_audio && d_masks && d_stems, "%s: NULL argument", fn);
+  DCS_REQUIRE(nx >= 1 && nx <= 16, "%s: nx %d not in [1, 16]", fn, nx);
+  DCS_REQUIRE(nsrc >= 1, "%s: nsrc %d must be >= 1", fn, nsrc);
+  DCS_REQUIRE(L > 0 && audio_stride >= L && stem_stride >= L, "%s: bad length / stride", fn);
+  return check_masks(fn, p, L, d_masks, m_stride);
+}
+
+// channel by channel through ONE mixture STFT plane of the workspace: X-only STFT of channel c, then the masked inverse
+// STFT of its nsrc stems, planes (s * nx + c)
+static int apply_masks(dcs_ctx* ctx, dcs_stft* p, const float* d_audio, int nx, int64_t audio_stride, int64_t L,
+                       const float* d_masks, int nsrc, int64_t m_stride, float* d_stems, int64_t stem_stride, cudaStream_t st) {
+  const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
+  DCS_TRY(ctx->X.ensure((size_t)plane * sizeof(float2), st));
+  float2* X = ctx->X.as<float2>();
+  for (int c = 0; c < nx; ++c) {
+    {
+      ProfScope ps(ctx, "stft_fwd", st);
+      DCS_TRY(launch_stft(p, d_audio + c * audio_stride, L, X, nullptr, nullptr, 1.f, ldf, st));
+    }
+    ProfScope ps(ctx, "istft_masked", st);
+    DCS_TRY(launch_istft(p, X, nullptr, nullptr, 1.f, nsrc, T, ldf, plane, d_stems + c * stem_stride, L, nx * stem_stride, st,
+                         d_masks, m_stride, 1));
+  }
+  return DCS_OK;
+}
+
+int dcs_apply_masks(dcs_ctx* ctx, dcs_stft* p, const float* d_audio, int nx, int64_t audio_stride, int64_t L,
+                    const float* d_masks, int nsrc, int64_t m_stride, float* d_stems, int64_t stem_stride, void* stream) {
+  DCS_TRY(check_apply_masks("dcs_apply_masks", ctx, p, d_audio, nx, audio_stride, L, d_masks, nsrc, m_stride, d_stems, stem_stride));
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  return apply_masks(ctx, p, d_audio, nx, audio_stride, L, d_masks, nsrc, m_stride, d_stems, stem_stride, (cudaStream_t)stream);
+}
+
+int dcs_separate_audio_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int nx, int64_t audio_stride,
+                                int64_t L, float scale_factor, int overlap, int patcher, float* d_stems, int64_t stem_stride,
+                                void* stream) {
+  const char* fn = "dcs_separate_audio_channels";
+  DCS_REQUIRE(!m || (m->arch != DCS_ARCH_DSD_ILD && !score_arch(m->arch)),
+              "%s does not serve architecture %d: use dcs_separate_masks* + dcs_apply_masks", fn, m->arch);
+  DCS_TRY(check_clip(fn, ctx, m, p, -1, d_audio, d_stems, L, audio_stride, stem_stride, overlap, patcher));
+  DCS_REQUIRE(nx >= 1 && nx <= 16, "%s: nx %d not in [1, 16]", fn, nx);
+  DCS_REQUIRE(!ctx->tap, "%s: a spectrum tap is set (dcs_set_spectrum_tap), and this path forms no masked spectra to copy", fn);
+  cudaStream_t st = (cudaStream_t)stream;
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  DCS_TRY(size_workspace(ctx, m, p, L, false, false, st, true, true));
+  const int64_t plane = dcs_num_frames(L, p->hop) * dcs_padded_bins(p->N);
+  float *mono = ctx->audio.as<float>(), *masks = ctx->masks.as<float>();
+  {
+    ProfScope ps(ctx, "downmix", st);
+    DCS_TRY(launch_downmix(ctx, d_audio, nx, audio_stride, L, mono, st));
+  }
+  DCS_TRY(separate_clip(ctx, m, p, mono, L, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher, masks, plane, st, true));
+  return apply_masks(ctx, p, d_audio, nx, audio_stride, L, masks, m->nsrc, plane, d_stems, stem_stride, st);
 }
 
 // ------------------------------------------------------------------------------------ Wiener post-filter

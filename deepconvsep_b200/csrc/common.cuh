@@ -83,6 +83,7 @@ struct dcs_ctx {
   std::vector<dcs_prof_rec> prof;
   // workspace of one in-flight pipeline (api.cu walks every buffer for dcs_destroy / dcs_workspace_bytes)
   dcs::DevBuf audio, X, mag, S, stems;
+  dcs::DevBuf masks;            // dcs_separate_audio_channels: the downmix's blended masks, nsrc float planes
   dcs::DevBuf net[dcs::NET_SLOTS];
   uint64_t net_sig[dcs::NET_SLOTS] = {0};   // layout signature of what each net[] buffer currently holds
   // multi-clip scheduler (dcs_separate_batch_pcm16_host): copy streams, double-buffered staging, hand-over events
@@ -198,15 +199,19 @@ namespace dcs {
 
 int launch_stft(dcs_stft* plan, const float* d_audio, int64_t L, float2* d_X, float* d_mag,
                 float* d_phase, float mag_scale, int64_t ldf, cudaStream_t st);
+// d_M set (masked inverse, d_mag / d_phase NULL): d_S is the mixture STFT of nx channels (src_stride apart), d_M the
+// float masks of nsrc sources [T][ldf] (m_stride apart); output plane s * nx + c = istft_norm(M_s * X_c)
 int launch_istft(dcs_stft* plan, const float2* d_S, const float* d_mag, const float* d_phase,
                  float polar_scale, int nsrc, int64_t T, int64_t ldf, int64_t src_stride, float* d_out,
-                 int64_t Lout, int64_t out_stride, cudaStream_t st);
+                 int64_t Lout, int64_t out_stride, cudaStream_t st, const float* d_M = nullptr, int64_t m_stride = 0,
+                 int nx = 1);
 
 int launch_stft_reg(dcs_stft* plan, const float* d_audio, int64_t L, float2* d_X, float* d_mag, float* d_phase,
                     float mag_scale, int64_t ldf, int64_t nframes, cudaStream_t st);
 bool istft_reg_supported(const dcs_stft* plan, const float* d_out, int64_t out_stride);
 int launch_istft_reg(dcs_stft* plan, const float2* d_S, int nsrc, int64_t nframes, int64_t ldf, int64_t src_stride,
-                     float* d_out, int64_t Lout, int64_t out_stride, cudaStream_t st);
+                     float* d_out, int64_t Lout, int64_t out_stride, cudaStream_t st, const float* d_M = nullptr,
+                     int64_t m_stride = 0, int nx = 1);
 
 // generic strided-operand GEMM  C = act(A*B + bias)
 struct GemmDesc {
@@ -330,6 +335,8 @@ int launch_pcm_decode_keep(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, float*
 int launch_downmix2(dcs_ctx* ctx, const float* d_audio, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st);
 int launch_pcm_encode_keep(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int64_t stem_stride, int16_t* d_out,
                            cudaStream_t st);
+// nx float planes -> (((a_0 + a_1) + a_2) + ...) * (1.0f / nx): launch_downmix2's bits at nx = 2, a copy at nx = 1
+int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st);
 
 // multichannel Wiener post-filter (wiener.cu): mixture channel c at X + c * x_plane, stem (j, c) at
 // S + (2 j + c) * src_stride, bins f < F filtered in place by `iterations` EM iterations; radius: the covariance window

@@ -73,12 +73,16 @@ stft_kernel(const float* __restrict__ audio, int64_t L, int hop, const float* __
   }
 }
 
-template <int N>
-__global__ void __launch_bounds__(N / 8)
-istft_kernel(const float2* __restrict__ S, const float* __restrict__ pmag, const float* __restrict__ pphase,
-             float polar_scale, int64_t T, int64_t ldf, int64_t src_stride, const float* __restrict__ wsyn,
-             const float* __restrict__ w2, const float2* __restrict__ tw, float* __restrict__ out, int64_t Lout,
-             int64_t out_stride, int hop, int hops_per_cta) {
+// The body of K4 and of its masked variant.  Not masked: CTA (x, y) owns span x of plane y of S (or of the polar pair).
+// MASKED: S is the mixture STFT (channel c = y at S + c * src_stride), Mk the masks (source s at Mk + s * m_stride, same
+// ldf), the spectrum M_s * X_c is formed as the row is read, output plane s * nx + c; x = span * nsrc + s, so the CTAs of
+// the nsrc sources that read the same rows of X are launched next to each other.
+template <int N, bool MASKED>
+__device__ __forceinline__ void
+istft_body(const float2* __restrict__ S, const float* __restrict__ pmag, const float* __restrict__ pphase,
+           float polar_scale, int64_t T, int64_t ldf, int64_t src_stride, const float* __restrict__ wsyn,
+           const float* __restrict__ w2, const float2* __restrict__ tw, float* __restrict__ out, int64_t Lout,
+           int64_t out_stride, int hop, int hops_per_cta, const float* __restrict__ Mk, int64_t m_stride, int nsrc, int nx) {
   constexpr int N2 = N / 2, T4 = N2 / 4;
   __shared__ __align__(16) float2 bufA[N2];
   __shared__ __align__(16) float2 bufB[N2];
@@ -88,7 +92,8 @@ istft_kernel(const float2* __restrict__ S, const float* __restrict__ pmag, const
   const int span = hops_per_cta * hop;
   // output sample i (after the first N/2 samples are dropped, transform.py:390) <-> padded
   // coordinate q = i + N/2.  This CTA owns q in [q_lo, q_lo + span).
-  const int64_t q_lo = (int64_t)blockIdx.x * span + N / 2;
+  const int msrc = MASKED ? (int)(blockIdx.x % nsrc) : 0;
+  const int64_t q_lo = (int64_t)(MASKED ? blockIdx.x / nsrc : blockIdx.x) * span + N / 2;
   for (int i = tid; i < span; i += T4) acc[i] = 0.f;
   // frames n with n*hop <= q < n*hop + N for some owned q
   int64_t n_lo = (q_lo - N) / hop + 1;  // q_lo >= N/2 > 0; for q_lo < N this is <= 0 -> clamp
@@ -104,7 +109,14 @@ istft_kernel(const float2* __restrict__ S, const float* __restrict__ pmag, const
     for (int m = 0; m < 4; ++m) {
       const int k = tid + m * T4;
       float2 xk, xn;
-      if (S) {
+      if constexpr (MASKED) {   // M * X componentwise: two roundings, never contracted into the sums that follow
+        const float* mrow = Mk + (int64_t)msrc * m_stride + n * ldf;
+        const float mk = mrow[k], mn = mrow[N2 - k];
+        xk = S[row + k];
+        xn = S[row + N2 - k];
+        xk = make_float2(__fmul_rn(mk, xk.x), __fmul_rn(mk, xk.y));
+        xn = make_float2(__fmul_rn(mn, xn.x), __fmul_rn(mn, xn.y));
+      } else if (S) {
         xk = S[row + k];
         xn = S[row + N2 - k];
       } else {
@@ -133,7 +145,7 @@ istft_kernel(const float2* __restrict__ S, const float* __restrict__ pmag, const
     }
     __syncthreads();
   }
-  float* o = out + (int64_t)src * out_stride;
+  float* o = out + (int64_t)(MASKED ? msrc * nx + src : src) * out_stride;
   for (int i = tid; i < span; i += T4) {
     const int64_t q = q_lo + i;
     const int64_t oi = q - N / 2;
@@ -147,6 +159,27 @@ istft_kernel(const float2* __restrict__ S, const float* __restrict__ pmag, const
     if (c == 0.f) c = 1.f;  // transform.py:392
     o[oi] = acc[i] / c;
   }
+}
+
+template <int N>
+__global__ void __launch_bounds__(N / 8)
+istft_kernel(const float2* __restrict__ S, const float* __restrict__ pmag, const float* __restrict__ pphase,
+             float polar_scale, int64_t T, int64_t ldf, int64_t src_stride, const float* __restrict__ wsyn,
+             const float* __restrict__ w2, const float2* __restrict__ tw, float* __restrict__ out, int64_t Lout,
+             int64_t out_stride, int hop, int hops_per_cta) {
+  istft_body<N, false>(S, pmag, pphase, polar_scale, T, ldf, src_stride, wsyn, w2, tw, out, Lout, out_stride, hop,
+                       hops_per_cta, nullptr, 0, 1, 1);
+}
+
+// K4 on M_s * X_c: X complex [nx][T][ldf] (x_plane apart), Mk float [nsrc][T][ldf] (m_stride apart); grid (spans * nsrc, nx)
+template <int N>
+__global__ void __launch_bounds__(N / 8)
+istft_masked_kernel(const float2* __restrict__ X, int64_t T, int64_t ldf, int64_t x_plane, const float* __restrict__ Mk,
+                    int64_t m_stride, int nsrc, int nx, const float* __restrict__ wsyn, const float* __restrict__ w2,
+                    const float2* __restrict__ tw, float* __restrict__ out, int64_t Lout, int64_t out_stride, int hop,
+                    int hops_per_cta) {
+  istft_body<N, true>(X, nullptr, nullptr, 1.f, T, ldf, x_plane, wsyn, w2, tw, out, Lout, out_stride, hop, hops_per_cta, Mk,
+                      m_stride, nsrc, nx);
 }
 
 __global__ void pcm_decode_kernel(const int16_t* __restrict__ pcm, int64_t L, int channels, int downmix,
@@ -194,6 +227,16 @@ __global__ void downmix2_kernel(const float* __restrict__ audio, int64_t stride,
   mono[i] = (audio[i] + audio[stride + i]) * 0.5f;
 }
 
+// nx float planes (stride apart) -> (((a_0 + a_1) + a_2) + ...) * (1.0f / nx), summed in that order: downmix2_kernel's
+// bits at nx = 2, the channel itself at nx = 1
+__global__ void downmix_kernel(const float* __restrict__ audio, int nx, int64_t stride, int64_t L, float* __restrict__ mono) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= L) return;
+  float a = audio[i];
+  for (int c = 1; c < nx; ++c) a += audio[c * stride + i];
+  mono[i] = a * (1.0f / (float)nx);
+}
+
 // stem planes (source s, channel c) at stems + (2 s + c) * stem_stride -> int16 [nsrc][L][2] (what writeAudioScipy
 // writes for a 2-channel stem), the truncation rule of pcm_encode_kernel
 __global__ void pcm_encode_keep_kernel(const float* __restrict__ stems, int64_t L, int64_t stem_stride,
@@ -236,13 +279,22 @@ int launch_stft(dcs_stft* p, const float* d_audio, int64_t L, float2* d_X, float
 template <int N>
 static int launch_istft_n(dcs_stft* p, const float2* d_S, const float* d_mag, const float* d_phase, float polar_scale,
                           int nsrc, int64_t T, int64_t ldf, int64_t src_stride, float* d_out, int64_t Lout,
-                          int64_t out_stride, cudaStream_t st) {
+                          int64_t out_stride, cudaStream_t st, const float* d_M = nullptr, int64_t m_stride = 0, int nx = 1) {
   // enough hops per CTA to amortise the N/hop-1 halo frames, small enough for many CTAs
   int hpc = 4 * (p->N / p->hop);
   if (hpc < 8) hpc = 8;
   while ((size_t)hpc * p->hop * sizeof(float) > 64 * 1024 && hpc > 1) hpc /= 2;
   const int64_t span = (int64_t)hpc * p->hop;
   const size_t dyn = (size_t)span * sizeof(float);
+  if (d_M) {   // d_S: the mixture STFT of nx channels; nsrc masks
+    dim3 grid((unsigned)(ceil_div64(Lout, span) * nsrc), (unsigned)nx);
+    DCS_TRY(ensure_smem_attr(istft_masked_kernel<N>, 96 * 1024));
+    istft_masked_kernel<N><<<grid, N / 8, dyn, st>>>(d_S, T, ldf, src_stride, d_M, m_stride, nsrc, nx, p->d_wsyn, p->d_w2,
+                                                     p->d_tw, d_out, Lout, out_stride, p->hop, hpc);
+    DCS_CHECK_LAUNCH();
+    p->ctx->launches++;
+    return DCS_OK;
+  }
   dim3 grid((unsigned)ceil_div64(Lout, span), (unsigned)nsrc);
   DCS_TRY(ensure_smem_attr(istft_kernel<N>, 96 * 1024));
   istft_kernel<N><<<grid, N / 8, dyn, st>>>(d_S, d_mag, d_phase, polar_scale, T, ldf, src_stride, p->d_wsyn, p->d_w2,
@@ -254,14 +306,16 @@ static int launch_istft_n(dcs_stft* p, const float2* d_S, const float* d_mag, co
 
 int launch_istft(dcs_stft* p, const float2* d_S, const float* d_mag, const float* d_phase, float polar_scale,
                  int nsrc, int64_t T, int64_t ldf, int64_t src_stride, float* d_out, int64_t Lout,
-                 int64_t out_stride, cudaStream_t st) {
+                 int64_t out_stride, cudaStream_t st, const float* d_M, int64_t m_stride, int nx) {
   DCS_REQUIRE(Lout <= (T - 1) * p->hop + p->N - p->N / 2, "num_out %lld exceeds the istft length", (long long)Lout);
-  if (Lout <= 0 || nsrc <= 0) return DCS_OK;
+  if (Lout <= 0 || nsrc <= 0 || nx <= 0) return DCS_OK;
+  // the register path stages rows with 16-byte cp.async: aligned spectrum rows, and aligned mask rows of whole pieces
+  const bool mask_rows_ok = !d_M || (ldf % 4 == 0 && m_stride % 4 == 0 && (uintptr_t)d_M % 16 == 0 && ldf >= p->N / 2 + 4);
   if (d_S && istft_reg_supported(p, d_out, out_stride) && ldf % 2 == 0 &&
-      src_stride % 2 == 0 && ((uintptr_t)d_S % 16 == 0) && ldf >= (p->N / 2 + 2) / 2 * 2)
-    return launch_istft_reg(p, d_S, nsrc, T, ldf, src_stride, d_out, Lout, out_stride, st);
+      src_stride % 2 == 0 && ((uintptr_t)d_S % 16 == 0) && ldf >= (p->N / 2 + 2) / 2 * 2 && mask_rows_ok)
+    return launch_istft_reg(p, d_S, nsrc, T, ldf, src_stride, d_out, Lout, out_stride, st, d_M, m_stride, nx);
 #define DCS_ISTFT_CASE(NN) \
-  case NN: return launch_istft_n<NN>(p, d_S, d_mag, d_phase, polar_scale, nsrc, T, ldf, src_stride, d_out, Lout, out_stride, st);
+  case NN: return launch_istft_n<NN>(p, d_S, d_mag, d_phase, polar_scale, nsrc, T, ldf, src_stride, d_out, Lout, out_stride, st, d_M, m_stride, nx);
   switch (p->N) {
     DCS_ISTFT_CASE(256)
     DCS_ISTFT_CASE(512)
@@ -293,6 +347,14 @@ int launch_pcm_decode_keep(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, float*
 int launch_downmix2(dcs_ctx* ctx, const float* d_audio, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st) {
   if (L <= 0) return DCS_OK;
   downmix2_kernel<<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(d_audio, audio_stride, L, d_mono);
+  DCS_CHECK_LAUNCH();
+  ctx->launches++;
+  return DCS_OK;
+}
+
+int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st) {
+  if (L <= 0) return DCS_OK;
+  downmix_kernel<<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(d_audio, nx, audio_stride, L, d_mono);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;

@@ -105,12 +105,18 @@ stft_reg_kernel(const float* __restrict__ audio, int64_t L, int hop, const float
   }
 }
 
-template <int T, int HS>  // HS = hop / 64: window slots (32 float2 each) per hop
-__global__ void __launch_bounds__(ISTFT_THREADS, 1)
-istft_reg_kernel(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int64_t src_stride,
-                 const float* __restrict__ wsyn, const float* __restrict__ w2, const float2* __restrict__ tw,
-                 float* __restrict__ out, int64_t Lout, int64_t out_stride, int hops_per_group, int64_t num_hops,
-                 int64_t groups_per_src, int64_t total_groups) {
+// The body of K4 and of its masked variant (MASKED: the spectrum is M_s * X_c, formed as the row is read).  Not masked:
+// group gi owns hops of plane gi / groups_per_src of S.  Masked: S is the mixture STFT (channel c at S + c * src_stride),
+// Mk the masks (source s at Mk + s * m_stride, same ldf), output plane s * nx + c; the source is the fastest-varying part
+// of gi, so the nsrc groups that walk the same frames of one channel are neighbours (same CTA, same wave) and their X
+// rows meet in L2 -- an ordering, not a guarantee.
+template <int T, int HS, bool MASKED>  // HS = hop / 64: window slots (32 float2 each) per hop
+__device__ __forceinline__ void
+istft_reg_body(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int64_t src_stride,
+               const float* __restrict__ wsyn, const float* __restrict__ w2, const float2* __restrict__ tw,
+               float* __restrict__ out, int64_t Lout, int64_t out_stride, int hops_per_group, int64_t num_hops,
+               int64_t groups_per_src, int64_t total_groups, const float* __restrict__ Mk, int64_t m_stride, int nsrc,
+               int nx) {
   using G = FftGroup<T>;
   constexpr int N2 = G::N2, N = 2 * N2, hop = 64 * HS, R = N / hop, C0 = (N / 2) / hop, GPC = ISTFT_THREADS / T;
   extern __shared__ __align__(16) float2 scratch[];
@@ -119,13 +125,18 @@ istft_reg_kernel(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int
   int64_t gi = (int64_t)blockIdx.x * GPC + gl;
   const bool active = gi < total_groups;
   if (!active) gi = total_groups - 1;  // keeps the warp convergent; nothing is stored
-  const int src = (int)(gi / groups_per_src);
+  int msrc = 0;   // masked: the source whose mask this group applies
+  if constexpr (MASKED) {
+    msrc = (int)(gi % nsrc);
+    gi /= nsrc;
+  }
+  const int src = (int)(gi / groups_per_src);   // plane of S (masked: the channel)
   const int64_t h0 = (gi % groups_per_src) * hops_per_group;
   const float inv_n2 = 1.0f / (float)N2;
   float2 acc[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) acc[i] = make_float2(0.f, 0.f);
-  float* o = out + (int64_t)src * out_stride;
+  float* o = out + (int64_t)(MASKED ? msrc * nx + src : src) * out_stride;
   // 1 / sum_r win*syn_win for the interior of the clip (every hop sees the same R frames)
   float2 cinv[G::Q * HS];
 #pragma unroll
@@ -152,6 +163,9 @@ istft_reg_kernel(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int
   float2* stw = scratch + GPC * (G::SCRATCH + ROWP);   // tw[0..N2): the real-FFT merge twiddles
   float2* stw2 = stw + N2;                              // inter-stage twiddles, lane-contiguous (FftGroup::fill_tw2)
   float2* swsyn = stw2 + N2;
+  // masked: the group's mask row, ROWP floats, staged like the spectrum row in 16-byte pieces covering bins 0..N2
+  constexpr int MCHUNKS = (N2 + 4) / 4;
+  float* smrow = reinterpret_cast<float*>(swsyn + N2) + gl * ROWP;
   for (int i = tid; i < N2; i += ISTFT_THREADS) stw[i] = __ldg(tw + i);
   G::fill_tw2(stw2, tw, tid, ISTFT_THREADS);
   for (int i = tid; i < N2; i += ISTFT_THREADS) swsyn[i] = __ldg(reinterpret_cast<const float2*>(wsyn) + i);
@@ -162,6 +176,13 @@ istft_reg_kernel(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int
       for (int c = b; c < CHUNKS; c += T) {
         const uint32_t dst = (uint32_t)__cvta_generic_to_shared(srow + 2 * c);
         asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(rowp + 2 * c) : "memory");
+      }
+      if constexpr (MASKED) {
+        const float* mrowp = Mk + (int64_t)msrc * m_stride + nn * ldf;
+        for (int c = b; c < MCHUNKS; c += T) {
+          const uint32_t dst = (uint32_t)__cvta_generic_to_shared(smrow + 4 * c);
+          asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(mrowp + 4 * c) : "memory");
+        }
       }
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
@@ -180,6 +201,11 @@ istft_reg_kernel(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int
       if (fvalid) {
         xk = srow[idx];
         xn = srow[N2 - idx];
+        if constexpr (MASKED) {   // M * X componentwise: two roundings, never contracted into the sums that follow
+          const float mk = smrow[idx], mn = smrow[N2 - idx];
+          xk = make_float2(__fmul_rn(mk, xk.x), __fmul_rn(mk, xk.y));
+          xn = make_float2(__fmul_rn(mn, xn.x), __fmul_rn(mn, xn.y));
+        }
       }
       if (idx == 0) { xk.y = 0.f; xn.y = 0.f; }  // irfft ignores Im of DC and Nyquist
       v[a] = real_pre_conj(xk, xn, stw[idx]);
@@ -241,6 +267,28 @@ istft_reg_kernel(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int
   }
 }
 
+template <int T, int HS>
+__global__ void __launch_bounds__(ISTFT_THREADS, 1)
+istft_reg_kernel(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int64_t src_stride,
+                 const float* __restrict__ wsyn, const float* __restrict__ w2, const float2* __restrict__ tw,
+                 float* __restrict__ out, int64_t Lout, int64_t out_stride, int hops_per_group, int64_t num_hops,
+                 int64_t groups_per_src, int64_t total_groups) {
+  istft_reg_body<T, HS, false>(S, nframes, ldf, src_stride, wsyn, w2, tw, out, Lout, out_stride, hops_per_group, num_hops,
+                               groups_per_src, total_groups, nullptr, 0, 1, 1);
+}
+
+// K4 on M_s * X_c: X complex [nx][nframes][ldf] (x_plane apart), Mk float [nsrc][nframes][ldf] (m_stride apart)
+template <int T, int HS>
+__global__ void __launch_bounds__(ISTFT_THREADS, 1)
+istft_masked_reg_kernel(const float2* __restrict__ X, int64_t nframes, int64_t ldf, int64_t x_plane,
+                        const float* __restrict__ Mk, int64_t m_stride, int nsrc, int nx, const float* __restrict__ wsyn,
+                        const float* __restrict__ w2, const float2* __restrict__ tw, float* __restrict__ out, int64_t Lout,
+                        int64_t out_stride, int hops_per_group, int64_t num_hops, int64_t groups_per_plane,
+                        int64_t total_groups) {
+  istft_reg_body<T, HS, true>(X, nframes, ldf, x_plane, wsyn, w2, tw, out, Lout, out_stride, hops_per_group, num_hops,
+                              groups_per_plane, total_groups, Mk, m_stride, nsrc, nx);
+}
+
 int launch_stft_reg(dcs_stft* p, const float* d_audio, int64_t L, float2* d_X, float* d_mag, float* d_phase,
                     float mag_scale, int64_t ldf, int64_t nframes, cudaStream_t st) {
   const int fpg = 4;
@@ -273,9 +321,12 @@ bool istft_reg_supported(const dcs_stft* p, const float* d_out, int64_t out_stri
          out_stride % 2 == 0;
 }
 
+// d_M NULL: nsrc planes of d_S.  d_M set: d_S is the mixture STFT of nx channels (src_stride apart), d_M nsrc masks
+// (m_stride apart), nsrc * nx output planes
 template <int T, int HS>
 static int launch_istft_reg_t(dcs_stft* p, const float2* d_S, int nsrc, int64_t nframes, int64_t ldf, int64_t src_stride,
-                              float* d_out, int64_t Lout, int64_t out_stride, cudaStream_t st) {
+                              float* d_out, int64_t Lout, int64_t out_stride, cudaStream_t st, const float* d_M = nullptr,
+                              int64_t m_stride = 0, int nx = 1) {
   using G = FftGroup<T>;
   constexpr int GPC = ISTFT_THREADS / T;
   const int hop = 64 * HS;
@@ -283,29 +334,43 @@ static int launch_istft_reg_t(dcs_stft* p, const float2* d_S, int nsrc, int64_t 
   // hops per group: as long as possible (each group recomputes N/hop-1 halo frames) while every SM
   // still gets its resident warps: ONE full wave of equal-sized groups
   const int64_t target_groups = (int64_t)p->ctx->num_sms * (ISTFT_THREADS / 32) * (32 / T);
-  int64_t hpg = ceil_div64((int64_t)nsrc * num_hops, target_groups);
+  const int nplanes = nsrc * nx;
+  int64_t hpg = ceil_div64((int64_t)nplanes * num_hops, target_groups);
   if (hpg < 12) hpg = 12;
   if (hpg > 64) hpg = 64;
   const int64_t groups_per_src = ceil_div64(num_hops, hpg);
-  const int64_t total = groups_per_src * nsrc;
+  const int64_t total = groups_per_src * nplanes;
   const unsigned grid = (unsigned)ceil_div64(total, GPC);
   constexpr int ROWP = (G::N2 + 1 + 7) / 8 * 8;
   const size_t smem = ((size_t)GPC * (G::SCRATCH + ROWP) + 2 * G::N2 + G::N2) * sizeof(float2);   // + twiddles + window
-  DCS_TRY(ensure_smem_attr(istft_reg_kernel<T, HS>, (int)smem));
-  istft_reg_kernel<T, HS><<<grid, ISTFT_THREADS, smem, st>>>(
-      d_S, nframes, ldf, src_stride, p->d_wsyn, p->d_w2, p->d_tw, d_out, Lout, out_stride, (int)hpg, num_hops,
-      groups_per_src, total);
+  if (d_M) {
+    const size_t smem_m = smem + (size_t)GPC * ROWP * sizeof(float);   // + a mask row per group: 191232 B (N = 2048), 181760 B (N = 1024)
+    DCS_TRY(ensure_smem_attr(istft_masked_reg_kernel<T, HS>, (int)smem_m));
+    istft_masked_reg_kernel<T, HS><<<grid, ISTFT_THREADS, smem_m, st>>>(
+        d_S, nframes, ldf, src_stride, d_M, m_stride, nsrc, nx, p->d_wsyn, p->d_w2, p->d_tw, d_out, Lout, out_stride,
+        (int)hpg, num_hops, groups_per_src, total);
+  } else {
+    DCS_TRY(ensure_smem_attr(istft_reg_kernel<T, HS>, (int)smem));
+    istft_reg_kernel<T, HS><<<grid, ISTFT_THREADS, smem, st>>>(
+        d_S, nframes, ldf, src_stride, p->d_wsyn, p->d_w2, p->d_tw, d_out, Lout, out_stride, (int)hpg, num_hops,
+        groups_per_src, total);
+  }
   DCS_CHECK_LAUNCH();
   p->ctx->launches++;
   return DCS_OK;
 }
 
 int launch_istft_reg(dcs_stft* p, const float2* d_S, int nsrc, int64_t nframes, int64_t ldf, int64_t src_stride,
-                     float* d_out, int64_t Lout, int64_t out_stride, cudaStream_t st) {
-  if (p->N == 2048 && p->hop == 512) return launch_istft_reg_t<32, 8>(p, d_S, nsrc, nframes, ldf, src_stride, d_out, Lout, out_stride, st);
-  if (p->N == 2048 && p->hop == 256) return launch_istft_reg_t<32, 4>(p, d_S, nsrc, nframes, ldf, src_stride, d_out, Lout, out_stride, st);
-  if (p->N == 1024 && p->hop == 512) return launch_istft_reg_t<16, 8>(p, d_S, nsrc, nframes, ldf, src_stride, d_out, Lout, out_stride, st);
-  if (p->N == 1024 && p->hop == 256) return launch_istft_reg_t<16, 4>(p, d_S, nsrc, nframes, ldf, src_stride, d_out, Lout, out_stride, st);
+                     float* d_out, int64_t Lout, int64_t out_stride, cudaStream_t st, const float* d_M, int64_t m_stride,
+                     int nx) {
+#define DCS_ISTFT_REG_CASE(NN, HOP) \
+  if (p->N == NN && p->hop == HOP)  \
+    return launch_istft_reg_t<NN / 64, HOP / 64>(p, d_S, nsrc, nframes, ldf, src_stride, d_out, Lout, out_stride, st, d_M, m_stride, nx);
+  DCS_ISTFT_REG_CASE(2048, 512)
+  DCS_ISTFT_REG_CASE(2048, 256)
+  DCS_ISTFT_REG_CASE(1024, 512)
+  DCS_ISTFT_REG_CASE(1024, 256)
+#undef DCS_ISTFT_REG_CASE
   DCS_REQUIRE(false, "istft_reg: unsupported frame size / hop");
 }
 

@@ -68,13 +68,36 @@ def wiener_stereo(ctx, X, S, iterations, stream=None, num_bins=None, radius=0):
     return S
 
 
-def check_stereo_options(family, keep_channels=False, wiener=0, wiener_radius=0):
+# the networks whose input is not one magnitude plane: their masks cannot come from a downmix inside the library
+MASKS_BY_HAND = ("dsd_ild", "bach10_score", "bach10_score_1x1")
+
+
+def check_channels_family(family):
+    """Separator.separate_channels (the downmix's masks applied to every channel) serves the single-channel networks;
+    raises ValueError naming the alternative for the others."""
+    if family in MASKS_BY_HAND:
+        raise ValueError("the %s network does not take a downmix: get its masks with Separator.separate_masks and apply "
+                         "them to the channels with Separator.apply_masks" % (family,))
+
+
+def check_stereo_options(family, keep_channels=False, wiener=0, wiener_radius=0, channels=None):
     """The rule for the options of two-channel stems, by network family (the keys of models.FAMILY_DEFAULTS, which
     are also the Separator's architecture names): keep_channels (the soft masks of the downmix applied to each
     channel) exists for the DSD100 / hiphopss network "dsd" only; wiener (EM iterations of the multichannel Wiener
     post-filter) cannot be negative and needs two-channel stems: keep_channels, or the stereo / ILD network
     "dsd_ild"; wiener_radius (the filter's covariance window in chunks to either side, 0 = the whole clip) cannot be
-    negative and needs wiener > 0.  Raises ValueError with the reason otherwise."""
+    negative and needs wiener > 0.  channels: the recording's channel count where it is known and keep_channels is
+    asked for -- None or 2 is the rule above; 1 is refused; C > 2 (5.1, arrays: Separator.separate_channels) is served
+    for every single-channel network, without the Wiener filter, whose 2 x 2 algebra has no C-channel form.  Raises
+    ValueError with the reason otherwise."""
+    if keep_channels and channels is not None and channels != 2:
+        if channels < 2:
+            raise ValueError("--keep-channels needs at least a 2-channel recording, this one has %d channel(s)" % channels)
+        check_channels_family(family)
+        if wiener:
+            raise ValueError("--wiener %d: the Wiener post-filter works on two-channel stems, this recording has %d "
+                             "channels" % (wiener, channels))
+        return check_wiener_radius(wiener, wiener_radius)
     if keep_channels and family != "dsd":
         raise ValueError("--keep-channels: only the DSD100 / hiphopss network (family dsd) keeps the stereo channels, "
                          "not %s" % (family,))
@@ -94,14 +117,18 @@ def check_wiener_radius(wiener, wiener_radius):
         raise ValueError("--wiener-radius needs --wiener K > 0: it is the window of the Wiener post-filter's covariances")
 
 
-def clip_call(sep, filters=None, melody=None, frame0=0, keep_channels=False, wiener=0, wiener_radius=0):
+def clip_call(sep, filters=None, melody=None, frame0=0, keep_channels=False, wiener=0, wiener_radius=0, channels=None):
     """The call that separates a whole clip with Separator `sep`'s network and these inputs, as a function of the
-    audio: sep.separate_keep_channels (keep_channels=True), sep.separate_notes (the note table melody, from table frame
+    audio: sep.separate_channels (keep_channels=True on a recording of `channels` > 2 channels),
+    sep.separate_keep_channels (keep_channels=True otherwise), sep.separate_notes (the note table melody, from table frame
     frame0), sep.separate_score (a score-informed net and its score filters), sep.separate_stereo (the stereo / ILD
     net) or sep.separate.  wiener: EM iterations of the Wiener post-filter, and wiener_radius its covariance window
     (passed only when set), given to the two-channel calls and refused for the others here, before anything runs.
     Only sep.model.arch and the method picked are used, so stand-ins with just those work too."""
     rkw = {"wiener_radius": wiener_radius} if wiener_radius else {}
+    if keep_channels and channels is not None and channels != 2:
+        check_stereo_options(sep.model.arch, True, wiener, wiener_radius, channels)
+        return sep.separate_channels
     if keep_channels:
         return partial(sep.separate_keep_channels, wiener=wiener, **rkw)
     if melody is not None:
@@ -274,6 +301,26 @@ class Stft(object):
         n = self.out_length(T) if num_out is None else int(num_out)
         out = torch.empty((nsrc, n), dtype=torch.float32, device=S.device)
         _lib.check(self.lib.dcs_istft(self.handle, _ptr(S), nsrc, T, ldf, T * ldf, _ptr(out), n, n, _stream_ptr(stream, self.device)))
+        return out
+
+    def inverse_masked(self, X, M, num_out=None, stream=None):
+        """istft_norm(M_s * X_c) with the product formed inside the kernel (dcs_istft_masked): X torch complex64 cuda
+        [nx, T, ldf] (or [T, ldf]), M float32 cuda [nsrc, T, ldf] (or [T, ldf]) with rows of the same ldf -> float32
+        [nsrc * nx, num_out], plane (s * nx + c).  The planes may be views with gaps between them; rows are contiguous."""
+        import torch
+        X = X.unsqueeze(0) if X.dim() == 2 else X
+        M = M.unsqueeze(0) if M.dim() == 2 else M
+        if X.dim() != 3 or M.dim() != 3 or tuple(X.shape[1:]) != tuple(M.shape[1:]):
+            raise ValueError("inverse_masked needs X [nx, T, ldf] and M [nsrc, T, ldf], got %r and %r" % (tuple(X.shape), tuple(M.shape)))
+        if X.dtype != torch.complex64 or M.dtype != torch.float32 or not (X.is_cuda and M.is_cuda):
+            raise ValueError("inverse_masked needs a complex64 X and a float32 M on the device")
+        nx, T, ldf = X.shape
+        if any(t.stride(2) != 1 or t.stride(1) != ldf for t in (X, M)) or ldf < self.F:
+            raise ValueError("inverse_masked needs contiguous rows of ldf >= %d" % self.F)
+        n = self.out_length(T) if num_out is None else int(num_out)
+        out = torch.empty((M.shape[0] * nx, n), dtype=torch.float32, device=X.device)
+        _lib.check(self.lib.dcs_istft_masked(self.handle, _ptr(X), nx, X.stride(0), _ptr(M), M.shape[0], M.stride(0), T, ldf,
+                                             _ptr(out), n, n, _stream_ptr(stream, self.device)))
         return out
 
     def inverse_polar(self, mag, phase, mag_scale=1.0, num_out=None, stream=None):
@@ -509,26 +556,98 @@ class Separator(object):
         """audio float [L, 2] (numpy) or [2, L] (cuda tensor) through the two-channel clip entry point `entry`, with
         `wiener` EM iterations of the Wiener post-filter over covariance windows of `wiener_radius` chunks -> float32
         [L, nsrc, 2] (numpy) or the device planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out)."""
-        import torch
         check_wiener_radius(wiener, wiener_radius)
-        host = not hasattr(audio, "is_cuda")
-        if host:
-            a = np.asarray(audio, dtype=np.float32)
-            if a.ndim != 2 or a.shape[1] != 2:
-                raise ValueError("two-channel separation needs stereo audio [L, 2], got shape %r" % (a.shape,))
-            x = torch.as_tensor(np.ascontiguousarray(a.T), device=self.stft.dev)
-        else:
-            x = audio.contiguous()
-            assert x.dim() == 2 and x.shape[0] == 2 and x.dtype == torch.float32
+        host, x, outd = self._channel_planes(audio, out, self.nsrc, 2)
         L = x.shape[1]
-        outd = out if (out is not None and not host) else torch.empty((self.nsrc * 2, L), dtype=torch.float32, device=x.device)
         self.ctx.set_wiener(wiener)
         self.ctx.set_wiener_radius(wiener_radius)
         _lib.check(entry(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), x.stride(0), L, self.scale_factor,
                          self.overlap, self.patcher, _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
+        return self._channel_stems(host, outd, out, 2)
+
+    def _channel_planes(self, audio, out, nsrc, channels=None):
+        """The marshalling of every multi-channel clip call: audio float [L, C] (numpy) or [C, L] (cuda tensor), C =
+        `channels` when given, else 1..16 -> (host: audio was numpy, x: float32 cuda planes [C, L], outd: the device stem
+        planes [nsrc * C, L], `out` itself for cuda audio)."""
+        import torch
+        host = not hasattr(audio, "is_cuda")
+        want = "%d" % channels if channels else "1 to 16"
+        if host:
+            a = np.asarray(audio, dtype=np.float32)
+            if a.ndim != 2 or not (a.shape[1] == channels if channels else 1 <= a.shape[1] <= 16):
+                raise ValueError("this call needs audio [L, C] with C = %s channels%s, got shape %r"
+                                 % (want, " (two-channel separation needs stereo audio [L, 2])" if channels == 2 else "", a.shape))
+            x = torch.as_tensor(np.ascontiguousarray(a.T), device=self.stft.dev)
+        else:
+            x = audio.contiguous()
+            if x.dim() != 2 or x.dtype != torch.float32 or not (x.shape[0] == channels if channels else 1 <= x.shape[0] <= 16):
+                raise ValueError("this call needs float32 device planes [C, L] with C = %s channels, got %r %s"
+                                 % (want, tuple(x.shape), x.dtype))
+        if x.shape[0] == 1:
+            x = x.reshape(-1).unsqueeze(0)       # a single plane still reports a plane stride of L
+        C_, L = x.shape
+        if out is not None and not host:
+            assert out.is_cuda and out.dtype == torch.float32 and tuple(out.shape) == (nsrc * C_, L) and out.stride(1) == 1
+            return host, x, out
+        return host, x, torch.empty((nsrc * C_, L), dtype=torch.float32, device=x.device)
+
+    @staticmethod
+    def _channel_stems(host, outd, out, channels):
+        """device stem planes [nsrc * C, L] ordered (source, channel) -> as they are (cuda audio), or float32
+        [L, nsrc, C] numpy (into `out` when given)"""
         if not host:
             return outd
-        return np.ascontiguousarray(outd.cpu().numpy().reshape(self.nsrc, 2, L).transpose(2, 0, 1))
+        nplanes, L = outd.shape
+        stems = outd.cpu().numpy().reshape(nplanes // channels, channels, L).transpose(2, 0, 1)
+        if out is not None:
+            out[...] = stems
+            return out
+        return np.ascontiguousarray(stems)
+
+    def separate_channels(self, audio, out=None, stream=None):
+        """Stems for any number of channels from a single-channel network (dcs_separate_audio_channels): the network
+        sees the downmix (((a_0 + a_1) + a_2) + ...) * (1 / C) in fp32, its blended soft masks are applied to the STFT
+        of every channel inside the inverse STFT -- no masked spectra in memory, a workspace that does not grow with C.
+        audio float [L, C] (numpy) or [C, L] (cuda tensor), C in 1..16 -> float32 [L, nsrc, C] (numpy; at C = 2 the
+        layout and, for the DSD100 network, the bits of separate_keep_channels) or the device planes [nsrc * C, L]
+        ordered (source, channel).  No Wiener post-filter (two-channel stems only) and no spectrum tap; the stereo /
+        ILD and score-informed networks are refused: separate_masks + apply_masks serve them."""
+        check_channels_family(self.model.arch)
+        host, x, outd = self._channel_planes(audio, out, self.nsrc)
+        C_, L = x.shape
+        _lib.check(self.lib.dcs_separate_audio_channels(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), C_,
+                                                        x.stride(0), L, self.scale_factor, self.overlap, self.patcher,
+                                                        _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
+        return self._channel_stems(host, outd, out, C_)
+
+    def apply_masks(self, audio, masks, out=None, stream=None):
+        """The caller's masks -- separate_masks' of any network, edited or not -- applied to every channel of `audio`
+        inside the inverse STFT (dcs_apply_masks): plane (s, c) = iSTFT(masks_s * STFT(channel c)).  audio float [L, C]
+        (numpy) with masks [nsrc, T, F], or device planes [C, L] with masks float32 cuda [nsrc, T, ldf] (planes may be
+        views with gaps, rows contiguous; pad columns are not read) -> float32 [L, nsrc, C] (numpy) or the device
+        planes [nsrc * C, L] ordered (source, channel).  nsrc is the masks' own: any number >= 1."""
+        import torch
+        host = not hasattr(audio, "is_cuda")
+        L = np.shape(audio)[0] if host else audio.shape[-1]
+        T, ldf, F = self.stft.num_frames(L), self.stft.ldf, self.stft.F
+        if host:
+            m = np.asarray(masks, dtype=np.float32)
+            if m.ndim != 3 or m.shape[0] < 1 or tuple(m.shape[1:]) != (T, F):
+                raise ValueError("apply_masks needs masks [nsrc, T, F] = [nsrc, %d, %d] for this audio, got %r" % (T, F, m.shape))
+            md = torch.zeros((m.shape[0], T, ldf), dtype=torch.float32, device=self.stft.dev)
+            md[:, :, :F] = torch.as_tensor(m, device=self.stft.dev)
+        else:
+            md = masks
+            if not (md.is_cuda and md.dtype == torch.float32 and md.dim() == 3 and md.shape[0] >= 1 and
+                    tuple(md.shape[1:]) == (T, ldf) and md.stride(2) == 1 and md.stride(1) == ldf):
+                raise ValueError("apply_masks needs float32 device masks [nsrc, T, ldf] = [nsrc, %d, %d] with contiguous "
+                                 "rows for this audio, got %r" % (T, ldf, tuple(md.shape)))
+        nsrc = int(md.shape[0])
+        host, x, outd = self._channel_planes(audio, out, nsrc)
+        C_ = x.shape[0]
+        _lib.check(self.lib.dcs_apply_masks(self.ctx.handle, self.stft.handle, _ptr(x), C_, x.stride(0), L, _ptr(md), nsrc,
+                                            md.stride(0), _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
+        return self._channel_stems(host, outd, out, C_)
 
     def separate_masks(self, audio, filters=None, melody=None, frame0=0, out=None, stream=None):
         """The network's blended soft masks, from a pipeline that stops before the inverse STFT (dcs_separate_masks*):

@@ -42,15 +42,32 @@ def decode(audioObj, family):
     return a if a.ndim == 1 else a[:, 0]
 
 
+def wav_channels(path):
+    """Channel count of a wav, or of the first wav of a directory, from the header (memory-mapped: nothing is read);
+    None where there is none to read."""
+    try:
+        if os.path.isdir(path):
+            path = sorted(os.path.join(path, f) for f in os.listdir(path) if f.lower().endswith(".wav"))[0]
+        a = scipy.io.wavfile.read(path, mmap=True)[1]
+        return 1 if a.ndim == 1 else int(a.shape[1])
+    except Exception:  # noqa: BLE001  (unreadable: the read in run() reports it)
+        return None
+
+
 def run(family, filein, outdir, model, scale_factor, time_context, overlap, batch_size, input_size, frame_size, hop,
         out_name, window=None, device=0, slot=0, keep_channels=False, wiener=0, wiener_radius=0):
     """wav in -> one int16 wav per source in `outdir`.  `batch_size` is accepted for signature
     compatibility; the CUDA path has no patch batches.  keep_channels (DSD100 / hiphopss, 2-channel wav): one
     2-channel wav per source -- the soft masks of the downmix applied to each channel; wiener: that many EM iterations
     of the multichannel Wiener post-filter on them (keep_channels only), wiener_radius: its covariance window in chunks
-    to either side (0 = the whole clip).  A device list cuts the recording into segments over the devices; with
+    to either side (0 = the whole clip).  keep_channels on a wav of C > 2 channels (5.1, arrays; every single-channel
+    family): one C-channel wav per source, the masks of the mean of the channels applied to each
+    (Separator.separate_channels; no Wiener filter, one device).  A device list cuts the recording into segments over the devices; with
     keep_channels and wiener that needs wiener_radius >= 1."""
-    check_stereo_options(family, keep_channels, wiener, wiener_radius)
+    nch = wav_channels(filein) if keep_channels else None
+    if nch == 1:
+        raise ValueError("--keep-channels needs at least a 2-channel recording; %s has 1 channel" % (filein,))
+    check_stereo_options(family, keep_channels, wiener, wiener_radius, channels=nch)
     wkw = {"wiener": wiener} if wiener else {}
     if wiener_radius:
         wkw["wiener_radius"] = wiener_radius
@@ -63,11 +80,18 @@ def run(family, filein, outdir, model, scale_factor, time_context, overlap, batc
         return None
     arch = None if family in ("ikala",) else family
     if keep_channels:
-        if audioObj.ndim != 2 or audioObj.shape[1] != 2:
-            raise ValueError("--keep-channels needs a 2-channel recording; %s has %d channel(s)"
-                             % (filein, 1 if audioObj.ndim == 1 else audioObj.shape[1]))
         maxv = np.finfo(audioObj.dtype).max if np.issubdtype(audioObj.dtype, np.floating) else np.iinfo(audioObj.dtype).max
-        if isinstance(device, (list, tuple)):
+        if audioObj.shape[1] > 2:
+            if isinstance(device, (list, tuple)):
+                if len(device) > 1:
+                    raise ValueError("--keep-channels on %d channels runs on one device; cutting such a recording over "
+                                     "several is not implemented" % audioObj.shape[1])
+                device = device[0]
+            sep = get_separator(model, arch, frame_size, hop, d["window"], scale_factor, time_context, overlap, input_size,
+                                device=device, slot=slot)
+            stems = sep.separate_channels(audioObj.astype('float') / maxv)              # [L, nsrc, C]
+            stems16 = (stems.transpose(1, 0, 2).astype(np.float64) * np.iinfo(np.int16).max).astype('int16')
+        elif isinstance(device, (list, tuple)):
             # one stereo recording over several GPUs: segments on the chunk grid of the Wiener filter's windows
             from .. import longclip
             seps = [get_separator(model, arch, frame_size, hop, d["window"], scale_factor, time_context, overlap, input_size,
@@ -118,7 +142,8 @@ LONG_OPTS = ["ifile=", "odir=", "mfile=", "frame-size=", "window=", "devices=", 
 EXTRA_USAGE = ("  optional: --frame-size N (STFT frame, feat_size = N/2+1)  --window hanning|blackmanharris|sinebell\n"
                "            --devices 0,1,...  --batch-clips K (clips in flight per device); with these, -i may be a directory of wavs\n"
                "            (one wav and several devices: the recording itself is cut into segments over the devices)\n"
-               "            --keep-channels (DSD100 / hiphopss, 2-channel wavs): 2-channel stems, the downmix's masks on each channel\n"
+               "            --keep-channels (DSD100 / hiphopss, 2-channel wavs): 2-channel stems, the downmix's masks on each channel;\n"
+               "            on wavs of more than 2 channels (5.1, arrays), for every script: stems of as many channels\n"
                "            --wiener K (with --keep-channels): K EM iterations of the multichannel Wiener post-filter on them\n"
                "            --wiener-radius R (with --wiener): covariances over a window of R chunks of 128 frames to either\n"
                "            side instead of the whole clip; needed to cut one recording over several devices with --wiener")
@@ -174,8 +199,11 @@ def cli_main(argv, usage, train_auto_default, run_one, family=None):
     only the DSD100 / hiphopss script, family "dsd", takes them)."""
     import sys
     o = parse_cli(argv, usage)
+    # more than 2 channels (of the wav, or of the first wav of a directory) widens --keep-channels to every
+    # single-channel family; a 1-channel file is reported by run(), with its name
+    nch = wav_channels(o["inputfile"]) if o["keep_channels"] else None
     try:
-        check_stereo_options(family, o["keep_channels"], o["wiener"], o["wiener_radius"])
+        check_stereo_options(family, o["keep_channels"], o["wiener"], o["wiener_radius"], channels=nch if nch and nch > 2 else None)
     except ValueError as e:
         sys.exit(str(e))
     one_over_devices = not os.path.isdir(o["inputfile"]) and len(o["devices"] or []) > 1

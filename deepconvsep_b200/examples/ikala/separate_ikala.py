@@ -42,8 +42,9 @@ def main(argv):
     return _common.cli_main(
         argv, USAGE,
         lambda i, o, m: train_auto(i, o, m, 0.3, 30, 20, 32, 513),   # separate_ikala.py:275
-        lambda f, o, m, N, w, dev, slot, several: _common.run(FAMILY, f, o, m, 0.3, 30, 20, 32, (N or 1024) // 2 + 1, frame_size=N or 1024, hop=512,
-                                                     out_name=lambda fn, src: fn.replace(".wav", "-" + src + ".wav"), window=w, device=dev, slot=slot))
+        lambda f, o, m, N, w, dev, slot, several, **kw: _common.run(FAMILY, f, o, m, 0.3, 30, 20, 32, (N or 1024) // 2 + 1, frame_size=N or 1024, hop=512,
+                                                     out_name=lambda fn, src: fn.replace(".wav", "-" + src + ".wav"), window=w, device=dev, slot=slot, **kw),
+        family=FAMILY)
 
 
 if __name__ == "__main__":

@@ -121,6 +121,16 @@ def _write_stems(paths, stems, sampleRate, bitrate):
         util.writeAudioScipy(path, stem.astype(np.float64), sampleRate, bitrate)
 
 
+def _first_channels(jobs):
+    """Channel count of the first mixture from its wav header; None where there is none to read."""
+    try:
+        import scipy.io.wavfile
+        a = scipy.io.wavfile.read(jobs[0][0], mmap=True)[1]
+        return 1 if a.ndim == 1 else int(a.shape[1])
+    except Exception:  # noqa: BLE001
+        return None
+
+
 def separate_dataset(family, testdir, outdir, model, scale_factor=None, time_context=30, rank=0, world_size=1, device=0,
                      keep_channels=False, wiener=0, wiener_radius=0, **overrides):
     """scale_factor: None = the family's trainer value (0.2 for bach10_score, else 0.3).
@@ -131,8 +141,10 @@ def separate_dataset(family, testdir, outdir, model, scale_factor=None, time_con
     channel of the mixture (Separator.separate_keep_channels), so that a multichannel evaluation scores real stereo
     images.  wiener (family dsd with keep_channels, or dsd_ild): that many EM iterations of the multichannel Wiener
     post-filter on the stereo stems; wiener_radius: its covariance window in chunks of 128 frames to either side
-    (0 = the whole song)."""
-    check_stereo_options(family, keep_channels, wiener, wiener_radius)
+    (0 = the whole song).  keep_channels on mixtures of C > 2 channels (any single-channel family; the first mixture
+    decides): C-channel stems, the masks of the mean of the channels applied to each (Separator.separate_channels)."""
+    nch = _first_channels(list_jobs(family, testdir, outdir)) if keep_channels and family != "bach10_score" else None
+    check_stereo_options(family, keep_channels, wiener, wiener_radius, channels=nch if nch and nch > 2 else None)
     wkw = {"wiener": wiener} if wiener else {}
     if wiener_radius:
         wkw["wiener_radius"] = wiener_radius
@@ -161,7 +173,10 @@ def separate_dataset(family, testdir, outdir, model, scale_factor=None, time_con
         else:
             audio, sampleRate, bitrate = util.readAudioScipy(wav)
             assert sampleRate == 44100, "Sample rate needs to be 44100"
-            if family == "dsd_ild" or keep_channels:             # both channels in, stereo stems out
+            if keep_channels and audio.ndim == 2 and audio.shape[1] > 2:     # C channels in, C-channel stems out
+                check_stereo_options(family, True, wiener, wiener_radius, channels=audio.shape[1])
+                stems = sep.separate_channels(audio).transpose(1, 0, 2)
+            elif family == "dsd_ild" or keep_channels:             # both channels in, stereo stems out
                 assert audio.ndim == 2 and audio.shape[1] == 2, "%s needs 2-channel mixtures" % (
                     "--keep-channels" if keep_channels else "the stereo / ILD network")
                 stereo = sep.separate_keep_channels(audio, **wkw) if keep_channels else sep.separate_stereo(audio, **wkw)
@@ -184,7 +199,8 @@ def main(argv=None):
     ap.add_argument("--scale-factor", type=float, default=None,
                     help="magnitude scale of the network input (default: 0.2 for --family bach10_score, else 0.3)")
     ap.add_argument("--keep-channels", action="store_true",
-                    help="--family dsd: 2-channel stems, the soft masks of the downmix applied to each channel")
+                    help="--family dsd: 2-channel stems, the soft masks of the downmix applied to each channel; mixtures of "
+                         "more than 2 channels, any single-channel family: stems of as many channels")
     ap.add_argument("--wiener", type=int, default=0, metavar="K",
                     help="K EM iterations of the multichannel Wiener post-filter on the stereo stems "
                          "(--family dsd --keep-channels, or --family dsd_ild)")
@@ -192,8 +208,12 @@ def main(argv=None):
                     help="with --wiener: spatial covariances over a sliding window of R chunks of 128 frames to either "
                          "side (default 0: one per song)")
     args = ap.parse_args(argv)
+    nch = None
+    if args.keep_channels and args.family != "bach10_score" and os.path.isdir(args.db):
+        nch = _first_channels(list_jobs(args.family, args.db, args.out))
     try:
-        check_stereo_options(args.family, args.keep_channels, args.wiener, args.wiener_radius)
+        check_stereo_options(args.family, args.keep_channels, args.wiener, args.wiener_radius,
+                             channels=nch if nch and nch > 2 else None)
     except ValueError as e:
         ap.error(str(e))
     world, rank, local = (int(os.environ.get(k, d)) for k, d in (("WORLD_SIZE", "1"), ("RANK", "0"), ("LOCAL_RANK", "0")))

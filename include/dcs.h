@@ -430,6 +430,48 @@ int dcs_separate_masks_notes(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, con
                              float scale_factor, int overlap, int patcher, float* d_masks, int64_t m_stride,
                              void* stream);
 
+/* ---- masks applied to any number of channels: stems for 5.1, microphone arrays, edited masks ------------------------ */
+/* istft_norm(M_s * X_c): d_X complex[nx][T][ldf] (x_plane apart), d_M float[nsrc][T][ldf] (m_stride apart, same ldf)
+ * -> d_out float[nsrc*nx][out_stride], plane (s*nx + c), the first num_out samples of each; the product is formed
+ * componentwise in fp32 as a spectrum row is loaded -- make_float2(m * x.x, m * x.y), the expression of the mask kernels
+ * -- so no masked spectrum is ever in memory and the samples are, bit for bit, those of dcs_istft on that product.  The
+ * groups of the nsrc sources that walk the same frames of one channel are launched next to each other, so that their X
+ * rows are shared through L2 rather than fetched nsrc times (an ordering, not a guarantee).
+ * Never read into the result, so free to hold anything, NaN included: Im of the DC and Nyquist bins of d_X, the pad
+ * columns F..ldf-1 of d_X and of d_M (dcs_separate_masks* leaves them unwritten), the gaps between planes.
+ * Refused with DCS_EINVAL before anything is queued: a NULL pointer, num_frames <= 0, nx outside [1, 16], nsrc < 1,
+ * ldf < N/2 + 1, a negative stride, x_plane < T*ldf with nx > 1, m_stride < T*ldf with nsrc > 1, out_stride < num_out
+ * with more than one output plane, num_out > (T-1)*hop + N - N/2, d_X not 8-byte or d_M not 4-byte aligned. */
+int dcs_istft_masked(dcs_stft* plan, const dcs_complex* d_X, int nx, int64_t x_plane, const float* d_M, int nsrc,
+                     int64_t m_stride, int64_t num_frames, int64_t ldf, float* d_out, int64_t num_out,
+                     int64_t out_stride, void* stream);
+/* The caller's masks (from dcs_separate_masks*, edited or not) applied to nx audio channels: d_audio float[nx][audio_stride]
+ * (first num_samples valid), d_masks float[nsrc][T][ldf] (T = dcs_num_frames(num_samples, hop), ldf = dcs_padded_bins(N),
+ * m_stride >= T*ldf apart) -> d_stems float[nsrc*nx][stem_stride], plane (s*nx + c) = iSTFT(M_s * STFT(channel c)).
+ * Per channel one X-only forward STFT into ONE workspace plane, then dcs_istft_masked for its nsrc planes: the workspace
+ * does not depend on nx.  nsrc is the caller's (>= 1), with no link to a model.  Refused with DCS_EINVAL before anything
+ * is queued: a NULL pointer, nx outside [1, 16], nsrc < 1, num_samples <= 0, audio_stride or stem_stride < num_samples,
+ * m_stride < T*ldf, a misaligned d_masks. */
+int dcs_apply_masks(dcs_ctx* ctx, dcs_stft* plan, const float* d_audio, int nx, int64_t audio_stride,
+                    int64_t num_samples, const float* d_masks, int nsrc, int64_t m_stride, float* d_stems,
+                    int64_t stem_stride, void* stream);
+/* Stems for nx channels from a single-channel network (every architecture but the stereo / ILD and score-informed nets,
+ * which are refused with a message naming dcs_separate_masks* + dcs_apply_masks): the network sees the downmix
+ * (((a_0 + a_1) + a_2) + ...) * (1.0f / nx) in fp32 -- (l + r) * 0.5f at nx = 2, the channel itself at nx = 1 -- and its
+ * blended masks, bit for bit those dcs_separate_masks returns for that downmix, go to every channel as in
+ * dcs_apply_masks.  d_audio float[nx][audio_stride] -> d_stems float[nsrc*nx][stem_stride], plane (s*nx + c).  At nx = 1
+ * the stems are those of dcs_separate_audio and at nx = 2 (DCS_ARCH_DSD) those of dcs_separate_audio_keep_channels,
+ * bit for bit.  The workspace holds the downmix, its magnitude, nsrc float mask planes and one mixture STFT plane: no
+ * masked spectra, and nothing that grows with nx.
+ *  - dcs_set_wiener is ignored, as by the masks calls: the 2 x 2 filter has no nx-channel form here.
+ *  - There are no masked spectra to copy: a spectrum tap set on the ctx is DCS_EINVAL before anything is queued.  The
+ *    routing tap (dcs_set_pool_tap) is honoured as by the masks calls.
+ *  - A clip shorter than one patch gives all-zero masks, so silent stems.
+ *  - Refused with DCS_EINVAL before anything is queued: nx outside [1, 16] and what dcs_separate_audio refuses. */
+int dcs_separate_audio_channels(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const float* d_audio, int nx,
+                                int64_t audio_stride, int64_t num_samples, float scale_factor, int overlap,
+                                int patcher, float* d_stems, int64_t stem_stride, void* stream);
+
 /* ---- multichannel Wiener filter with EM spatial covariances (Duong, Vincent & Gribonval 2010; util.py:633-719) -- */
 /* In place on caller-owned spectra, the plane layout of the stereo entry points: mixture channel c at d_X + c*x_plane,
  * stem (source j, channel c) at d_S + (2j + c)*src_stride, each complex[T][ldf]; only bins f < F are read or written.
