@@ -101,7 +101,7 @@ class DsdMaskView(C.Structure):
     _fields_ = [("G", _p), ("ldg", C.c_int), ("W1t", _p), ("ldw", C.c_int), ("bout", _p), ("X", _p), ("S", _p),
                 ("ldf", _i64), ("src_stride", _i64),
                 ("T", C.c_int), ("P", C.c_int), ("tc", C.c_int), ("overlap", C.c_int), ("F", C.c_int),
-                ("ndec", C.c_int), ("nx", C.c_int), ("x_plane", _i64)]
+                ("ndec", C.c_int)]
 
 
 class SconvMaskView(C.Structure):

@@ -469,55 +469,43 @@ static int dsd_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaS
   g5.kc_rows = (int)(P * ndec); g5.kc_unit = C2p; g5.kc_pad = kh2 - 1; g5.kc_n = h2; g5.kc_taps = kh2;
   { ProfScope ps(ctx, "dec_convT2_gemm", st); DCS_TRY(run_gemm(ctx, g5, ds.tWt2, st)); }
   // InverseLayer(conv1) + bias + ReLU + mask + cross-fade + phase; the stereo net: once per channel
-  // with that channel's conv1 weights, output biases and mixture STFT (trainCNN_ILD_DSD100.py:183-186).
-  // n.nx = 2 (DSD100 net, keep-channels): the downmix's masks times the STFT of each channel, planes (s * 2 + c) --
-  // one tensor-core launch for both channels, or the FFMA kernel once per channel
+  // with that channel's conv1 weights, output biases and mixture STFT (trainCNN_ILD_DSD100.py:183-186)
   ProfScope ps(ctx, "dec_convT1_mask_xfade", st);
-  const bool tc_path = !ctx->debug_simt_gemm && (tc + step - 1) / step <= 6;   // else the FFMA kernel: > 6 patches
-  const int nplanes = nch * n.nx;                                               // per frame, cross-check
+  // else the FFMA kernel: > 6 patches per frame, cross-check
+  const bool tc_path = !ctx->debug_simt_gemm && (tc + step - 1) / step <= 6;
   for (int ch = 0; ch < nch; ++ch) {
     DsdMaskArgs a;
     a.G = G; a.ldg = ldg; a.W1t = ds.W1t + (int64_t)ch * C1 * ds.ldw; a.ldw = (int)ds.ldw; a.bout = ds.bout + 4 * ch;
     a.ldf = ldf; a.T = (int)T; a.P = (int)P; a.tc = tc; a.overlap = n.overlap; a.F = m->F;
     a.ndec = ndec;
-    a.x_plane = n.x_plane;
-    if (tc_path && n.nx == 2) {
-      a.X = n.X; a.S = n.S; a.src_stride = n.src_stride; a.nx = 2;
-      DCS_REQUIRE(dsd_mask_tc_supported(a), "dsd_forward: tensor-core mask kernel does not take this shape");
-      DCS_TRY(launch_dsd_mask_tc(ctx, a, st));
-      continue;
+    a.src_stride = nch * n.src_stride;
+    float* M = nullptr;   // masks mode: plane (s * nch + ch), the layout of the spectra
+    if (n.M) {
+      a.X = nullptr; a.S = nullptr; M = n.M + ch * n.src_stride;
+    } else {
+      a.X = n.X + ch * n.x_plane; a.S = n.S + ch * n.src_stride;
     }
-    for (int c = 0; c < n.nx; ++c) {   // ch + c: the channel (nch and n.nx are never both 2)
-      a.src_stride = nplanes * n.src_stride; a.nx = 1;
-      float* M = nullptr;   // masks mode: plane (s * nch + ch), the layout of the spectra
-      if (n.M) {
-        a.X = nullptr; a.S = nullptr; M = n.M + (ch + c) * n.src_stride;
-      } else {
-        a.X = n.X + (ch + c) * n.x_plane; a.S = n.S + (ch + c) * n.src_stride;
-      }
-      if (tc_path) {
-        DCS_REQUIRE(dsd_mask_tc_supported(a), "dsd_forward: tensor-core mask kernel does not take this shape");
-        DCS_TRY(launch_dsd_mask_tc(ctx, a, st, M));
-      } else {
-        DCS_TRY(launch_dsd_mask(ctx, a, st, M));
-      }
+    if (tc_path) {
+      DCS_REQUIRE(dsd_mask_tc_supported(a), "dsd_forward: tensor-core mask kernel does not take this shape");
+      DCS_TRY(launch_dsd_mask_tc(ctx, a, st, M));
+    } else {
+      DCS_TRY(launch_dsd_mask(ctx, a, st, M));
     }
   }
   return DCS_OK;
 }
 
 // the network stage of every entry point: the input planes (plane stride in_plane) and the mixture STFT
-// (channel stride x_plane) -> masked spectra, nsrc x nch planes of stride src_stride; nx = 2 (DSD100 net only): the
-// masks applied to two mixture channels, nsrc x 2 planes (source, channel).  M (masks mode, nx = 1): the blended masks
-// instead, float planes ordered like the spectra, bins < F of each frame written; X and S are not used
+// (channel stride x_plane) -> masked spectra, nsrc x nch planes of stride src_stride.  M (masks mode): the blended
+// masks instead, float planes ordered like the spectra, bins < F of each frame written; X and S are not used
 static int run_network(dcs_ctx* ctx, const dcs_model* m, const float* in, int64_t in_plane, const float2* X, int64_t x_plane,
-                       int nx, int64_t T, int64_t ldf, int overlap, int patcher, float2* S, int64_t src_stride, cudaStream_t st,
+                       int64_t T, int64_t ldf, int overlap, int patcher, float2* S, int64_t src_stride, cudaStream_t st,
                        float* M = nullptr) {
   const bool dsd = m->arch == DCS_ARCH_DSD || m->arch == DCS_ARCH_DSD_ILD;
   NetCall n;
   n.P = dcs_num_patches(T, m->tc, overlap, patcher);
   if (n.P == 0) {  // clip shorter than one patch: nothing is predicted, every stem is silence (every mask 0)
-    for (int s = 0; s < m->nsrc * m->nch * nx; ++s) {
+    for (int s = 0; s < m->nsrc * m->nch; ++s) {
       if (M)
         DCS_CUDA(cudaMemset2DAsync(M + s * src_stride, (size_t)ldf * sizeof(float), 0, (size_t)m->F * sizeof(float), (size_t)T, st));
       else
@@ -525,7 +513,7 @@ static int run_network(dcs_ctx* ctx, const dcs_model* m, const float* in, int64_
     }
     return DCS_OK;
   }
-  n.in = in; n.in_plane = in_plane; n.X = X; n.x_plane = x_plane; n.nx = nx; n.S = S; n.src_stride = src_stride; n.M = M;
+  n.in = in; n.in_plane = in_plane; n.X = X; n.x_plane = x_plane; n.S = S; n.src_stride = src_stride; n.M = M;
   n.T = T; n.ldf = ldf; n.overlap = overlap; n.step = m->tc - overlap;
   n.Tp = std::max<int64_t>(T, (n.P - 1) * n.step + m->tc);
   // the zero-padded slots are re-zeroed when the model changes; those of the 30-channel nets also when the overlap does
@@ -565,64 +553,63 @@ static int check_clip(const char* fn, const dcs_ctx* ctx, const dcs_model* m, co
 }
 
 // the workspace of a clip of L samples: nch STFT planes, nsrc x nch masked spectra, the score-informed net's input
-// channels; with `staged` also the device copies of host audio and stems.  keep (keep-channels mode of the DSD100
-// net): two STFT planes, one magnitude plane, nsrc x 2 spectra; staged: three audio planes (downmix, left, right).
-// Two-channel stems with the Wiener post-filter on: its partial sums and covariances.  masks (masks-output mode): the
-// magnitude planes and the network's buffers only -- no mixture STFT, no spectra, no Wiener workspace.  channels (with
-// masks: the downmix's masks applied to any number of channels): also the downmix, the nsrc mask planes and ONE mixture
-// STFT plane, whatever the channel count
-static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, bool staged, bool keep,
-                          cudaStream_t st, bool masks = false, bool channels = false) {
+// channels; with `staged` also the device copies of host audio and stems.  The stereo net with the Wiener post-filter
+// on: its partial sums and covariances.  masks (masks-output mode): the magnitude planes and the network's buffers only
+// -- no mixture STFT, no spectra, no Wiener workspace
+static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, bool staged, cudaStream_t st,
+                          bool masks = false) {
   const int64_t plane = dcs_num_frames(L, p->hop) * dcs_padded_bins(p->N);
-  if (channels) {
-    DCS_TRY(ctx->audio.ensure((size_t)L * sizeof(float), st));
-    DCS_TRY(ctx->X.ensure((size_t)plane * sizeof(float2), st));
-    DCS_TRY(ctx->masks.ensure((size_t)m->nsrc * plane * sizeof(float), st));
-  }
-  const int nx = keep ? 2 : m->nch;   // mixture STFT planes = stem planes per source
-  if (!masks) DCS_TRY(ctx->X.ensure((size_t)nx * plane * sizeof(float2), st));
+  if (!masks) DCS_TRY(ctx->X.ensure((size_t)m->nch * plane * sizeof(float2), st));
   DCS_TRY(ctx->mag.ensure((size_t)m->nch * plane * sizeof(float), st));
-  if (!masks) DCS_TRY(ctx->S.ensure((size_t)m->nsrc * nx * plane * sizeof(float2), st));
+  if (!masks) DCS_TRY(ctx->S.ensure((size_t)m->nsrc * m->nch * plane * sizeof(float2), st));
   if (score_arch(m->arch)) DCS_TRY(ctx->net[NET_CHANS].ensure((size_t)score_planes(m) * plane * sizeof(float), st));
-  if (!masks && ctx->wiener_iters > 0 && m->nch * nx == 2)
+  if (!masks && ctx->wiener_iters > 0 && m->nch == 2)
     DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, dcs_num_frames(L, p->hop), m->F, ctx->wiener_radius), st));
   if (staged) {
-    DCS_TRY(ctx->audio.ensure((size_t)(keep ? 3 : 1) * L * sizeof(float), st));
-    DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * (keep ? 2 : 1) * L * sizeof(float), st));
+    DCS_TRY(ctx->audio.ensure((size_t)L * sizeof(float), st));
+    DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * L * sizeof(float), st));
   }
   return DCS_OK;
 }
 
+// the workspace of downmix_clip: the masks-output workspace, the downmix, the nsrc mask planes and ONE mixture STFT
+// plane, whatever the channel count.  wiener (two channels, the filter on): two STFT planes, nsrc x 2 masked spectra
+// and the filter's sums.  staged (the int16 keep-channels batch): three audio planes (downmix, left, right) and
+// nsrc x 2 stem planes
+static int size_downmix_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, bool wiener, bool staged,
+                                  cudaStream_t st) {
+  const int64_t plane = dcs_num_frames(L, p->hop) * dcs_padded_bins(p->N);
+  DCS_TRY(size_workspace(ctx, m, p, L, false, st, true));
+  DCS_TRY(ctx->audio.ensure((size_t)(staged ? 3 : 1) * L * sizeof(float), st));
+  DCS_TRY(ctx->masks.ensure((size_t)m->nsrc * plane * sizeof(float), st));
+  DCS_TRY(ctx->X.ensure((size_t)(wiener ? 2 : 1) * plane * sizeof(float2), st));
+  if (wiener) {
+    DCS_TRY(ctx->S.ensure((size_t)m->nsrc * 2 * plane * sizeof(float2), st));
+    DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, dcs_num_frames(L, p->hop), m->F, ctx->wiener_radius), st));
+  }
+  if (staged) DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * 2 * L * sizeof(float), st));
+  return DCS_OK;
+}
+
 // one clip, device to device: nch audio planes (audio_stride apart) -> nsrc x nch stem planes; d_filters: the
-// score filters that form the score-informed net's input channels.  d_mono (keep-channels mode, DSD100 net): the
-// downmix of the two audio planes; the network sees its magnitude, its masks are applied to the STFT of each
-// channel -> nsrc x 2 stem planes ordered (source, channel).  Two-channel stems (keep-channels, the stereo net) go
-// through the Wiener post-filter between the network and the iSTFT when dcs_set_wiener is above 0, with the covariance
-// window of dcs_set_wiener_radius.  masks (masks-output mode, not with d_mono): d_stems receives the network's blended
-// masks instead, float planes [T][ldf] stem_stride apart in the order of the stems; the STFT writes the magnitude only
-// and there is no Wiener pass, spectrum tap or iSTFT
+// score filters that form the score-informed net's input channels.  The stereo net's stems go through the Wiener
+// post-filter between the network and the iSTFT when dcs_set_wiener is above 0, with the covariance window of
+// dcs_set_wiener_radius.  masks (masks-output mode): d_stems receives the network's blended masks instead, float planes
+// [T][ldf] stem_stride apart in the order of the stems; the STFT writes the magnitude only and there is no Wiener pass,
+// spectrum tap or iSTFT
 static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,
-                         const float* d_filters, const NoteTable* notes, const float* d_mono, float scale_factor,
-                         int overlap, int patcher, float* d_stems, int64_t stem_stride, cudaStream_t st, bool masks = false) {
-  const bool keep = d_mono != nullptr;
-  DCS_TRY(size_workspace(ctx, m, p, L, false, keep, st, masks));
-  const int nch = m->nch, nx = keep ? 2 : 1;
+                         const float* d_filters, const NoteTable* notes, float scale_factor, int overlap, int patcher,
+                         float* d_stems, int64_t stem_stride, cudaStream_t st, bool masks = false) {
+  DCS_TRY(size_workspace(ctx, m, p, L, false, st, masks));
+  const int nch = m->nch;
   const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
   float2 *X = masks ? nullptr : ctx->X.as<float2>(), *S = masks ? nullptr : ctx->S.as<float2>();
   float* mag = ctx->mag.as<float>();
   {
     ProfScope ps(ctx, "stft_fwd", st);   // compute_transform: one STFT per channel (transform.py:105-119)
-    if (masks) {
-      for (int ch = 0; ch < nch; ++ch)
-        DCS_TRY(launch_stft(p, d_audio + ch * audio_stride, L, nullptr, mag + ch * plane, nullptr, scale_factor, ldf, st));
-    } else if (keep) {
-      DCS_TRY(launch_stft(p, d_mono, L, nullptr, mag, nullptr, scale_factor, ldf, st));
-      for (int c = 0; c < 2; ++c)
-        DCS_TRY(launch_stft(p, d_audio + c * audio_stride, L, X + c * plane, nullptr, nullptr, scale_factor, ldf, st));
-    } else {
-      for (int ch = 0; ch < nch; ++ch)
-        DCS_TRY(launch_stft(p, d_audio + ch * audio_stride, L, X + ch * plane, mag + ch * plane, nullptr, scale_factor, ldf, st));
-    }
+    for (int ch = 0; ch < nch; ++ch)
+      DCS_TRY(launch_stft(p, d_audio + ch * audio_stride, L, masks ? nullptr : X + ch * plane, mag + ch * plane, nullptr,
+                          scale_factor, ldf, st));
   }
   const float* in = mag;
   if (d_filters || notes) {
@@ -634,13 +621,71 @@ static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const fl
       DCS_TRY(launch_channel_mul(ctx, mag, d_filters, chans, plane, score_planes(m), st));
     in = chans;
   }
-  if (masks) return run_network(ctx, m, in, plane, nullptr, 0, 1, T, ldf, overlap, patcher, nullptr, stem_stride, st, d_stems);
-  DCS_TRY(run_network(ctx, m, in, plane, X, plane, nx, T, ldf, overlap, patcher, S, plane, st));
-  if (ctx->wiener_iters > 0 && nch * nx == 2)
+  if (masks) return run_network(ctx, m, in, plane, nullptr, 0, T, ldf, overlap, patcher, nullptr, stem_stride, st, d_stems);
+  DCS_TRY(run_network(ctx, m, in, plane, X, plane, T, ldf, overlap, patcher, S, plane, st));
+  if (ctx->wiener_iters > 0 && nch == 2)
     DCS_TRY(launch_wiener(ctx, X, plane, S, plane, m->nsrc, T, ldf, m->F, ctx->wiener_iters, ctx->wiener_radius, st));
-  DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * nch * nx * plane, st));
+  DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * nch * plane, st));
   ProfScope ps(ctx, "istft_ola", st);
-  return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc * nch * nx, T, ldf, plane, d_stems, L, stem_stride, st);
+  return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc * nch, T, ldf, plane, d_stems, L, stem_stride, st);
+}
+
+// channel by channel through ONE mixture STFT plane of the workspace: X-only STFT of channel c, then the masked inverse
+// STFT of its nsrc stems, planes (s * nx + c)
+static int apply_masks(dcs_ctx* ctx, dcs_stft* p, const float* d_audio, int nx, int64_t audio_stride, int64_t L,
+                       const float* d_masks, int nsrc, int64_t m_stride, float* d_stems, int64_t stem_stride, cudaStream_t st) {
+  const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
+  DCS_TRY(ctx->X.ensure((size_t)plane * sizeof(float2), st));
+  float2* X = ctx->X.as<float2>();
+  for (int c = 0; c < nx; ++c) {
+    {
+      ProfScope ps(ctx, "stft_fwd", st);
+      DCS_TRY(launch_stft(p, d_audio + c * audio_stride, L, X, nullptr, nullptr, 1.f, ldf, st));
+    }
+    ProfScope ps(ctx, "istft_masked", st);
+    DCS_TRY(launch_istft(p, X, nullptr, nullptr, 1.f, nsrc, T, ldf, plane, d_stems + c * stem_stride, L, nx * stem_stride, st,
+                         d_masks, m_stride, 1));
+  }
+  return DCS_OK;
+}
+
+// keep-channels without the Wiener post-filter forms no masked spectra: a spectrum tap is refused before anything is
+// queued
+static int check_keep_tap(const char* fn, const dcs_ctx* ctx) {
+  DCS_REQUIRE(!ctx->tap || ctx->wiener_iters > 0,
+              "%s: a spectrum tap is set (dcs_set_spectrum_tap), and without the Wiener post-filter this path forms no masked "
+              "spectra to copy", fn);
+  return DCS_OK;
+}
+
+// Stems of nx channels (audio_stride apart) from the masks of their downmix d_mono, single-channel nets: the network
+// in masks mode into ctx->masks, then those masks applied to every channel inside the inverse STFT, planes (s * nx + c).
+// d_mono NULL: the downmix is formed here, into ctx->audio.  wiener (keep-channels, nx = 2): with dcs_set_wiener above
+// 0 the filter's first pass forms the masked spectra M_s * X_c in memory; they are filtered, copied to the spectrum tap
+// and inverted
+static int downmix_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const float* d_mono, const float* d_audio, int nx,
+                        int64_t audio_stride, int64_t L, bool wiener, float scale_factor, int overlap, int patcher,
+                        float* d_stems, int64_t stem_stride, cudaStream_t st) {
+  const bool filter = wiener && ctx->wiener_iters > 0;
+  DCS_TRY(size_downmix_workspace(ctx, m, p, L, filter, false, st));
+  const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
+  float* masks = ctx->masks.as<float>();
+  if (!d_mono) {
+    ProfScope ps(ctx, "downmix", st);
+    DCS_TRY(launch_downmix(ctx, d_audio, nx, audio_stride, L, ctx->audio.as<float>(), st));
+    d_mono = ctx->audio.as<float>();
+  }
+  DCS_TRY(separate_clip(ctx, m, p, d_mono, L, L, nullptr, nullptr, scale_factor, overlap, patcher, masks, plane, st, true));
+  if (!filter) return apply_masks(ctx, p, d_audio, nx, audio_stride, L, masks, m->nsrc, plane, d_stems, stem_stride, st);
+  float2 *X = ctx->X.as<float2>(), *S = ctx->S.as<float2>();
+  {
+    ProfScope ps(ctx, "stft_fwd", st);
+    for (int c = 0; c < 2; ++c) DCS_TRY(launch_stft(p, d_audio + c * audio_stride, L, X + c * plane, nullptr, nullptr, 1.f, ldf, st));
+  }
+  DCS_TRY(launch_wiener(ctx, X, plane, S, plane, m->nsrc, T, ldf, m->F, ctx->wiener_iters, ctx->wiener_radius, st, masks, plane));
+  DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * 2 * plane, st));
+  ProfScope ps(ctx, "istft_ola", st);
+  return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc * 2, T, ldf, plane, d_stems, L, stem_stride, st);
 }
 
 int dcs_separate_spec(dcs_ctx* ctx, dcs_model* m, const float* d_mag, const dcs_complex* d_X, int64_t T, int64_t ldf,
@@ -649,7 +694,7 @@ int dcs_separate_spec(dcs_ctx* ctx, dcs_model* m, const float* d_mag, const dcs_
   DCS_REQUIRE(d_mag && d_X && d_S, "dcs_separate_spec: NULL argument");
   DCS_REQUIRE(T > 0 && ldf >= m->F && src_stride >= T * ldf, "dcs_separate_spec: bad shape");
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return run_network(ctx, m, d_mag, 0, (const float2*)d_X, 0, 1, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
+  return run_network(ctx, m, d_mag, 0, (const float2*)d_X, 0, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
                      (cudaStream_t)stream);
 }
 
@@ -660,7 +705,7 @@ int dcs_separate_spec_channels(dcs_ctx* ctx, dcs_model* m, const float* d_in, in
   DCS_REQUIRE(d_in && d_X && d_S, "dcs_separate_spec_channels: NULL argument");
   DCS_REQUIRE(T > 0 && ldf >= m->F && src_stride >= T * ldf && in_plane >= T * ldf, "dcs_separate_spec_channels: bad shape");
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return run_network(ctx, m, d_in, in_plane, (const float2*)d_X, 0, 1, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
+  return run_network(ctx, m, d_in, in_plane, (const float2*)d_X, 0, T, ldf, overlap, patcher, (float2*)d_S, src_stride,
                      (cudaStream_t)stream);
 }
 
@@ -670,7 +715,7 @@ int dcs_separate_audio_score(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const floa
                      overlap, patcher));
   DCS_REQUIRE(d_filters, "dcs_separate_audio_score: NULL filters");
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return separate_clip(ctx, m, p, d_audio, L, L, d_filters, nullptr, nullptr, scale_factor, overlap, patcher, d_stems,
+  return separate_clip(ctx, m, p, d_audio, L, L, d_filters, nullptr, scale_factor, overlap, patcher, d_stems,
                        stem_stride, (cudaStream_t)stream);
 }
 
@@ -701,7 +746,7 @@ int dcs_separate_audio_notes(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const floa
   cudaStream_t st = (cudaStream_t)stream;
   DCS_CUDA(cudaSetDevice(ctx->device));
   DCS_TRY(notes_stage(ctx, tab, &nt, st));
-  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, &nt, nullptr, scale_factor, overlap, patcher, d_stems, stem_stride,
+  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, &nt, scale_factor, overlap, patcher, d_stems, stem_stride,
                        st);
 }
 
@@ -767,8 +812,8 @@ int dcs_gemm_view_f32(dcs_ctx* ctx, int engine, int epi, const dcs_gemm_view* vi
 static_assert(sizeof(dcs_dsd_mask_view) == sizeof(DsdMaskArgs) && offsetof(dcs_dsd_mask_view, ldw) == offsetof(DsdMaskArgs, ldw) &&
                   offsetof(dcs_dsd_mask_view, X) == offsetof(DsdMaskArgs, X) &&
                   offsetof(dcs_dsd_mask_view, src_stride) == offsetof(DsdMaskArgs, src_stride) &&
-                  offsetof(dcs_dsd_mask_view, F) == offsetof(DsdMaskArgs, F) && offsetof(dcs_dsd_mask_view, nx) == offsetof(DsdMaskArgs, nx) &&
-                  offsetof(dcs_dsd_mask_view, x_plane) == offsetof(DsdMaskArgs, x_plane),
+                  offsetof(dcs_dsd_mask_view, F) == offsetof(DsdMaskArgs, F) &&
+                  offsetof(dcs_dsd_mask_view, ndec) == offsetof(DsdMaskArgs, ndec),
               "dcs_dsd_mask_view must mirror DsdMaskArgs");
 static_assert(sizeof(dcs_sconv_mask_view) == sizeof(SconvMaskArgs) && offsetof(dcs_sconv_mask_view, G) == offsetof(SconvMaskArgs, G) &&
                   offsetof(dcs_sconv_mask_view, S) == offsetof(SconvMaskArgs, S) &&
@@ -795,11 +840,9 @@ int dcs_dsd_mask_f32(dcs_ctx* ctx, int engine, const dcs_dsd_mask_view* view, vo
   const int64_t plane = (int64_t)a.T * a.ldf;
   DCS_REQUIRE(a.T > 0 && a.P > 0 && a.tc > a.overlap && a.overlap >= 0 && a.F >= 2 && a.ldf >= a.F && a.ldw >= a.F && a.ldg >= 50,
               "dcs_dsd_mask_f32: bad shape");
-  DCS_REQUIRE((a.ndec == 3 || a.ndec == 4) && (a.nx == 1 || (a.nx == 2 && a.ndec == 3)),
-              "dcs_dsd_mask_f32: ndec %d with nx %d (nx = 2 needs ndec = 3)", a.ndec, a.nx);
-  DCS_REQUIRE(a.src_stride >= plane && (a.nx == 1 || a.x_plane >= plane), "dcs_dsd_mask_f32: planes overlap");
+  DCS_REQUIRE(a.ndec == 3 || a.ndec == 4, "dcs_dsd_mask_f32: ndec %d not 3 or 4", a.ndec);
+  DCS_REQUIRE(a.src_stride >= plane, "dcs_dsd_mask_f32: planes overlap");
   DCS_REQUIRE((uintptr_t)a.X % 8 == 0 && (uintptr_t)a.S % 8 == 0, "dcs_dsd_mask_f32: misaligned X or S");
-  DCS_REQUIRE(engine == 1 || a.nx == 1, "dcs_dsd_mask_f32: engine 0 applies the masks to one channel per call (nx = 1)");
   DCS_REQUIRE(engine == 0 || dsd_mask_tc_supported(a),
               "dcs_dsd_mask_f32: engine 1 takes at most 6 patches per frame, ldg >= 52 with ldg %% 4 == 0 and a 16-byte aligned G");
   DCS_CUDA(cudaSetDevice(ctx->device));
@@ -847,7 +890,7 @@ int dcs_separate_audio_stereo(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const flo
   DCS_TRY(check_clip("dcs_separate_audio_stereo", ctx, m, p, DCS_ARCH_DSD_ILD, d_audio, d_stems, L, audio_stride, stem_stride,
                      overlap, patcher));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher, d_stems,
+  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, nullptr, scale_factor, overlap, patcher, d_stems,
                        stem_stride, (cudaStream_t)stream);
 }
 
@@ -862,7 +905,7 @@ int dcs_separate_audio(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_a
                        int overlap, int patcher, float* d_stems, int64_t stem_stride, void* stream) {
   DCS_TRY(check_clip("dcs_separate_audio", ctx, m, p, -1, d_audio, d_stems, L, L, stem_stride, overlap, patcher));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher, d_stems,
+  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, nullptr, scale_factor, overlap, patcher, d_stems,
                        stem_stride, (cudaStream_t)stream);
 }
 
@@ -871,9 +914,9 @@ int dcs_separate_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* h_au
   DCS_TRY(check_clip("dcs_separate_host", ctx, m, p, -1, h_audio, h_stems, L, L, stem_stride, overlap, patcher));
   cudaStream_t st = (cudaStream_t)stream;
   DCS_CUDA(cudaSetDevice(ctx->device));
-  DCS_TRY(size_workspace(ctx, m, p, L, true, false, st));
+  DCS_TRY(size_workspace(ctx, m, p, L, true, st));
   DCS_CUDA(cudaMemcpyAsync(ctx->audio.p, h_audio, (size_t)L * sizeof(float), cudaMemcpyHostToDevice, st));
-  DCS_TRY(separate_clip(ctx, m, p, ctx->audio.as<float>(), L, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher,
+  DCS_TRY(separate_clip(ctx, m, p, ctx->audio.as<float>(), L, L, nullptr, nullptr, scale_factor, overlap, patcher,
                         ctx->stems.as<float>(), L, st));
   DCS_CUDA(cudaMemcpy2DAsync(h_stems, (size_t)stem_stride * sizeof(float), ctx->stems.p, (size_t)L * sizeof(float),
                              (size_t)L * sizeof(float), m->nsrc, cudaMemcpyDeviceToHost, st));
@@ -918,12 +961,11 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, c
     if (keep) {
       DCS_TRY(launch_pcm_decode_keep(ctx, ctx->pcm_in[b].as<int16_t>(), L, audio, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
-      DCS_TRY(separate_clip(ctx, m, p, audio + L, L, L, nullptr, nullptr, audio, scale_factor, overlap, patcher, stems, L,
-                            st));
+      DCS_TRY(downmix_clip(ctx, m, p, audio, audio + L, 2, L, L, true, scale_factor, overlap, patcher, stems, L, st));
     } else {
       DCS_TRY(launch_pcm_decode(ctx, ctx->pcm_in[b].as<int16_t>(), L, channels, downmix, audio, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
-      DCS_TRY(separate_clip(ctx, m, p, audio, L, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher, stems, L,
+      DCS_TRY(separate_clip(ctx, m, p, audio, L, L, nullptr, nullptr, scale_factor, overlap, patcher, stems, L,
                             st));
     }
     if (i >= 2) DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_out[b], 0));     // D2H of clip i-2 has drained the output staging
@@ -955,6 +997,7 @@ static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, i
     Lmax = std::max(Lmax, num_samples[i]);
   }
   DCS_TRY(check_clip(fn, ctx, m, p, keep ? DCS_ARCH_DSD : -1, h_pcm, h_out, Lmax, Lmax, Lmax, overlap, patcher));
+  if (keep) DCS_TRY(check_keep_tap(fn, ctx));
   DCS_CUDA(cudaSetDevice(ctx->device));
   // each resource on its own: a call that failed half-way through this block must not leave later calls with null handles
   if (!ctx->s_h2d) DCS_CUDA(cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
@@ -971,7 +1014,10 @@ static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, i
     DCS_TRY(ctx->pcm_in[b].ensure((size_t)Lmax * channels * sizeof(int16_t), st));
     DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * (keep ? 2 : 1) * Lmax * sizeof(int16_t), st));
   }
-  DCS_TRY(size_workspace(ctx, m, p, Lmax, true, keep, st));
+  if (keep)
+    DCS_TRY(size_downmix_workspace(ctx, m, p, Lmax, ctx->wiener_iters > 0, true, st));
+  else
+    DCS_TRY(size_workspace(ctx, m, p, Lmax, true, st));
   const int rc = batch_pipeline(ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, keep, scale_factor, overlap, patcher,
                                 h_out, out_strides, st);
   // drain everything, success or not, before the host buffers go back to the caller
@@ -1002,18 +1048,12 @@ int dcs_separate_batch_pcm16_keep_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_
 int dcs_separate_audio_keep_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride,
                                      int64_t L, float scale_factor, int overlap, int patcher, float* d_stems,
                                      int64_t stem_stride, void* stream) {
-  DCS_TRY(check_clip("dcs_separate_audio_keep_channels", ctx, m, p, DCS_ARCH_DSD, d_audio, d_stems, L, audio_stride,
-                     stem_stride, overlap, patcher));
-  cudaStream_t st = (cudaStream_t)stream;
+  const char* fn = "dcs_separate_audio_keep_channels";
+  DCS_TRY(check_clip(fn, ctx, m, p, DCS_ARCH_DSD, d_audio, d_stems, L, audio_stride, stem_stride, overlap, patcher));
+  DCS_TRY(check_keep_tap(fn, ctx));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  DCS_TRY(ctx->audio.ensure((size_t)L * sizeof(float), st));
-  float* mono = ctx->audio.as<float>();
-  {
-    ProfScope ps(ctx, "downmix", st);
-    DCS_TRY(launch_downmix2(ctx, d_audio, audio_stride, L, mono, st));
-  }
-  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, nullptr, mono, scale_factor, overlap, patcher, d_stems,
-                       stem_stride, st);
+  return downmix_clip(ctx, m, p, nullptr, d_audio, 2, audio_stride, L, true, scale_factor, overlap, patcher, d_stems,
+                      stem_stride, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------ masks output
@@ -1031,7 +1071,7 @@ int dcs_separate_masks(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_a
   DCS_TRY(check_clip("dcs_separate_masks", ctx, m, p, arch, d_audio, d_masks, L, audio_stride, L, overlap, patcher));
   DCS_TRY(check_masks("dcs_separate_masks", p, L, d_masks, m_stride));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher, d_masks,
+  return separate_clip(ctx, m, p, d_audio, audio_stride, L, nullptr, nullptr, scale_factor, overlap, patcher, d_masks,
                        m_stride, (cudaStream_t)stream, true);
 }
 
@@ -1041,7 +1081,7 @@ int dcs_separate_masks_score(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const floa
   DCS_REQUIRE(d_filters, "dcs_separate_masks_score: NULL filters");
   DCS_TRY(check_masks("dcs_separate_masks_score", p, L, d_masks, m_stride));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return separate_clip(ctx, m, p, d_audio, L, L, d_filters, nullptr, nullptr, scale_factor, overlap, patcher, d_masks, m_stride,
+  return separate_clip(ctx, m, p, d_audio, L, L, d_filters, nullptr, scale_factor, overlap, patcher, d_masks, m_stride,
                        (cudaStream_t)stream, true);
 }
 
@@ -1057,7 +1097,7 @@ int dcs_separate_masks_notes(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const floa
   cudaStream_t st = (cudaStream_t)stream;
   DCS_CUDA(cudaSetDevice(ctx->device));
   DCS_TRY(notes_stage(ctx, tab, &nt, st));
-  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, &nt, nullptr, scale_factor, overlap, patcher, d_masks, m_stride, st,
+  return separate_clip(ctx, m, p, d_audio, L, L, nullptr, &nt, scale_factor, overlap, patcher, d_masks, m_stride, st,
                        true);
 }
 
@@ -1101,25 +1141,6 @@ static int check_apply_masks(const char* fn, const dcs_ctx* ctx, const dcs_stft*
   return check_masks(fn, p, L, d_masks, m_stride);
 }
 
-// channel by channel through ONE mixture STFT plane of the workspace: X-only STFT of channel c, then the masked inverse
-// STFT of its nsrc stems, planes (s * nx + c)
-static int apply_masks(dcs_ctx* ctx, dcs_stft* p, const float* d_audio, int nx, int64_t audio_stride, int64_t L,
-                       const float* d_masks, int nsrc, int64_t m_stride, float* d_stems, int64_t stem_stride, cudaStream_t st) {
-  const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
-  DCS_TRY(ctx->X.ensure((size_t)plane * sizeof(float2), st));
-  float2* X = ctx->X.as<float2>();
-  for (int c = 0; c < nx; ++c) {
-    {
-      ProfScope ps(ctx, "stft_fwd", st);
-      DCS_TRY(launch_stft(p, d_audio + c * audio_stride, L, X, nullptr, nullptr, 1.f, ldf, st));
-    }
-    ProfScope ps(ctx, "istft_masked", st);
-    DCS_TRY(launch_istft(p, X, nullptr, nullptr, 1.f, nsrc, T, ldf, plane, d_stems + c * stem_stride, L, nx * stem_stride, st,
-                         d_masks, m_stride, 1));
-  }
-  return DCS_OK;
-}
-
 int dcs_apply_masks(dcs_ctx* ctx, dcs_stft* p, const float* d_audio, int nx, int64_t audio_stride, int64_t L,
                     const float* d_masks, int nsrc, int64_t m_stride, float* d_stems, int64_t stem_stride, void* stream) {
   DCS_TRY(check_apply_masks("dcs_apply_masks", ctx, p, d_audio, nx, audio_stride, L, d_masks, nsrc, m_stride, d_stems, stem_stride));
@@ -1136,17 +1157,9 @@ int dcs_separate_audio_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const f
   DCS_TRY(check_clip(fn, ctx, m, p, -1, d_audio, d_stems, L, audio_stride, stem_stride, overlap, patcher));
   DCS_REQUIRE(nx >= 1 && nx <= 16, "%s: nx %d not in [1, 16]", fn, nx);
   DCS_REQUIRE(!ctx->tap, "%s: a spectrum tap is set (dcs_set_spectrum_tap), and this path forms no masked spectra to copy", fn);
-  cudaStream_t st = (cudaStream_t)stream;
   DCS_CUDA(cudaSetDevice(ctx->device));
-  DCS_TRY(size_workspace(ctx, m, p, L, false, false, st, true, true));
-  const int64_t plane = dcs_num_frames(L, p->hop) * dcs_padded_bins(p->N);
-  float *mono = ctx->audio.as<float>(), *masks = ctx->masks.as<float>();
-  {
-    ProfScope ps(ctx, "downmix", st);
-    DCS_TRY(launch_downmix(ctx, d_audio, nx, audio_stride, L, mono, st));
-  }
-  DCS_TRY(separate_clip(ctx, m, p, mono, L, L, nullptr, nullptr, nullptr, scale_factor, overlap, patcher, masks, plane, st, true));
-  return apply_masks(ctx, p, d_audio, nx, audio_stride, L, masks, m->nsrc, plane, d_stems, stem_stride, st);
+  return downmix_clip(ctx, m, p, nullptr, d_audio, nx, audio_stride, L, false, scale_factor, overlap, patcher, d_stems,
+                      stem_stride, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------ Wiener post-filter

@@ -179,7 +179,6 @@ bool shape_is(const int64_t* s, int nd, int want_nd, int64_t a, int64_t b = 1, i
 struct NetCall {
   const float* in; int64_t in_plane;
   const float2* X; int64_t x_plane;
-  int nx;           // mixture channels the masks apply to (2: DSD100 net in keep-channels mode, planes (s * 2 + c))
   float2* S; int64_t src_stride;
   float* M;         // masks mode (non-NULL): the blended masks, float plane p at M + p * src_stride; X and S unused
   int64_t T, ldf;
@@ -267,22 +266,19 @@ struct DsdMaskArgs {
   const float* W1t;    // [50][ldw]  W1t[c][b] = conv1.W[c,0,0,F-1-b]
   int ldw;
   const float* bout;   // [4]
-  const float2* X;     // [nx][T][ldf], channel c at X + c * x_plane
-  float2* S;           // [4][nx][T][ldf]: source s, channel c at S + (s * nx + c) * src_stride
+  const float2* X;     // [T][ldf]
+  float2* S;           // [4][T][ldf]: source s at S + s * src_stride
   int64_t ldf, src_stride;
   int T, P, tc, overlap, F;
   int ndec;            // 3: DSD100 (4th output = decoder 2, all-zero bins get 1/4); 4: one decoder per source,
                        //    all-zero bins get 0 (stereo / ILD net, one launch per channel)
-  int nx;              // mixture channels the masks are applied to: 1, or 2 (DSD100 net, stereo stems from the
-                       //    downmix's masks; tensor-core kernel only)
-  int64_t x_plane;
 };
 // every mask kernel takes a total of the rectified sources at or below this as "all sources zero" (the rule's 1/nsrc or
 // 0): the reciprocal of a subnormal total overflows, and the masks would be inf * 0 = NaN.  dsd_tc.cu tests the same value.
 constexpr float MASK_TOT_MIN = 1.2e-38f;
 // Every mask launcher has a masks-output mode: with M set, the blended masks -- the fp32 values the other mode multiplies
 // by X -- are stored instead, float plane of source s at M + s * src_stride (bins < F of each frame); X and S are not
-// read or written (nx must be 1).
+// read or written.
 int launch_dsd_mask(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st, float* M = nullptr);
 bool dsd_mask_tc_supported(const DsdMaskArgs& a);
 int launch_dsd_mask_tc(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st, float* M = nullptr);   // wgmma (dsd_tc.cu)
@@ -329,22 +325,25 @@ int launch_pcm_decode(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int channel
                       cudaStream_t st);
 int launch_pcm_encode(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int64_t stem_stride, int16_t* d_out,
                       int64_t out_stride, cudaStream_t st);
-// stereo stems: interleaved int16 [L][2] -> three float planes L apart (downmix, left, right); float left / right planes
-// -> the downmix; nsrc x 2 stem planes (source, channel) -> int16 [nsrc][L][2], source s at d_out + s * 2 * L
+// stereo stems: interleaved int16 [L][2] -> three float planes L apart (downmix, left, right); nsrc x 2 stem planes
+// (source, channel) -> int16 [nsrc][L][2], source s at d_out + s * 2 * L
 int launch_pcm_decode_keep(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, float* d_planes, cudaStream_t st);
-int launch_downmix2(dcs_ctx* ctx, const float* d_audio, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st);
 int launch_pcm_encode_keep(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int64_t stem_stride, int16_t* d_out,
                            cudaStream_t st);
-// nx float planes -> (((a_0 + a_1) + a_2) + ...) * (1.0f / nx): launch_downmix2's bits at nx = 2, a copy at nx = 1
+// nx float planes -> (((a_0 + a_1) + a_2) + ...) * (1.0f / nx): the downmix of launch_pcm_decode_keep at nx = 2, a copy
+// at nx = 1
 int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st);
 
 // multichannel Wiener post-filter (wiener.cu): mixture channel c at X + c * x_plane, stem (j, c) at
 // S + (2 j + c) * src_stride, bins f < F filtered in place by `iterations` EM iterations; radius: the covariance window
-// in chunks of DCS_WIENER_CHUNK_FRAMES frames to either side (0 = the whole clip)
+// in chunks of DCS_WIENER_CHUNK_FRAMES frames to either side (0 = the whole clip).  M set (nsrc = 4): the stems are not
+// in S yet; the first pass forms stem (j, c) as M_j * X_c (float masks [T][ldf], m_stride apart), componentwise in fp32,
+// and stores it to S
 int wiener_check(const char* fn, int nsrc, int64_t T, int64_t ldf, int F, int64_t x_plane, int64_t src_stride, int iterations,
                  int radius);
 size_t wiener_workspace_bytes(int nsrc, int64_t T, int F, int radius);
 int launch_wiener(dcs_ctx* ctx, const float2* X, int64_t x_plane, float2* S, int64_t src_stride, int nsrc, int64_t T,
-                  int64_t ldf, int F, int iterations, int radius, cudaStream_t st);
+                  int64_t ldf, int F, int iterations, int radius, cudaStream_t st, const float* M = nullptr,
+                  int64_t m_stride = 0);
 
 }  // namespace dcs

@@ -57,8 +57,6 @@ constexpr int MT_BAR_A = 4;              // + consumer: its A half of a new tile
 //           separate_dsd.py:228,258-266), 8 frames per group, 144 columns (m64n144k8);
 // NDEC = 4: the stereo / ILD net, one launch per input channel (one decoder per source, all-zero bins get 0,
 //           trainCNN_ILD_DSD100.py:99-106,183-186), 4 frames per group, 96 columns (m64n96k8).
-// NX: mixture channels the cross-faded masks are applied to -- 1, or 2 with NDEC = 3 (stereo stems from the masks of
-//     the downmix: the same m times each channel's X; GEMM, gather and cross-fade run once).
 // Value v = slot * NDEC + decoder.  Fragment (tc.cuh): d[4j + 2i + e] = D[16w + l/4 + 8i][8j + 2(l%4) + e].
 //   NDEC = 3: column 8v + f          -> thread holds frames f = 2(l%4) + e, all v: d[4v + 2i + e]
 //   NDEC = 4: column 8(v/2) + 2f + v%2 -> thread holds frame f = l%4, all v:     d[4(v/2) + 2i + v%2]
@@ -193,7 +191,7 @@ __device__ __forceinline__ void mask_slot(const float4 c, float y0, float y1, fl
 
 // the Nyquist bin of frame t from the producer's dot products of its group (f = frame in the group, xf = the group's
 // fade-table entries); MASKS: the masks themselves to M (source s at M + s * src_stride), no X read
-template <int NDEC, int NX, bool MASKS>
+template <int NDEC, bool MASKS>
 __device__ __forceinline__ void mask_nyquist_epilogue(const DsdMaskArgs& a, float* M, const float4* xf, int t, int f, const float* nyq,
                                                       float bo0, float bo1, float bo2, float bo3) {
   using MT = MaskTile<NDEC>;
@@ -211,27 +209,23 @@ __device__ __forceinline__ void mask_nyquist_epilogue(const DsdMaskArgs& a, floa
 #pragma unroll
     for (int s = 0; s < 4; ++s) M[o + s * a.src_stride] = mm[s];
   } else {
-#pragma unroll
-    for (int c = 0; c < NX; ++c) {
-      const float2 xx = a.X[c * a.x_plane + (int64_t)t * a.ldf + bin];
-      const int64_t o = (int64_t)t * a.ldf + bin + c * a.src_stride;
-      a.S[o] = make_float2(mm[0] * xx.x, mm[0] * xx.y);
-      a.S[o + NX * a.src_stride] = make_float2(mm[1] * xx.x, mm[1] * xx.y);
-      a.S[o + 2 * NX * a.src_stride] = make_float2(mm[2] * xx.x, mm[2] * xx.y);
-      a.S[o + 3 * NX * a.src_stride] = make_float2(mm[3] * xx.x, mm[3] * xx.y);
-    }
+    const int64_t o = (int64_t)t * a.ldf + bin;
+    const float2 xx = a.X[o];
+    a.S[o] = make_float2(mm[0] * xx.x, mm[0] * xx.y);
+    a.S[o + a.src_stride] = make_float2(mm[1] * xx.x, mm[1] * xx.y);
+    a.S[o + 2 * a.src_stride] = make_float2(mm[2] * xx.x, mm[2] * xx.y);
+    a.S[o + 3 * a.src_stride] = make_float2(mm[3] * xx.x, mm[3] * xx.y);
   }
 }
 
 // nyq_tiles > 0: the tiles cover bins [0, F - 1) and item (tile, g) with tile == g % nyq_tiles also computes bin F - 1
 // of group g on the producer; 0: the tiles cover all F bins.
-// MASKS (NX = 1): the cross-faded masks themselves -- the fp32 values the other mode multiplies by X -- go to M,
-// source s at M + s * src_stride; X and S are not touched.
-template <int NDEC, int NX, bool MASKS>
+// MASKS: the cross-faded masks themselves -- the fp32 values the other mode multiplies by X -- go to M, source s at
+// M + s * src_stride; X and S are not touched.
+template <int NDEC, bool MASKS>
 __global__ void __launch_bounds__(MT_THREADS, 1)
 dsd_mask_tc_kernel(const DsdMaskArgs a, float* __restrict__ M, const float4* __restrict__ xtab, int num_groups, int num_items,
                    int nyq_tiles) {
-  static_assert(!MASKS || NX == 1, "the masks do not depend on the mixture channel");
   using MT = MaskTile<NDEC>;
   constexpr int FRAMES = MT::FRAMES, TF = MT::TFRAMES;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -297,7 +291,7 @@ dsd_mask_tc_kernel(const DsdMaskArgs a, float* __restrict__ M, const float4* __r
         nb ^= 1;
         bar_sync(MT_BAR_PROD, MT_PRODUCER);
         if (ptid < FRAMES)
-          mask_nyquist_epilogue<NDEC, NX, MASKS>(a, M, sXf + (it & 3) * MT::XF, g * FRAMES + ptid, ptid, nq, bo0, bo1, bo2, bo3);
+          mask_nyquist_epilogue<NDEC, MASKS>(a, M, sXf + (it & 3) * MT::XF, g * FRAMES + ptid, ptid, nq, bo0, bo1, bo2, bo3);
       }
     }
     return;
@@ -347,7 +341,7 @@ dsd_mask_tc_kernel(const DsdMaskArgs a, float* __restrict__ M, const float4* __r
     if (wg == 0) bar_arrive(MT_BAR_TURN1, MT_CONSUMERS);
     else if (w + 1 < w_end) bar_arrive(MT_BAR_TURN0, MT_CONSUMERS);
 
-    // ---- while they run: this item's X (of every channel)
+    // ---- while they run: this item's X
     int bin[2];
     bool bok[2];
 #pragma unroll
@@ -355,17 +349,15 @@ dsd_mask_tc_kernel(const DsdMaskArgs a, float* __restrict__ M, const float4* __r
       bin[i] = tile * MT_BINS + row0 + 8 * i;
       bok[i] = bin[i] < a.F;
     }
-    float2 x[NX][TF][2];
+    float2 x[TF][2];
     if constexpr (!MASKS) {
 #pragma unroll
-      for (int c = 0; c < NX; ++c)
+      for (int e = 0; e < TF; ++e) {
+        const int t = g * FRAMES + MT::thread_frame(lane, e);
 #pragma unroll
-        for (int e = 0; e < TF; ++e) {
-          const int t = g * FRAMES + MT::thread_frame(lane, e);
-#pragma unroll
-          for (int i = 0; i < 2; ++i)
-            x[c][e][i] = (bok[i] && t < a.T) ? a.X[c * a.x_plane + (int64_t)t * a.ldf + bin[i]] : make_float2(0.f, 0.f);
-        }
+        for (int i = 0; i < 2; ++i)
+          x[e][i] = (bok[i] && t < a.T) ? a.X[(int64_t)t * a.ldf + bin[i]] : make_float2(0.f, 0.f);
+      }
     }
     wgmma_wait<0>();
     wgmma_fence_acc(acc);
@@ -399,25 +391,23 @@ dsd_mask_tc_kernel(const DsdMaskArgs a, float* __restrict__ M, const float4* __r
           }
         }
       }
-    } else {   // source s, channel c at S + (s * NX + c) * src_stride
+    } else {   // source s at S + s * src_stride
 #pragma unroll
-      for (int c = 0; c < NX; ++c)
+      for (int e = 0; e < TF; ++e) {
+        const int t = g * FRAMES + MT::thread_frame(lane, e);
 #pragma unroll
-        for (int e = 0; e < TF; ++e) {
-          const int t = g * FRAMES + MT::thread_frame(lane, e);
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            if (bok[i] && t < a.T) {
-              const float2 xx = x[c][e][i];
-              const float* mm = m[e][i];
-              const int64_t o = (int64_t)t * a.ldf + bin[i] + c * a.src_stride;
-              a.S[o] = make_float2(mm[0] * xx.x, mm[0] * xx.y);
-              a.S[o + NX * a.src_stride] = make_float2(mm[1] * xx.x, mm[1] * xx.y);
-              a.S[o + 2 * NX * a.src_stride] = make_float2(mm[2] * xx.x, mm[2] * xx.y);
-              a.S[o + 3 * NX * a.src_stride] = make_float2(mm[3] * xx.x, mm[3] * xx.y);
-            }
+        for (int i = 0; i < 2; ++i) {
+          if (bok[i] && t < a.T) {
+            const float2 xx = x[e][i];
+            const float* mm = m[e][i];
+            const int64_t o = (int64_t)t * a.ldf + bin[i];
+            a.S[o] = make_float2(mm[0] * xx.x, mm[0] * xx.y);
+            a.S[o + a.src_stride] = make_float2(mm[1] * xx.x, mm[1] * xx.y);
+            a.S[o + 2 * a.src_stride] = make_float2(mm[2] * xx.x, mm[2] * xx.y);
+            a.S[o + 3 * a.src_stride] = make_float2(mm[3] * xx.x, mm[3] * xx.y);
           }
         }
+      }
     }
   }
 }
@@ -446,16 +436,16 @@ __global__ void dsd_xfade_table_kernel(float4* __restrict__ tab, int T, int Tpad
 
 bool dsd_mask_tc_supported(const DsdMaskArgs& a) {
   const int step = a.tc - a.overlap;
-  return step > 0 && (a.ndec == 3 || a.ndec == 4) && (a.nx == 1 || (a.nx == 2 && a.ndec == 3)) && (a.tc + step - 1) / step <= MT_SLOTS && a.ldg % 4 == 0 && a.ldg >= 52 &&
+  return step > 0 && (a.ndec == 3 || a.ndec == 4) && (a.tc + step - 1) / step <= MT_SLOTS && a.ldg % 4 == 0 && a.ldg >= 52 &&
          ((uintptr_t)a.G % 16 == 0);
 }
 
 // F = 128 m + 1 (the DSD nets' F = N / 2 + 1) with m >= 1: m tiles, and the producer computes the Nyquist bin, which
 // would otherwise take a tile of its own; any other F: ceil(F / 128) tiles
-template <int NDEC, int NX, bool MASKS = false>
+template <int NDEC, bool MASKS>
 static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, float* M, cudaStream_t st) {
   using MT = MaskTile<NDEC>;
-  DCS_TRY(ensure_smem_attr(dsd_mask_tc_kernel<NDEC, NX, MASKS>, MT::SMEM));
+  DCS_TRY(ensure_smem_attr(dsd_mask_tc_kernel<NDEC, MASKS>, MT::SMEM));
   const bool nyq = a.F > MT_BINS && (a.F - 1) % MT_BINS == 0;
   const int m_tiles = nyq ? (a.F - 1) / MT_BINS : (a.F + MT_BINS - 1) / MT_BINS;
   const int num_groups = (a.T + MT::FRAMES - 1) / MT::FRAMES;
@@ -467,8 +457,8 @@ static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, float* M, cu
   dsd_xfade_table_kernel<<<(unsigned)ceil_div64((int64_t)Tpad * MT_SLOTS, 256), 256, 0, st>>>(xtab, a.T, Tpad, a.P, a.tc, a.overlap);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
-  dsd_mask_tc_kernel<NDEC, NX, MASKS><<<(unsigned)ctas, MT_THREADS, MT::SMEM, st>>>(a, M, xtab, num_groups, num_items,
-                                                                                   nyq ? m_tiles : 0);
+  dsd_mask_tc_kernel<NDEC, MASKS><<<(unsigned)ctas, MT_THREADS, MT::SMEM, st>>>(a, M, xtab, num_groups, num_items,
+                                                                               nyq ? m_tiles : 0);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;
@@ -477,12 +467,8 @@ static int launch_dsd_mask_tc_t(dcs_ctx* ctx, const DsdMaskArgs& a, float* M, cu
 int launch_dsd_mask_tc(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st, float* M) {
   if (a.T <= 0) return DCS_OK;
   DCS_REQUIRE(dsd_mask_tc_supported(a), "dsd_mask_tc: unsupported shape");
-  if (M) {
-    DCS_REQUIRE(a.nx == 1, "dsd_mask_tc: the masks are written once, not per mixture channel (nx = 1)");
-    return a.ndec == 4 ? launch_dsd_mask_tc_t<4, 1, true>(ctx, a, M, st) : launch_dsd_mask_tc_t<3, 1, true>(ctx, a, M, st);
-  }
-  if (a.ndec == 4) return launch_dsd_mask_tc_t<4, 1>(ctx, a, nullptr, st);
-  return a.nx == 2 ? launch_dsd_mask_tc_t<3, 2>(ctx, a, nullptr, st) : launch_dsd_mask_tc_t<3, 1>(ctx, a, nullptr, st);
+  if (M) return a.ndec == 4 ? launch_dsd_mask_tc_t<4, true>(ctx, a, M, st) : launch_dsd_mask_tc_t<3, true>(ctx, a, M, st);
+  return a.ndec == 4 ? launch_dsd_mask_tc_t<4, false>(ctx, a, nullptr, st) : launch_dsd_mask_tc_t<3, false>(ctx, a, nullptr, st);
 }
 
 }  // namespace dcs

@@ -220,15 +220,8 @@ __global__ void pcm_decode_keep_kernel(const int16_t* __restrict__ pcm, int64_t 
   planes[2 * L + i] = r;
 }
 
-// float left / right planes (stride apart) -> their downmix, the same expression
-__global__ void downmix2_kernel(const float* __restrict__ audio, int64_t stride, int64_t L, float* __restrict__ mono) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= L) return;
-  mono[i] = (audio[i] + audio[stride + i]) * 0.5f;
-}
-
-// nx float planes (stride apart) -> (((a_0 + a_1) + a_2) + ...) * (1.0f / nx), summed in that order: downmix2_kernel's
-// bits at nx = 2, the channel itself at nx = 1
+// nx float planes (stride apart) -> (((a_0 + a_1) + a_2) + ...) * (1.0f / nx), summed in that order: the bits of
+// pcm_decode_keep_kernel's downmix at nx = 2, the channel itself at nx = 1
 __global__ void downmix_kernel(const float* __restrict__ audio, int nx, int64_t stride, int64_t L, float* __restrict__ mono) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= L) return;
@@ -339,14 +332,6 @@ int launch_pcm_decode(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int channel
 int launch_pcm_decode_keep(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, float* d_planes, cudaStream_t st) {
   if (L <= 0) return DCS_OK;
   pcm_decode_keep_kernel<<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(d_pcm, L, d_planes);
-  DCS_CHECK_LAUNCH();
-  ctx->launches++;
-  return DCS_OK;
-}
-
-int launch_downmix2(dcs_ctx* ctx, const float* d_audio, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st) {
-  if (L <= 0) return DCS_OK;
-  downmix2_kernel<<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(d_audio, audio_stride, L, d_mono);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;

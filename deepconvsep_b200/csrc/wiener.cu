@@ -56,9 +56,11 @@ __device__ __forceinline__ void store_partials(const WienerArgs& a, const double
     for (int q = 0; q < 4; ++q) p[(int64_t)(j * 4 + q) * a.F] = acc[j][q];
 }
 
-// the network's stems -> per-chunk partial sums, and the per-block max of |x|^2
-template <int NSRC>
-__global__ void __launch_bounds__(kWienerBins) wiener_init_kernel(const WienerArgs a) {
+// the network's stems -> per-chunk partial sums, and the per-block max of |x|^2.  MASKED: the stems are formed here,
+// y_jc = M_j * x_c per component (the product the masked inverse STFT forms), source j's float mask plane at
+// M + j * m_stride, and stored to S
+template <int NSRC, bool MASKED>
+__global__ void __launch_bounds__(kWienerBins) wiener_init_kernel(const WienerArgs a, const float* __restrict__ M, int64_t m_stride) {
   const int f = blockIdx.x * kWienerBins + threadIdx.x;
   const int64_t t0 = (int64_t)blockIdx.y * kWienerFrames, t1 = min(a.T, t0 + kWienerFrames);
   double mx = 0.0;
@@ -73,7 +75,17 @@ __global__ void __launch_bounds__(kWienerBins) wiener_init_kernel(const WienerAr
       const float2 xl = a.X[o], xr = a.X[a.x_plane + o];
       mx = fmax(mx, fmax((double)xl.x * xl.x + (double)xl.y * xl.y, (double)xr.x * xr.x + (double)xr.y * xr.y));
 #pragma unroll
-      for (int j = 0; j < NSRC; ++j) accumulate(acc[j], a.S[(2 * j) * a.src_stride + o], a.S[(2 * j + 1) * a.src_stride + o]);
+      for (int j = 0; j < NSRC; ++j) {
+        if constexpr (MASKED) {
+          const float m = M[j * m_stride + o];
+          const float2 l = make_float2(__fmul_rn(m, xl.x), __fmul_rn(m, xl.y)), r = make_float2(__fmul_rn(m, xr.x), __fmul_rn(m, xr.y));
+          a.S[(2 * j) * a.src_stride + o] = l;
+          a.S[(2 * j + 1) * a.src_stride + o] = r;
+          accumulate(acc[j], l, r);
+        } else {
+          accumulate(acc[j], a.S[(2 * j) * a.src_stride + o], a.S[(2 * j + 1) * a.src_stride + o]);
+        }
+      }
     }
     store_partials<NSRC>(a, acc, f);
   }
@@ -217,13 +229,14 @@ void launch_reduce(const WienerArgs& a, int64_t n, int radius, cudaStream_t st) 
     wiener_reduce_window_kernel<<<dim3(rgrid, (unsigned)a.nchunks), kReduceThreads, 0, st>>>(a, n, min(radius, a.nchunks - 1));
 }
 
-template <int NSRC>
-int launch_wiener_n(dcs_ctx* ctx, const WienerArgs& a, int iterations, int radius, cudaStream_t st) {
+template <int NSRC, bool MASKED = false>
+int launch_wiener_n(dcs_ctx* ctx, const WienerArgs& a, int iterations, int radius, cudaStream_t st, const float* M = nullptr,
+                    int64_t m_stride = 0) {
   const dim3 grid((unsigned)a.ntiles, (unsigned)a.nchunks);
   const int64_t n = (int64_t)NSRC * 4 * a.F;
   {
     ProfScope ps(ctx, "wiener_init", st);
-    wiener_init_kernel<NSRC><<<grid, kWienerBins, 0, st>>>(a);
+    wiener_init_kernel<NSRC, MASKED><<<grid, kWienerBins, 0, st>>>(a, M, m_stride);
     DCS_CHECK_LAUNCH();
     ctx->launches++;
     launch_reduce(a, n, radius, st);
@@ -284,8 +297,9 @@ size_t wiener_workspace_bytes(int nsrc, int64_t T, int F, int radius) {
 }
 
 int launch_wiener(dcs_ctx* ctx, const float2* X, int64_t x_plane, float2* S, int64_t src_stride, int nsrc, int64_t T,
-                  int64_t ldf, int F, int iterations, int radius, cudaStream_t st) {
+                  int64_t ldf, int F, int iterations, int radius, cudaStream_t st, const float* M, int64_t m_stride) {
   if (iterations <= 0) return DCS_OK;
+  DCS_REQUIRE(!M || nsrc == 4, "wiener: stems formed from masks need nsrc 4, got %d", nsrc);
   const WienerLayout l = wiener_layout(nsrc, T, F, radius);
   DCS_TRY(ctx->wiener.ensure((size_t)l.total * sizeof(double), st));
   double* w = ctx->wiener.as<double>();
@@ -295,6 +309,7 @@ int launch_wiener(dcs_ctx* ctx, const float2* X, int64_t x_plane, float2* S, int
   a.part = w + l.part; a.Q = w + l.Q; a.pmax = w + l.pmax; a.scale = w + l.scale;
   a.q_stride = radius > 0 ? (int64_t)nsrc * 4 * F : 0;
   a.s_stride = radius > 0 ? 1 : 0;
+  if (M) return launch_wiener_n<4, true>(ctx, a, iterations, radius, st, M, m_stride);
   switch (nsrc) {
     case 1: return launch_wiener_n<1>(ctx, a, iterations, radius, st);
     case 2: return launch_wiener_n<2>(ctx, a, iterations, radius, st);

@@ -724,13 +724,22 @@ class Separator(object):
         pool=True: also the routing decisions of this call (dcs_set_pool_tap) -- max-pool net: the tie bits uint8
         [T, WP, 32]; 1x1 score net: the gate codes of conv1..conv6, a list of uint8 [rows, W, C] (gate_code_layout).
         wiener: EM iterations of the Wiener post-filter (two-channel stems only), wiener_radius its covariance window;
-        the tap then holds the filtered spectra.
+        the tap then holds the filtered spectra.  keep_channels without the filter forms no masked spectra in the
+        library: S is built here from the masks of the (l + r) * 0.5 downmix times each channel's STFT, componentwise in
+        fp32 -- the products the masked inverse STFT consumed.
         melody (score-informed nets): the note table instead of `filters`, through separate_notes(audio, melody, frame0)."""
         import torch
         run = clip_call(self, filters, melody, frame0, keep_channels, wiener, wiener_radius)
         a = np.asarray(audio)
         L = a.shape[0]
         T = self.stft.num_frames(L)
+        if keep_channels and not wiener:
+            out = run(a)
+            x = torch.as_tensor(np.ascontiguousarray(a.T, dtype=np.float32), device=self.stft.dev)
+            M = self.separate_masks((x[0] + x[1]) * 0.5)
+            X = [torch.view_as_real(self.stft.forward(x[c], want_mag=False)[0]) for c in range(2)]
+            S = torch.view_as_complex(torch.stack([X[c] * M[s, :, :, None] for s in range(self.nsrc) for c in range(2)]))
+            return out, S[:, :, :self.model.F].cpu().numpy()
         nplanes = self.nsrc * (2 if self.model.arch == "dsd_ild" or keep_channels else 1)
         tap = torch.zeros((nplanes, T, self.stft.ldf), dtype=torch.complex64, device=self.stft.dev)
         _lib.check(self.lib.dcs_set_spectrum_tap(self.ctx.handle, _ptr(tap), tap.numel()))

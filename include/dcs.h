@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DCS_VERSION 100
+#define DCS_VERSION 101
 
 /* frames per chunk of the Wiener post-filter's sums over time (dcs_wiener_stereo_windowed) */
 #define DCS_WIENER_CHUNK_FRAMES 128
@@ -82,7 +82,8 @@ int64_t dcs_launch_count(const dcs_ctx* ctx);
 /* Inspection tap (used by the parity tests): while set, every dcs_separate_audio* / *_host call on this ctx
  * also copies the blended masked spectra its inverse STFT consumed -- complex[nplanes][T][ldf],
  * ldf = dcs_padded_bins(N), nplanes = nsrc (x 2 channels, ordered (source, channel), for the stereo net and for
- * dcs_separate_*keep_channels*) -- to d_S (capacity in
+ * dcs_separate_*keep_channels* with the Wiener post-filter on; without it those form no masked spectra and refuse the
+ * tap, as dcs_separate_audio_channels does) -- to d_S (capacity in
  * elements; the call fails if it is too small).  d_S = NULL switches it off.  These are the tensors
  * `overlapadd_multi(...)/scale * exp(j*phase)` of separate_dsd.py:301-304. */
 int dcs_set_spectrum_tap(dcs_ctx* ctx, dcs_complex* d_S, int64_t capacity);
@@ -275,10 +276,9 @@ int dcs_gemm_view_f32(dcs_ctx* ctx, int engine, int epi, const dcs_gemm_view* vi
  *   W1t   [50][ldw]           W1t[c][b] = conv1.W[c, ch, 0, F-1-b] for bins b < F
  *   bout  [4]                 output biases (ndec 3: source 4 is decoder 2 with bias 4; all-zero bins get 1/4 each;
  *                             ndec 4: one decoder per source, all-zero bins get 0)
- *   X     complex [nx][T][ldf], channel c at X + c * x_plane;  S complex, source s / channel c at S + (s*nx + c) * src_stride
+ *   X     complex [T][ldf];  S complex [4][T][ldf], source s at S + s * src_stride
  *   patch k covers frames [k*(tc-overlap), k*(tc-overlap) + tc); frames no patch covers get S = 0.
- *   engine 1 takes at most 6 patches per frame, ldg >= 52 with ldg % 4 == 0 and a 16-byte aligned G; nx = 2 (the
- *   masks of one mixture applied to two channels) needs ndec 3.  engine 0 takes nx = 1 only.
+ *   engine 1 takes at most 6 patches per frame, ldg >= 52 with ldg % 4 == 0 and a 16-byte aligned G.
  *   Pad elements read: engine 1 multiplies G columns 50..51 by zero W1t rows, so they must be finite.  No other pad
  *   element (G columns >= 52, W1t columns >= F, X / S columns >= F) is read.
  */
@@ -290,8 +290,7 @@ typedef struct {
   dcs_complex* S;
   int64_t ldf, src_stride;
   int T, P, tc, overlap, F;
-  int ndec, nx;
-  int64_t x_plane;
+  int ndec;
 } dcs_dsd_mask_view;
 int dcs_dsd_mask_f32(dcs_ctx* ctx, int engine, const dcs_dsd_mask_view* view, void* stream);
 
@@ -384,9 +383,12 @@ int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan
  * is applied to the STFT X_c of channel c and inverted with that channel's phase: plane (s*2 + c) = iSTFT(M_s * X_c).
  * With l == r every channel equals the mono call's stem; (stem_L + stem_R) / 2 equals it up to STFT rounding.
  * d_audio float[2][audio_stride] (left, right; first num_samples valid) -> d_stems float[nsrc*2][stem_stride], plane
- * (s*2 + c) = source s, channel c (the layout of dcs_separate_audio_stereo).  Other architectures are refused before
- * anything is queued (the stereo / ILD net: dcs_separate_audio_stereo).  With the spectrum tap set, it holds nsrc*2
- * planes ordered (source, channel). */
+ * (s*2 + c) = source s, channel c (the layout of dcs_separate_audio_stereo).  This is dcs_separate_audio_channels at
+ * nx = 2, bit for bit, with the same workspace, and with the Wiener post-filter (dcs_set_wiener) in addition: its first
+ * pass forms the masked spectra M_s * X_c (fp32, componentwise) in memory, filters them and inverts them.  Other
+ * architectures are refused before anything is queued (the stereo / ILD net: dcs_separate_audio_stereo).  With the
+ * filter on, the spectrum tap holds the nsrc*2 filtered planes ordered (source, channel); with it off, a spectrum tap is
+ * refused before anything is queued. */
 int dcs_separate_audio_keep_channels(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const float* d_audio,
                                      int64_t audio_stride, int64_t num_samples, float scale_factor, int overlap,
                                      int patcher, float* d_stems, int64_t stem_stride, void* stream);

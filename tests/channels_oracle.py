@@ -2,10 +2,11 @@
 
 The network sees the downmix (((a_0 + a_1) + a_2) + ...) / C exactly as `oracle.pipeline.separate` runs it (float32
 scaled magnitude, the patcher, batches of 32, the soft-mask rule); its per-patch soft masks are applied to the patches
-of each channel's scaled magnitude, cross-faded with `overlapadd_multi`, and inverted with that channel's phase: the
-construction of tests/keep_channels_oracle.py for any channel count and any single-channel family, and at C = 2 with
-the DSD100 network its values exactly.  The blended masks and the kink map are those of
-tests/masks_oracle.separate_masks on the downmix."""
+of each channel's scaled magnitude, cross-faded with `overlapadd_multi`, and inverted with that channel's phase.  That
+is M~_s * X_c per (source, channel), M~_s = overlapadd_multi of the per-patch masks, formed without dividing anything by
+the downmix's magnitude (which vanishes where the channels are in anti-phase).  At C = 2 with the DSD100 network this is
+the keep-channels mode.  The blended masks and the kink map are those of tests/masks_oracle.separate_masks on the
+downmix."""
 import numpy as np
 
 from oracle import dsp, patch, nets

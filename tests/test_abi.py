@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), "libdcs.so does not export %s" % name
     assert sorted(declared) == _lib.exported_symbols()
-    assert lib.dcs_version() == 100
+    assert lib.dcs_version() == 101
 
 
 def test_no_cpu_fallback():

@@ -1,6 +1,6 @@
-"""C-channel stems without a GPU: the float64 oracle (tests/channels_oracle.py) against the keep-channels oracle, the
-shape and layout marshalling of Separator.separate_channels / apply_masks and Stft.inverse_masked against a stand-in
-library working on host memory, and the option rules of --keep-channels on recordings of more than two channels in
+"""C-channel stems without a GPU: the float64 oracle (tests/channels_oracle.py) against the mono oracle, the shape
+and layout marshalling of Separator.separate_channels / apply_masks and Stft.inverse_masked against a stand-in library
+working on host memory, and the option rules of --keep-channels on recordings of more than two channels in
 check_stereo_options, clip_call, the stand-alone scripts and the dataset runner."""
 import ctypes as C
 import os
@@ -12,7 +12,6 @@ import scipy.io.wavfile
 
 from oracle import nets, pipeline
 import channels_oracle as co
-from keep_channels_oracle import separate_keep_channels
 
 from deepconvsep_b200 import engine, runner
 from deepconvsep_b200.engine import Separator, Stft, check_stereo_options, clip_call
@@ -21,23 +20,6 @@ from deepconvsep_b200.models import FAMILY_DEFAULTS
 
 
 # ---------------------------------------------------------------------------------------------- the oracle
-@pytest.mark.parametrize("patcher", ["standalone", "util"])
-def test_oracle_at_two_channels_is_the_keep_channels_oracle(patcher):
-    N, hop = 512, 256
-    params = nets.make_synthetic_params("dsd", N // 2 + 1, seed=12)
-    a, _ = pipeline.synth_mixture(1.0, 21)
-    b, _ = pipeline.synth_mixture(1.0, 22)
-    audio = np.stack([0.7 * a + 0.3 * b, 0.4 * a - 0.6 * np.roll(b, 11)], axis=1)
-    kw = dict(frameSize=N, hopSize=hop, overlap=25, patcher=patcher)
-    stems, mags, phs, mms, masks, kmap = co.separate_channels(audio, params, **kw)
-    k_stems, k_mags, k_phs, k_mms, k_kmap = separate_keep_channels(audio, params, **kw)
-    assert stems.shape == (len(a), 4, 2) and np.array_equal(stems, k_stems) and np.linalg.norm(stems) > 0
-    for c in range(2):
-        assert np.array_equal(mags[c], k_mags[c]) and np.array_equal(phs[c], k_phs[c]) and np.array_equal(mms[c], k_mms[c])
-    T = masks.shape[1]
-    assert np.array_equal(kmap, k_kmap) and np.array_equal(masks, separate_keep_channels.last_masks[:, :T])
-
-
 def test_oracle_one_channel_is_the_mono_oracle_and_six_share_the_masks():
     N, hop = 512, 256
     params = nets.make_synthetic_params("dsd", N // 2 + 1, seed=3)

@@ -174,7 +174,7 @@ def test_workspace_is_independent_of_the_channel_count_and_the_tap_is_refused():
     plane = T * ldf
     # the masks call's buffers (magnitude, network) + the downmix, ONE mixture STFT plane and the nsrc mask planes
     assert ws["c6"] == ws["masks"] + rounded(4 * L) + rounded(8 * plane) + rounded(4 * 4 * plane), ws
-    assert ws["c6"] == ws["c2"] and ws["c6"] < ws["keep"]
+    assert ws["c6"] == ws["c2"] == ws["keep"]              # keep-channels is the C = 2 path
     record("channels_workspace_N2048_30s", **ws)
     # a spectrum tap on the ctx: refused before anything is queued
     tap = torch.zeros((4, T, ldf), dtype=torch.complex64, device="cuda")

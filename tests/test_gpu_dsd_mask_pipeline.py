@@ -10,7 +10,7 @@ device's SM count S, put the schedule at its edges:
 - 2 S and 3 S items: every CTA runs an even or an odd number of items, so the last item ends on either consumer;
 - a CTA range that starts on the last item of a tile: the consumers reload A after their first item;
 - F = 129: one full tile and the Nyquist bin is all there is;
-- F = 513 and F = 2049 with the DSD100 net (3 decoders) on one and two mixture channels and the stereo net (4).
+- F = 513 and F = 2049 with the DSD100 net (3 decoders) and the stereo net (4).
 
 Every case runs twice with identical bits, leaves the NaN sentinels around and between the output planes untouched,
 and reports the worst error / bound ratio at the Nyquist bin apart from the bins below it."""
@@ -47,20 +47,18 @@ def _tile_last_start(F, ndec, sms, t_min):
     raise AssertionError("no such T")
 
 
-# name -> (F, T(S), ndec, nx)
+# name -> (F, T(S), ndec)
 CASES = {
-    "items_sms_plus_1": lambda S: (129, 8 * S + 3, 3, 1),
-    "items_2sms_even": lambda S: (129, 16 * S, 3, 1),
-    "items_3sms_odd": lambda S: (129, 24 * S, 3, 1),
-    "ild_items_3sms_odd": lambda S: (129, 12 * S, 4, 1),
-    "range_starts_on_tile_last": lambda S: (257, _tile_last_start(257, 3, S, 4 * S), 3, 1),
-    "F129": lambda S: (129, 300, 3, 1),
-    "F513": lambda S: (513, 200, 3, 1),
-    "F513_keep": lambda S: (513, 200, 3, 2),
-    "F513_ild": lambda S: (513, 150, 4, 1),
-    "F2049": lambda S: (2049, 150, 3, 1),
-    "F2049_keep": lambda S: (2049, 150, 3, 2),
-    "F2049_ild": lambda S: (2049, 101, 4, 1),
+    "items_sms_plus_1": lambda S: (129, 8 * S + 3, 3),
+    "items_2sms_even": lambda S: (129, 16 * S, 3),
+    "items_3sms_odd": lambda S: (129, 24 * S, 3),
+    "ild_items_3sms_odd": lambda S: (129, 12 * S, 4),
+    "range_starts_on_tile_last": lambda S: (257, _tile_last_start(257, 3, S, 4 * S), 3),
+    "F129": lambda S: (129, 300, 3),
+    "F513": lambda S: (513, 200, 3),
+    "F513_ild": lambda S: (513, 150, 4),
+    "F2049": lambda S: (2049, 150, 3),
+    "F2049_ild": lambda S: (2049, 101, 4),
 }
 
 
@@ -83,8 +81,8 @@ def _bins(ref, sl):
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_mask_pipeline_edges_match_float64(ctx, name):
-    F, T, ndec, nx = CASES[name](_sms())
-    case = dsd_case("pipeline_" + name, F, T, 30, 25, ndec=ndec, nx=nx)
+    F, T, ndec = CASES[name](_sms())
+    case = dsd_case("pipeline_" + name, F, T, 30, 25, ndec=ndec)
     case["engine"] = "tc"
     b = Buffers(case)
     Sb = _run(ctx, case, b, 1)
@@ -113,7 +111,7 @@ def test_mask_pipeline_edges_match_float64(ctx, name):
                 wo, fa = evaluate(_bins(ref, sl), S[idx][:, :, sl], case["X"][xpl][:, sl])
                 worst[part] = max(worst[part], wo)
                 fails += ["%s: %s" % (part, f) for f in fa]
-    record("mask_pipeline:" + name, F=F, T=T, ndec=ndec, nx=nx, well_conditioned=wf,
+    record("mask_pipeline:" + name, F=F, T=T, ndec=ndec, well_conditioned=wf,
            worst_error_over_bound=max(worst.values()), worst_below_nyquist=worst["below"],
            worst_at_nyquist=worst["nyquist"])
     assert not fails, (name, fails)

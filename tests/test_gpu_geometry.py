@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 
 from oracle import dsp, nets, pipeline  # noqa: E402
 from parity import strict_check  # noqa: E402
-from keep_channels_oracle import separate_keep_channels  # noqa: E402
+from channels_oracle import separate_channels  # noqa: E402
 
 
 def slots(tc, overlap):
@@ -123,15 +123,15 @@ def test_ild_geometry(tc, overlap):
 
 
 def test_keep_channels_tc23_5slots_nx2_wgmma():
-    """keep-channels mode (the <3, 2> tensor-core mask kernel: one launch for both channels) at time_context 23,
-    overlap 18: 5 patches per frame"""
+    """keep-channels mode (the downmix's masks from the tensor-core mask kernel, applied to both channels) at
+    time_context 23, overlap 18: 5 patches per frame"""
     from deepconvsep_b200.engine import Separator
     N, hop, F, tc, overlap = 1024, 512, 513, 23, 18
     params = nets.make_synthetic_params("dsd", F, tc=tc, seed=123)
     sep = Separator(params, frame_size=N, hop=hop, window="hanning", time_context=tc, overlap=overlap)
     audio = stereo_clip(1.5, 321)
-    want, mags, phs, mms, kmap = separate_keep_channels(audio, params, frameSize=N, hopSize=hop, time_context=tc,
-                                                        overlap=overlap)
+    want, mags, phs, mms, _, kmap = separate_channels(audio, params, frameSize=N, hopSize=hop, time_context=tc,
+                                                      overlap=overlap)
     got, S = sep.separate_tapped(audio, keep_channels=True)
     assert got.shape == want.shape == (audio.shape[0], 4, 2) and got.dtype == np.float32
     for c in range(2):

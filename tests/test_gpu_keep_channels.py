@@ -1,14 +1,15 @@
 """Keep-channels mode of the DSD100 / hiphopss network on the GPU (dcs_separate_audio_keep_channels,
 dcs_separate_batch_pcm16_keep_channels_host): the soft masks of the downmix (l + r) * 0.5f applied to the STFT of each
-channel by the <3,2> instantiation of the wgmma mask kernel (dsd_tc.cu), or by its FFMA twin (dsd.cu) once per channel.
+channel inside the masked inverse STFT (the C-channel path at C = 2); the masks come from the wgmma mask kernel
+(dsd_tc.cu) in masks mode, or from its FFMA twin (dsd.cu).
 
 - equal channels: each output channel is byte-identical to the mono call;
-- parity per (source, channel) against the float64 oracle (tests/keep_channels_oracle.py) under tests/parity.strict_check,
+- parity per (source, channel) against the float64 oracle (tests/channels_oracle.py at C = 2) under tests/parity.strict_check,
   the downmix's ill-conditioned bins taken out bin by bin;
 - one mask for both channels: S_c / X_c agrees across the channels and with the mono call;
 - the tensor-core kernel against the FFMA twin at the schedule edge of test_gpu_dsd_mask_schedule.py;
 - the int16 batch path against one-clip calls and the float path;
-- refusals before anything is queued."""
+- refusals before anything is queued, a spectrum tap without the Wiener post-filter included."""
 import ctypes as C
 
 import numpy as np
@@ -19,7 +20,7 @@ pytestmark = pytest.mark.gpu
 
 from oracle import nets, pipeline  # noqa: E402
 from parity import strict_check, TOL  # noqa: E402
-from keep_channels_oracle import separate_keep_channels  # noqa: E402
+from channels_oracle import separate_channels  # noqa: E402
 
 
 def rel(a, b):
@@ -65,8 +66,8 @@ def test_equal_channels_match_the_mono_call_bytes(N):
 
 
 def run_strict(name, sep, params, audio, N, hop, overlap=25, patcher="standalone"):
-    want, mags, phs, mms, kmap = separate_keep_channels(audio, params, frameSize=N, hopSize=hop, overlap=overlap,
-                                                        patcher=patcher)
+    want, mags, phs, mms, _, kmap = separate_channels(audio, params, frameSize=N, hopSize=hop, overlap=overlap,
+                                                      patcher=patcher)
     got, S = sep.separate_tapped(audio, keep_channels=True)     # got [L, 4, 2]; S planes (source, channel)
     assert got.shape == want.shape == (audio.shape[0], 4, 2) and got.dtype == np.float32
     for c in range(2):
@@ -207,7 +208,17 @@ def test_refusals_queue_nothing():
     refused["audio, stride < length"] = (lambda: audio_call(sep.model, stride=L - 1), None)
     refused["audio, overlap = time_context"] = (lambda: audio_call(sep.model, overlap=sep.model.tc), None)
     refused["batch, overlap = time_context"] = (lambda: batch_call(sep.model, overlap=sep.model.tc), None)
-    for name, (call, _) in refused.items():
+    tap = torch.zeros((8, sep.stft.num_frames(L), sep.stft.ldf), dtype=torch.complex64, device="cuda")
+
+    def tapped(call):
+        _lib.check(lib.dcs_set_spectrum_tap(ctx.handle, _ptr(tap), tap.numel()))
+        try:
+            return call()
+        finally:
+            _lib.check(lib.dcs_set_spectrum_tap(ctx.handle, None, 0))
+    refused["audio, spectrum tap without Wiener"] = (lambda: tapped(lambda: audio_call(sep.model)), "spectrum tap")
+    refused["batch, spectrum tap without Wiener"] = (lambda: tapped(lambda: batch_call(sep.model)), "spectrum tap")
+    for name, (call, msg) in refused.items():
         torch.cuda.synchronize()
         n0 = ctx.launch_count()
         with pytest.raises(_lib.DcsError) as e:
@@ -215,6 +226,8 @@ def test_refusals_queue_nothing():
         assert ctx.launch_count() == n0, name
         if name == "audio, dsd_ild":
             assert "dcs_separate_audio_stereo" in str(e.value)
+        if msg:
+            assert msg in str(e.value), name
     with pytest.raises(ValueError):
         sep.separate_keep_channels(audio[:, 0])
     assert np.array_equal(sep.separate_keep_channels(audio), ref)

@@ -356,7 +356,7 @@ def well_fraction(ref):
 
 
 # ---------------------------------------------------------------------------------------------- cases
-def dsd_case(name, F, T, tc, ov, patcher="util", ndec=3, nx=1, ldg=52, coherent=False, zero_slots=()):
+def dsd_case(name, F, T, tc, ov, patcher="util", ndec=3, ldg=52, coherent=False, zero_slots=()):
     """a DSD-family argument set: Lasagne conv1.W [50, nch, 1, F], G [P, ndec, tc, ldg], bout [nch][4], X planes"""
     rng = _rng(name)
     nch = 2 if ndec == 4 else 1
@@ -374,9 +374,8 @@ def dsd_case(name, F, T, tc, ov, patcher="util", ndec=3, nx=1, ldg=52, coherent=
         G[k, :, p] = 0.0
     if zero_slots:
         bout[:] = np.float32([1e-40, -1, -1, -1])
-    nxp = max(nch, nx)
-    X = (rng.standard_normal((nxp, T, F)) + 1j * rng.standard_normal((nxp, T, F))).astype(np.complex64)
-    return dict(kind="dsd", name=name, F=F, T=T, tc=tc, ov=ov, P=P, ndec=ndec, nx=nx, nch=nch, ldg=ldg, ldf=_ldf(F),
+    X = (rng.standard_normal((nch, T, F)) + 1j * rng.standard_normal((nch, T, F))).astype(np.complex64)
+    return dict(kind="dsd", name=name, F=F, T=T, tc=tc, ov=ov, P=P, ndec=ndec, nch=nch, ldg=ldg, ldf=_ldf(F),
                 W=W, G=G, bout=bout, X=X, p_base=0, t0=0, t1=T)
 
 
@@ -409,7 +408,7 @@ def k3s_case(name, arch, F, T, tc, ov, patcher="util", chunk=None, coherent=Fals
     tie = rng.integers(1, 16, (T, WP, 32)).astype(np.uint8) if pool else None   # single, double, ..., all-four ties
     X = (rng.standard_normal((T, F)) + 1j * rng.standard_normal((T, F))).astype(np.complex64)
     return dict(kind="k3s", name=name, arch=arch, F=F, T=T, tc=tc, ov=ov, P=P, J=J, WP=WP, ldf=_ldf(F), W=W, G=G,
-                bout=bout, X=X, tie=tie, p_base=p_base, t0=t0, t1=t1, nx=1, nch=1)
+                bout=bout, X=X, tie=tie, p_base=p_base, t0=t0, t1=t1, nch=1)
 
 
 SLOT_GEOMS = [(30, 0), (10, 5), (12, 8), (4, 3), (30, 24), (30, 25)]   # 1 .. 6 patches per frame
@@ -425,7 +424,6 @@ DSD_CASES = {
     "dsd_ldg56": lambda n: dsd_case(n, 257, 100, 30, 25, ldg=56),
     "dsd_ild": lambda n: dsd_case(n, 513, 150, 30, 25, ndec=4),
     "dsd_ild_standalone": lambda n: dsd_case(n, 129, 97, 20, 15, "standalone", ndec=4),
-    "dsd_keep": lambda n: dsd_case(n, 513, 150, 30, 25, nx=2),
     "dsd_coherent": lambda n: dsd_case(n, 257, 60, 30, 25, coherent=True),
     # defect: subnormal totals, in a one-slot frame, a zero-weight first frame of a later patch and a faded frame
     "dsd_subnormal": lambda n: dsd_case(n, 129, 400, 30, 25, zero_slots=((0, 2), (1, 0), (3, 2))),
@@ -668,7 +666,7 @@ class Buffers:
             self.W1t = dev(_padded(np.stack([w1t_layout(case["W"], ch, ldf) for ch in range(case["nch"])])))
             self.bout = dev(_padded(case["bout"]))
             self.tie = None
-            self.nplanes = 4 * case["nch"] * case["nx"]
+            self.nplanes = 4 * case["nch"]
             Xp = case["X"]
         else:
             KW, stride, nsrc, ndec, nw, pool, _ = K3S[case["arch"]]
@@ -694,25 +692,20 @@ def _ptr(t, floats=SLACK):
 
 
 def dsd_views(case, b, S, engine):
-    """the argument sets dsd_forward builds: mono, ILD (one call per channel, planes (s, ch)), keep-channels (nx = 2
-    on engine 1, two nx = 1 calls on engine 0, planes (s, c))"""
+    """the argument sets dsd_forward builds: mono, ILD (one call per channel, planes (s, ch))"""
     from deepconvsep_b200 import _lib
     T, F, ldf = case["T"], case["F"], case["ldf"]
     calls = []
     for ch in range(case["nch"]):
-        for c in range(case["nx"] if engine == 0 else 1):
-            v = _lib.DsdMaskView()
-            v.G, v.ldg = _ptr(b.G), case["ldg"]
-            v.W1t, v.ldw = _ptr(b.W1t) + 4 * ch * 50 * ldf, ldf
-            v.bout = _ptr(b.bout) + 16 * ch
-            i = ch + c
-            v.X = _ptr(b.X) + 8 * i * b.xp
-            v.S = _ptr(S, 2 * SLACK) + 8 * i * b.sp
-            v.ldf, v.T, v.P, v.tc, v.overlap, v.F, v.ndec = ldf, T, case["P"], case["tc"], case["ov"], F, case["ndec"]
-            v.src_stride = b.sp * (case["nch"] * case["nx"] if engine == 0 or case["nch"] == 2 else 1)
-            v.nx = case["nx"] if engine == 1 else 1
-            v.x_plane = b.xp
-            calls.append(v)
+        v = _lib.DsdMaskView()
+        v.G, v.ldg = _ptr(b.G), case["ldg"]
+        v.W1t, v.ldw = _ptr(b.W1t) + 4 * ch * 50 * ldf, ldf
+        v.bout = _ptr(b.bout) + 16 * ch
+        v.X = _ptr(b.X) + 8 * ch * b.xp
+        v.S = _ptr(S, 2 * SLACK) + 8 * ch * b.sp
+        v.ldf, v.T, v.P, v.tc, v.overlap, v.F, v.ndec = ldf, T, case["P"], case["tc"], case["ov"], F, case["ndec"]
+        v.src_stride = b.sp * case["nch"]
+        calls.append(v)
     return calls
 
 
@@ -748,8 +741,7 @@ def _plane_map(case):
     """output plane -> (source, mask set, mixture plane)"""
     if case["kind"] == "k3s":
         return [(s, 0, 0) for s in range(K3S[case["arch"]][2])]
-    npl = case["nch"] * case["nx"]
-    return [(s, c if case["nch"] == 2 else 0, c) for s in range(4) for c in range(npl)]
+    return [(s, c, c) for s in range(4) for c in range(case["nch"])]
 
 
 ENGINES = {"tc": 1, "ffma": 0}
@@ -830,7 +822,7 @@ def test_dsd_ffma_clip_longer_than_grid_y(ctx):
     v = _lib.DsdMaskView()
     v.G, v.ldg, v.W1t, v.ldw, v.bout = G.data_ptr(), ldg, W1t.data_ptr(), ldf, bo.data_ptr()
     v.X, v.S, v.ldf, v.src_stride = X.data_ptr(), S.data_ptr(), ldf, plane
-    v.T, v.P, v.tc, v.overlap, v.F, v.ndec, v.nx, v.x_plane = T, P, tc, ov, F, 3, 1, plane
+    v.T, v.P, v.tc, v.overlap, v.F, v.ndec = T, P, tc, ov, F, 3
     assert ctx.lib.dcs_dsd_mask_f32(ctx.handle, 1, ctypes.byref(v), None) == -1    # 7 patches per frame
     _lib.check(ctx.lib.dcs_dsd_mask_f32(ctx.handle, 0, ctypes.byref(v), None))
     case = dict(kind="dsd", T=T, P=P, tc=tc, ov=ov, F=F, ndec=3, W=W, G=G, bout=bout, engine="ffma")
@@ -852,7 +844,7 @@ def test_dsd_ffma_clip_longer_than_grid_y(ctx):
 @pytest.mark.gpu
 def test_mask_views_refuse_what_the_engine_does_not_take(ctx):
     """each refusal returns DCS_EINVAL with nothing launched and S untouched"""
-    case = make_case("dsd_keep", "tc")
+    case = make_case("dsd_F513", "tc")
     b = Buffers(case)
     S = b.fresh_S()
     n0 = ctx.launch_count()
@@ -863,13 +855,12 @@ def test_mask_views_refuse_what_the_engine_does_not_take(ctx):
             setattr(v, k, x)
         assert ctx.lib.dcs_dsd_mask_f32(ctx.handle, engine, ctypes.byref(v), None) == -1, (engine, kw)
 
-    bad(0)                                   # nx = 2 on the FFMA engine
-    bad(1, ndec=4)                           # nx = 2 with the ILD net
-    bad(1, nx=1, ldg=50)
-    bad(1, nx=1, ldg=54)
-    bad(1, nx=1, G=_ptr(b.G) + 4)            # G not 16-byte aligned
-    bad(2, nx=1)
-    bad(1, nx=1, src_stride=b.plane - 1)     # overlapping output planes
+    bad(1, ndec=5)
+    bad(1, ldg=50)
+    bad(1, ldg=54)
+    bad(1, G=_ptr(b.G) + 4)                  # G not 16-byte aligned
+    bad(2)
+    bad(1, src_stride=b.plane - 1)           # overlapping output planes
     kc = make_case("bach10_F129", "tc")
     kb = Buffers(kc)
     S2 = kb.fresh_S()

@@ -1,5 +1,5 @@
-"""Keep-channels mode of the DSD100 / hiphopss network without a GPU: the float64 oracle (tests/keep_channels_oracle.py)
-against the mono oracle, and the --keep-channels flags of the stand-alone scripts and of the dataset runner with
+"""Keep-channels mode of the DSD100 / hiphopss network without a GPU: the float64 oracle (tests/channels_oracle.py at
+C = 2) against the mono oracle, and the --keep-channels flags of the stand-alone scripts and of the dataset runner with
 stand-in separators."""
 import os
 import numpy as np
@@ -8,7 +8,7 @@ import scipy.io.wavfile
 from types import SimpleNamespace
 
 from oracle import dsp, nets, pipeline
-from keep_channels_oracle import separate_keep_channels
+from channels_oracle import separate_channels
 
 N, HOP = 512, 256
 
@@ -30,7 +30,7 @@ def test_equal_channels_are_the_mono_oracle_bit_for_bit(patcher):
     kw = dict(frameSize=N, hopSize=HOP, overlap=25, patcher=patcher)
     want, mag, ph, mm = pipeline.separate(mono, params, "dsd", return_spec=True, count_kinks=True, **kw)
     kmap = pipeline.separate.last_kink_map
-    stems, mags, phs, mms, km = separate_keep_channels(np.stack([mono, mono], axis=1), params, **kw)
+    stems, mags, phs, mms, _, km = separate_channels(np.stack([mono, mono], axis=1), params, **kw)
     assert stems.shape == (len(mono), 4, 2)
     for c in range(2):
         assert np.array_equal(stems[:, :, c].T, want)
@@ -43,8 +43,7 @@ def test_different_channels_share_the_downmix_masks():
     params = _params(12)
     audio = _stereo(1.0, 21)
     kw = dict(frameSize=N, hopSize=HOP, overlap=25)
-    stems, mags, phs, mms, _ = separate_keep_channels(audio, params, **kw)
-    M = separate_keep_channels.last_masks
+    stems, mags, phs, mms, M, _ = separate_channels(audio, params, **kw)
     T = phs[0].shape[0]
     # per channel: the blended masks of the downmix times that channel's magnitude
     for c in range(2):
@@ -71,7 +70,7 @@ def test_different_channels_share_the_downmix_masks():
 def test_anti_phase_channels_give_finite_stems():
     params = _params(13)
     x, _ = pipeline.synth_mixture(0.6, 8)
-    stems, mags, phs, mms, _ = separate_keep_channels(np.stack([x, -x], axis=1), params, frameSize=N, hopSize=HOP, overlap=25)
+    stems, mags, phs, mms, _, _ = separate_channels(np.stack([x, -x], axis=1), params, frameSize=N, hopSize=HOP, overlap=25)
     assert np.isfinite(stems).all() and all(np.isfinite(m).all() for m in mms)
     # the downmix is silent, the channels are not: the masks (of a silent input) still carry each channel through
     assert np.linalg.norm(stems) > 0

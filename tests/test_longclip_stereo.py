@@ -14,7 +14,7 @@ import torch.multiprocessing as mp
 
 from deepconvsep_b200 import longclip
 from oracle import dsp, nets, pipeline
-import keep_channels_oracle as kco
+import channels_oracle as co
 import wiener_local_oracle as WL
 
 CHUNK = WL.CHUNK
@@ -34,7 +34,7 @@ class OracleKeepSeparator(object):
         audio = np.asarray(audio, dtype=np.float64)
         self.calls.append((audio.shape[0], wiener, wiener_radius))
         N, H = self.frame_size, self.hop
-        stems, _, phs, mms, _ = kco.separate_keep_channels(audio, self.params, frameSize=N, hopSize=H, overlap=self.overlap)
+        stems, _, phs, mms, _, _ = co.separate_channels(audio, self.params, frameSize=N, hopSize=H, overlap=self.overlap)
         if not wiener:
             return stems
         win = np.hanning(N)

@@ -18,7 +18,7 @@ pytestmark = pytest.mark.gpu
 
 from oracle import dsp, pipeline  # noqa: E402
 from parity import record, TOL  # noqa: E402
-import keep_channels_oracle as kco  # noqa: E402
+import channels_oracle as co  # noqa: E402
 import wiener_local_oracle as WL  # noqa: E402
 from test_gpu_wiener import separator, stereo_clip  # noqa: E402
 
@@ -29,7 +29,7 @@ def oracle_spectra(sep, audio):
     """the network's spectra in float64 [4, 2, T, F] and the flagged bins [2, T, F]"""
     N, H = sep.frame_size, sep.hop
     if sep.model.arch == "dsd":
-        _, _, phs, mms, kmap = kco.separate_keep_channels(audio, sep._params, frameSize=N, hopSize=H, overlap=sep.overlap)
+        _, _, phs, mms, _, kmap = co.separate_channels(audio, sep._params, frameSize=N, hopSize=H, overlap=sep.overlap)
         kmaps = np.stack([kmap, kmap])
     else:
         _, _, phs, mms = pipeline.separate_stereo(audio, sep._params, frameSize=N, hopSize=H, overlap=sep.overlap,

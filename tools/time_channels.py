@@ -1,5 +1,6 @@
 """Device timing of C-channel stems (Separator.separate_channels: the downmix's masks applied inside the inverse STFT)
-against the keep-channels mode and the mono call (development aid, not the bench).
+against the keep-channels mode and the mono call (development aid, not the bench).  Keep-channels without the Wiener
+post-filter takes the C = 2 path; timing it next to separate_channels at C = 2 shows what its entry point adds.
 
 One seeded 180 s clip at N = 2048 and N = 1024: warm-up, then separate_keep_channels and separate_channels at C = 2
 alternated, then separate and separate_channels at C = 1 alternated, then separate_channels at C = 6 on its own, >= 10
@@ -12,15 +13,66 @@ It reads the card's name, power limit and max SM clock in the same run.
 import argparse
 import json
 import os
+import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
 from deepconvsep_b200.engine import Separator  # noqa: E402
-from time_keep_channels import SR, synth_params, card, stages  # noqa: E402
+
+SR = 44100
+
+
+def synth_params(F, seed=0):
+    """DSD100 parameter list with Glorot-uniform weights (the shapes of tools/quick_time.py)"""
+    rng = np.random.default_rng(seed)
+    shapes = [(50, 1, 1, F), (50,), (50,), (50, 50, 15, 1), (50,), (50,), (800, 128), (128,), (128, 800), (800,),
+              (128, 800), (800,), (128, 800), (800,), (4,)]
+    out = []
+    for s in shapes:
+        if len(s) == 4:
+            a = np.sqrt(6.0 / ((s[0] + s[1]) * s[2] * s[3]))
+        elif len(s) == 2:
+            a = np.sqrt(6.0 / (s[0] + s[1]))
+        else:
+            a = 0.1
+        out.append(rng.uniform(-a, a, size=s).astype(np.float32))
+    return out
+
+
+def stereo_clip(seconds, seed=1234):
+    rng = np.random.default_rng(seed)
+    L = int(seconds * SR)
+    t = np.arange(L) / SR
+    common = 0.2 * np.sin(2 * np.pi * 220 * t) + 0.1 * rng.standard_normal(L)
+    left = common + 0.1 * np.sin(2 * np.pi * 330 * t) + 0.05 * rng.standard_normal(L)
+    right = 0.8 * common + 0.1 * np.sin(2 * np.pi * 550 * t) + 0.05 * rng.standard_normal(L)
+    return np.stack([left, right], axis=1).clip(-0.99, 0.99).astype(np.float32)
+
+
+def card():
+    name = torch.cuda.get_device_name(0)
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+        power, sm_max = [v.strip() for v in q.split(",")]
+    except Exception:  # noqa: BLE001
+        power, sm_max = None, None
+    return {"gpu": name, "power_limit_w": power, "sm_max_mhz": sm_max}
+
+
+def stages(sep, call):
+    sep.ctx.profile(True)
+    call()
+    torch.cuda.synchronize()
+    rec = sep.ctx.profile_read()
+    sep.ctx.profile(False)
+    out = {}
+    for name, ms in rec:
+        out[name] = out.get(name, 0.0) + ms
+    return out
 
 
 def clip(seconds, nch, seed=1234):
@@ -39,13 +91,9 @@ def shape_bytes(N, L, nch, nsrc=4, hop=512):
     """MB the mask stage writes and the inverse STFT reads at the least (every plane once), and the spectra held"""
     plane = ((L + hop - 1) // hop + 2) * ((N // 2 + 1 + 7) // 8 * 8)
     mb = 1e-6
-    return {
-        "keep_channels": {"mask_stage_writes_S": nsrc * nch * plane * 8 * mb, "mask_stage_reads_X": nch * plane * 8 * mb,
-                          "istft_reads_S": nsrc * nch * plane * 8 * mb, "spectra_held": (nch + nsrc * nch) * plane * 8 * mb},
-        "channels": {"mask_stage_writes_M": nsrc * plane * 4 * mb, "mask_stage_reads_X": 0.0,
-                     "istft_reads_X_once": nch * plane * 8 * mb, "istft_reads_M_once": nsrc * plane * 4 * mb,
-                     "istft_reads_no_reuse": nsrc * nch * plane * 12 * mb, "spectra_held": (plane * 8 + nsrc * plane * 4) * mb},
-    }
+    return {"mask_stage_writes_M": nsrc * plane * 4 * mb, "mask_stage_reads_X": 0.0,
+            "istft_reads_X_once": nch * plane * 8 * mb, "istft_reads_M_once": nsrc * plane * 4 * mb,
+            "istft_reads_no_reuse": nsrc * nch * plane * 12 * mb, "spectra_held": (plane * 8 + nsrc * plane * 4) * mb}
 
 
 def timed(runs, reps):
@@ -104,7 +152,7 @@ def main():
         cfg = {"N": N, "ms": ms, "launches": launches, "stages_ms": {k: stages(s, f) for k, (s, f) in calls.items()},
                "workspace_MB": {"keep_channels": keep.ctx.workspace_bytes() / 1e6, "channels": chan.ctx.workspace_bytes() / 1e6,
                                 "mono": mono.ctx.workspace_bytes() / 1e6},
-               "shape_MB": {"C2": shape_bytes(N, L, 2), "C6": shape_bytes(N, L, 6)["channels"]}}
+               "shape_MB": {"C2": shape_bytes(N, L, 2), "C6": shape_bytes(N, L, 6)}}
         res["configs"].append(cfg)
         print(json.dumps(cfg), flush=True)
         del keep, chan, mono

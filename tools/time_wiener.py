@@ -24,7 +24,7 @@ import torch  # noqa: E402
 
 from deepconvsep_b200 import longclip  # noqa: E402
 from deepconvsep_b200.engine import Separator  # noqa: E402
-from time_keep_channels import synth_params, stereo_clip, stages  # noqa: E402
+from time_channels import synth_params, stereo_clip, stages  # noqa: E402
 
 NSRC, CHUNK = 4, 128      # sources; frames per partial-sum chunk (csrc/wiener.cu kWienerFrames)
 
@@ -38,7 +38,8 @@ def card():
 
 
 def wiener_bytes(T, F, nsrc=NSRC, radius=0):
-    """bytes each stage must move: the init pass reads the stems and X; an EM pass reads them and writes the stems;
+    """bytes each stage must move: the init pass reads the float masks and X and writes the stems; an EM pass reads
+    the stems and X and writes the stems;
     every pass but the last EM one writes per-chunk partial sums that its reduce reads back -- with a radius W >= 1
     each chunk reads the partials of its (up to 2W + 1) window chunks and writes its own R"""
     n = -(-T // CHUNK)
@@ -46,7 +47,7 @@ def wiener_bytes(T, F, nsrc=NSRC, radius=0):
     partials = n * nsrc * 4 * F * 8
     reread = partials if radius == 0 else sum(min(n - 1, c + radius) - max(0, c - radius) + 1 for c in range(n)) * partials // n
     write_q = 0 if radius == 0 else partials
-    init = (2 * nsrc + 2) * plane + partials + reread + write_q
+    init = (nsrc // 2 + 2 + 2 * nsrc) * plane + partials + reread + write_q
     em = (4 * nsrc + 2) * plane
     return {"plane_MB": plane / 1e6, "partials_MB": partials / 1e6, "reduce_read_MB": reread / 1e6,
             "init_GB": init / 1e9, "em_last_GB": em / 1e9, "em_GB": (em + partials + reread + write_q) / 1e9}
