@@ -32,6 +32,7 @@ _SIGS = {
     "dcs_wiener_stereo": (C.c_int, [_p, _p, _i64, _p, _i64, C.c_int, _i64, _i64, C.c_int, C.c_int, _p]),
     "dcs_set_wiener_radius": (C.c_int, [_p, C.c_int]),
     "dcs_wiener_stereo_windowed": (C.c_int, [_p, _p, _i64, _p, _i64, C.c_int, _i64, _i64, C.c_int, C.c_int, C.c_int, _p]),
+    "dcs_wiener_channels": (C.c_int, [_p, _p, C.c_int, _i64, _p, _i64, C.c_int, _i64, _i64, C.c_int, C.c_int, C.c_int, _p]),
     "dcs_profile": (C.c_int, [_p, C.c_int]),
     "dcs_profile_read": (C.c_int, [_p, C.c_char_p, C.c_int, _p, C.c_int]),
     "dcs_stft_plan": (C.c_int, [_p, C.c_int, C.c_int, _p, _p, C.POINTER(_p)]),
@@ -60,6 +61,8 @@ _SIGS = {
     "dcs_istft_masked": (C.c_int, [_p, _p, C.c_int, _i64, _p, C.c_int, _i64, _i64, _i64, _p, _i64, _i64, _p]),
     "dcs_apply_masks": (C.c_int, [_p, _p, _p, C.c_int, _i64, _i64, _p, C.c_int, _i64, _p, _i64, _p]),
     "dcs_separate_audio_channels": (C.c_int, [_p, _p, _p, _p, C.c_int, _i64, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
+    "dcs_separate_audio_channels_wiener": (C.c_int, [_p, _p, _p, _p, C.c_int, _i64, _i64, C.c_float, C.c_int, C.c_int, C.c_int,
+                                                     C.c_int, _p, _i64, _p]),
     "dcs_xcorr_lags": (C.c_int, [_p, _p, _p, C.c_int, _i64, C.c_int, _p, _p]),
     "dcs_gemm_f32": (C.c_int, [_p, C.c_int, _p, _i64, _p, _i64, _p, _p, _i64, C.c_int, C.c_int, C.c_int, C.c_int, _p]),
     "dcs_gemm_view_f32": (C.c_int, [_p, C.c_int, C.c_int, _p, _p, _p]),

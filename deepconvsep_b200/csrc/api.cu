@@ -564,7 +564,7 @@ static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, i
   if (!masks) DCS_TRY(ctx->S.ensure((size_t)m->nsrc * m->nch * plane * sizeof(float2), st));
   if (score_arch(m->arch)) DCS_TRY(ctx->net[NET_CHANS].ensure((size_t)score_planes(m) * plane * sizeof(float), st));
   if (!masks && ctx->wiener_iters > 0 && m->nch == 2)
-    DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, dcs_num_frames(L, p->hop), m->F, ctx->wiener_radius), st));
+    DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, 2, dcs_num_frames(L, p->hop), m->F, ctx->wiener_radius), st));
   if (staged) {
     DCS_TRY(ctx->audio.ensure((size_t)L * sizeof(float), st));
     DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * L * sizeof(float), st));
@@ -573,19 +573,19 @@ static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, i
 }
 
 // the workspace of downmix_clip: the masks-output workspace, the downmix, the nsrc mask planes and ONE mixture STFT
-// plane, whatever the channel count.  wiener (two channels, the filter on): two STFT planes, nsrc x 2 masked spectra
-// and the filter's sums.  staged (the int16 keep-channels batch): three audio planes (downmix, left, right) and
-// nsrc x 2 stem planes
-static int size_downmix_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, bool wiener, bool staged,
+// plane, whatever the channel count.  wx > 0 (the filter on, wx channels): wx STFT planes, nsrc x wx masked spectra
+// and the filter's sums over covariance windows of `radius` chunks.  staged (the int16 keep-channels batch): three audio
+// planes (downmix, left, right) and nsrc x 2 stem planes
+static int size_downmix_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, int wx, int radius, bool staged,
                                   cudaStream_t st) {
   const int64_t plane = dcs_num_frames(L, p->hop) * dcs_padded_bins(p->N);
   DCS_TRY(size_workspace(ctx, m, p, L, false, st, true));
   DCS_TRY(ctx->audio.ensure((size_t)(staged ? 3 : 1) * L * sizeof(float), st));
   DCS_TRY(ctx->masks.ensure((size_t)m->nsrc * plane * sizeof(float), st));
-  DCS_TRY(ctx->X.ensure((size_t)(wiener ? 2 : 1) * plane * sizeof(float2), st));
-  if (wiener) {
-    DCS_TRY(ctx->S.ensure((size_t)m->nsrc * 2 * plane * sizeof(float2), st));
-    DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, dcs_num_frames(L, p->hop), m->F, ctx->wiener_radius), st));
+  DCS_TRY(ctx->X.ensure((size_t)(wx > 0 ? wx : 1) * plane * sizeof(float2), st));
+  if (wx > 0) {
+    DCS_TRY(ctx->S.ensure((size_t)m->nsrc * wx * plane * sizeof(float2), st));
+    DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, wx, dcs_num_frames(L, p->hop), m->F, radius), st));
   }
   if (staged) DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * 2 * L * sizeof(float), st));
   return DCS_OK;
@@ -660,14 +660,14 @@ static int check_keep_tap(const char* fn, const dcs_ctx* ctx) {
 
 // Stems of nx channels (audio_stride apart) from the masks of their downmix d_mono, single-channel nets: the network
 // in masks mode into ctx->masks, then those masks applied to every channel inside the inverse STFT, planes (s * nx + c).
-// d_mono NULL: the downmix is formed here, into ctx->audio.  wiener (keep-channels, nx = 2): with dcs_set_wiener above
-// 0 the filter's first pass forms the masked spectra M_s * X_c in memory; they are filtered, copied to the spectrum tap
-// and inverted
+// d_mono NULL: the downmix is formed here, into ctx->audio.  iterations > 0 (nx in [2, 8]): the Wiener post-filter's
+// first pass forms the masked spectra M_s * X_c of all nx channels in memory; `iterations` EM iterations over covariance
+// windows of `radius` chunks filter them, and they are copied to the spectrum tap and inverted
 static int downmix_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const float* d_mono, const float* d_audio, int nx,
-                        int64_t audio_stride, int64_t L, bool wiener, float scale_factor, int overlap, int patcher,
-                        float* d_stems, int64_t stem_stride, cudaStream_t st) {
-  const bool filter = wiener && ctx->wiener_iters > 0;
-  DCS_TRY(size_downmix_workspace(ctx, m, p, L, filter, false, st));
+                        int64_t audio_stride, int64_t L, int iterations, int radius, float scale_factor, int overlap,
+                        int patcher, float* d_stems, int64_t stem_stride, cudaStream_t st) {
+  const bool filter = iterations > 0;
+  DCS_TRY(size_downmix_workspace(ctx, m, p, L, filter ? nx : 0, radius, false, st));
   const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
   float* masks = ctx->masks.as<float>();
   if (!d_mono) {
@@ -680,12 +680,12 @@ static int downmix_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const flo
   float2 *X = ctx->X.as<float2>(), *S = ctx->S.as<float2>();
   {
     ProfScope ps(ctx, "stft_fwd", st);
-    for (int c = 0; c < 2; ++c) DCS_TRY(launch_stft(p, d_audio + c * audio_stride, L, X + c * plane, nullptr, nullptr, 1.f, ldf, st));
+    for (int c = 0; c < nx; ++c) DCS_TRY(launch_stft(p, d_audio + c * audio_stride, L, X + c * plane, nullptr, nullptr, 1.f, ldf, st));
   }
-  DCS_TRY(launch_wiener(ctx, X, plane, S, plane, m->nsrc, T, ldf, m->F, ctx->wiener_iters, ctx->wiener_radius, st, masks, plane));
-  DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * 2 * plane, st));
+  DCS_TRY(launch_wiener(ctx, X, plane, S, plane, m->nsrc, T, ldf, m->F, iterations, radius, st, masks, plane, nx));
+  DCS_TRY(copy_tap(ctx, S, (int64_t)m->nsrc * nx * plane, st));
   ProfScope ps(ctx, "istft_ola", st);
-  return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc * 2, T, ldf, plane, d_stems, L, stem_stride, st);
+  return launch_istft(p, S, nullptr, nullptr, 1.f, m->nsrc * nx, T, ldf, plane, d_stems, L, stem_stride, st);
 }
 
 int dcs_separate_spec(dcs_ctx* ctx, dcs_model* m, const float* d_mag, const dcs_complex* d_X, int64_t T, int64_t ldf,
@@ -961,7 +961,8 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, c
     if (keep) {
       DCS_TRY(launch_pcm_decode_keep(ctx, ctx->pcm_in[b].as<int16_t>(), L, audio, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
-      DCS_TRY(downmix_clip(ctx, m, p, audio, audio + L, 2, L, L, true, scale_factor, overlap, patcher, stems, L, st));
+      DCS_TRY(downmix_clip(ctx, m, p, audio, audio + L, 2, L, L, ctx->wiener_iters, ctx->wiener_radius, scale_factor, overlap,
+                           patcher, stems, L, st));
     } else {
       DCS_TRY(launch_pcm_decode(ctx, ctx->pcm_in[b].as<int16_t>(), L, channels, downmix, audio, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
@@ -1015,7 +1016,7 @@ static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, i
     DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * (keep ? 2 : 1) * Lmax * sizeof(int16_t), st));
   }
   if (keep)
-    DCS_TRY(size_downmix_workspace(ctx, m, p, Lmax, ctx->wiener_iters > 0, true, st));
+    DCS_TRY(size_downmix_workspace(ctx, m, p, Lmax, ctx->wiener_iters > 0 ? 2 : 0, ctx->wiener_radius, true, st));
   else
     DCS_TRY(size_workspace(ctx, m, p, Lmax, true, st));
   const int rc = batch_pipeline(ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, keep, scale_factor, overlap, patcher,
@@ -1052,8 +1053,8 @@ int dcs_separate_audio_keep_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, co
   DCS_TRY(check_clip(fn, ctx, m, p, DCS_ARCH_DSD, d_audio, d_stems, L, audio_stride, stem_stride, overlap, patcher));
   DCS_TRY(check_keep_tap(fn, ctx));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return downmix_clip(ctx, m, p, nullptr, d_audio, 2, audio_stride, L, true, scale_factor, overlap, patcher, d_stems,
-                      stem_stride, (cudaStream_t)stream);
+  return downmix_clip(ctx, m, p, nullptr, d_audio, 2, audio_stride, L, ctx->wiener_iters, ctx->wiener_radius, scale_factor,
+                      overlap, patcher, d_stems, stem_stride, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------ masks output
@@ -1148,18 +1149,43 @@ int dcs_apply_masks(dcs_ctx* ctx, dcs_stft* p, const float* d_audio, int nx, int
   return apply_masks(ctx, p, d_audio, nx, audio_stride, L, d_masks, nsrc, m_stride, d_stems, stem_stride, (cudaStream_t)stream);
 }
 
-int dcs_separate_audio_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int nx, int64_t audio_stride,
-                                int64_t L, float scale_factor, int overlap, int patcher, float* d_stems, int64_t stem_stride,
-                                void* stream) {
-  const char* fn = "dcs_separate_audio_channels";
+// the checks of dcs_separate_audio_channels(_wiener): with iterations > 0 also those of the filter on the clip's spectra
+static int check_channels(const char* fn, const dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, const float* d_audio, int nx,
+                          int64_t audio_stride, int64_t L, int overlap, int patcher, const float* d_stems, int64_t stem_stride,
+                          int iterations, int radius) {
   DCS_REQUIRE(!m || (m->arch != DCS_ARCH_DSD_ILD && !score_arch(m->arch)),
               "%s does not serve architecture %d: use dcs_separate_masks* + dcs_apply_masks", fn, m->arch);
   DCS_TRY(check_clip(fn, ctx, m, p, -1, d_audio, d_stems, L, audio_stride, stem_stride, overlap, patcher));
   DCS_REQUIRE(nx >= 1 && nx <= 16, "%s: nx %d not in [1, 16]", fn, nx);
-  DCS_REQUIRE(!ctx->tap, "%s: a spectrum tap is set (dcs_set_spectrum_tap), and this path forms no masked spectra to copy", fn);
+  DCS_REQUIRE(iterations >= 0, "%s: iterations %d must be >= 0", fn, iterations);
+  DCS_REQUIRE(radius >= 0, "%s: radius %d must be >= 0", fn, radius);
+  if (iterations == 0) {
+    DCS_REQUIRE(!ctx->tap, "%s: a spectrum tap is set (dcs_set_spectrum_tap), and this path forms no masked spectra to copy", fn);
+    return DCS_OK;
+  }
+  DCS_REQUIRE(nx >= 2 && nx <= 8, "%s: the Wiener post-filter needs nx in [2, 8], got %d", fn, nx);
+  const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N);
+  return wiener_check(fn, m->nsrc, T, ldf, m->F, T * ldf, T * ldf, iterations, radius);
+}
+
+int dcs_separate_audio_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int nx, int64_t audio_stride,
+                                int64_t L, float scale_factor, int overlap, int patcher, float* d_stems, int64_t stem_stride,
+                                void* stream) {
+  DCS_TRY(check_channels("dcs_separate_audio_channels", ctx, m, p, d_audio, nx, audio_stride, L, overlap, patcher, d_stems,
+                         stem_stride, 0, 0));
   DCS_CUDA(cudaSetDevice(ctx->device));
-  return downmix_clip(ctx, m, p, nullptr, d_audio, nx, audio_stride, L, false, scale_factor, overlap, patcher, d_stems,
+  return downmix_clip(ctx, m, p, nullptr, d_audio, nx, audio_stride, L, 0, 0, scale_factor, overlap, patcher, d_stems,
                       stem_stride, (cudaStream_t)stream);
+}
+
+int dcs_separate_audio_channels_wiener(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int nx,
+                                       int64_t audio_stride, int64_t L, float scale_factor, int overlap, int patcher,
+                                       int iterations, int radius, float* d_stems, int64_t stem_stride, void* stream) {
+  DCS_TRY(check_channels("dcs_separate_audio_channels_wiener", ctx, m, p, d_audio, nx, audio_stride, L, overlap, patcher,
+                         d_stems, stem_stride, iterations, radius));
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  return downmix_clip(ctx, m, p, nullptr, d_audio, nx, audio_stride, L, iterations, radius, scale_factor, overlap, patcher,
+                      d_stems, stem_stride, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------ Wiener post-filter
@@ -1182,6 +1208,18 @@ int dcs_wiener_stereo_windowed(dcs_ctx* ctx, const dcs_complex* d_X, int64_t x_p
                                int nsrc, int64_t T, int64_t ldf, int F, int iterations, int radius, void* stream) {
   return wiener_stereo("dcs_wiener_stereo_windowed", ctx, d_X, x_plane, d_S, src_stride, nsrc, T, ldf, F, iterations, radius,
                        stream);
+}
+
+int dcs_wiener_channels(dcs_ctx* ctx, const dcs_complex* d_X, int nx, int64_t x_plane, dcs_complex* d_S, int64_t src_stride,
+                        int nsrc, int64_t T, int64_t ldf, int F, int iterations, int radius, void* stream) {
+  const char* fn = "dcs_wiener_channels";
+  DCS_REQUIRE(nx >= 2 && nx <= 8, "%s: nx %d not in [2, 8] (one channel has no spatial covariance)", fn, nx);
+  DCS_REQUIRE(ctx && d_X && d_S, "%s: NULL argument", fn);
+  DCS_REQUIRE((uintptr_t)d_X % sizeof(float2) == 0 && (uintptr_t)d_S % sizeof(float2) == 0, "%s: spectra not 8-byte aligned", fn);
+  DCS_TRY(wiener_check(fn, nsrc, T, ldf, F, x_plane, src_stride, iterations, radius));
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  return launch_wiener(ctx, (const float2*)d_X, x_plane, (float2*)d_S, src_stride, nsrc, T, ldf, F, iterations, radius,
+                       (cudaStream_t)stream, nullptr, 0, nx);
 }
 
 }  // extern "C"

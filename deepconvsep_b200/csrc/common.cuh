@@ -334,16 +334,16 @@ int launch_pcm_encode_keep(dcs_ctx* ctx, const float* d_stems, int64_t L, int ns
 // at nx = 1
 int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st);
 
-// multichannel Wiener post-filter (wiener.cu): mixture channel c at X + c * x_plane, stem (j, c) at
-// S + (2 j + c) * src_stride, bins f < F filtered in place by `iterations` EM iterations; radius: the covariance window
-// in chunks of DCS_WIENER_CHUNK_FRAMES frames to either side (0 = the whole clip).  M set (nsrc = 4): the stems are not
-// in S yet; the first pass forms stem (j, c) as M_j * X_c (float masks [T][ldf], m_stride apart), componentwise in fp32,
-// and stores it to S
+// multichannel Wiener post-filter (wiener.cu): nch (2..8) mixture channels, channel c at X + c * x_plane, stem (j, c) at
+// S + (j * nch + c) * src_stride, bins f < F filtered in place by `iterations` EM iterations; radius: the covariance
+// window in chunks of DCS_WIENER_CHUNK_FRAMES frames to either side (0 = the whole clip).  M set: the stems are not in S
+// yet; the first pass forms stem (j, c) as M_j * X_c (float masks [T][ldf], m_stride apart), componentwise in fp32, and
+// stores it to S.  nch 2 runs the 2 x 2 kernels, more channels the C x C ones
 int wiener_check(const char* fn, int nsrc, int64_t T, int64_t ldf, int F, int64_t x_plane, int64_t src_stride, int iterations,
                  int radius);
-size_t wiener_workspace_bytes(int nsrc, int64_t T, int F, int radius);
+size_t wiener_workspace_bytes(int nsrc, int nch, int64_t T, int F, int radius);
 int launch_wiener(dcs_ctx* ctx, const float2* X, int64_t x_plane, float2* S, int64_t src_stride, int nsrc, int64_t T,
                   int64_t ldf, int F, int iterations, int radius, cudaStream_t st, const float* M = nullptr,
-                  int64_t m_stride = 0);
+                  int64_t m_stride = 0, int nch = 2);
 
 }  // namespace dcs

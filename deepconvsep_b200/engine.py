@@ -68,6 +68,40 @@ def wiener_stereo(ctx, X, S, iterations, stream=None, num_bins=None, radius=0):
     return S
 
 
+# the channel counts the C-channel Wiener post-filter serves (dcs_wiener_channels): one channel has no spatial covariance
+WIENER_CHANNELS = (2, 8)
+
+
+def check_wiener_channels(nx):
+    """ValueError unless the Wiener post-filter serves `nx` channels."""
+    lo, hi = WIENER_CHANNELS
+    if not lo <= nx <= hi:
+        raise ValueError("the Wiener post-filter works on %d to %d channels (one channel has no spatial covariance), got %d"
+                         % (lo, hi, nx))
+
+
+def wiener_channels(ctx, X, S, iterations, stream=None, num_bins=None, radius=0):
+    """The multichannel Wiener post-filter on nx = 2 .. 8 channels (dcs_wiener_channels), in place on device spectra:
+    X torch complex64 cuda [nx, T, ldf] (the mixture's channels), S [nsrc * nx, T, ldf] (the stems, planes ordered
+    (source, channel), nsrc <= 4).  At nx = 2 the bytes of wiener_stereo.  Bins >= num_bins (default ldf) are left
+    alone; radius as in wiener_stereo.  Returns S."""
+    import torch
+    if X.dim() != 3 or S.dim() != 3 or tuple(S.shape[1:]) != tuple(X.shape[1:]) or S.shape[0] % max(X.shape[0], 1):
+        raise ValueError("wiener_channels needs X [nx, T, ldf] and S [nsrc * nx, T, ldf], got %r and %r"
+                         % (tuple(X.shape), tuple(S.shape)))
+    nx = int(X.shape[0])
+    check_wiener_channels(nx)
+    if X.dtype != torch.complex64 or S.dtype != torch.complex64 or not (X.is_cuda and S.is_cuda):
+        raise ValueError("wiener_channels needs complex64 cuda tensors")
+    if X.stride(2) != 1 or X.stride(1) != X.shape[2] or S.stride(2) != 1 or S.stride(1) != S.shape[2]:
+        raise ValueError("wiener_channels needs contiguous [T, ldf] planes")
+    T, ldf = int(X.shape[1]), int(X.shape[2])
+    F = ldf if num_bins is None else int(num_bins)
+    _lib.check(ctx.lib.dcs_wiener_channels(ctx.handle, _ptr(X), nx, X.stride(0), _ptr(S), S.stride(0), S.shape[0] // nx, T,
+                                           ldf, F, int(iterations), int(radius), _stream_ptr(stream, ctx.device)))
+    return S
+
+
 # the networks whose input is not one magnitude plane: their masks cannot come from a downmix inside the library
 MASKS_BY_HAND = ("dsd_ild", "bach10_score", "bach10_score_1x1")
 
@@ -88,8 +122,9 @@ def check_stereo_options(family, keep_channels=False, wiener=0, wiener_radius=0,
     "dsd_ild"; wiener_radius (the filter's covariance window in chunks to either side, 0 = the whole clip) cannot be
     negative and needs wiener > 0.  channels: the recording's channel count where it is known and keep_channels is
     asked for -- None or 2 is the rule above; 1 is refused; C > 2 (5.1, arrays: Separator.separate_channels) is served
-    for every single-channel network, without the Wiener filter, whose 2 x 2 algebra has no C-channel form.  Raises
-    ValueError with the reason otherwise."""
+    for every single-channel network, without the Wiener filter here: the filtered C-channel stems (C <= 8) are
+    Separator.separate_channels(wiener=K), which the command-line options do not reach yet.  Raises ValueError with the
+    reason otherwise."""
     if keep_channels and channels is not None and channels != 2:
         if channels < 2:
             raise ValueError("--keep-channels needs at least a 2-channel recording, this one has %d channel(s)" % channels)
@@ -604,20 +639,37 @@ class Separator(object):
             return out
         return np.ascontiguousarray(stems)
 
-    def separate_channels(self, audio, out=None, stream=None):
+    def separate_channels(self, audio, out=None, stream=None, wiener=0, wiener_radius=0):
         """Stems for any number of channels from a single-channel network (dcs_separate_audio_channels): the network
         sees the downmix (((a_0 + a_1) + a_2) + ...) * (1 / C) in fp32, its blended soft masks are applied to the STFT
         of every channel inside the inverse STFT -- no masked spectra in memory, a workspace that does not grow with C.
         audio float [L, C] (numpy) or [C, L] (cuda tensor), C in 1..16 -> float32 [L, nsrc, C] (numpy; at C = 2 the
         layout and, for the DSD100 network, the bits of separate_keep_channels) or the device planes [nsrc * C, L]
-        ordered (source, channel).  No Wiener post-filter (two-channel stems only) and no spectrum tap; the stereo /
-        ILD and score-informed networks are refused: separate_masks + apply_masks serve them."""
+        ordered (source, channel).  No spectrum tap; the stereo / ILD and score-informed networks are refused:
+        separate_masks + apply_masks serve them.
+        wiener > 0 (C in 2..8): that many EM iterations of the multichannel Wiener post-filter on the masked spectra
+        M_s * X_c, over covariance windows of wiener_radius chunks to either side (0 = the whole clip), between the
+        masks and the inverse STFT (dcs_separate_audio_channels_wiener); the spectra are then in memory, so the
+        workspace grows with C.  At C = 2 with the DSD100 network, the bits of separate_keep_channels with the same
+        wiener and wiener_radius."""
         check_channels_family(self.model.arch)
+        check_wiener_radius(wiener, wiener_radius)
+        if wiener < 0:
+            raise ValueError("wiener %d: the number of EM iterations cannot be negative" % wiener)
+        if wiener:
+            shape = np.shape(audio) if not hasattr(audio, "is_cuda") else tuple(audio.shape)[::-1]
+            check_wiener_channels(shape[1] if len(shape) == 2 else 1)
         host, x, outd = self._channel_planes(audio, out, self.nsrc)
         C_, L = x.shape
-        _lib.check(self.lib.dcs_separate_audio_channels(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), C_,
-                                                        x.stride(0), L, self.scale_factor, self.overlap, self.patcher,
-                                                        _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
+        if wiener:
+            _lib.check(self.lib.dcs_separate_audio_channels_wiener(
+                self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), C_, x.stride(0), L, self.scale_factor,
+                self.overlap, self.patcher, int(wiener), int(wiener_radius), _ptr(outd), outd.stride(0),
+                _stream_ptr(stream, self.ctx.device)))
+        else:
+            _lib.check(self.lib.dcs_separate_audio_channels(self.ctx.handle, self.model.handle, self.stft.handle, _ptr(x), C_,
+                                                            x.stride(0), L, self.scale_factor, self.overlap, self.patcher,
+                                                            _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
         return self._channel_stems(host, outd, out, C_)
 
     def apply_masks(self, audio, masks, out=None, stream=None):

@@ -103,8 +103,9 @@ int dcs_set_pool_tap(dcs_ctx* ctx, uint8_t* d_bits, int64_t capacity);
 /* Multichannel Wiener post-filter of two-channel stems (see dcs_wiener_stereo): while iterations > 0, the entry points
  * that produce stereo stems -- dcs_separate_audio_keep_channels, dcs_separate_batch_pcm16_keep_channels_host and
  * dcs_separate_audio_stereo -- run that many EM iterations on the network's spectra before the inverse STFT (the
- * spectrum tap then holds the filtered spectra).  Single-channel entry points ignore the setting.  Default 0 (off:
- * the network's spectra, bit for bit); negative values are refused. */
+ * spectrum tap then holds the filtered spectra).  Single-channel entry points ignore the setting, and so does
+ * dcs_separate_audio_channels: its filtered form, for 2 to 8 channels, is dcs_separate_audio_channels_wiener, which takes
+ * the iterations as an argument.  Default 0 (off: the network's spectra, bit for bit); negative values are refused. */
 int dcs_set_wiener(dcs_ctx* ctx, int iterations);
 /* The covariance window of that filter on the same entry points (see dcs_wiener_stereo_windowed): 0 (the default) =
  * one R_j(f) and one scale for the whole clip, bit for bit the filter without this setting; radius >= 1 = per chunk
@@ -465,7 +466,8 @@ int dcs_apply_masks(dcs_ctx* ctx, dcs_stft* plan, const float* d_audio, int nx, 
  * the stems are those of dcs_separate_audio and at nx = 2 (DCS_ARCH_DSD) those of dcs_separate_audio_keep_channels,
  * bit for bit.  The workspace holds the downmix, its magnitude, nsrc float mask planes and one mixture STFT plane: no
  * masked spectra, and nothing that grows with nx.
- *  - dcs_set_wiener is ignored, as by the masks calls: the 2 x 2 filter has no nx-channel form here.
+ *  - dcs_set_wiener is ignored, as by the masks calls: the Wiener post-filter on these stems is
+ *    dcs_separate_audio_channels_wiener, which takes its iterations and radius as arguments.
  *  - There are no masked spectra to copy: a spectrum tap set on the ctx is DCS_EINVAL before anything is queued.  The
  *    routing tap (dcs_set_pool_tap) is honoured as by the masks calls.
  *  - A clip shorter than one patch gives all-zero masks, so silent stems.
@@ -498,6 +500,39 @@ int dcs_wiener_stereo(dcs_ctx* ctx, const dcs_complex* d_X, int64_t x_plane, dcs
 int dcs_wiener_stereo_windowed(dcs_ctx* ctx, const dcs_complex* d_X, int64_t x_plane, dcs_complex* d_S,
                                int64_t src_stride, int nsrc, int64_t num_frames, int64_t ldf, int F, int iterations,
                                int radius, void* stream);
+/* The same filter on nx = 2 .. 8 channels: mixture channel c at d_X + c*x_plane, stem (source j, channel c) at
+ * d_S + (j*nx + c)*src_stride (the stereo layout at nx = 2), in place, with the constants, chunks and windows of
+ * dcs_wiener_stereo_windowed and C x C algebra:
+ *     v_j = (1/nx) sum_c |y_jc|^2,   R_j(f) = sum_t y_j y_j^H / (eps s^2 + sum_t v_j),
+ *     C = sum_j v_j R_j + sqrt(eps) s^2 I  (Hermitian, positive definite),   y_j <- v_j R_j C^-1 x,
+ * s over every channel.  C is factored L D L^H without pivoting and solved by two triangular substitutions, in fp64, in
+ * a fixed order of operations: the same bits on every run, W >= n-1 gives the bits of radius 0, and a chunk depends only
+ * on the frames within K*W chunks of it.  nx = 2 runs the 2 x 2 kernels: the bytes of dcs_wiener_stereo_windowed.
+ * Launch count 2 * iterations + 1.  The workspace (bytes) is
+ *     8 * (n * P + q * P + n * ceil(F / b) + q),   P = nsrc * nx^2 * F,  q = (radius > 0 ? n : 1),  n = ceil(T / 128),
+ * b = 128 at nx = 2 and 32 above: the per-chunk partial sums, the summed covariances, the per-block maxima and the scales.
+ * Refused with DCS_EINVAL before anything is queued: nx outside [2, 8] (one channel has no spatial covariance) and what
+ * dcs_wiener_stereo_windowed refuses. */
+int dcs_wiener_channels(dcs_ctx* ctx, const dcs_complex* d_X, int nx, int64_t x_plane, dcs_complex* d_S,
+                        int64_t src_stride, int nsrc, int64_t num_frames, int64_t ldf, int F, int iterations,
+                        int radius, void* stream);
+/* dcs_separate_audio_channels with the Wiener post-filter (dcs_wiener_channels) between the masks and the inverse STFT:
+ * the filter's first pass forms the masked spectra M_s * X_c of every channel (fp32, componentwise, the product the
+ * masked inverse STFT forms) in memory, `iterations` EM iterations over covariance windows of `radius` chunks filter
+ * them, and the plain inverse STFT gives plane (s*nx + c).  The iterations and radius are arguments: dcs_set_wiener and
+ * dcs_set_wiener_radius are not read.
+ *  - iterations 0: the bits of dcs_separate_audio_channels, with its workspace and its refusal of a spectrum tap.
+ *  - nx = 2, DCS_ARCH_DSD: the bits of dcs_separate_audio_keep_channels with the same iterations and radius set on the
+ *    ctx.
+ *  - iterations > 0: the spectrum tap holds the nsrc*nx filtered planes, ordered (source, channel).  The workspace adds
+ *    to that of dcs_separate_audio_channels nx - 1 mixture STFT planes, nsrc*nx masked-spectrum planes (8 * T * ldf bytes
+ *    each) and the filter's workspace of dcs_wiener_channels at F = N/2 + 1.
+ *  - Refused with DCS_EINVAL before anything is queued: iterations or radius negative, nx outside [2, 8] with
+ *    iterations > 0, and what dcs_separate_audio_channels refuses. */
+int dcs_separate_audio_channels_wiener(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const float* d_audio, int nx,
+                                       int64_t audio_stride, int64_t num_samples, float scale_factor, int overlap,
+                                       int patcher, int iterations, int radius, float* d_stems, int64_t stem_stride,
+                                       void* stream);
 
 #ifdef __cplusplus
 }
