@@ -460,14 +460,25 @@ static int dsd_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaS
   GemmDesc g4 = gemm_plain(z, nfc, ds.Wdec, ndec * h2 * C2p, ds.bdec, ap, (int64_t)ndec * HP * C2p, (int)P, ndec * h2 * C2p, nfc, 1);
   g4.n_seg = h2 * C2p; g4.n_ss = (int64_t)HP * C2p; g4.c_col0 = (int64_t)(kh2 - 1) * C2p;
   { ProfScope ps(ctx, "dec_dense_gemm", st); DCS_TRY(run_gemm(ctx, g4, ds.tWdec, st)); }
-  // InverseLayer(conv2): full correlation on the padded activations, rows (k, d, u)
-  // Rows are ordered (u, k, d) -- u-major -- so that a 128-row tile holds one output position
-  // u and can skip the taps that only see the zero padding (on average 8 of the 15).
-  GemmDesc g5 = gemm_plain(ap, 0, ds.Wt2, C1, nullptr, G, ldg, (int)(P * ndec * tc), C1, kh2 * C2p, 0);
-  g5.m_inner = (int)(P * ndec); g5.a_so = C2p; g5.a_si = (int64_t)HP * C2p;
-  g5.cm_inner = (int)(P * ndec); g5.c_so = ldg; g5.c_si = (int64_t)tc * ldg;
-  g5.kc_rows = (int)(P * ndec); g5.kc_unit = C2p; g5.kc_pad = kh2 - 1; g5.kc_n = h2; g5.kc_taps = kh2;
-  { ProfScope ps(ctx, "dec_convT2_gemm", st); DCS_TRY(run_gemm(ctx, g5, ds.tWt2, st)); }
+  // InverseLayer(conv2): full correlation on the padded activations, rows (k, d, u).  The tensor-core
+  // kernel reads each (patch, decoder) pair's interior rows once into shared memory (dsd_convT2_tc.cu).
+  // The FFMA cross-check runs the same layer as a GEMM on an overlapping view of apad, rows ordered
+  // (u, k, d) -- u-major -- so that a tile holds one output position u and skips the taps that only see
+  // the zero padding.
+  {
+    ProfScope ps(ctx, "dec_convT2_gemm", st);
+    if (ctx->debug_simt_gemm) {
+      GemmDesc g5 = gemm_plain(ap, 0, ds.Wt2, C1, nullptr, G, ldg, (int)(P * ndec * tc), C1, kh2 * C2p, 0);
+      g5.m_inner = (int)(P * ndec); g5.a_so = C2p; g5.a_si = (int64_t)HP * C2p;
+      g5.cm_inner = (int)(P * ndec); g5.c_so = ldg; g5.c_si = (int64_t)tc * ldg;
+      g5.kc_rows = (int)(P * ndec); g5.kc_unit = C2p; g5.kc_pad = kh2 - 1; g5.kc_n = h2; g5.kc_taps = kh2;
+      DCS_TRY(launch_gemm(ctx, g5, st));
+    } else {
+      DsdConvT2Args a5;
+      a5.apad = ap; a5.G = G; a5.ldg = ldg; a5.npairs = (int)(P * ndec); a5.tc = tc;
+      DCS_TRY(launch_dsd_convT2_tc(ctx, a5, ds.tWt2, st));
+    }
+  }
   // InverseLayer(conv1) + bias + ReLU + mask + cross-fade + phase; the stereo net: once per channel
   // with that channel's conv1 weights, output biases and mixture STFT (trainCNN_ILD_DSD100.py:183-186)
   ProfScope ps(ctx, "dec_convT1_mask_xfade", st);
@@ -815,6 +826,10 @@ static_assert(sizeof(dcs_dsd_mask_view) == sizeof(DsdMaskArgs) && offsetof(dcs_d
                   offsetof(dcs_dsd_mask_view, F) == offsetof(DsdMaskArgs, F) &&
                   offsetof(dcs_dsd_mask_view, ndec) == offsetof(DsdMaskArgs, ndec),
               "dcs_dsd_mask_view must mirror DsdMaskArgs");
+static_assert(sizeof(dcs_dsd_convt2_view) == sizeof(DsdConvT2Args) && offsetof(dcs_dsd_convt2_view, G) == offsetof(DsdConvT2Args, G) &&
+                  offsetof(dcs_dsd_convt2_view, ldg) == offsetof(DsdConvT2Args, ldg) &&
+                  offsetof(dcs_dsd_convt2_view, tc) == offsetof(DsdConvT2Args, tc),
+              "dcs_dsd_convt2_view must mirror DsdConvT2Args");
 static_assert(sizeof(dcs_sconv_mask_view) == sizeof(SconvMaskArgs) && offsetof(dcs_sconv_mask_view, G) == offsetof(SconvMaskArgs, G) &&
                   offsetof(dcs_sconv_mask_view, S) == offsetof(SconvMaskArgs, S) &&
                   offsetof(dcs_sconv_mask_view, src_stride) == offsetof(SconvMaskArgs, src_stride) &&
@@ -848,6 +863,25 @@ int dcs_dsd_mask_f32(dcs_ctx* ctx, int engine, const dcs_dsd_mask_view* view, vo
   DCS_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = (cudaStream_t)stream;
   return sync_after("dcs_dsd_mask_f32", engine == 1 ? launch_dsd_mask_tc(ctx, a, st) : launch_dsd_mask(ctx, a, st), st);
+}
+
+int dcs_dsd_convt2_f32(dcs_ctx* ctx, const dcs_dsd_convt2_view* view, const float* h_Wt2, void* stream) {
+  DCS_REQUIRE(ctx && view && h_Wt2 && view->apad && view->G, "dcs_dsd_convt2_f32: NULL argument");
+  DsdConvT2Args a;
+  memcpy(&a, view, sizeof a);
+  DCS_REQUIRE(a.npairs > 0 && a.tc >= 4 && a.tc <= 64 && a.ldg >= 50 && a.ldg % 2 == 0 && (int64_t)a.npairs * a.tc < ((int64_t)1 << 31),
+              "dcs_dsd_convt2_f32: bad shape");
+  DCS_REQUIRE((uintptr_t)a.apad % 16 == 0 && (uintptr_t)a.G % 8 == 0, "dcs_dsd_convt2_f32: apad must be 16-byte and G 8-byte aligned");
+  DCS_REQUIRE(dsd_convT2_tc_supported(a), "dcs_dsd_convt2_f32: unsupported arguments");
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int kh2 = a.tc / 2;
+  TcWeight w;
+  int r = tc_weight_create(h_Wt2, 50, kh2 * 52, 50, &w);
+  if (r == DCS_OK) r = launch_dsd_convT2_tc(ctx, a, w, st);
+  r = sync_after("dcs_dsd_convt2_f32", r, st);
+  tc_weight_destroy(&w);
+  return r;
 }
 
 int dcs_sconv_mask_f32(dcs_ctx* ctx, int engine, const dcs_sconv_mask_view* view, void* stream) {

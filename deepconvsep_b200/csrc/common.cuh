@@ -282,6 +282,17 @@ constexpr float MASK_TOT_MIN = 1.2e-38f;
 int launch_dsd_mask(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st, float* M = nullptr);
 bool dsd_mask_tc_supported(const DsdMaskArgs& a);
 int launch_dsd_mask_tc(dcs_ctx* ctx, const DsdMaskArgs& a, cudaStream_t st, float* M = nullptr);   // wgmma (dsd_tc.cu)
+// InverseLayer(conv2) of the DSD nets: G[pair][u][c] = sum_{q, f} apad[pair][u + q][f] * Wt2[q][f][c] for the
+// npairs = P * ndec (patch, decoder) pairs, u < tc; only the h2 interior rows [kh2 - 1, kh2 - 1 + h2) of apad are read
+struct DsdConvT2Args {
+  const float* apad;   // [npairs][h2 + 2 (kh2 - 1)][52], 16-byte aligned
+  float* G;            // [npairs][tc][ldg]: columns 0..49 written, 8-byte aligned
+  int ldg;
+  int npairs, tc;
+};
+bool dsd_convT2_tc_supported(const DsdConvT2Args& a);
+// w: the transposed conv2 weight as tc_weight_create lays it out (K = kh2 * 52, N = 50)
+int launch_dsd_convT2_tc(dcs_ctx* ctx, const DsdConvT2Args& a, const TcWeight& w, cudaStream_t st);   // dsd_convT2_tc.cu
 // strided-conv1 families (iKala / Bach10): K3s arguments
 struct SconvMaskArgs {
   int arch;

@@ -178,6 +178,19 @@ template <int BN> __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2],
   else if constexpr (BN == 128) wgmma_tf32_n128(d, adesc, bdesc, accumulate);
   else wgmma_tf32_n144(d, adesc, bdesc, accumulate);
 }
+// D (+)= A[registers] * B[smem]^T, M = 64, N = 56, K = 8.  A fragment (the mma.m16n8k8 tf32 layout per warp): thread
+// t = 32 * w + l holds a[0] = A[16w + l/4][l%4], a[1] = A[16w + l/4 + 8][l%4], a[2] = A[16w + l/4][l%4 + 4],
+// a[3] = A[16w + l/4 + 8][l%4 + 4]
+__device__ __forceinline__ void wgmma_tf32_rs_n56(float (&d)[28], const float (&a)[4], uint64_t bdesc, int accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %33, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n56k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27}, {%28, %29, %30, %31}, %32, p, 1, 1;\n\t"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27])
+      : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])), "l"(bdesc), "r"(accumulate));
+}
 // after wgmma_wait: ties every accumulator register to this point, so no read of the accumulators is
 // scheduled above the wait
 template <int N> __device__ __forceinline__ void wgmma_fence_acc(float (&d)[N]) {
@@ -191,6 +204,25 @@ __device__ __forceinline__ float4 ld_stream(const float4* p) {
   float4 v;
   asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
   return v;
+}
+
+// ---- asynchronous copies into shared memory -----------------------------------------------------
+// cp.async (generic proxy): 16 bytes, L2 only; a thread sees its own copies after cp_async_wait
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// wait until at most N of this thread's committed groups are still in flight
+template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+// one arrival that also expects `bytes` of bulk-copy completions on the barrier's current phase
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+// bulk copy global -> shared (async proxy), completion counted in bytes on `bar`; dst, src and bytes multiples of 16
+__device__ __forceinline__ void bulk_copy_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
 }
 
 // ---- 3xTF32 operand split ---------------------------------------------------------------------

@@ -295,6 +295,22 @@ typedef struct {
 } dcs_dsd_mask_view;
 int dcs_dsd_mask_f32(dcs_ctx* ctx, int engine, const dcs_dsd_mask_view* view, void* stream);
 
+/* Bring-up and test entry: InverseLayer(conv2) of the DSD nets on the tensor cores, on buffers laid out as the layer
+ * sequence lays them out, for npairs = P * ndec (patch, decoder) pairs, time_context tc in 4..64, kh2 = tc / 2,
+ * h2 = tc - kh2 + 1:
+ *   apad  [npairs][h2 + 2 (kh2 - 1)][52]  decoder activations; only the h2 interior rows kh2 - 1 .. kh2 + h2 - 2 are
+ *                                        read (channels 50..51 meet zero weights and must be finite); 16-byte aligned
+ *   G     [npairs][tc][ldg]              G[i][u][c] = sum_{q < kh2, f < 52} apad[i][u + q][f] * h_Wt2[52 q + f][c];
+ *                                        columns 0..49 are written, nothing else; ldg >= 50 even, 8-byte aligned
+ *   h_Wt2 HOST [52 kh2][50]              transposed and split for the tensor cores on every call
+ * Every argument is checked before anything is queued.  Synchronises the stream before returning. */
+typedef struct {
+  const float* apad;
+  float* G; int ldg;
+  int npairs, tc;
+} dcs_dsd_convt2_view;
+int dcs_dsd_convt2_f32(dcs_ctx* ctx, const dcs_dsd_convt2_view* view, const float* h_Wt2, void* stream);
+
 /* The strided-conv1 networks (K3s): arch DCS_ARCH_BACH10, _BACH10_SCORE, _BACH10_SCORE_1X1, _IKALA, _IKALA_NOPOOL.
  * conv1 has KW taps at stride STRIDE over frequency (Bach10 nets 30 / 4, iKala 30 / 3, build_ca_1x1 5 / 2); J = (F-KW) /
  * STRIDE + 1 windows, WP = J / 4 pooled windows (DCS_ARCH_IKALA) or J; ND = ceil(KW / STRIDE).
