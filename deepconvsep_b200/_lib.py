@@ -11,6 +11,8 @@ ARCH_IDS = {"dsd": 0, "ikala": 1, "ikala_nopool": 2, "bach10": 3, "bach10_score"
 PATCHER_IDS = {"standalone": 0, "util": 1}
 # frames per chunk of the Wiener post-filter's sums over time (DCS_WIENER_CHUNK_FRAMES, include/dcs.h)
 WIENER_CHUNK_FRAMES = 128
+# the largest polyphase bank a resampler takes (DCS_RESAMPLE_MAX_BANK_BYTES, include/dcs.h)
+RESAMPLE_MAX_BANK_BYTES = 112 * 1024
 
 
 class DcsError(RuntimeError):
@@ -77,6 +79,10 @@ _SIGS = {
     "dcs_separate_audio_keep_channels": (C.c_int, [_p, _p, _p, _p, _i64, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
     "dcs_separate_batch_pcm16_keep_channels_host": (C.c_int, [_p, _p, _p, C.c_int, _p, _p, C.c_float, C.c_int, C.c_int,
                                                               _p, _p, _p]),
+    "dcs_resampler_create": (C.c_int, [_p, C.c_int, C.c_int, _p, C.c_int, C.POINTER(_p)]),
+    "dcs_resampler_destroy": (C.c_int, [_p]),
+    "dcs_resampled_length": (_i64, [_i64, C.c_int, C.c_int]),
+    "dcs_resample": (C.c_int, [_p, _p, C.c_int, _i64, _i64, _p, _i64, _i64, _p]),
 }
 
 

@@ -214,6 +214,110 @@ def score_filters(ctx, melody, T, F, start=0, mag=None, ldf=None, stream=None):
     return out
 
 
+# every network was trained on spectra of 44.1 kHz audio; other rates go through a Resampler
+MODEL_RATE = 44100
+# the sample rates a Resampler takes: integers in this range whose polyphase bank fits, in both directions
+RESAMPLE_RATES = (8000, 192000)
+
+
+def resample_ratio(rate_in, rate_out):
+    """(up, down): rate_out / rate_in in lowest terms."""
+    from math import gcd
+    g = gcd(int(rate_in), int(rate_out))
+    return int(rate_out) // g, int(rate_in) // g
+
+
+def resample_taps(up, down):
+    """The filter scipy.signal.resample_poly(x, up, down) designs by default, float64 [20 * max(up, down) + 1]:
+    firwin(2 * half_len + 1, 1 / max(up, down), window=('kaiser', 5.0)) * up, half_len = 10 * max(up, down)."""
+    from scipy.signal import firwin
+    m = max(int(up), int(down))
+    return np.ascontiguousarray(firwin(2 * 10 * m + 1, 1.0 / m, window=("kaiser", 5.0)) * int(up), dtype=np.float64)
+
+
+def resample_bank_bytes(up, down):
+    """Bytes of the polyphase bank of resample_taps(up, down): ceil(ntaps / up) taps for each of the up phases."""
+    ntaps = 20 * max(up, down) + 1
+    return -(-ntaps // up) * up * 8
+
+
+def check_resample_rates(rate_in, rate_out):
+    """(up, down) for resampling rate_in -> rate_out; ValueError naming the rate unless both are integers in
+    RESAMPLE_RATES whose bank is at most _lib.RESAMPLE_MAX_BANK_BYTES in both directions."""
+    lo, hi = RESAMPLE_RATES
+    for r in (rate_in, rate_out):
+        if isinstance(r, bool) or not isinstance(r, (int, float, np.integer, np.floating)) or r != int(r):
+            raise ValueError("sample rate %r Hz: only integer rates are resampled" % (r,))
+        if not lo <= int(r) <= hi:
+            raise ValueError("sample rate %d Hz: rates from %d to %d Hz are resampled" % (int(r), lo, hi))
+    up, down = resample_ratio(rate_in, rate_out)
+    worst = max(resample_bank_bytes(up, down), resample_bank_bytes(down, up))
+    if worst > _lib.RESAMPLE_MAX_BANK_BYTES:
+        odd = int(rate_in) if int(rate_out) == MODEL_RATE else int(rate_out)
+        raise ValueError("sample rate %d Hz: %d <-> %d Hz reduces to %d/%d, whose polyphase filter bank (%d bytes) is over "
+                         "the %d a resampler takes; resample it to a nearby common rate first"
+                         % (odd, int(rate_in), int(rate_out), up, down, worst, _lib.RESAMPLE_MAX_BANK_BYTES))
+    return up, down
+
+
+class Resampler(object):
+    """rate_in -> rate_out on the device (dcs_resample): scipy.signal.resample_poly with its default filter and zero
+    padding, the taps in fp64, rounded once to fp32.  Rates as check_resample_rates accepts them."""
+
+    def __init__(self, ctx, rate_in, rate_out):
+        self.up, self.down = check_resample_rates(rate_in, rate_out)
+        self.rate_in, self.rate_out = int(rate_in), int(rate_out)
+        self.ctx, self.lib = ctx, ctx.lib
+        self.taps = resample_taps(self.up, self.down)
+        h = C.c_void_p()
+        _lib.check(self.lib.dcs_resampler_create(ctx.handle, self.up, self.down, self.taps.ctypes.data, self.taps.size,
+                                                 C.byref(h)))
+        self.handle = h
+
+    def length(self, num_in):
+        """ceil(num_in * up / down): the samples of the whole resampled signal"""
+        return int(self.lib.dcs_resampled_length(int(num_in), self.up, self.down))
+
+    def resample(self, planes, num_out=None, stream=None, out=None):
+        """planes: float32 cuda [P, L] (rows contiguous, gaps between planes allowed) -> float32 cuda [P, num_out]
+        (default self.length(L); shorter trims the tail), into `out` when given ([P, num_out], rows contiguous)."""
+        import torch
+        if planes.dim() != 2 or planes.dtype != torch.float32 or not planes.is_cuda or planes.stride(1) != 1:
+            raise ValueError("resample needs float32 cuda planes [P, L] with contiguous rows, got %r %s"
+                             % (tuple(planes.shape), planes.dtype))
+        P, L = planes.shape
+        n = self.length(L) if num_out is None else int(num_out)
+        if out is None:
+            out = torch.empty((P, n), dtype=torch.float32, device=planes.device)
+        elif not (out.is_cuda and out.dtype == torch.float32 and tuple(out.shape) == (P, n) and out.stride(1) == 1):
+            raise ValueError("resample: out must be float32 cuda [%d, %d] with contiguous rows" % (P, n))
+        _lib.check(self.lib.dcs_resample(self.handle, _ptr(planes), P, planes.stride(0), L, _ptr(out), out.stride(0), n,
+                                         _stream_ptr(stream, self.ctx.device)))
+        return out
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self.lib.dcs_resampler_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+_SCORE_AT_RATE = "resample the audio to 44.1 kHz with Resampler first, and give the score on that grid"
+_MASKS_AT_RATE = ("resample the audio to 44.1 kHz with Resampler first, or use separate / separate_channels with "
+                  "sample_rate=, which resample for you")
+
+
+def check_model_rate(sample_rate, call, alternative):
+    """ValueError unless sample_rate is the networks' 44.1 kHz, for the calls whose inputs are on its grids."""
+    if sample_rate != MODEL_RATE:
+        raise ValueError("%s works at %d Hz only (sample_rate %r): %s" % (call, MODEL_RATE, sample_rate, alternative))
+
+
 class Context(object):
     """One dcs_ctx = one device + the workspace of one in-flight pipeline."""
 
@@ -441,11 +545,51 @@ class Separator(object):
         self.nsrc = self.model.nsrc
         self.sources = d["sources"]
         self.lib = self.ctx.lib
+        self._resamplers = {}
+
+    def resampler(self, rate_in, rate_out):
+        """The Resampler rate_in -> rate_out on this separator's context, made on first use and kept."""
+        key = (rate_in, rate_out)
+        if key not in self._resamplers:
+            self._resamplers[key] = Resampler(self.ctx, rate_in, rate_out)
+        return self._resamplers[key]
+
+    def _at_rate(self, call, audio, sample_rate, out, stream, channels=None, mono=False):
+        """A stems call on audio at sample_rate != MODEL_RATE: the audio planes to MODEL_RATE, call(planes, stream=stream)
+        on them (the device entry point), the nsrc x C stem planes back in one launch, trimmed to the input's length.
+        audio as the channel calls take it with `channels` (None: 1 to 16), or mono float [L] (numpy or cuda tensor)
+        -> the layout of the call at MODEL_RATE: numpy [nsrc, L] (mono) or [L, nsrc, C], or device planes [nsrc * C, L]."""
+        down = self.resampler(sample_rate, MODEL_RATE)     # the rate is checked before any device work
+        back = self.resampler(MODEL_RATE, sample_rate)
+        if mono:
+            import torch
+            host = not hasattr(audio, "is_cuda")
+            x = torch.as_tensor(np.ascontiguousarray(audio, dtype=np.float32), device=self.stft.dev) if host else audio
+            if x.dim() != 1 or x.dtype != torch.float32:
+                raise ValueError("this network needs mono float audio [L], got %r" % (tuple(x.shape),))
+            x = x.contiguous().unsqueeze(0)
+            outd = out if (out is not None and not host) else None
+            stems = back.resample(call(down.resample(x, stream=stream)[0], stream=stream), num_out=x.shape[1],
+                                  stream=stream, out=outd)
+            if not host:
+                return stems
+            if out is not None:
+                out[...] = stems.cpu().numpy()
+                return out
+            return stems.cpu().numpy()
+        host, x, outd = self._channel_planes(audio, out, self.nsrc, channels)
+        back.resample(call(down.resample(x, stream=stream), stream=stream), num_out=x.shape[1], stream=stream, out=outd)
+        return self._channel_stems(host, outd, out, x.shape[0])
 
     # ---- host buffers (numpy): H2D + pipeline + D2H inside the call ----
-    def separate(self, audio, out=None):
+    def separate(self, audio, out=None, sample_rate=MODEL_RATE):
         """audio: 1-D float array (any float dtype) -> float32 [nsrc, L].  `audio` / `out` may be
-        pinned (torch.from_numpy(...).pin_memory() views) for asynchronous copies."""
+        pinned (torch.from_numpy(...).pin_memory() views) for asynchronous copies.
+        sample_rate: the audio's rate.  At MODEL_RATE (44.1 kHz) this call; at another rate (check_resample_rates) the
+        audio is resampled to 44.1 kHz on the device, separated there (separate_device) and the stems resampled back to
+        the input's rate and length -- a float32 cuda tensor [L] in then gives the device stems [nsrc, L]."""
+        if sample_rate != MODEL_RATE:
+            return self._at_rate(self.separate_device, audio, sample_rate, out, None, mono=True)
         a = np.ascontiguousarray(audio, dtype=np.float32)
         L = a.size
         if out is None:
@@ -526,10 +670,12 @@ class Separator(object):
                                                _stream_ptr(stream, self.ctx.device)))
         return out
 
-    def separate_score(self, audio, filters, out=None, stream=None):
+    def separate_score(self, audio, filters, out=None, stream=None, sample_rate=MODEL_RATE):
         """Score-informed Bach10: audio float [L] (numpy or cuda tensor) + normalised score filters
         [4, T, F] float32 (deepconvsep_b200.score.score_filters; or a cuda tensor [4, T, ldf] already on the
-        device) -> stems float32 [4, L] (same kind as `audio`).  The four input channels are formed on the device."""
+        device) -> stems float32 [4, L] (same kind as `audio`).  The four input channels are formed on the device.
+        sample_rate other than 44.1 kHz is refused: the score is on the 44.1 kHz frame grid."""
+        check_model_rate(sample_rate, "separate_score", _SCORE_AT_RATE)
         import torch
         host = not hasattr(audio, "is_cuda")
         T = self.stft.num_frames(np.size(audio) if host else audio.numel())
@@ -544,11 +690,13 @@ class Separator(object):
             fd[:, :, :self.model.F] = torch.as_tensor(f, device=dev)
         return self._score_clip(self.lib.dcs_separate_audio_score, audio, (_ptr(fd),), out, stream)
 
-    def separate_notes(self, audio, melody, frame0=0, out=None, stream=None):
+    def separate_notes(self, audio, melody, frame0=0, out=None, stream=None, sample_rate=MODEL_RATE):
         """separate_score with the filters rasterised on the device from the note table (dcs_separate_audio_notes):
         audio float [L] (numpy or cuda tensor) + melody float64 [4, nnotes, ncols] (deepconvsep_b200.score.score_melody)
         -> stems float32 [4, L] (same kind as `audio`), the bits of separate_score(audio, filterSpec(..., frame0,
-        frame0 + T)).  frame0: the table frame of the clip's first STFT frame (a segment of a longer recording)."""
+        frame0 + T)).  frame0: the table frame of the clip's first STFT frame (a segment of a longer recording).
+        sample_rate other than 44.1 kHz is refused: the note table is on the 44.1 kHz frame grid."""
+        check_model_rate(sample_rate, "separate_notes", _SCORE_AT_RATE)
         if self.model.arch not in ("bach10_score", "bach10_score_1x1"):
             raise ValueError("separate_notes needs a score-informed network, this one is %r" % self.model.arch)
         if int(frame0) < 0:
@@ -570,28 +718,36 @@ class Separator(object):
                          self.overlap, self.patcher, _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
         return outd.cpu().numpy() if host else outd
 
-    def separate_stereo(self, audio, out=None, stream=None, wiener=0, wiener_radius=0):
+    def separate_stereo(self, audio, out=None, stream=None, wiener=0, wiener_radius=0, sample_rate=MODEL_RATE):
         """Stereo / ILD network (examples/dsd100_2ch_ILD/trainCNN_ILD_DSD100.py:299-327): audio float
         [L, 2] (numpy) or [2, L] (cuda tensor) -> `sep_audio` float32 [L, nsrc, 2] (numpy) or the device
         planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> cuda tensor out).  wiener: EM iterations of
         the multichannel Wiener post-filter (dcs_set_wiener) on the network's spectra, 0 = off; wiener_radius: its
-        covariance window in chunks to either side (dcs_set_wiener_radius), 0 = the whole clip."""
-        return self._two_channel_clip(self.lib.dcs_separate_audio_stereo, audio, out, stream, wiener, wiener_radius)
+        covariance window in chunks to either side (dcs_set_wiener_radius), 0 = the whole clip.  sample_rate: as in
+        separate (resampled to 44.1 kHz and back on the device at other rates)."""
+        return self._two_channel_clip(self.lib.dcs_separate_audio_stereo, audio, out, stream, wiener, wiener_radius,
+                                      sample_rate, self.separate_stereo)
 
-    def separate_keep_channels(self, audio, out=None, stream=None, wiener=0, wiener_radius=0):
+    def separate_keep_channels(self, audio, out=None, stream=None, wiener=0, wiener_radius=0, sample_rate=MODEL_RATE):
         """Stereo stems from the DSD100 / hiphopss network (dcs_separate_audio_keep_channels): the network sees the
         downmix (l + r) * 0.5, its soft masks are applied to each channel's STFT and inverted with that channel's
         phase.  audio float [L, 2] (numpy) or [2, L] (cuda tensor) -> float32 [L, nsrc, 2] (numpy, the layout of
         separate_stereo) or the device planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out).
         wiener: EM iterations of the multichannel Wiener post-filter (dcs_set_wiener) on the masked spectra, 0 = off;
-        wiener_radius: its covariance window in chunks to either side (dcs_set_wiener_radius), 0 = the whole clip."""
-        return self._two_channel_clip(self.lib.dcs_separate_audio_keep_channels, audio, out, stream, wiener, wiener_radius)
+        wiener_radius: its covariance window in chunks to either side (dcs_set_wiener_radius), 0 = the whole clip.
+        sample_rate: as in separate (resampled to 44.1 kHz and back on the device at other rates)."""
+        return self._two_channel_clip(self.lib.dcs_separate_audio_keep_channels, audio, out, stream, wiener, wiener_radius,
+                                      sample_rate, self.separate_keep_channels)
 
-    def _two_channel_clip(self, entry, audio, out, stream, wiener, wiener_radius):
+    def _two_channel_clip(self, entry, audio, out, stream, wiener, wiener_radius, sample_rate=MODEL_RATE, method=None):
         """audio float [L, 2] (numpy) or [2, L] (cuda tensor) through the two-channel clip entry point `entry`, with
         `wiener` EM iterations of the Wiener post-filter over covariance windows of `wiener_radius` chunks -> float32
-        [L, nsrc, 2] (numpy) or the device planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out)."""
+        [L, nsrc, 2] (numpy) or the device planes [nsrc * 2, L] ordered (source, channel) (cuda tensor in -> out).
+        At another sample_rate: `method`, the public call of `entry`, on the audio resampled to MODEL_RATE."""
         check_wiener_radius(wiener, wiener_radius)
+        if sample_rate != MODEL_RATE:
+            return self._at_rate(partial(method, wiener=wiener, wiener_radius=wiener_radius), audio, sample_rate, out,
+                                 stream, channels=2)
         host, x, outd = self._channel_planes(audio, out, self.nsrc, 2)
         L = x.shape[1]
         self.ctx.set_wiener(wiener)
@@ -639,7 +795,7 @@ class Separator(object):
             return out
         return np.ascontiguousarray(stems)
 
-    def separate_channels(self, audio, out=None, stream=None, wiener=0, wiener_radius=0):
+    def separate_channels(self, audio, out=None, stream=None, wiener=0, wiener_radius=0, sample_rate=MODEL_RATE):
         """Stems for any number of channels from a single-channel network (dcs_separate_audio_channels): the network
         sees the downmix (((a_0 + a_1) + a_2) + ...) * (1 / C) in fp32, its blended soft masks are applied to the STFT
         of every channel inside the inverse STFT -- no masked spectra in memory, a workspace that does not grow with C.
@@ -651,7 +807,9 @@ class Separator(object):
         M_s * X_c, over covariance windows of wiener_radius chunks to either side (0 = the whole clip), between the
         masks and the inverse STFT (dcs_separate_audio_channels_wiener); the spectra are then in memory, so the
         workspace grows with C.  At C = 2 with the DSD100 network, the bits of separate_keep_channels with the same
-        wiener and wiener_radius."""
+        wiener and wiener_radius.
+        sample_rate: as in separate (resampled to 44.1 kHz and back on the device at other rates, all C channels and
+        then all nsrc * C stem planes in one launch each)."""
         check_channels_family(self.model.arch)
         check_wiener_radius(wiener, wiener_radius)
         if wiener < 0:
@@ -659,6 +817,9 @@ class Separator(object):
         if wiener:
             shape = np.shape(audio) if not hasattr(audio, "is_cuda") else tuple(audio.shape)[::-1]
             check_wiener_channels(shape[1] if len(shape) == 2 else 1)
+        if sample_rate != MODEL_RATE:
+            return self._at_rate(partial(self.separate_channels, wiener=wiener, wiener_radius=wiener_radius), audio,
+                                 sample_rate, out, stream)
         host, x, outd = self._channel_planes(audio, out, self.nsrc)
         C_, L = x.shape
         if wiener:
@@ -672,12 +833,14 @@ class Separator(object):
                                                             _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
         return self._channel_stems(host, outd, out, C_)
 
-    def apply_masks(self, audio, masks, out=None, stream=None):
+    def apply_masks(self, audio, masks, out=None, stream=None, sample_rate=MODEL_RATE):
         """The caller's masks -- separate_masks' of any network, edited or not -- applied to every channel of `audio`
         inside the inverse STFT (dcs_apply_masks): plane (s, c) = iSTFT(masks_s * STFT(channel c)).  audio float [L, C]
         (numpy) with masks [nsrc, T, F], or device planes [C, L] with masks float32 cuda [nsrc, T, ldf] (planes may be
         views with gaps, rows contiguous; pad columns are not read) -> float32 [L, nsrc, C] (numpy) or the device
-        planes [nsrc * C, L] ordered (source, channel).  nsrc is the masks' own: any number >= 1."""
+        planes [nsrc * C, L] ordered (source, channel).  nsrc is the masks' own: any number >= 1.
+        sample_rate other than 44.1 kHz is refused: the masks are on the 44.1 kHz STFT grid."""
+        check_model_rate(sample_rate, "apply_masks", _MASKS_AT_RATE)
         import torch
         host = not hasattr(audio, "is_cuda")
         L = np.shape(audio)[0] if host else audio.shape[-1]
@@ -701,14 +864,16 @@ class Separator(object):
                                             md.stride(0), _ptr(outd), outd.stride(0), _stream_ptr(stream, self.ctx.device)))
         return self._channel_stems(host, outd, out, C_)
 
-    def separate_masks(self, audio, filters=None, melody=None, frame0=0, out=None, stream=None):
+    def separate_masks(self, audio, filters=None, melody=None, frame0=0, out=None, stream=None, sample_rate=MODEL_RATE):
         """The network's blended soft masks, from a pipeline that stops before the inverse STFT (dcs_separate_masks*):
         the fp32 values the stems calls multiply by the mixture STFT, so Stft.inverse(X * masks) gives the stems.
         audio as the stems call of this network takes it -- float [L] (single-channel nets), [L, 2] numpy or [2, L] cuda
         tensor (stereo / ILD net); score-informed nets also need the score filters `filters` (as separate_score) or the
         note table `melody` from table frame `frame0` (as separate_notes).  numpy in -> float32 [nsrc, T, F] ([nsrc, 2,
         T, F] for the stereo net); cuda tensor in -> the device planes [nplanes, T, ldf] (or into `out`, whose rows must be
-        contiguous; its pad columns and the gaps between planes are not written), planes ordered (source, channel)."""
+        contiguous; its pad columns and the gaps between planes are not written), planes ordered (source, channel).
+        sample_rate other than 44.1 kHz is refused: the masks are on the 44.1 kHz STFT grid."""
+        check_model_rate(sample_rate, "separate_masks", _MASKS_AT_RATE)
         import torch
         arch = self.model.arch
         score = arch in ("bach10_score", "bach10_score_1x1")

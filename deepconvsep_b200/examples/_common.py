@@ -5,7 +5,7 @@ import threading
 import numpy as np
 import scipy.io.wavfile
 
-from ..engine import Separator, check_stereo_options
+from ..engine import MODEL_RATE, Separator, check_resample_rates, check_stereo_options
 from ..models import load_model, FAMILY_DEFAULTS
 
 _cache = {}
@@ -54,8 +54,21 @@ def wav_channels(path):
         return None
 
 
+def wav_rate(path):
+    """Sample rate of a wav from its header (memory-mapped: nothing else is read); None where there is none to read."""
+    try:
+        return int(scipy.io.wavfile.read(path, mmap=True)[0])
+    except Exception:  # noqa: BLE001  (unreadable: the read in run() reports it)
+        return None
+
+
+def _one_over_devices_at_rate(filein, rate):
+    return ("--resample: %s is at %d Hz, and one recording at a rate other than 44100 Hz runs on one device; cutting it "
+            "over several is not implemented (a directory of wavs goes over the devices file by file)" % (filein, rate))
+
+
 def run(family, filein, outdir, model, scale_factor, time_context, overlap, batch_size, input_size, frame_size, hop,
-        out_name, window=None, device=0, slot=0, keep_channels=False, wiener=0, wiener_radius=0):
+        out_name, window=None, device=0, slot=0, keep_channels=False, wiener=0, wiener_radius=0, resample=False):
     """wav in -> one int16 wav per source in `outdir`.  `batch_size` is accepted for signature
     compatibility; the CUDA path has no patch batches.  keep_channels (DSD100 / hiphopss, 2-channel wav): one
     2-channel wav per source -- the soft masks of the downmix applied to each channel; wiener: that many EM iterations
@@ -63,7 +76,9 @@ def run(family, filein, outdir, model, scale_factor, time_context, overlap, batc
     to either side (0 = the whole clip).  keep_channels on a wav of C > 2 channels (5.1, arrays; every single-channel
     family): one C-channel wav per source, the masks of the mean of the channels applied to each
     (Separator.separate_channels; no Wiener filter, one device).  A device list cuts the recording into segments over the devices; with
-    keep_channels and wiener that needs wiener_radius >= 1."""
+    keep_channels and wiener that needs wiener_radius >= 1.  resample: a wav at another rate than 44100 Hz is separated
+    through the float Separator calls with sample_rate= (resampled to 44.1 kHz and back on the device, one device) and its
+    stems are written at the wav's rate and length; without it such a wav is reported and skipped, as by the reference."""
     nch = wav_channels(filein) if keep_channels else None
     if nch == 1:
         raise ValueError("--keep-channels needs at least a 2-channel recording; %s has 1 channel" % (filein,))
@@ -75,11 +90,30 @@ def run(family, filein, outdir, model, scale_factor, time_context, overlap, batc
     if window is not None:
         d["window"] = window
     sampleRate, audioObj = scipy.io.wavfile.read(filein)
-    if sampleRate != 44100:
+    if sampleRate != 44100 and not resample:
         print("Sample rate is not 44100")        # separate_dsd.py:313
         return None
     arch = None if family in ("ikala",) else family
-    if keep_channels:
+    if sampleRate != 44100:
+        if isinstance(device, (list, tuple)):
+            if len(device) > 1:
+                raise ValueError(_one_over_devices_at_rate(filein, sampleRate))
+            device = device[0]
+        check_resample_rates(sampleRate, MODEL_RATE)        # a rate it cannot take is refused before the model loads
+        sep = get_separator(model, arch, frame_size, hop, d["window"], scale_factor, time_context, overlap, input_size,
+                            device=device, slot=slot)
+        if keep_channels:
+            maxv = np.finfo(audioObj.dtype).max if np.issubdtype(audioObj.dtype, np.floating) else np.iinfo(audioObj.dtype).max
+            audio = audioObj.astype('float') / maxv
+            if audioObj.shape[1] > 2:
+                stems = sep.separate_channels(audio, sample_rate=sampleRate)                # [L, nsrc, C]
+            else:
+                stems = sep.separate_keep_channels(audio, sample_rate=sampleRate, **wkw)    # [L, nsrc, 2]
+            stems16 = (stems.transpose(1, 0, 2).astype(np.float64) * np.iinfo(np.int16).max).astype('int16')
+        else:
+            stems = sep.separate(decode(audioObj, family), sample_rate=sampleRate)
+            stems16 = (stems.astype(np.float64) * np.iinfo(np.int16).max).astype('int16')
+    elif keep_channels:
         maxv = np.finfo(audioObj.dtype).max if np.issubdtype(audioObj.dtype, np.floating) else np.iinfo(audioObj.dtype).max
         if audioObj.shape[1] > 2:
             if isinstance(device, (list, tuple)):
@@ -138,7 +172,7 @@ def run(family, filein, outdir, model, scale_factor, time_context, overlap, batc
 
 # ---- command line shared by the separate_*.py scripts ------------------------------------------------------
 LONG_OPTS = ["ifile=", "odir=", "mfile=", "frame-size=", "window=", "devices=", "batch-clips=", "keep-channels", "wiener=",
-             "wiener-radius="]
+             "wiener-radius=", "resample"]
 EXTRA_USAGE = ("  optional: --frame-size N (STFT frame, feat_size = N/2+1)  --window hanning|blackmanharris|sinebell\n"
                "            --devices 0,1,...  --batch-clips K (clips in flight per device); with these, -i may be a directory of wavs\n"
                "            (one wav and several devices: the recording itself is cut into segments over the devices)\n"
@@ -146,7 +180,9 @@ EXTRA_USAGE = ("  optional: --frame-size N (STFT frame, feat_size = N/2+1)  --wi
                "            on wavs of more than 2 channels (5.1, arrays), for every script: stems of as many channels\n"
                "            --wiener K (with --keep-channels): K EM iterations of the multichannel Wiener post-filter on them\n"
                "            --wiener-radius R (with --wiener): covariances over a window of R chunks of 128 frames to either\n"
-               "            side instead of the whole clip; needed to cut one recording over several devices with --wiener")
+               "            side instead of the whole clip; needed to cut one recording over several devices with --wiener\n"
+               "            --resample: wavs at other rates (8 to 192 kHz, e.g. 48000, 96000) are resampled to 44.1 kHz and\n"
+               "            back on the GPU and their stems written at their own rate and length (one wav: one device)")
 
 
 def parse_cli(argv, usage):
@@ -160,7 +196,7 @@ def parse_cli(argv, usage):
         print(EXTRA_USAGE)
         sys.exit(2)
     o = {"inputfile": None, "outdir": None, "model": None, "frame_size": None, "window": None, "devices": None, "batch_clips": 1,
-         "keep_channels": False, "wiener": 0, "wiener_radius": 0}
+         "keep_channels": False, "wiener": 0, "wiener_radius": 0, "resample": False}
     for opt, arg in opts:
         if opt == "-h":
             print(usage)
@@ -186,6 +222,8 @@ def parse_cli(argv, usage):
             o["wiener"] = int(arg)
         elif opt == "--wiener-radius":
             o["wiener_radius"] = int(arg)
+        elif opt == "--resample":
+            o["resample"] = True
     if o["inputfile"] is None or o["outdir"] is None or o["model"] is None:
         print(usage)
         sys.exit(2)
@@ -196,7 +234,7 @@ def cli_main(argv, usage, train_auto_default, run_one, family=None):
     """`train_auto_default(inputfile, outdir, model)` = the script's literal reference call (no extra flag given);
     `run_one(filein, outdir, model, frame_size, window, device, slot, several_clips)` = the same with the overrides
     (with --keep-channels also keep_channels=True, wiener=K with --wiener K and wiener_radius=R with --wiener-radius R;
-    only the DSD100 / hiphopss script, family "dsd", takes them)."""
+    only the DSD100 / hiphopss script, family "dsd", takes them; with --resample also resample=True)."""
     import sys
     o = parse_cli(argv, usage)
     # more than 2 channels (of the wav, or of the first wav of a directory) widens --keep-channels to every
@@ -210,19 +248,23 @@ def cli_main(argv, usage, train_auto_default, run_one, family=None):
     if o["wiener"] and not o["wiener_radius"] and one_over_devices:
         sys.exit("--wiener %d over several devices needs --wiener-radius R >= 1: the recording is cut into segments, and "
                  "whole-clip covariances (wiener_radius 0) need the whole recording in one" % o["wiener"])
+    if o["resample"] and one_over_devices and wav_rate(o["inputfile"]) not in (None, 44100):
+        sys.exit(_one_over_devices_at_rate(o["inputfile"], wav_rate(o["inputfile"])))
+    kw = {"resample": True} if o["resample"] else {}
     if o["keep_channels"]:
-        base = run_one
-        kw = {"keep_channels": True}
+        kw["keep_channels"] = True
         if o["wiener"]:
             kw["wiener"] = o["wiener"]
         if o["wiener_radius"]:
             kw["wiener_radius"] = o["wiener_radius"]
+    if kw:
+        base = run_one
 
         def run_one(*args):
             return base(*args, **kw)
     plain = o["frame_size"] is None and o["window"] is None and o["devices"] is None and o["batch_clips"] == 1 \
         and not os.path.isdir(o["inputfile"])
-    if plain and o["keep_channels"]:
+    if plain and kw:
         return run_one(o["inputfile"], o["outdir"], o["model"], None, None, 0, 0, False)
     if plain:
         return train_auto_default(o["inputfile"], o["outdir"], o["model"])

@@ -43,14 +43,14 @@ def train_auto(filein, outdir, model, scale_factor=0.3, time_context=30, overlap
 
 
 def main(argv):
-    """`-i -o -m` as separate_dsd.py:316-332; extra long options (--keep-channels, --wiener and --wiener-radius among
+    """`-i -o -m` as separate_dsd.py:316-332; extra long options (--keep-channels, --wiener, --wiener-radius and --resample among
     them): see _common.parse_cli."""
-    def run_one(f, o, m, N, w, dev, slot, several, keep_channels=False, wiener=0, wiener_radius=0):
+    def run_one(f, o, m, N, w, dev, slot, several, keep_channels=False, wiener=0, wiener_radius=0, resample=False):
         # several clips into one directory: keep them apart the way the iKala / Bach10 scripts name their outputs
         name = (lambda fn, src: fn.replace(".wav", "_" + src + ".wav")) if several else (lambda fn, src: src + ".wav")
         return _common.run(FAMILY, f, o, m, 0.3, 30, 25, 32, (N or 1024) // 2 + 1, frame_size=N or 1024, hop=512,
                            out_name=name, window=w, device=dev, slot=slot, keep_channels=keep_channels, wiener=wiener,
-                           wiener_radius=wiener_radius)
+                           wiener_radius=wiener_radius, resample=resample)
     return _common.cli_main(argv, USAGE, lambda i, o, m: train_auto(i, o, m, 0.3, 30, 25, 32, 513), run_one,
                             family=FAMILY)  # separate_dsd.py:332
 

@@ -550,6 +550,34 @@ int dcs_separate_audio_channels_wiener(dcs_ctx* ctx, dcs_model* model, dcs_stft*
                                        int patcher, int iterations, int radius, float* d_stems, int64_t stem_stride,
                                        void* stream);
 
+/* ---- polyphase resampling by up/down (scipy.signal.resample_poly, padtype='constant') -------------------------- */
+/* The networks work on 44.1 kHz spectra; these take a recording at another rate to 44.1 kHz and its stems back.  The
+ * reference has no counterpart: its scripts refuse such files (separate_dsd.py:313).
+ * A resampler holds the polyphase bank of the caller's taps h[ntaps] (host double, already scaled by up, zero-phase about
+ * half_len = (ntaps - 1)/2; scipy.signal.resample_poly designs firwin(2*10*max(up, down) + 1, 1/max(up, down),
+ * window=('kaiser', 5.0)) * up).  The output is
+ *     y[n] = sum_j x[j] * h[n*down + half_len - j*up],   0 <= j < num_in,   0 <= n*down + half_len - j*up < ntaps,
+ * for n < num_out <= dcs_resampled_length(num_in, up, down): samples outside [0, num_in) are zeros.  The taps stay fp64 as
+ * given, the fp32 input is widened exactly, the ceil(ntaps/up) products of an output are summed in fp64 in a fixed order
+ * and rounded once to fp32: the same bits on every run.
+ *  - Refused with DCS_EINVAL: up or down < 1 or not coprime, ntaps even or < 1, a bank (ceil(ntaps/up) * up doubles)
+ *    over DCS_RESAMPLE_MAX_BANK_BYTES, a NULL argument.
+ *  - The bank lives in the resampler (device memory of ctx's device) until dcs_resampler_destroy; the ctx's workspace
+ *    does not change. */
+#define DCS_RESAMPLE_MAX_BANK_BYTES (112 * 1024)
+typedef struct dcs_resampler dcs_resampler;
+int dcs_resampler_create(dcs_ctx* ctx, int up, int down, const double* h, int ntaps, dcs_resampler** out);
+int dcs_resampler_destroy(dcs_resampler* resampler);
+/* ceil(num_in * up / down); -1 for a negative num_in or up, down < 1 */
+int64_t dcs_resampled_length(int64_t num_in, int up, int down);
+/* nplanes planes: plane p of the input at d_in + p*in_stride (first num_in samples valid; nothing else is read), plane p
+ * of the output at d_out + p*out_stride (num_out samples written).  A num_out shorter than the resampled length trims
+ * the tail (the way back to a recording's own length).  One launch on `stream`.
+ * Refused with DCS_EINVAL before anything is queued: a NULL pointer, nplanes < 1, num_in < 1, num_out < 1 or over
+ * dcs_resampled_length, negative strides, strides shorter than the rows with nplanes > 1, planes not 4-byte aligned. */
+int dcs_resample(dcs_resampler* resampler, const float* d_in, int nplanes, int64_t in_stride, int64_t num_in,
+                 float* d_out, int64_t out_stride, int64_t num_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
