@@ -70,6 +70,7 @@ _SIGS = {
     "dcs_gemm_view_f32": (C.c_int, [_p, C.c_int, C.c_int, _p, _p, _p]),
     "dcs_dsd_mask_f32": (C.c_int, [_p, C.c_int, _p, _p]),
     "dcs_dsd_convt2_f32": (C.c_int, [_p, _p, _p, _p]),
+    "dcs_dsd_dense_f32": (C.c_int, [_p, _p, _p, C.c_int, C.c_int, _p]),
     "dcs_sconv_mask_f32": (C.c_int, [_p, C.c_int, _p, _p]),
     "dcs_separate_audio": (C.c_int, [_p, _p, _p, _p, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
     "dcs_separate_host": (C.c_int, [_p, _p, _p, _p, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
@@ -117,6 +118,11 @@ class DsdMaskView(C.Structure):
 class DsdConvT2View(C.Structure):
     """dcs_dsd_convt2_view (include/dcs.h): the arguments of dcs_dsd_convt2_f32, field for field."""
     _fields_ = [("apad", _p), ("G", _p), ("ldg", C.c_int), ("npairs", C.c_int), ("tc", C.c_int)]
+
+
+class DsdDenseView(C.Structure):
+    """dcs_dsd_dense_view (include/dcs.h): the arguments of dcs_dsd_dense_f32, field for field."""
+    _fields_ = [("z", _p), ("bias", _p), ("apad", _p), ("P", C.c_int), ("tc", C.c_int), ("ndec", C.c_int), ("nfc", C.c_int)]
 
 
 class SconvMaskView(C.Structure):

@@ -456,10 +456,20 @@ static int dsd_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaS
   // bottleneck: patch k reads H2 rows k*step .. k*step+h2-1 (contiguous h2*C2p floats)
   GemmDesc g3 = gemm_plain(H2, (int64_t)step * C2p, ds.Wfc, nfc, ds.bfc, z, nfc, (int)P, nfc, h2 * C2p, 1);
   { ProfScope ps(ctx, "bottleneck_gemm", st); DCS_TRY(run_gemm(ctx, g3, ds.tWfc, st)); }
-  // the decoder dense layers side by side, scattered into the zero-padded buffer
-  GemmDesc g4 = gemm_plain(z, nfc, ds.Wdec, ndec * h2 * C2p, ds.bdec, ap, (int64_t)ndec * HP * C2p, (int)P, ndec * h2 * C2p, nfc, 1);
-  g4.n_seg = h2 * C2p; g4.n_ss = (int64_t)HP * C2p; g4.c_col0 = (int64_t)(kh2 - 1) * C2p;
-  { ProfScope ps(ctx, "dec_dense_gemm", st); DCS_TRY(run_gemm(ctx, g4, ds.tWdec, st)); }
+  // the decoder dense layers side by side, scattered into the interior rows of the zero-padded buffer: the
+  // tensor-core kernel keeps a slab of the weight in shared memory over many patches (dsd_dense_tc.cu)
+  {
+    ProfScope ps(ctx, "dec_dense_gemm", st);
+    if (ctx->debug_simt_gemm) {
+      GemmDesc g4 = gemm_plain(z, nfc, ds.Wdec, ndec * h2 * C2p, ds.bdec, ap, (int64_t)ndec * HP * C2p, (int)P, ndec * h2 * C2p, nfc, 1);
+      g4.n_seg = h2 * C2p; g4.n_ss = (int64_t)HP * C2p; g4.c_col0 = (int64_t)(kh2 - 1) * C2p;
+      DCS_TRY(launch_gemm(ctx, g4, st));
+    } else {
+      DsdDenseArgs a4;
+      a4.z = z; a4.bias = ds.bdec; a4.apad = ap; a4.P = (int)P; a4.tc = tc; a4.ndec = ndec; a4.nfc = nfc;
+      DCS_TRY(launch_dsd_dense_tc(ctx, a4, ds.tWdec, st));
+    }
+  }
   // InverseLayer(conv2): full correlation on the padded activations, rows (k, d, u).  The tensor-core
   // kernel reads each (patch, decoder) pair's interior rows once into shared memory (dsd_convT2_tc.cu).
   // The FFMA cross-check runs the same layer as a GEMM on an overlapping view of apad, rows ordered
@@ -830,6 +840,9 @@ static_assert(sizeof(dcs_dsd_convt2_view) == sizeof(DsdConvT2Args) && offsetof(d
                   offsetof(dcs_dsd_convt2_view, ldg) == offsetof(DsdConvT2Args, ldg) &&
                   offsetof(dcs_dsd_convt2_view, tc) == offsetof(DsdConvT2Args, tc),
               "dcs_dsd_convt2_view must mirror DsdConvT2Args");
+static_assert(sizeof(dcs_dsd_dense_view) == sizeof(DsdDenseArgs) && offsetof(dcs_dsd_dense_view, apad) == offsetof(DsdDenseArgs, apad) &&
+                  offsetof(dcs_dsd_dense_view, nfc) == offsetof(DsdDenseArgs, nfc),
+              "dcs_dsd_dense_view must mirror DsdDenseArgs");
 static_assert(sizeof(dcs_sconv_mask_view) == sizeof(SconvMaskArgs) && offsetof(dcs_sconv_mask_view, G) == offsetof(SconvMaskArgs, G) &&
                   offsetof(dcs_sconv_mask_view, S) == offsetof(SconvMaskArgs, S) &&
                   offsetof(dcs_sconv_mask_view, src_stride) == offsetof(SconvMaskArgs, src_stride) &&
@@ -880,6 +893,27 @@ int dcs_dsd_convt2_f32(dcs_ctx* ctx, const dcs_dsd_convt2_view* view, const floa
   int r = tc_weight_create(h_Wt2, 50, kh2 * 52, 50, &w);
   if (r == DCS_OK) r = launch_dsd_convT2_tc(ctx, a, w, st);
   r = sync_after("dcs_dsd_convt2_f32", r, st);
+  tc_weight_destroy(&w);
+  return r;
+}
+
+int dcs_dsd_dense_f32(dcs_ctx* ctx, const dcs_dsd_dense_view* view, const float* h_W, int w_rows, int w_cols, void* stream) {
+  DCS_REQUIRE(ctx && view && h_W && view->z && view->bias && view->apad, "dcs_dsd_dense_f32: NULL argument");
+  DsdDenseArgs a;
+  memcpy(&a, view, sizeof a);
+  DCS_REQUIRE(a.P > 0 && a.tc >= 4 && a.tc <= 64 && (a.ndec == 3 || a.ndec == 4) && a.nfc > 0 && a.nfc % 32 == 0 && a.nfc <= 256,
+              "dcs_dsd_dense_f32: bad shape");
+  DCS_REQUIRE((uintptr_t)a.z % 4 == 0 && (uintptr_t)a.bias % 4 == 0 && (uintptr_t)a.apad % 8 == 0,
+              "dcs_dsd_dense_f32: z and bias must be 4-byte and apad 8-byte aligned");
+  const int N = a.ndec * (a.tc - a.tc / 2 + 1) * 52;
+  DCS_REQUIRE(w_rows == a.nfc && w_cols == N, "dcs_dsd_dense_f32: weight is %dx%d, the layer wants %dx%d", w_rows, w_cols, a.nfc, N);
+  DCS_REQUIRE(dsd_dense_tc_supported(a), "dcs_dsd_dense_f32: unsupported arguments");
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  TcWeight w;
+  int r = tc_weight_create(h_W, N, a.nfc, N, &w);
+  if (r == DCS_OK) r = launch_dsd_dense_tc(ctx, a, w, st);
+  r = sync_after("dcs_dsd_dense_f32", r, st);
   tc_weight_destroy(&w);
   return r;
 }

@@ -293,6 +293,17 @@ struct DsdConvT2Args {
 bool dsd_convT2_tc_supported(const DsdConvT2Args& a);
 // w: the transposed conv2 weight as tc_weight_create lays it out (K = kh2 * 52, N = 50)
 int launch_dsd_convT2_tc(dcs_ctx* ctx, const DsdConvT2Args& a, const TcWeight& w, cudaStream_t st);   // dsd_convT2_tc.cu
+// the decoder dense layers of the DSD nets, N = ndec h2 52 columns, scattered into the interior rows of apad:
+// apad[k][d][kh2 - 1 + i][c] = ReLU(z[k] . W[:, n] + bias[n]), n = (d h2 + i) 52 + c
+struct DsdDenseArgs {
+  const float* z;      // [P][nfc], 4-byte aligned
+  const float* bias;   // [ndec h2 52]
+  float* apad;         // [P][ndec][h2 + 2 (kh2 - 1)][52]: interior rows written, 8-byte aligned
+  int P, tc, ndec, nfc;
+};
+bool dsd_dense_tc_supported(const DsdDenseArgs& a);
+// w: the dense weight as tc_weight_create lays it out (K = nfc, N = ndec h2 52)
+int launch_dsd_dense_tc(dcs_ctx* ctx, const DsdDenseArgs& a, const TcWeight& w, cudaStream_t st);   // dsd_dense_tc.cu
 // strided-conv1 families (iKala / Bach10): K3s arguments
 struct SconvMaskArgs {
   int arch;

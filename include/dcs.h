@@ -311,6 +311,23 @@ typedef struct {
 } dcs_dsd_convt2_view;
 int dcs_dsd_convt2_f32(dcs_ctx* ctx, const dcs_dsd_convt2_view* view, const float* h_Wt2, void* stream);
 
+/* Bring-up and test entry: the decoder dense layers of the DSD nets on the tensor cores, on buffers laid out as the
+ * layer sequence lays them out, for P patches, ndec 3 or 4 decoders, time_context tc in 4..64, kh2 = tc / 2,
+ * h2 = tc - kh2 + 1, bottleneck width nfc (a multiple of 32, at most 256), N = ndec * h2 * 52:
+ *   z     [P][nfc]                            bottleneck activations; 4-byte aligned
+ *   bias  [N]                                 device memory; 4-byte aligned
+ *   apad  [P][ndec][h2 + 2 (kh2 - 1)][52]     apad[k][d][kh2 - 1 + i][c] = ReLU(z[k] . h_W[:, n] + bias[n]) with
+ *                                            n = (d h2 + i) 52 + c; only these interior rows are written; 8-byte aligned
+ *   h_W   HOST [w_rows][w_cols] = [nfc][N]    transposed and split for the tensor cores on every call
+ * Every argument is checked before anything is queued.  Synchronises the stream before returning. */
+typedef struct {
+  const float* z;
+  const float* bias;
+  float* apad;
+  int P, tc, ndec, nfc;
+} dcs_dsd_dense_view;
+int dcs_dsd_dense_f32(dcs_ctx* ctx, const dcs_dsd_dense_view* view, const float* h_W, int w_rows, int w_cols, void* stream);
+
 /* The strided-conv1 networks (K3s): arch DCS_ARCH_BACH10, _BACH10_SCORE, _BACH10_SCORE_1X1, _IKALA, _IKALA_NOPOOL.
  * conv1 has KW taps at stride STRIDE over frequency (Bach10 nets 30 / 4, iKala 30 / 3, build_ca_1x1 5 / 2); J = (F-KW) /
  * STRIDE + 1 windows, WP = J / 4 pooled windows (DCS_ARCH_IKALA) or J; ND = ceil(KW / STRIDE).
