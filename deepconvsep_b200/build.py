@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdcs.so")
-SOURCES = ["api.cu", "stft.cu", "stft_reg.cu", "gemm.cu", "gemm_tc.cu", "dsd.cu", "dsd_tc.cu", "dsd_convT2_tc.cu", "dsd_dense_tc.cu", "sconv.cu", "sconv_tc.cu", "sconv_model.cu", "bsseval.cu",
+SOURCES = ["api.cu", "stft.cu", "stft_reg.cu", "gemm.cu", "gemm_tc.cu", "dsd.cu", "dsd_tc.cu", "dsd_convT2_tc.cu", "dsd_dense_tc.cu", "dsd_model.cu", "sconv.cu", "sconv_tc.cu", "sconv_model.cu", "bsseval.cu",
            "wiener.cu", "score1x1.cu", "score_notes.cu", "resample.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-O2,-Wall", "-DDCS_BUILD"]

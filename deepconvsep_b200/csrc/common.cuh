@@ -141,8 +141,8 @@ struct dcs_dsd {     // DSD100 / hiphopss and the stereo / ILD net
   int C1, C2, kh2, h2, nfc, ndec;
   int C1p, C2p;   // channel pitch of the activation buffers (multiple of 4 floats)
   int64_t ldw;
-  float *W1f, *b1, *W2c, *b2, *Wfc, *bfc, *Wdec, *bdec, *Wt2, *W1t, *bout;   // W1t is [nch][C1][ldw], bout [nch][4]
-  // tensor-core copies of the GEMM weights (K-major, 3xTF32 split)
+  float *b1, *b2, *bfc, *bdec, *W1t, *bout;   // W1t is [nch][C1][ldw], bout [nch][4]
+  // conv1, conv2, bottleneck, decoder dense and InverseLayer(conv2) weights for the tensor cores (K-major, 3xTF32 split)
   dcs::TcWeight tW1f, tW2c, tWfc, tWdec, tWt2;
 };
 struct dcs_sconv {   // strided-conv1 families: iKala (pool / no pool), Bach10
@@ -170,6 +170,7 @@ struct dcs_model {
 namespace dcs {
 // owned: a list the allocation is recorded in (a model's, which dcs_model_destroy frees)
 int upload(const std::vector<float>& h, float** d, std::vector<void*>* owned = nullptr);
+int model_create_dsd(dcs_model* m, int nparams, const float* const* hp, const int64_t* shp, const int* nd);
 int model_create_sconv(dcs_model* m, int nparams, const float* const* hp, const int64_t* shp, const int* nd);
 int model_create_s1x1(dcs_model* m, int nparams, const float* const* hp, const int64_t* shp, const int* nd);
 bool shape_is(const int64_t* s, int nd, int want_nd, int64_t a, int64_t b = 1, int64_t c = 1, int64_t d = 1);
@@ -186,7 +187,8 @@ struct NetCall {
   int overlap, step;
   uint64_t sig;     // layout signature of the zero-padded slots for this model and overlap
 };
-// the layer sequence of the 30-channel nets (DSD's: api.cu)
+// the layer sequence of each family (dsd_model.cu, sconv_model.cu, score1x1.cu)
+int dsd_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaStream_t st);
 int sconv_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaStream_t st);
 int s1x1_forward(dcs_ctx* ctx, const dcs_model* m, const NetCall& n, cudaStream_t st);
 // (re)zero a workspace slot whenever what it holds changes layout: zero padding is relied upon
@@ -261,7 +263,7 @@ int launch_gemm_tc(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, cudaStrea
 int launch_gemm_tc_epi(dcs_ctx* ctx, const GemmDesc& d, const TcWeight& w, int epi, cudaStream_t st);
 
 struct DsdMaskArgs {
-  const float* G;      // [P][3][tc][ldg]  decoder activations after the transposed conv2
+  const float* G;      // [P][ndec][tc][ldg]  decoder activations after the transposed conv2
   int ldg;
   const float* W1t;    // [50][ldw]  W1t[c][b] = conv1.W[c,0,0,F-1-b]
   int ldw;

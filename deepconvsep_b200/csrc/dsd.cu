@@ -1,8 +1,8 @@
 // dsd.cu -- K3 for the DSD100 / hiphopss network, exact-fp32 FFMA version: InverseLayer(conv1) +
 // ConcatLayer + output bias + ReLU + soft ratio mask + patch cross-fade + mixture-phase re-apply, fused.
 // The product path for the reference settings is the wgmma kernel in dsd_tc.cu; this one serves
-// (time_context, overlap) settings with more than 6 patches per frame and the DCS_DEBUG_SIMT_GEMM=1
-// cross-check.
+// (time_context, overlap) settings with more than 6 patches per frame and, under DCS_DEBUG_SIMT_GEMM=1,
+// the cross-check of the mask stage (every other layer stays on the tensor cores).
 //
 // Reference: examples/dsd100/separate_dsd.py:212-234 (l_inverse4x, l_merge, l_out), :258-271 (masks),
 // :139-169 (overlapadd_multi), :304 + :36-41 (compute_inverse).  Because conv1 spans the whole

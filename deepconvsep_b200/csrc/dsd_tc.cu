@@ -2,8 +2,8 @@
 // frame as ONE wgmma GEMM per tile, with bias + ReLU + soft ratio mask + patch cross-fade +
 // mixture-phase re-apply fused into the epilogue.  Same math as dsd.cu (reference:
 // separate_dsd.py:212-234, :258-271, :139-169, :304); dsd.cu remains the path for
-// (time_context, overlap) settings with more than 6 patches per frame and the DCS_DEBUG_SIMT_GEMM
-// cross-check.
+// (time_context, overlap) settings with more than 6 patches per frame and, under DCS_DEBUG_SIMT_GEMM=1,
+// the cross-check of this kernel alone.
 //
 // GEMM view (D = A * B^T, fp32-accurate 3xTF32):
 //   M = frequency bins  (128 per tile, one 64-row half per consumer warpgroup)

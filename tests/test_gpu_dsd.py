@@ -182,8 +182,9 @@ def test_full_size_properties():
 
 @pytest.mark.parametrize("arch,N,seconds", [("dsd", 1024, 1.5), ("dsd", 2048, 6.0), ("dsd_ild", 1024, 3.0)])
 def test_tensor_core_mask_matches_ffma_twin(monkeypatch, arch, N, seconds):
-    """the wgmma mask + cross-fade kernel (dsd_tc.cu) against its exact-fp32 FFMA twin (dsd.cu, selected with the GEMMs by
-    DCS_DEBUG_SIMT_GEMM=1, read when a context is created): same stems within the parity bar"""
+    """the wgmma mask + cross-fade kernel (dsd_tc.cu) against its exact-fp32 FFMA twin (dsd.cu, selected by
+    DCS_DEBUG_SIMT_GEMM=1, read when a context is created; every other layer stays on the tensor cores): same stems
+    within the parity bar"""
     from deepconvsep_b200.engine import Separator
     F = N // 2 + 1
     params = nets.make_synthetic_params(arch, F, seed=2)

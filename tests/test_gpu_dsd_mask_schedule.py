@@ -1,5 +1,6 @@
 """Edges of the persistent schedule of the wgmma mask + cross-fade kernel (dsd_tc.cu), checked against its
-exact-fp32 FFMA twin (dsd.cu, selected with the GEMMs by DCS_DEBUG_SIMT_GEMM=1, read when a context is created):
+exact-fp32 FFMA twin (dsd.cu, selected by DCS_DEBUG_SIMT_GEMM=1, read when a context is created; every other layer
+stays on the tensor cores):
 
 - DSD100 at N=2048 on a 0.5 s clip: fewer (tile, group) work items than SMs, and a last group of 8 frames that is
   only partly inside the clip;

@@ -1,7 +1,7 @@
 """Every operand view and epilogue of the GEMM (csrc/common.cuh GemmDesc) on both engines against a float64 reference,
 element by element, through dcs_gemm_view_f32.
 
-The views are built the way the layers build them (api.cu dsd_forward, sconv_model.cu sconv_forward, score1x1.cu
+The views are built the way the layers build them (dsd_model.cu dsd_forward, sconv_model.cu sconv_forward, score1x1.cu
 s1x1_forward), at their real shapes, plus the edges of the kernels' control logic.  Every case
   - requires |C - C64| <= bound (below) for every stored element;
   - fills every C element outside the view with a NaN-payload sentinel and every A element outside the view with NaN,
@@ -287,7 +287,7 @@ def _bias(rng, n, s=0.1):
 
 def dsd_layer(name):
     """the DSD100 net at N = 2048 (F = 1025, ldf 1032), time_context 30, overlap 25, util patcher, on a 180 s clip at
-    hop 512 (T = 15506, P = 3097, Tp = 15510), as api.cu dsd_forward builds each view"""
+    hop 512 (T = 15506, P = 3097, Tp = 15510), as dsd_model.cu dsd_forward builds each view"""
     rng = _rng(name)
     T, P, Tp, F, ldf, step = 15506, 3097, 15510, 1025, 1032, 5
     C1 = C2 = 50

@@ -167,7 +167,7 @@ def test_separate_spec_channels_matches_audio_score():
                                                               ("ikala", 513, 1024, 512, "hanning", 20, 3.0),
                                                               ("ikala_nopool", 513, 1024, 512, "hanning", 20, 3.0)])
 def test_tensor_core_mask_matches_ffma_twin(monkeypatch, arch, F, N, hop, win, overlap, seconds):
-    """the wgmma K3s kernel (sconv_tc.cu) against its exact-fp32 FFMA twin (sconv.cu, selected with the GEMMs by
+    """the wgmma K3s kernel (sconv_tc.cu) against its exact-fp32 FFMA twin (sconv.cu, selected by
     DCS_DEBUG_SIMT_GEMM=1, read when a context is created): same stems within the parity bar"""
     from deepconvsep_b200.engine import Separator
     params = nets.make_synthetic_params(arch, F, seed=5)
