@@ -61,7 +61,7 @@ enum NetSlot {
   NET_CHANS,                                // score-informed net: the 4 input channel planes
   NET_SPLITK,                               // split-K partial sums of the tensor-core GEMM
   NET_XC_PTRS, NET_XC_PARTIAL,              // dcs_xcorr_lags
-  NET_XTAB,                                 // DSD mask kernel's frame table
+  NET_XTAB, NET_AIMG,                       // DSD mask kernel's fade table and pre-split A operand image
   NET_ENC, NET_CODES, NET_DEC,              // 1x1 score net: encoder activations, ReLU gate codes, decoder chunk
   NET_NOTES,                                // compacted note table of the score-informed nets (score_notes.cu)
   NET_SLOTS
