@@ -65,6 +65,8 @@ _SIGS = {
     "dcs_separate_audio_channels": (C.c_int, [_p, _p, _p, _p, C.c_int, _i64, _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
     "dcs_separate_audio_channels_wiener": (C.c_int, [_p, _p, _p, _p, C.c_int, _i64, _i64, C.c_float, C.c_int, C.c_int, C.c_int,
                                                      C.c_int, _p, _i64, _p]),
+    "dcs_separate_batch_pcm16_channels_host": (C.c_int, [_p, _p, _p, C.c_int, _p, _p, C.c_int, C.c_int, C.c_int, C.c_float,
+                                                         C.c_int, C.c_int, _p, _p, _p]),
     "dcs_xcorr_lags": (C.c_int, [_p, _p, _p, C.c_int, _i64, C.c_int, _p, _p]),
     "dcs_gemm_f32": (C.c_int, [_p, C.c_int, _p, _i64, _p, _i64, _p, _p, _i64, C.c_int, C.c_int, C.c_int, C.c_int, _p]),
     "dcs_gemm_view_f32": (C.c_int, [_p, C.c_int, C.c_int, _p, _p, _p]),

@@ -420,20 +420,20 @@ static int size_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, i
 
 // the workspace of downmix_clip: the masks-output workspace, the downmix, the nsrc mask planes and ONE mixture STFT
 // plane, whatever the channel count.  wx > 0 (the filter on, wx channels): wx STFT planes, nsrc x wx masked spectra
-// and the filter's sums over covariance windows of `radius` chunks.  staged (the int16 keep-channels batch): three audio
-// planes (downmix, left, right) and nsrc x 2 stem planes
-static int size_downmix_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, int wx, int radius, bool staged,
+// and the filter's sums over covariance windows of `radius` chunks.  staged > 0 (the int16 batch of `staged` channels):
+// staged + 1 audio planes (the downmix, then the channels) and nsrc x staged stem planes
+static int size_downmix_workspace(dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, int64_t L, int wx, int radius, int staged,
                                   cudaStream_t st) {
   const int64_t plane = dcs_num_frames(L, p->hop) * dcs_padded_bins(p->N);
   DCS_TRY(size_workspace(ctx, m, p, L, false, st, true));
-  DCS_TRY(ctx->audio.ensure((size_t)(staged ? 3 : 1) * L * sizeof(float), st));
+  DCS_TRY(ctx->audio.ensure((size_t)(staged + 1) * L * sizeof(float), st));
   DCS_TRY(ctx->masks.ensure((size_t)m->nsrc * plane * sizeof(float), st));
   DCS_TRY(ctx->X.ensure((size_t)(wx > 0 ? wx : 1) * plane * sizeof(float2), st));
   if (wx > 0) {
     DCS_TRY(ctx->S.ensure((size_t)m->nsrc * wx * plane * sizeof(float2), st));
     DCS_TRY(ctx->wiener.ensure(wiener_workspace_bytes(m->nsrc, wx, dcs_num_frames(L, p->hop), m->F, radius), st));
   }
-  if (staged) DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * 2 * L * sizeof(float), st));
+  if (staged > 0) DCS_TRY(ctx->stems.ensure((size_t)m->nsrc * staged * L * sizeof(float), st));
   return DCS_OK;
 }
 
@@ -513,7 +513,7 @@ static int downmix_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const flo
                         int64_t audio_stride, int64_t L, int iterations, int radius, float scale_factor, int overlap,
                         int patcher, float* d_stems, int64_t stem_stride, cudaStream_t st) {
   const bool filter = iterations > 0;
-  DCS_TRY(size_downmix_workspace(ctx, m, p, L, filter ? nx : 0, radius, false, st));
+  DCS_TRY(size_downmix_workspace(ctx, m, p, L, filter ? nx : 0, radius, 0, st));
   const int64_t T = dcs_num_frames(L, p->hop), ldf = dcs_padded_bins(p->N), plane = T * ldf;
   float* masks = ctx->masks.as<float>();
   if (!d_mono) {
@@ -830,13 +830,17 @@ int dcs_separate_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const int16
 // int16 staging on the device and events for the hand-overs.  The reference's only multi-clip driver starts a Python
 // process per file (examples/dsd100/separate_multiple.ipynb cell 3); per clip this is the wav contract of train_auto
 // (separate_dsd.py:275-287,307-309), exactly dcs_separate_pcm16_host.  Host buffers should be pinned.
-// the pipelined loop of dcs_separate_batch_pcm16_host; on any failure the caller drains the copy streams before it
-// returns, because the copies in flight read and write the user's host buffers.  keep (keep-channels mode, 2 channels):
-// the clip is decoded into (downmix, left, right) planes, the stems are encoded as interleaved [L][2] per source
+// the pipelined loop of the int16 batch entry points; on any failure the caller drains the copy streams before it
+// returns, because the copies in flight read and write the user's host buffers.  nx == 0: mono stems, the clip decoded
+// into one plane (channel 0 or the downmix of `downmix`), int16 [nsrc][L] out.  nx > 0 (C-channel stems, nx ==
+// channels): the clip is decoded into nx + 1 planes (the downmix, then the channels), separated as
+// dcs_separate_audio_channels_wiener with `iterations` and `radius`, and the stems encoded as interleaved [L][nx] per
+// source
 static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
-                          const int64_t* num_samples, int channels, int downmix, bool keep, float scale_factor, int overlap,
-                          int patcher, int16_t* const* h_out, const int64_t* out_strides, cudaStream_t st) {
-  const int w = keep ? 2 : 1;   // int16 values per sample of a stem
+                          const int64_t* num_samples, int channels, int downmix, int nx, int iterations, int radius,
+                          float scale_factor, int overlap, int patcher, int16_t* const* h_out, const int64_t* out_strides,
+                          cudaStream_t st) {
+  const int w = nx > 0 ? nx : 1;   // int16 values per sample of a stem
   float *audio = ctx->audio.as<float>(), *stems = ctx->stems.as<float>();
   // the copy streams start after whatever the caller queued on `st` (and after the memsets of fresh buffers)
   DCS_CUDA(cudaEventRecord(ctx->ev_dec[0], st));
@@ -851,11 +855,12 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, c
     DCS_CUDA(cudaEventRecord(ctx->ev_in[b], ctx->s_h2d));
     // kernels of clip i
     DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_in[b], 0));
-    if (keep) {
-      DCS_TRY(launch_pcm_decode_keep(ctx, ctx->pcm_in[b].as<int16_t>(), L, audio, st));
+    if (nx > 0) {
+      ProfScope ps(ctx, "pcm16_decode_separate", st);   // the clip's kernels up to its stem planes
+      DCS_TRY(launch_pcm_decode_channels(ctx, ctx->pcm_in[b].as<int16_t>(), L, nx, audio, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
-      DCS_TRY(downmix_clip(ctx, m, p, audio, audio + L, 2, L, L, ctx->wiener_iters, ctx->wiener_radius, scale_factor, overlap,
-                           patcher, stems, L, st));
+      DCS_TRY(downmix_clip(ctx, m, p, audio, audio + L, nx, L, L, iterations, radius, scale_factor, overlap, patcher, stems, L,
+                           st));
     } else {
       DCS_TRY(launch_pcm_decode(ctx, ctx->pcm_in[b].as<int16_t>(), L, channels, downmix, audio, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
@@ -863,9 +868,10 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, c
                             st));
     }
     if (i >= 2) DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_out[b], 0));     // D2H of clip i-2 has drained the output staging
-    if (keep)
-      DCS_TRY(launch_pcm_encode_keep(ctx, stems, L, m->nsrc, L, ctx->pcm_out[b].as<int16_t>(), st));
-    else
+    if (nx > 0) {
+      ProfScope ps(ctx, "pcm16_encode", st);
+      DCS_TRY(launch_pcm_encode_channels(ctx, stems, L, m->nsrc, nx, L, ctx->pcm_out[b].as<int16_t>(), st));
+    } else
       DCS_TRY(launch_pcm_encode(ctx, stems, L, m->nsrc, L, ctx->pcm_out[b].as<int16_t>(), L, st));
     DCS_CUDA(cudaEventRecord(ctx->ev_enc[b], st));
     // D2H of clip i
@@ -878,20 +884,24 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, c
   return DCS_OK;
 }
 
-// the checks, resources and drain of both int16 batch entry points around batch_pipeline
+// the checks, resources and drain of every int16 batch entry point around batch_pipeline (nx, iterations, radius as
+// there).  check_model(Lmax): the entry point's own checks of the model, plan and options, run on the longest clip
+// after the per-clip checks and before anything is queued
+extern "C++" {
+template <class CheckModel>
 static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
-                      const int64_t* num_samples, int channels, int downmix, bool keep, float scale_factor, int overlap,
-                      int patcher, int16_t* const* h_out, const int64_t* out_strides, cudaStream_t st) {
+                      const int64_t* num_samples, int channels, int downmix, int nx, int iterations, int radius,
+                      float scale_factor, int overlap, int patcher, int16_t* const* h_out, const int64_t* out_strides,
+                      cudaStream_t st, CheckModel check_model) {
   DCS_REQUIRE(ctx && m && p && h_pcm && num_samples && h_out && out_strides && nclips >= 0, "%s: bad argument", fn);
-  DCS_REQUIRE(channels >= 1 && channels <= 8 && downmix >= 0 && downmix <= 2, "bad channels/downmix");
+  DCS_REQUIRE(nx > 0 || (channels >= 1 && channels <= 8 && downmix >= 0 && downmix <= 2), "bad channels/downmix");
   if (nclips == 0) return DCS_OK;
   int64_t Lmax = 0;
   for (int i = 0; i < nclips; ++i) {
     DCS_REQUIRE(h_pcm[i] && h_out[i] && num_samples[i] > 0 && out_strides[i] >= num_samples[i], "clip %d: bad buffer / length", i);
     Lmax = std::max(Lmax, num_samples[i]);
   }
-  DCS_TRY(check_clip(fn, ctx, m, p, keep ? DCS_ARCH_DSD : -1, h_pcm, h_out, Lmax, Lmax, Lmax, overlap, patcher));
-  if (keep) DCS_TRY(check_keep_tap(fn, ctx));
+  DCS_TRY(check_model(Lmax));
   DCS_CUDA(cudaSetDevice(ctx->device));
   // each resource on its own: a call that failed half-way through this block must not leave later calls with null handles
   if (!ctx->s_h2d) DCS_CUDA(cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
@@ -906,14 +916,14 @@ static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, i
   // re-allocated mid-batch would synchronise the stream
   for (int b = 0; b < std::min(nclips, 2); ++b) {
     DCS_TRY(ctx->pcm_in[b].ensure((size_t)Lmax * channels * sizeof(int16_t), st));
-    DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * (keep ? 2 : 1) * Lmax * sizeof(int16_t), st));
+    DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * (nx > 0 ? nx : 1) * Lmax * sizeof(int16_t), st));
   }
-  if (keep)
-    DCS_TRY(size_downmix_workspace(ctx, m, p, Lmax, ctx->wiener_iters > 0 ? 2 : 0, ctx->wiener_radius, true, st));
+  if (nx > 0)
+    DCS_TRY(size_downmix_workspace(ctx, m, p, Lmax, iterations > 0 ? nx : 0, radius, nx, st));
   else
     DCS_TRY(size_workspace(ctx, m, p, Lmax, true, st));
-  const int rc = batch_pipeline(ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, keep, scale_factor, overlap, patcher,
-                                h_out, out_strides, st);
+  const int rc = batch_pipeline(ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, nx, iterations, radius, scale_factor,
+                                overlap, patcher, h_out, out_strides, st);
   // drain everything, success or not, before the host buffers go back to the caller
   const cudaError_t e0 = cudaStreamSynchronize(ctx->s_h2d), e1 = cudaStreamSynchronize(ctx->s_d2h), e2 = cudaStreamSynchronize(st);
   if (rc != DCS_OK) return rc;
@@ -922,21 +932,31 @@ static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, i
   DCS_CUDA(e2);
   return DCS_OK;
 }
+}  // extern "C++"
 
 int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
                                   const int64_t* num_samples, int channels, int downmix, float scale_factor, int overlap,
                                   int patcher, int16_t* const* h_out, const int64_t* out_strides, void* stream) {
-  return batch_host("dcs_separate_batch_pcm16_host", ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, false,
-                    scale_factor, overlap, patcher, h_out, out_strides, (cudaStream_t)stream);
+  const char* fn = "dcs_separate_batch_pcm16_host";
+  return batch_host(fn, ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, 0, 0, 0, scale_factor, overlap, patcher,
+                    h_out, out_strides, (cudaStream_t)stream, [&](int64_t Lmax) {
+                      return check_clip(fn, ctx, m, p, -1, h_pcm, h_out, Lmax, Lmax, Lmax, overlap, patcher);
+                    });
 }
 
 // ------------------------------------------------------------------------------------ keep-channels (DSD100 net)
+// the C = 2 batch with the filter settings of the ctx
 int dcs_separate_batch_pcm16_keep_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips,
                                                 const int16_t* const* h_pcm, const int64_t* num_samples, float scale_factor,
                                                 int overlap, int patcher, int16_t* const* h_out, const int64_t* out_strides,
                                                 void* stream) {
-  return batch_host("dcs_separate_batch_pcm16_keep_channels_host", ctx, m, p, nclips, h_pcm, num_samples, 2, 1, true,
-                    scale_factor, overlap, patcher, h_out, out_strides, (cudaStream_t)stream);
+  const char* fn = "dcs_separate_batch_pcm16_keep_channels_host";
+  return batch_host(fn, ctx, m, p, nclips, h_pcm, num_samples, 2, 1, 2, ctx ? ctx->wiener_iters : 0,
+                    ctx ? ctx->wiener_radius : 0, scale_factor, overlap, patcher, h_out, out_strides, (cudaStream_t)stream,
+                    [&](int64_t Lmax) {
+                      DCS_TRY(check_clip(fn, ctx, m, p, DCS_ARCH_DSD, h_pcm, h_out, Lmax, Lmax, Lmax, overlap, patcher));
+                      return check_keep_tap(fn, ctx);
+                    });
 }
 
 int dcs_separate_audio_keep_channels(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride,
@@ -1043,8 +1063,8 @@ int dcs_apply_masks(dcs_ctx* ctx, dcs_stft* p, const float* d_audio, int nx, int
 }
 
 // the checks of dcs_separate_audio_channels(_wiener): with iterations > 0 also those of the filter on the clip's spectra
-static int check_channels(const char* fn, const dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, const float* d_audio, int nx,
-                          int64_t audio_stride, int64_t L, int overlap, int patcher, const float* d_stems, int64_t stem_stride,
+static int check_channels(const char* fn, const dcs_ctx* ctx, const dcs_model* m, const dcs_stft* p, const void* d_audio, int nx,
+                          int64_t audio_stride, int64_t L, int overlap, int patcher, const void* d_stems, int64_t stem_stride,
                           int iterations, int radius) {
   DCS_REQUIRE(!m || (m->arch != DCS_ARCH_DSD_ILD && !score_arch(m->arch)),
               "%s does not serve architecture %d: use dcs_separate_masks* + dcs_apply_masks", fn, m->arch);
@@ -1079,6 +1099,25 @@ int dcs_separate_audio_channels_wiener(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, 
   DCS_CUDA(cudaSetDevice(ctx->device));
   return downmix_clip(ctx, m, p, nullptr, d_audio, nx, audio_stride, L, iterations, radius, scale_factor, overlap, patcher,
                       d_stems, stem_stride, (cudaStream_t)stream);
+}
+
+// the int16 batch of C-channel clips: per clip dcs_separate_audio_channels_wiener on the decoded planes, with the checks
+// of that call on the longest clip
+int dcs_separate_batch_pcm16_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
+                                           const int64_t* num_samples, int channels, int iterations, int radius,
+                                           float scale_factor, int overlap, int patcher, int16_t* const* h_out,
+                                           const int64_t* out_strides, void* stream) {
+  const char* fn = "dcs_separate_batch_pcm16_channels_host";
+  DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
+  DCS_REQUIRE(iterations >= 0, "%s: iterations %d must be >= 0", fn, iterations);
+  DCS_REQUIRE(radius >= 0, "%s: radius %d must be >= 0", fn, radius);
+  DCS_REQUIRE(iterations == 0 || (channels >= 2 && channels <= 8), "%s: the Wiener post-filter needs channels in [2, 8], got %d",
+              fn, channels);
+  return batch_host(fn, ctx, m, p, nclips, h_pcm, num_samples, channels, 0, channels, iterations, radius, scale_factor, overlap,
+                    patcher, h_out, out_strides, (cudaStream_t)stream, [&](int64_t Lmax) {
+                      return check_channels(fn, ctx, m, p, h_pcm, channels, Lmax, Lmax, overlap, patcher, h_out, Lmax,
+                                            iterations, radius);
+                    });
 }
 
 // ------------------------------------------------------------------------------------ Wiener post-filter

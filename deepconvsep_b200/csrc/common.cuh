@@ -349,12 +349,13 @@ int launch_pcm_decode(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int channel
                       cudaStream_t st);
 int launch_pcm_encode(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int64_t stem_stride, int16_t* d_out,
                       int64_t out_stride, cudaStream_t st);
-// stereo stems: interleaved int16 [L][2] -> three float planes L apart (downmix, left, right); nsrc x 2 stem planes
-// (source, channel) -> int16 [nsrc][L][2], source s at d_out + s * 2 * L
-int launch_pcm_decode_keep(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, float* d_planes, cudaStream_t st);
-int launch_pcm_encode_keep(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int64_t stem_stride, int16_t* d_out,
-                           cudaStream_t st);
-// nx float planes -> (((a_0 + a_1) + a_2) + ...) * (1.0f / nx): the downmix of launch_pcm_decode_keep at nx = 2, a copy
+// C-channel stems, C in [1, 16]: interleaved int16 [L][C] -> C + 1 float planes L apart (the downmix of
+// launch_downmix, then the C channels); nsrc x C stem planes (source, channel) -> int16 [nsrc][L][C], source s at
+// d_out + s * C * L
+int launch_pcm_decode_channels(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int C, float* d_planes, cudaStream_t st);
+int launch_pcm_encode_channels(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int C, int64_t stem_stride,
+                               int16_t* d_out, cudaStream_t st);
+// nx float planes -> (((a_0 + a_1) + a_2) + ...) * (1.0f / nx): the downmix of launch_pcm_decode_channels, a copy
 // at nx = 1
 int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st);
 

@@ -208,20 +208,26 @@ __global__ void pcm_encode_kernel(const float* __restrict__ stems, int64_t L, in
   out[(int64_t)s * out_stride + i] = (int16_t)(int)v;
 }
 
-// keep-channels mode: interleaved int16 [L][2] -> planes (downmix, left, right), L apart; the downmix is the
-// expression of pcm_decode_kernel's downmix 1, so the network sees what the mono call would see
-__global__ void pcm_decode_keep_kernel(const int16_t* __restrict__ pcm, int64_t L, float* __restrict__ planes) {
+// C-channel stems: interleaved int16 [L][C] -> C + 1 float planes L apart: the downmix, then channel c at plane 1 + c.
+// Each channel is pcm / 32767 and the downmix is downmix_kernel's expression on those planes, so at C = 2 it is
+// pcm_decode_kernel's downmix 1 and the network sees what the mono call would see
+__global__ void pcm_decode_channels_kernel(const int16_t* __restrict__ pcm, int64_t L, int C, float* __restrict__ planes) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= L) return;
   const float maxv = 32767.0f;
-  const float l = (float)pcm[2 * i] / maxv, r = (float)pcm[2 * i + 1] / maxv;
-  planes[i] = (l + r) * 0.5f;
-  planes[L + i] = l;
-  planes[2 * L + i] = r;
+  const int16_t* row = pcm + i * C;
+  float a = (float)row[0] / maxv;
+  planes[L + i] = a;
+  for (int c = 1; c < C; ++c) {
+    const float v = (float)row[c] / maxv;
+    planes[(int64_t)(1 + c) * L + i] = v;
+    a += v;
+  }
+  planes[i] = a * (1.0f / (float)C);
 }
 
 // nx float planes (stride apart) -> (((a_0 + a_1) + a_2) + ...) * (1.0f / nx), summed in that order: the bits of
-// pcm_decode_keep_kernel's downmix at nx = 2, the channel itself at nx = 1
+// pcm_decode_channels_kernel's downmix, the channel itself at nx = 1
 __global__ void downmix_kernel(const float* __restrict__ audio, int nx, int64_t stride, int64_t L, float* __restrict__ mono) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= L) return;
@@ -230,16 +236,40 @@ __global__ void downmix_kernel(const float* __restrict__ audio, int nx, int64_t 
   mono[i] = a * (1.0f / (float)nx);
 }
 
-// stem planes (source s, channel c) at stems + (2 s + c) * stem_stride -> int16 [nsrc][L][2] (what writeAudioScipy
-// writes for a 2-channel stem), the truncation rule of pcm_encode_kernel
-__global__ void pcm_encode_keep_kernel(const float* __restrict__ stems, int64_t L, int64_t stem_stride,
-                                       int16_t* __restrict__ out) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= L) return;
+constexpr int kPcmEncodeRows = 256;   // rows (samples) of one CTA's tile, one per thread
+constexpr int kPcmMaxChannels = 16;
+
+// stem planes (source s, channel c) at stems + (s C + c) * stem_stride -> int16 [nsrc][L][C] (what
+// scipy.io.wavfile.write takes for a C-channel stem), source s at out + s C L, the truncation rule of
+// pcm_encode_kernel; grid (ceil(L / 256), nsrc).  A thread's C samples are not an aligned vector for most C, so the
+// tile of 256 interleaved rows is staged in shared memory at the byte offset its destination has modulo 16: the
+// 16-byte-aligned middle of the destination then meets 16-byte-aligned shared memory, and each warp stores 512
+// contiguous bytes with 16-byte stores.  The up to 7 values before the first and after the last aligned piece (a
+// source's rows start at s C L 2 bytes, not always a multiple of 16) go out one int16 at a time.
+__global__ void __launch_bounds__(kPcmEncodeRows)
+pcm_encode_channels_kernel(const float* __restrict__ stems, int64_t L, int C, int64_t stem_stride, int16_t* __restrict__ out) {
+  __shared__ __align__(16) int16_t tile[kPcmEncodeRows * kPcmMaxChannels + 8];
   const int s = blockIdx.y;
-  const float l = stems[(int64_t)(2 * s) * stem_stride + i] * 32767.0f;
-  const float r = stems[(int64_t)(2 * s + 1) * stem_stride + i] * 32767.0f;
-  reinterpret_cast<short2*>(out + (int64_t)s * 2 * L)[i] = make_short2((int16_t)(int)l, (int16_t)(int)r);
+  const int64_t i0 = (int64_t)blockIdx.x * kPcmEncodeRows;
+  const int rows = (int)(L - i0 < kPcmEncodeRows ? L - i0 : kPcmEncodeRows);
+  int16_t* dst = out + ((int64_t)s * L + i0) * C;                   // the tile's first value
+  const int shift = (int)(((uintptr_t)dst & 15) >> 1);              // in int16 values
+  if ((int)threadIdx.x < rows) {
+    const float* src = stems + (int64_t)s * C * stem_stride + i0 + threadIdx.x;
+    for (int c = 0; c < C; ++c)
+      tile[shift + threadIdx.x * C + c] = (int16_t)(int)(src[(int64_t)c * stem_stride] * 32767.0f);
+  }
+  __syncthreads();
+  const int n = rows * C;                                           // values of the tile
+  const int head = min(n, (8 - shift) & 7);                         // values before the first 16-byte boundary
+  const int nvec = (n - head) >> 3;
+  const int tail0 = head + nvec * 8;
+  const uint4* vsrc = reinterpret_cast<const uint4*>(tile + shift + head);
+  uint4* vdst = reinterpret_cast<uint4*>(dst + head);
+  for (int k = threadIdx.x; k < nvec; k += kPcmEncodeRows) vdst[k] = vsrc[k];
+  if ((int)threadIdx.x < head) dst[threadIdx.x] = tile[shift + threadIdx.x];
+  const int t = tail0 + (int)threadIdx.x;
+  if (t < n) dst[t] = tile[shift + t];
 }
 
 template <int N>
@@ -329,9 +359,10 @@ int launch_pcm_decode(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int channel
   return DCS_OK;
 }
 
-int launch_pcm_decode_keep(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, float* d_planes, cudaStream_t st) {
+int launch_pcm_decode_channels(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int C, float* d_planes, cudaStream_t st) {
   if (L <= 0) return DCS_OK;
-  pcm_decode_keep_kernel<<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(d_pcm, L, d_planes);
+  DCS_REQUIRE(C >= 1 && C <= kPcmMaxChannels, "pcm_decode_channels: %d channels not in [1, %d]", C, kPcmMaxChannels);
+  pcm_decode_channels_kernel<<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(d_pcm, L, C, d_planes);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;
@@ -345,12 +376,13 @@ int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_str
   return DCS_OK;
 }
 
-int launch_pcm_encode_keep(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int64_t stem_stride, int16_t* d_out,
-                           cudaStream_t st) {
+int launch_pcm_encode_channels(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int C, int64_t stem_stride,
+                               int16_t* d_out, cudaStream_t st) {
   if (L <= 0) return DCS_OK;
-  DCS_REQUIRE((uintptr_t)d_out % 4 == 0, "pcm_encode_keep: output not 4-byte aligned");
-  dim3 grid((unsigned)ceil_div64(L, 256), (unsigned)nsrc);
-  pcm_encode_keep_kernel<<<grid, 256, 0, st>>>(d_stems, L, stem_stride, d_out);
+  DCS_REQUIRE(C >= 1 && C <= kPcmMaxChannels, "pcm_encode_channels: %d channels not in [1, %d]", C, kPcmMaxChannels);
+  DCS_REQUIRE((uintptr_t)d_out % 2 == 0, "pcm_encode_channels: output not 2-byte aligned");
+  dim3 grid((unsigned)ceil_div64(L, kPcmEncodeRows), (unsigned)nsrc);
+  pcm_encode_channels_kernel<<<grid, kPcmEncodeRows, 0, st>>>(d_stems, L, C, stem_stride, d_out);
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;

@@ -642,6 +642,37 @@ class Separator(object):
         assert all((1 if p_.ndim == 1 else p_.shape[1]) == ch for p_ in ps), "all clips must have the same channel count"
         return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_host, ps, outs, (), (ch, int(downmix if ch > 1 else 0)))
 
+    def separate_pcm16_channels_batch(self, clips, outs=None, wiener=0, wiener_radius=0):
+        """C-channel int16 clips through the context's multi-clip scheduler (dcs_separate_batch_pcm16_channels_host):
+        H2D of clip i+1, the kernels of clip i and D2H of clip i-1 overlap, and the decode to fp32 and the encode of the
+        stems to int16 run on the device.  clips: list of int16 arrays [L, C] with the same C in 1..16 (pinned for real
+        overlap) -> list of int16 [nsrc, L, C] (into `outs` when given, which may be pinned): per clip
+        (separate_channels(clip / 32767, wiener, wiener_radius) * 32767) truncated to int16 in fp32, source by source.
+        wiener > 0 (C in 2..8): EM iterations of the Wiener post-filter, over covariance windows of wiener_radius
+        chunks.  At C = 2 with the DSD100 network, the bytes of separate_pcm16_batch(keep_channels=True) with the same
+        wiener and wiener_radius."""
+        check_channels_family(self.model.arch)
+        check_wiener_radius(wiener, wiener_radius)
+        if wiener < 0:
+            raise ValueError("wiener %d: the number of EM iterations cannot be negative" % wiener)
+        ps = []
+        for c in clips:
+            a = np.asarray(c)
+            if a.dtype != np.int16 or a.ndim != 2:
+                raise ValueError("separate_pcm16_channels_batch needs int16 clips [L, C], got %s %r" % (a.dtype, a.shape))
+            ps.append(np.ascontiguousarray(a))
+        if not ps:
+            return []
+        ch = ps[0].shape[1]
+        if any(p_.shape[1] != ch for p_ in ps):
+            raise ValueError("all clips of a batch must have the same channel count, got %r" % sorted({p_.shape[1] for p_ in ps}))
+        if not 1 <= ch <= 16:
+            raise ValueError("separate_pcm16_channels_batch takes 1 to 16 channels, got %d" % ch)
+        if wiener:
+            check_wiener_channels(ch)
+        return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_channels_host, ps, outs, (ch,),
+                                 (ch, int(wiener), int(wiener_radius)))
+
     def _pcm16_batch(self, entry, ps, outs, channels, args):
         """int16 clips ps through the multi-clip entry point `entry` -> outs, int16 [nsrc, L, *channels] each (made
         when None).  args: the entry's arguments between the clip lengths and scale_factor."""

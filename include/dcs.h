@@ -566,6 +566,37 @@ int dcs_separate_audio_channels_wiener(dcs_ctx* ctx, dcs_model* model, dcs_stft*
                                        int64_t audio_stride, int64_t num_samples, float scale_factor, int overlap,
                                        int patcher, int iterations, int radius, float* d_stems, int64_t stem_stride,
                                        void* stream);
+/* C-channel int16 clips through the multi-clip scheduler of dcs_separate_batch_pcm16_host (5.1, 7.1, arrays of up to 16
+ * channels): h_pcm[i] int16[num_samples[i]][channels] (pinned for real overlap) -> source s of clip i at
+ * h_out[i] + s*channels*out_strides[i] as int16 [num_samples[i]][channels], interleaved (what scipy.io.wavfile.write
+ * takes for a C-channel stem).  One launch decodes a clip into channels + 1 fp32 planes -- the downmix of
+ * dcs_separate_audio_channels, then a_c = pcm/32767 per channel -- the clip is dcs_separate_audio_channels_wiener on
+ * those planes with `iterations` and `radius` (dcs_set_wiener and dcs_set_wiener_radius are not read), and one launch
+ * encodes its nsrc*channels stem planes as (int16)(int)(stem*32767) (C truncation, no clipping, as in
+ * dcs_separate_pcm16_host).  Launches per clip: those of dcs_separate_audio_channels(_wiener) on the clip, plus one
+ * (the decode forms the downmix in place of the downmix launch, and the encode is added).
+ *  - channels = 1: the bytes of dcs_separate_batch_pcm16_host on the same clips (channels 1).
+ *  - channels = 2, DCS_ARCH_DSD: the bytes of dcs_separate_batch_pcm16_keep_channels_host with the same iterations and
+ *    radius set on the ctx.
+ *  - any channels: per clip the bytes of (int16)(int)(stem*32767) on the stems of dcs_separate_audio_channels_wiener on
+ *    the planes pcm/32767 (fp32).
+ * With the filter on, the spectrum tap holds the last clip's nsrc*channels filtered planes; without it a tap is refused.
+ * Workspace: every buffer is sized once from the longest clip, Lmax samples, before the pipeline starts.  With
+ * B(x) = x rounded up to a multiple of 2^20 bytes and n = min(nclips, 2), a fresh ctx holds after the call
+ *     W(Lmax) - B(4 Lmax) + B(4 (channels + 1) Lmax) + B(4 nsrc channels Lmax)
+ *       + n B(2 channels Lmax) + n B(2 nsrc channels Lmax)
+ * where W(Lmax) is what a fresh ctx holds after dcs_separate_audio_channels_wiener with the same iterations and radius
+ * on one clip of Lmax samples: the fp32 staging of the audio planes replaces that call's downmix plane, and the stem
+ * planes and the double-buffered int16 staging are added.
+ * Synchronises before returning, also on an error (the copies in flight have drained).  Refused with DCS_EINVAL before
+ * anything is queued: channels outside [1, 16], iterations or radius negative, iterations > 0 with channels outside
+ * [2, 8], a NULL buffer, a non-positive length or out_strides[i] < num_samples[i] (the message names the clip), and what
+ * dcs_separate_audio_channels_wiener refuses on the longest clip (the stereo / ILD and score-informed nets with a
+ * message naming dcs_separate_masks*, a spectrum tap without the filter). */
+int dcs_separate_batch_pcm16_channels_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, int nclips,
+                                           const int16_t* const* h_pcm, const int64_t* num_samples, int channels,
+                                           int iterations, int radius, float scale_factor, int overlap, int patcher,
+                                           int16_t* const* h_out, const int64_t* out_strides, void* stream);
 
 /* ---- polyphase resampling by up/down (scipy.signal.resample_poly, padtype='constant') -------------------------- */
 /* The networks work on 44.1 kHz spectra; these take a recording at another rate to 44.1 kHz and its stems back.  The
