@@ -86,6 +86,8 @@ _SIGS = {
     "dcs_resampler_destroy": (C.c_int, [_p]),
     "dcs_resampled_length": (_i64, [_i64, C.c_int, C.c_int]),
     "dcs_resample": (C.c_int, [_p, _p, C.c_int, _i64, _i64, _p, _i64, _i64, _p]),
+    "dcs_separate_batch_pcm16_channels_resampled_host": (C.c_int, [_p, _p, _p, _p, _p, C.c_int, _p, _p, C.c_int, C.c_int,
+                                                                   C.c_int, C.c_float, C.c_int, C.c_int, _p, _p, _p]),
 }
 
 

@@ -835,11 +835,12 @@ int dcs_separate_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const int16
 // into one plane (channel 0 or the downmix of `downmix`), int16 [nsrc][L] out.  nx > 0 (C-channel stems, nx ==
 // channels): the clip is decoded into nx + 1 planes (the downmix, then the channels), separated as
 // dcs_separate_audio_channels_wiener with `iterations` and `radius`, and the stems encoded as interleaved [L][nx] per
-// source
-static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
-                          const int64_t* num_samples, int channels, int downmix, int nx, int iterations, int radius,
-                          float scale_factor, int overlap, int patcher, int16_t* const* h_out, const int64_t* out_strides,
-                          cudaStream_t st) {
+// source.  to / from (nx > 0, both or neither): the clip is at another rate; the decode resamples it to L' =
+// resampler_length(to, L) samples, the clip is separated at L', and the encode resamples its stems back to L
+static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to, const dcs_resampler* from,
+                          int nclips, const int16_t* const* h_pcm, const int64_t* num_samples, int channels, int downmix,
+                          int nx, int iterations, int radius, float scale_factor, int overlap, int patcher,
+                          int16_t* const* h_out, const int64_t* out_strides, cudaStream_t st) {
   const int w = nx > 0 ? nx : 1;   // int16 values per sample of a stem
   float *audio = ctx->audio.as<float>(), *stems = ctx->stems.as<float>();
   // the copy streams start after whatever the caller queued on `st` (and after the memsets of fresh buffers)
@@ -855,7 +856,14 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, c
     DCS_CUDA(cudaEventRecord(ctx->ev_in[b], ctx->s_h2d));
     // kernels of clip i
     DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_in[b], 0));
-    if (nx > 0) {
+    const int64_t Lm = to ? resampler_length(to, L) : L;   // the clip's samples at the networks' rate
+    if (to) {
+      DCS_TRY(launch_resample_decode_pcm16(to, ctx->pcm_in[b].as<int16_t>(), L, nx, audio, Lm, st));
+      DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
+      ProfScope ps(ctx, "pcm16_separate", st);
+      DCS_TRY(downmix_clip(ctx, m, p, audio, audio + Lm, nx, Lm, Lm, iterations, radius, scale_factor, overlap, patcher, stems,
+                           Lm, st));
+    } else if (nx > 0) {
       ProfScope ps(ctx, "pcm16_decode_separate", st);   // the clip's kernels up to its stem planes
       DCS_TRY(launch_pcm_decode_channels(ctx, ctx->pcm_in[b].as<int16_t>(), L, nx, audio, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
@@ -868,7 +876,9 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, c
                             st));
     }
     if (i >= 2) DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_out[b], 0));     // D2H of clip i-2 has drained the output staging
-    if (nx > 0) {
+    if (from) {
+      DCS_TRY(launch_resample_encode_pcm16(from, stems, Lm, m->nsrc, nx, ctx->pcm_out[b].as<int16_t>(), L, st));
+    } else if (nx > 0) {
       ProfScope ps(ctx, "pcm16_encode", st);
       DCS_TRY(launch_pcm_encode_channels(ctx, stems, L, m->nsrc, nx, L, ctx->pcm_out[b].as<int16_t>(), st));
     } else
@@ -884,12 +894,14 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, c
   return DCS_OK;
 }
 
-// the checks, resources and drain of every int16 batch entry point around batch_pipeline (nx, iterations, radius as
-// there).  check_model(Lmax): the entry point's own checks of the model, plan and options, run on the longest clip
-// after the per-clip checks and before anything is queued
+// the checks, resources and drain of every int16 batch entry point around batch_pipeline (nx, iterations, radius, to,
+// from as there; the entry point has checked the resampler pair).  check_model(Lmax): the entry point's own checks of
+// the model, plan and options, run on the longest clip (its length at the networks' rate) after the per-clip checks and
+// before anything is queued
 extern "C++" {
 template <class CheckModel>
-static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
+static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to,
+                      const dcs_resampler* from, int nclips, const int16_t* const* h_pcm,
                       const int64_t* num_samples, int channels, int downmix, int nx, int iterations, int radius,
                       float scale_factor, int overlap, int patcher, int16_t* const* h_out, const int64_t* out_strides,
                       cudaStream_t st, CheckModel check_model) {
@@ -901,7 +913,8 @@ static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, i
     DCS_REQUIRE(h_pcm[i] && h_out[i] && num_samples[i] > 0 && out_strides[i] >= num_samples[i], "clip %d: bad buffer / length", i);
     Lmax = std::max(Lmax, num_samples[i]);
   }
-  DCS_TRY(check_model(Lmax));
+  const int64_t Lwork = to ? resampler_length(to, Lmax) : Lmax;   // the longest clip at the networks' rate
+  DCS_TRY(check_model(Lwork));
   DCS_CUDA(cudaSetDevice(ctx->device));
   // each resource on its own: a call that failed half-way through this block must not leave later calls with null handles
   if (!ctx->s_h2d) DCS_CUDA(cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
@@ -919,11 +932,11 @@ static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, i
     DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * (nx > 0 ? nx : 1) * Lmax * sizeof(int16_t), st));
   }
   if (nx > 0)
-    DCS_TRY(size_downmix_workspace(ctx, m, p, Lmax, iterations > 0 ? nx : 0, radius, nx, st));
+    DCS_TRY(size_downmix_workspace(ctx, m, p, Lwork, iterations > 0 ? nx : 0, radius, nx, st));
   else
     DCS_TRY(size_workspace(ctx, m, p, Lmax, true, st));
-  const int rc = batch_pipeline(ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, nx, iterations, radius, scale_factor,
-                                overlap, patcher, h_out, out_strides, st);
+  const int rc = batch_pipeline(ctx, m, p, to, from, nclips, h_pcm, num_samples, channels, downmix, nx, iterations, radius,
+                                scale_factor, overlap, patcher, h_out, out_strides, st);
   // drain everything, success or not, before the host buffers go back to the caller
   const cudaError_t e0 = cudaStreamSynchronize(ctx->s_h2d), e1 = cudaStreamSynchronize(ctx->s_d2h), e2 = cudaStreamSynchronize(st);
   if (rc != DCS_OK) return rc;
@@ -938,7 +951,8 @@ int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int n
                                   const int64_t* num_samples, int channels, int downmix, float scale_factor, int overlap,
                                   int patcher, int16_t* const* h_out, const int64_t* out_strides, void* stream) {
   const char* fn = "dcs_separate_batch_pcm16_host";
-  return batch_host(fn, ctx, m, p, nclips, h_pcm, num_samples, channels, downmix, 0, 0, 0, scale_factor, overlap, patcher,
+  return batch_host(fn, ctx, m, p, nullptr, nullptr, nclips, h_pcm, num_samples, channels, downmix, 0, 0, 0, scale_factor,
+                    overlap, patcher,
                     h_out, out_strides, (cudaStream_t)stream, [&](int64_t Lmax) {
                       return check_clip(fn, ctx, m, p, -1, h_pcm, h_out, Lmax, Lmax, Lmax, overlap, patcher);
                     });
@@ -951,7 +965,7 @@ int dcs_separate_batch_pcm16_keep_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_
                                                 int overlap, int patcher, int16_t* const* h_out, const int64_t* out_strides,
                                                 void* stream) {
   const char* fn = "dcs_separate_batch_pcm16_keep_channels_host";
-  return batch_host(fn, ctx, m, p, nclips, h_pcm, num_samples, 2, 1, 2, ctx ? ctx->wiener_iters : 0,
+  return batch_host(fn, ctx, m, p, nullptr, nullptr, nclips, h_pcm, num_samples, 2, 1, 2, ctx ? ctx->wiener_iters : 0,
                     ctx ? ctx->wiener_radius : 0, scale_factor, overlap, patcher, h_out, out_strides, (cudaStream_t)stream,
                     [&](int64_t Lmax) {
                       DCS_TRY(check_clip(fn, ctx, m, p, DCS_ARCH_DSD, h_pcm, h_out, Lmax, Lmax, Lmax, overlap, patcher));
@@ -1102,22 +1116,42 @@ int dcs_separate_audio_channels_wiener(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, 
 }
 
 // the int16 batch of C-channel clips: per clip dcs_separate_audio_channels_wiener on the decoded planes, with the checks
-// of that call on the longest clip
-int dcs_separate_batch_pcm16_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
-                                           const int64_t* num_samples, int channels, int iterations, int radius,
-                                           float scale_factor, int overlap, int patcher, int16_t* const* h_out,
-                                           const int64_t* out_strides, void* stream) {
-  const char* fn = "dcs_separate_batch_pcm16_channels_host";
+// of that call on the longest clip.  to / from: the resampler pair of a clip rate other than the networks' (NULL: none)
+static int pcm16_channels(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to,
+                          const dcs_resampler* from, int nclips, const int16_t* const* h_pcm, const int64_t* num_samples,
+                          int channels, int iterations, int radius, float scale_factor, int overlap, int patcher,
+                          int16_t* const* h_out, const int64_t* out_strides, void* stream) {
   DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
   DCS_REQUIRE(iterations >= 0, "%s: iterations %d must be >= 0", fn, iterations);
   DCS_REQUIRE(radius >= 0, "%s: radius %d must be >= 0", fn, radius);
   DCS_REQUIRE(iterations == 0 || (channels >= 2 && channels <= 8), "%s: the Wiener post-filter needs channels in [2, 8], got %d",
               fn, channels);
-  return batch_host(fn, ctx, m, p, nclips, h_pcm, num_samples, channels, 0, channels, iterations, radius, scale_factor, overlap,
-                    patcher, h_out, out_strides, (cudaStream_t)stream, [&](int64_t Lmax) {
+  return batch_host(fn, ctx, m, p, to, from, nclips, h_pcm, num_samples, channels, 0, channels, iterations, radius,
+                    scale_factor, overlap, patcher, h_out, out_strides, (cudaStream_t)stream, [&](int64_t Lmax) {
                       return check_channels(fn, ctx, m, p, h_pcm, channels, Lmax, Lmax, overlap, patcher, h_out, Lmax,
                                             iterations, radius);
                     });
+}
+
+int dcs_separate_batch_pcm16_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int nclips, const int16_t* const* h_pcm,
+                                           const int64_t* num_samples, int channels, int iterations, int radius,
+                                           float scale_factor, int overlap, int patcher, int16_t* const* h_out,
+                                           const int64_t* out_strides, void* stream) {
+  return pcm16_channels("dcs_separate_batch_pcm16_channels_host", ctx, m, p, nullptr, nullptr, nclips, h_pcm, num_samples,
+                        channels, iterations, radius, scale_factor, overlap, patcher, h_out, out_strides, stream);
+}
+
+int dcs_separate_batch_pcm16_channels_resampled_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to_model,
+                                                     const dcs_resampler* from_model, int nclips, const int16_t* const* h_pcm,
+                                                     const int64_t* num_samples, int channels, int iterations, int radius,
+                                                     float scale_factor, int overlap, int patcher, int16_t* const* h_out,
+                                                     const int64_t* out_strides, void* stream) {
+  const char* fn = "dcs_separate_batch_pcm16_channels_resampled_host";
+  DCS_REQUIRE(ctx, "%s: NULL ctx", fn);
+  DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
+  DCS_TRY(check_resample_pcm16(fn, ctx, to_model, from_model, channels));
+  return pcm16_channels(fn, ctx, m, p, to_model, from_model, nclips, h_pcm, num_samples, channels, iterations, radius,
+                        scale_factor, overlap, patcher, h_out, out_strides, stream);
 }
 
 // ------------------------------------------------------------------------------------ Wiener post-filter

@@ -359,6 +359,18 @@ int launch_pcm_encode_channels(dcs_ctx* ctx, const float* d_stems, int64_t L, in
 // at nx = 1
 int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st);
 
+// the int16 batch at another rate (resample.cu), C in [1, 16], on the resampler's ctx.  check_resample_pcm16: what the
+// batch refuses of its resampler pair (NULL, another ctx, not inverse, no tile that fits).  decode: int16 [L][C] -> C + 1
+// float planes Lout apart at the resampler's output rate (the downmix, then the channels), each channel the bits of
+// dcs_resample on pcm / 32767; encode: nsrc x C stem planes (source, channel) Lin apart -> int16 [nsrc][L][C] at the
+// output rate, (int16_t)(int)(y * 32767) of dcs_resample's y trimmed to L
+int64_t resampler_length(const dcs_resampler* r, int64_t num_in);
+int check_resample_pcm16(const char* fn, const dcs_ctx* ctx, const dcs_resampler* to, const dcs_resampler* from, int C);
+int launch_resample_decode_pcm16(const dcs_resampler* r, const int16_t* d_pcm, int64_t L, int C, float* d_planes,
+                                 int64_t Lout, cudaStream_t st);
+int launch_resample_encode_pcm16(const dcs_resampler* r, const float* d_stems, int64_t Lin, int nsrc, int C, int16_t* d_out,
+                                 int64_t L, cudaStream_t st);
+
 // multichannel Wiener post-filter (wiener.cu): nch (2..8) mixture channels, channel c at X + c * x_plane, stem (j, c) at
 // S + (j * nch + c) * src_stride, bins f < F filtered in place by `iterations` EM iterations; radius: the covariance
 // window in chunks of DCS_WIENER_CHUNK_FRAMES frames to either side (0 = the whole clip).  M set: the stems are not in S

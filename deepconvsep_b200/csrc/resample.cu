@@ -11,6 +11,10 @@
 // each tap is loaded once for RS_V outputs, consecutive lanes take consecutive residues, so the tap loads are
 // conflict-free and the sample loads nearly so.  The sum is accumulated in fp64 with fma in increasing i and rounded
 // once to fp32: the same bits on every run.
+//
+// The int16 batch at another rate fuses the PCM conversions into the resampler (resample_decode_pcm16_kernel,
+// resample_encode_pcm16_kernel): the same bank, the same work items and the same inner sum (polyphase_sum), so each value
+// has the bits of resample_kernel on the fp32 planes the unfused route would have formed.
 #include <algorithm>
 #include "common.cuh"
 
@@ -37,6 +41,20 @@ struct ResampleArgs {
   int up, down, Q, half_len, c0, tp, span;
   int64_t tiles_per_plane, ntiles;
 };
+
+// the RS_V outputs of residue r, one period apart, from the staged samples x(base + v*down - i): fma in increasing tap
+// index i from the exactly widened fp32 sample, in fp64; the caller rounds each once to fp32
+template <class Sample>
+__device__ __forceinline__ void polyphase_sum(const double* __restrict__ bank, int up, int down, int Q, int r, int base,
+                                              Sample x, double (&acc)[RS_V]) {
+#pragma unroll
+  for (int v = 0; v < RS_V; ++v) acc[v] = 0.0;
+  for (int i = 0; i < Q; ++i) {
+    const double hv = bank[i * up + r];
+#pragma unroll
+    for (int v = 0; v < RS_V; ++v) acc[v] = fma(hv, (double)x(base + v * down - i), acc[v]);
+  }
+}
 
 __global__ void __launch_bounds__(RS_THREADS)
 resample_kernel(const ResampleArgs a) {
@@ -65,17 +83,124 @@ resample_kernel(const ResampleArgs a) {
       // sample of (period P0 + g*V + v, tap i) at xs[base + v*down - i]
       const int base = g * RS_V * a.down + c - a.c0 + a.Q - 1;
       double acc[RS_V];
-#pragma unroll
-      for (int v = 0; v < RS_V; ++v) acc[v] = 0.0;
-      for (int i = 0; i < a.Q; ++i) {
-        const double hv = bank[i * a.up + r];
-#pragma unroll
-        for (int v = 0; v < RS_V; ++v) acc[v] = fma(hv, (double)xs[base + v * a.down - i], acc[v]);
-      }
+      polyphase_sum(bank, a.up, a.down, a.Q, r, base, [&](int k) { return xs[k]; }, acc);
 #pragma unroll
       for (int v = 0; v < RS_V; ++v) {
         const int64_t n = n0 + (int64_t)v * a.up;
         if (n < a.num_out) y[n] = (float)acc[v];
+      }
+    }
+  }
+}
+
+// The int16 batch's conversions fused into the resampler.  Both take the bank and phase constants of a dcs_resampler,
+// tiles of tp periods as resample_kernel does, and a plan per (resampler, C) that fits shared memory.
+struct ResamplePcmArgs {
+  const void* in; int64_t num_in;    // decode: int16 [num_in][C]; encode: nsrc*C fp32 planes num_in apart
+  void* out; int64_t num_out;        // decode: C + 1 fp32 planes num_out apart; encode: int16 [nsrc][num_out][C]
+  const double* bank;
+  int up, down, Q, half_len, c0, tp, span;
+  int C, cn, cs;                     // channels; channels per tile and staged values per sample (encode)
+  int64_t tiles_t, ntiles;           // tiles along time, all tiles
+};
+
+// int16 [num_in][C] at the clip's rate -> plane 1 + c: resample_kernel on the fp32 plane (float)pcm_c / 32767.0f, and
+// plane 0: (((y_0 + y_1) + y_2) + ...) * (1.0f / C) on those rounded values, downmix_kernel's expression.  A tile is tp
+// periods of all C channels, so one thread forms the downmix of its outputs; its input span is staged as int16, channel
+// by channel ([C][span]), and converted per tap.  A work item is (residue r, RS_V periods) for every channel in turn.
+__global__ void __launch_bounds__(RS_THREADS)
+resample_decode_pcm16_kernel(const ResamplePcmArgs a) {
+  extern __shared__ __align__(16) unsigned char rs_smem[];
+  double* bank = reinterpret_cast<double*>(rs_smem);
+  int16_t* xs = reinterpret_cast<int16_t*>(bank + (size_t)a.Q * a.up);
+  const int16_t* __restrict__ pcm = static_cast<const int16_t*>(a.in);
+  float* __restrict__ planes = static_cast<float*>(a.out);
+  for (int k = threadIdx.x; k < a.Q * a.up; k += RS_THREADS) bank[k] = __ldg(a.bank + k);
+  const int C = a.C, items = a.up * (a.tp / RS_V), staged = a.span * C;
+  const float inv = 1.0f / (float)C;
+  for (int64_t tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
+    const int64_t P0 = tile * a.tp;
+    const int64_t jlo = P0 * a.down + a.c0 - (a.Q - 1);
+    __syncthreads();
+    for (int k = threadIdx.x; k < staged; k += RS_THREADS) {    // consecutive threads read consecutive int16 values
+      const int jj = k / C, c = k - jj * C;
+      const int64_t j = jlo + jj;
+      xs[c * a.span + jj] = (j >= 0 && j < a.num_in) ? pcm[j * C + c] : (int16_t)0;
+    }
+    __syncthreads();
+    for (int w = threadIdx.x; w < items; w += RS_THREADS) {
+      const int r = w % a.up, g = w / a.up;
+      const int64_t n0 = (P0 + (int64_t)g * RS_V) * a.up + r;
+      if (n0 >= a.num_out) continue;
+      const int cr = (int)(((int64_t)r * a.down + a.half_len) / a.up);
+      const int base = g * RS_V * a.down + cr - a.c0 + a.Q - 1;
+      float mix[RS_V];
+      for (int c = 0; c < C; ++c) {
+        const int16_t* xc = xs + c * a.span;
+        double acc[RS_V];
+        polyphase_sum(bank, a.up, a.down, a.Q, r, base, [&](int k) { return (float)xc[k] / 32767.0f; }, acc);
+        float* y = planes + (int64_t)(1 + c) * a.num_out;
+#pragma unroll
+        for (int v = 0; v < RS_V; ++v) {
+          const float yv = (float)acc[v];
+          const int64_t n = n0 + (int64_t)v * a.up;
+          if (n < a.num_out) y[n] = yv;
+          mix[v] = c == 0 ? yv : mix[v] + yv;
+        }
+      }
+#pragma unroll
+      for (int v = 0; v < RS_V; ++v) {
+        const int64_t n = n0 + (int64_t)v * a.up;
+        if (n < a.num_out) planes[n] = mix[v] * inv;
+      }
+    }
+  }
+}
+
+// nsrc*C fp32 stem planes (source s, channel c at (s*C + c) * num_in) at 44.1 kHz -> int16 [nsrc][num_out][C] at the
+// clip's rate: (int16_t)(int)(y * 32767.0f) with y resample_kernel's fp32 value, the truncation of
+// pcm_encode_channels_kernel.  A tile is tp periods of cn channels of one source (cn = C unless the bank leaves too
+// little room); its span is staged interleaved, cs = cn | 1 values per sample so that the staging stores and the tap loads
+// of neighbouring channels fall in different banks.  A work item is (channel, residue, RS_V periods) with the channel
+// fastest, so neighbouring lanes write neighbouring int16 values of the interleaved output.
+__global__ void __launch_bounds__(RS_THREADS)
+resample_encode_pcm16_kernel(const ResamplePcmArgs a) {
+  extern __shared__ __align__(16) unsigned char rs_smem[];
+  double* bank = reinterpret_cast<double*>(rs_smem);
+  float* xs = reinterpret_cast<float*>(bank + (size_t)a.Q * a.up);
+  const float* __restrict__ stems = static_cast<const float*>(a.in);
+  int16_t* __restrict__ out = static_cast<int16_t*>(a.out);
+  for (int k = threadIdx.x; k < a.Q * a.up; k += RS_THREADS) bank[k] = __ldg(a.bank + k);
+  const int C = a.C, cs = a.cs, groups = (C + a.cn - 1) / a.cn;
+  for (int64_t tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
+    const int64_t tt = tile % a.tiles_t, sg = tile / a.tiles_t;
+    const int s = (int)(sg / groups), c_lo = (int)(sg % groups) * a.cn;
+    const int cn = min(a.cn, C - c_lo);
+    const int64_t P0 = tt * a.tp;
+    const int64_t jlo = P0 * a.down + a.c0 - (a.Q - 1);
+    const float* __restrict__ x = stems + ((int64_t)s * C + c_lo) * a.num_in;
+    __syncthreads();
+    for (int k = threadIdx.x; k < a.span * cn; k += RS_THREADS) {   // plane by plane: coalesced reads
+      const int c = k / a.span, jj = k - c * a.span;
+      const int64_t j = jlo + jj;
+      xs[jj * cs + c] = (j >= 0 && j < a.num_in) ? __ldg(x + (int64_t)c * a.num_in + j) : 0.f;
+    }
+    __syncthreads();
+    const int items = cn * a.up * (a.tp / RS_V);
+    int16_t* __restrict__ o = out + (int64_t)s * a.num_out * C + c_lo;
+    for (int w = threadIdx.x; w < items; w += RS_THREADS) {
+      const int c = w % cn, rg = w / cn;
+      const int r = rg % a.up, g = rg / a.up;
+      const int64_t n0 = (P0 + (int64_t)g * RS_V) * a.up + r;
+      if (n0 >= a.num_out) continue;
+      const int cr = (int)(((int64_t)r * a.down + a.half_len) / a.up);
+      const int base = g * RS_V * a.down + cr - a.c0 + a.Q - 1;
+      double acc[RS_V];
+      polyphase_sum(bank, a.up, a.down, a.Q, r, base, [&](int k) { return xs[k * cs + c]; }, acc);
+#pragma unroll
+      for (int v = 0; v < RS_V; ++v) {
+        const int64_t n = n0 + (int64_t)v * a.up;
+        if (n < a.num_out) o[n * C + c] = (int16_t)(int)((float)acc[v] * 32767.0f);
       }
     }
   }
@@ -89,6 +214,93 @@ static int64_t gcd64(int64_t a, int64_t b) {
   while (b) { const int64_t t = a % b; a = b; b = t; }
   return a;
 }
+
+namespace dcs {
+
+// the tile of a fused int16 kernel for C channels: periods per tile (a multiple of RS_V, no more work items than 4
+// rounds of the CTA, counting each channel's outputs for the encode), channels per tile and staged values per sample;
+// false when even RS_V periods of one channel do not fit next to the bank
+struct PcmPlan { int tp, span, cn, cs; size_t smem; };
+
+static bool pcm_plan(const dcs_resampler* r, int C, bool encode, PcmPlan* pl) {
+  const int64_t bank = (int64_t)r->Q * r->up * (int64_t)sizeof(double);
+  const int64_t bytes = encode ? (int64_t)sizeof(float) : (int64_t)sizeof(int16_t);
+  // encode: the fewest equal channel groups that fit; decode: all C channels in one tile (it forms the downmix)
+  for (int groups = 1; groups <= (encode ? C : 1); ++groups) {
+    const int cn = encode ? (C + groups - 1) / groups : C;
+    const int cs = encode ? (cn | 1) : cn;
+    const int64_t per_round = (int64_t)r->up * (encode ? cn : 1);
+    for (int64_t tp = std::max<int64_t>(1, 4 * RS_THREADS / per_round) * RS_V; tp >= RS_V; tp -= RS_V) {
+      const int64_t span = (tp - 1) * r->down + r->cspan + r->Q;
+      const int64_t smem = bank + span * cs * bytes;
+      if (smem <= RS_SMEM_MAX) {
+        pl->tp = (int)tp; pl->span = (int)span; pl->cn = cn; pl->cs = cs; pl->smem = (size_t)smem;
+        return true;
+      }
+    }
+  }
+  return false;
+}
+
+template <class Kernel>
+static int launch_pcm(const dcs_resampler* r, Kernel kernel, const char* scope, const PcmPlan& pl, ResamplePcmArgs a,
+                      cudaStream_t st) {
+  dcs_ctx* ctx = r->ctx;
+  a.bank = r->d_bank;
+  a.up = r->up; a.down = r->down; a.Q = r->Q; a.half_len = r->half_len; a.c0 = r->c0;
+  a.tp = pl.tp; a.span = pl.span; a.cn = pl.cn; a.cs = pl.cs;
+  DCS_TRY(ensure_smem_attr(kernel, (int)pl.smem));
+  int per_sm = 0;
+  DCS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, RS_THREADS, pl.smem));
+  const int64_t grid = std::min<int64_t>(a.ntiles, (int64_t)ctx->num_sms * std::max(per_sm, 1));
+  ProfScope ps(ctx, scope, st);
+  kernel<<<(unsigned)grid, RS_THREADS, pl.smem, st>>>(a);
+  DCS_CHECK_LAUNCH();
+  ctx->launches++;
+  return DCS_OK;
+}
+
+int64_t resampler_length(const dcs_resampler* r, int64_t num_in) { return dcs_resampled_length(num_in, r->up, r->down); }
+
+int check_resample_pcm16(const char* fn, const dcs_ctx* ctx, const dcs_resampler* to, const dcs_resampler* from, int C) {
+  DCS_REQUIRE(to && from, "%s: NULL resampler", fn);
+  DCS_REQUIRE(to->ctx == ctx && from->ctx == ctx, "%s: a resampler was made on another ctx", fn);
+  DCS_REQUIRE(to->up == from->down && to->down == from->up,
+              "%s: the resamplers %d/%d and %d/%d are not inverse (to_model up/down must be from_model down/up)", fn,
+              to->up, to->down, from->up, from->down);
+  PcmPlan pl;
+  DCS_REQUIRE(pcm_plan(to, C, false, &pl), "%s: %d channels at %d/%d do not fit one tile in shared memory", fn, C, to->up,
+              to->down);
+  DCS_REQUIRE(pcm_plan(from, C, true, &pl), "%s: one channel at %d/%d does not fit one tile in shared memory", fn, from->up,
+              from->down);
+  return DCS_OK;
+}
+
+int launch_resample_decode_pcm16(const dcs_resampler* r, const int16_t* d_pcm, int64_t L, int C, float* d_planes,
+                                 int64_t Lout, cudaStream_t st) {
+  PcmPlan pl;
+  DCS_REQUIRE(L >= 1 && Lout >= 1 && Lout <= resampler_length(r, L) && C >= 1 && C <= 16 && pcm_plan(r, C, false, &pl),
+              "resample_decode_pcm16: bad arguments");
+  ResamplePcmArgs a;
+  a.in = d_pcm; a.num_in = L; a.out = d_planes; a.num_out = Lout; a.C = C;
+  a.tiles_t = ceil_div64(ceil_div64(Lout, r->up), pl.tp);
+  a.ntiles = a.tiles_t;
+  return launch_pcm(r, resample_decode_pcm16_kernel, "resample_decode", pl, a, st);
+}
+
+int launch_resample_encode_pcm16(const dcs_resampler* r, const float* d_stems, int64_t Lin, int nsrc, int C, int16_t* d_out,
+                                 int64_t L, cudaStream_t st) {
+  PcmPlan pl;
+  DCS_REQUIRE(Lin >= 1 && L >= 1 && L <= resampler_length(r, Lin) && nsrc >= 1 && C >= 1 && C <= 16 && pcm_plan(r, C, true, &pl),
+              "resample_encode_pcm16: bad arguments");
+  ResamplePcmArgs a;
+  a.in = d_stems; a.num_in = Lin; a.out = d_out; a.num_out = L; a.C = C;
+  a.tiles_t = ceil_div64(ceil_div64(L, r->up), pl.tp);
+  a.ntiles = a.tiles_t * ((C + pl.cn - 1) / pl.cn) * nsrc;
+  return launch_pcm(r, resample_encode_pcm16_kernel, "resample_encode", pl, a, st);
+}
+
+}  // namespace dcs
 
 extern "C" {
 

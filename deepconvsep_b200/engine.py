@@ -642,15 +642,19 @@ class Separator(object):
         assert all((1 if p_.ndim == 1 else p_.shape[1]) == ch for p_ in ps), "all clips must have the same channel count"
         return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_host, ps, outs, (), (ch, int(downmix if ch > 1 else 0)))
 
-    def separate_pcm16_channels_batch(self, clips, outs=None, wiener=0, wiener_radius=0):
+    def separate_pcm16_channels_batch(self, clips, outs=None, wiener=0, wiener_radius=0, sample_rate=MODEL_RATE):
         """C-channel int16 clips through the context's multi-clip scheduler (dcs_separate_batch_pcm16_channels_host):
         H2D of clip i+1, the kernels of clip i and D2H of clip i-1 overlap, and the decode to fp32 and the encode of the
         stems to int16 run on the device.  clips: list of int16 arrays [L, C] with the same C in 1..16 (pinned for real
         overlap) -> list of int16 [nsrc, L, C] (into `outs` when given, which may be pinned): per clip
-        (separate_channels(clip / 32767, wiener, wiener_radius) * 32767) truncated to int16 in fp32, source by source.
-        wiener > 0 (C in 2..8): EM iterations of the Wiener post-filter, over covariance windows of wiener_radius
-        chunks.  At C = 2 with the DSD100 network, the bytes of separate_pcm16_batch(keep_channels=True) with the same
-        wiener and wiener_radius."""
+        (separate_channels(clip / 32767, wiener, wiener_radius, sample_rate) * 32767) truncated to int16 in fp32, source
+        by source.  wiener > 0 (C in 2..8): EM iterations of the Wiener post-filter, over covariance windows of
+        wiener_radius chunks.  At C = 2 with the DSD100 network, the bytes of separate_pcm16_batch(keep_channels=True)
+        with the same wiener and wiener_radius.
+        sample_rate: the clips' rate, one for the whole call (a sequence of one rate per clip is taken if they are all
+        equal).  At another rate than MODEL_RATE (check_resample_rates) each clip is resampled to 44.1 kHz as it is
+        decoded and its stems back to its own rate and length as they are encoded, on the device with this separator's
+        resamplers (dcs_separate_batch_pcm16_channels_resampled_host): no more launches per clip than at 44.1 kHz."""
         check_channels_family(self.model.arch)
         check_wiener_radius(wiener, wiener_radius)
         if wiener < 0:
@@ -661,6 +665,14 @@ class Separator(object):
             if a.dtype != np.int16 or a.ndim != 2:
                 raise ValueError("separate_pcm16_channels_batch needs int16 clips [L, C], got %s %r" % (a.dtype, a.shape))
             ps.append(np.ascontiguousarray(a))
+        if not np.isscalar(sample_rate):
+            rates = list(sample_rate)
+            if len(rates) != len(ps) or any(r != rates[0] for r in rates):
+                raise ValueError("separate_pcm16_channels_batch takes one sample rate per call, got %r for %d clips"
+                                 % (rates, len(ps)))
+            sample_rate = rates[0] if rates else MODEL_RATE
+        if sample_rate != MODEL_RATE:
+            check_resample_rates(sample_rate, MODEL_RATE)   # the rate is refused before any library call
         if not ps:
             return []
         ch = ps[0].shape[1]
@@ -670,12 +682,16 @@ class Separator(object):
             raise ValueError("separate_pcm16_channels_batch takes 1 to 16 channels, got %d" % ch)
         if wiener:
             check_wiener_channels(ch)
-        return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_channels_host, ps, outs, (ch,),
-                                 (ch, int(wiener), int(wiener_radius)))
+        args = (ch, int(wiener), int(wiener_radius))
+        if sample_rate == MODEL_RATE:
+            return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_channels_host, ps, outs, (ch,), args)
+        pre = (self.resampler(sample_rate, MODEL_RATE).handle, self.resampler(MODEL_RATE, sample_rate).handle)
+        return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_channels_resampled_host, ps, outs, (ch,), args, pre)
 
-    def _pcm16_batch(self, entry, ps, outs, channels, args):
+    def _pcm16_batch(self, entry, ps, outs, channels, args, pre=()):
         """int16 clips ps through the multi-clip entry point `entry` -> outs, int16 [nsrc, L, *channels] each (made
-        when None).  args: the entry's arguments between the clip lengths and scale_factor."""
+        when None).  args: the entry's arguments between the clip lengths and scale_factor; pre: those between the
+        plan and the clip count."""
         n = len(ps)
         Ls = np.array([p_.shape[0] for p_ in ps], dtype=np.int64)
         if outs is None:
@@ -684,7 +700,7 @@ class Separator(object):
                    for o, L in zip(outs, Ls))
         pin = (C.c_void_p * n)(*[p_.ctypes.data for p_ in ps])
         pout = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
-        _lib.check(entry(self.ctx.handle, self.model.handle, self.stft.handle, n, pin, Ls.ctypes.data, *args,
+        _lib.check(entry(self.ctx.handle, self.model.handle, self.stft.handle, *pre, n, pin, Ls.ctypes.data, *args,
                          self.scale_factor, self.overlap, self.patcher, pout, Ls.ctypes.data,
                          _stream_ptr(None, self.ctx.device)))
         return outs

@@ -625,6 +625,34 @@ int64_t dcs_resampled_length(int64_t num_in, int up, int down);
  * dcs_resampled_length, negative strides, strides shorter than the rows with nplanes > 1, planes not 4-byte aligned. */
 int dcs_resample(dcs_resampler* resampler, const float* d_in, int nplanes, int64_t in_stride, int64_t num_in,
                  float* d_out, int64_t out_stride, int64_t num_out, void* stream);
+/* dcs_separate_batch_pcm16_channels_host for clips at another rate (48 kHz film and broadcast material, 8 to 192 kHz):
+ * to_model takes the clips' rate to the networks' 44.1 kHz and from_model brings the stems back, both made on ctx and
+ * inverse (to_model up/down = from_model down/up).  Clip i of L = num_samples[i] samples is separated at
+ * L' = dcs_resampled_length(L, to_model up, to_model down) samples and its stems come back at L, in the layout of
+ * dcs_separate_batch_pcm16_channels_host.  One launch resamples and decodes a clip into channels + 1 fp32 planes of L'
+ * samples -- channel c is the bits of dcs_resample(to_model) on the plane pcm_c/32767 (fp32), the downmix is
+ * dcs_separate_audio_channels' on those planes -- the clip is dcs_separate_audio_channels_wiener on them with
+ * `iterations` and `radius`, and one launch resamples and encodes its nsrc*channels stem planes as (int16)(int)(y*32767)
+ * with y the fp32 value of dcs_resample(from_model, num_out = L) (C truncation, no clipping).  So per clip the bytes are
+ * those of (int16)(int)(stem*32767) on the stems of: dcs_resample(to_model) of pcm/32767, then
+ * dcs_separate_audio_channels_wiener, then dcs_resample(from_model) trimmed to L.  Launches per clip: those of
+ * dcs_separate_audio_channels(_wiener) on a clip of L' samples, plus one -- one fewer than those three calls.
+ * Workspace: every buffer is sized once before the pipeline starts, the fp32 planes from the longest clip at 44.1 kHz,
+ * L'max samples, and the int16 staging from the longest clip, Lmax samples.  With B(x) and n as above, a fresh ctx holds
+ * after the call
+ *     W(L'max) - B(4 L'max) + B(4 (channels + 1) L'max) + B(4 nsrc channels L'max)
+ *       + n B(2 channels Lmax) + n B(2 nsrc channels Lmax)
+ * where W(L'max) is what a fresh ctx holds after dcs_separate_audio_channels_wiener with the same iterations and radius
+ * on one clip of L'max samples; the resamplers' banks are their own, not the workspace.
+ * Synchronises before returning, also on an error.  Refused with DCS_EINVAL before anything is queued: a NULL resampler,
+ * a resampler made on another ctx, a pair that is not inverse, and what dcs_separate_batch_pcm16_channels_host refuses
+ * (the model's checks on the longest clip at L'max). */
+int dcs_separate_batch_pcm16_channels_resampled_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan,
+                                                     const dcs_resampler* to_model, const dcs_resampler* from_model,
+                                                     int nclips, const int16_t* const* h_pcm, const int64_t* num_samples,
+                                                     int channels, int iterations, int radius, float scale_factor,
+                                                     int overlap, int patcher, int16_t* const* h_out,
+                                                     const int64_t* out_strides, void* stream);
 
 #ifdef __cplusplus
 }
