@@ -778,6 +778,85 @@ int dcs_sconv_mask_f32(dcs_ctx* ctx, int engine, const dcs_sconv_mask_view* view
   return sync_after("dcs_sconv_mask_f32", engine == 1 ? launch_sconv_mask_tc(ctx, a, st) : launch_sconv_mask(ctx, a, st), st);
 }
 
+// ------------------------------------------------------------------------------------ int16 PCM conversions
+// each one launch of the launcher the int16 batch entry points call, on the caller's buffers
+int dcs_pcm16_decode(dcs_ctx* ctx, const dcs_resampler* r, int mode, const int16_t* d_pcm, int64_t L, int channels,
+                     float* d_out, int64_t num_out, void* stream) {
+  const char* fn = "dcs_pcm16_decode";
+  DCS_REQUIRE(ctx && d_pcm && d_out, "%s: NULL argument", fn);
+  DCS_REQUIRE(!r || resampler_ctx(r) == ctx, "%s: the resampler was made on another ctx", fn);
+  DCS_REQUIRE(L >= 1, "%s: num_samples %lld must be >= 1", fn, (long long)L);
+  DCS_REQUIRE((uintptr_t)d_pcm % 2 == 0 && (uintptr_t)d_out % 4 == 0, "%s: d_pcm not 2-byte or d_out not 4-byte aligned", fn);
+  if (mode == DCS_PCM16_CHANNELS) {
+    DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
+    const int64_t most = r ? resampler_length(r, L) : L;
+    DCS_REQUIRE(num_out >= 1 && num_out <= most && (r || num_out == L), "%s: num_out %lld, want %s%lld", fn,
+                (long long)num_out, r ? "1 .. " : "", (long long)most);
+  } else {
+    DCS_REQUIRE(mode >= 0 && mode <= 2, "%s: unknown mode %d", fn, mode);
+    DCS_REQUIRE(!r, "%s: a resampler takes the C-channel mode only", fn);
+    DCS_REQUIRE(channels >= 1 && channels <= 8, "%s: channels %d not in [1, 8]", fn, channels);
+    DCS_REQUIRE(num_out == L, "%s: num_out %lld != num_samples %lld", fn, (long long)num_out, (long long)L);
+  }
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if (r)
+    rc = launch_resample_decode_pcm16(r, d_pcm, L, channels, d_out, num_out, st);
+  else if (mode == DCS_PCM16_CHANNELS)
+    rc = launch_pcm_decode_channels(ctx, d_pcm, L, channels, d_out, st);
+  else
+    rc = launch_pcm_decode(ctx, d_pcm, L, channels, mode, d_out, st);
+  return sync_after(fn, rc, st);
+}
+
+int dcs_pcm16_encode(dcs_ctx* ctx, const dcs_resampler* r, int mode, const float* d_stems, int64_t num_in, int nsrc,
+                     int channels, int64_t stem_stride, int16_t* d_out, int64_t num_out, int64_t out_stride, void* stream) {
+  const char* fn = "dcs_pcm16_encode";
+  DCS_REQUIRE(ctx && d_stems && d_out, "%s: NULL argument", fn);
+  DCS_REQUIRE(!r || resampler_ctx(r) == ctx, "%s: the resampler was made on another ctx", fn);
+  DCS_REQUIRE(num_in >= 1 && nsrc >= 1, "%s: num_in %lld and nsrc %d must be >= 1", fn, (long long)num_in, nsrc);
+  DCS_REQUIRE((uintptr_t)d_stems % 4 == 0 && (uintptr_t)d_out % 2 == 0, "%s: d_stems not 4-byte or d_out not 2-byte aligned",
+              fn);
+  if (mode == DCS_PCM16_CHANNELS) {
+    DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
+    DCS_REQUIRE(r ? stem_stride == num_in : stem_stride >= num_in, "%s: stem_stride %lld, num_in %lld", fn,
+                (long long)stem_stride, (long long)num_in);
+    const int64_t most = r ? resampler_length(r, num_in) : num_in;
+    DCS_REQUIRE(num_out >= 1 && num_out <= most && (r || num_out == num_in), "%s: num_out %lld, want %s%lld", fn,
+                (long long)num_out, r ? "1 .. " : "", (long long)most);
+    DCS_REQUIRE(out_stride == (int64_t)channels * num_out, "%s: out_stride %lld != channels * num_out", fn, (long long)out_stride);
+  } else {
+    DCS_REQUIRE(mode == DCS_PCM16_MONO, "%s: unknown mode %d", fn, mode);
+    DCS_REQUIRE(!r, "%s: a resampler takes the C-channel mode only", fn);
+    DCS_REQUIRE(channels == 1, "%s: the mono mode has one channel, not %d", fn, channels);
+    DCS_REQUIRE(num_out == num_in && stem_stride >= num_in && out_stride >= num_out,
+                "%s: num_out %lld, stem_stride %lld, out_stride %lld for num_in %lld", fn, (long long)num_out,
+                (long long)stem_stride, (long long)out_stride, (long long)num_in);
+  }
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc;
+  if (r)
+    rc = launch_resample_encode_pcm16(r, d_stems, num_in, nsrc, channels, d_out, num_out, st);
+  else if (mode == DCS_PCM16_CHANNELS)
+    rc = launch_pcm_encode_channels(ctx, d_stems, num_in, nsrc, channels, stem_stride, d_out, st);
+  else
+    rc = launch_pcm_encode(ctx, d_stems, num_in, nsrc, stem_stride, d_out, out_stride, st);
+  return sync_after(fn, rc, st);
+}
+
+int dcs_downmix_f32(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t L, float* d_mono, void* stream) {
+  const char* fn = "dcs_downmix_f32";
+  DCS_REQUIRE(ctx && d_audio && d_mono, "%s: NULL argument", fn);
+  DCS_REQUIRE(nx >= 1 && nx <= 16, "%s: nx %d not in [1, 16]", fn, nx);
+  DCS_REQUIRE(L >= 1 && audio_stride >= L, "%s: num_samples %lld, audio_stride %lld", fn, (long long)L, (long long)audio_stride);
+  DCS_REQUIRE((uintptr_t)d_audio % 4 == 0 && (uintptr_t)d_mono % 4 == 0, "%s: planes not 4-byte aligned", fn);
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  return sync_after(fn, launch_downmix(ctx, d_audio, nx, audio_stride, L, d_mono, st), st);
+}
+
 int dcs_separate_audio_stereo(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const float* d_audio, int64_t audio_stride, int64_t L,
                               float scale_factor, int overlap, int patcher, float* d_stems, int64_t stem_stride, void* stream) {
   DCS_TRY(check_clip("dcs_separate_audio_stereo", ctx, m, p, DCS_ARCH_DSD_ILD, d_audio, d_stems, L, audio_stride, stem_stride,

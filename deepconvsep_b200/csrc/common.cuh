@@ -365,6 +365,7 @@ int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_str
 // dcs_resample on pcm / 32767; encode: nsrc x C stem planes (source, channel) Lin apart -> int16 [nsrc][L][C] at the
 // output rate, (int16_t)(int)(y * 32767) of dcs_resample's y trimmed to L
 int64_t resampler_length(const dcs_resampler* r, int64_t num_in);
+const dcs_ctx* resampler_ctx(const dcs_resampler* r);
 int check_resample_pcm16(const char* fn, const dcs_ctx* ctx, const dcs_resampler* to, const dcs_resampler* from, int C);
 int launch_resample_decode_pcm16(const dcs_resampler* r, const int16_t* d_pcm, int64_t L, int C, float* d_planes,
                                  int64_t Lout, cudaStream_t st);

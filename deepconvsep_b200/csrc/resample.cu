@@ -261,6 +261,7 @@ static int launch_pcm(const dcs_resampler* r, Kernel kernel, const char* scope, 
 }
 
 int64_t resampler_length(const dcs_resampler* r, int64_t num_in) { return dcs_resampled_length(num_in, r->up, r->down); }
+const dcs_ctx* resampler_ctx(const dcs_resampler* r) { return r->ctx; }
 
 int check_resample_pcm16(const char* fn, const dcs_ctx* ctx, const dcs_resampler* to, const dcs_resampler* from, int C) {
   DCS_REQUIRE(to && from, "%s: NULL resampler", fn);

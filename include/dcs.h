@@ -391,7 +391,11 @@ int dcs_separate_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const floa
 /* int16 PCM in / int16 PCM out, the wav-file contract of train_auto (separate_dsd.py:275-287,
  * 307-309): h_pcm int16[L][channels] interleaved; mono = (L+R)/2/32767 (downmix 1) or (L+R)/32767
  * (downmix 2, iKala separate_ikala.py:229) or channel 0 (channels == 1);
- * h_out int16[nsrc][out_stride] = (int16)(stem*32767) (C truncation, no clipping, as astype does) */
+ * h_out int16[nsrc][out_stride] = (int16)(stem*32767) (C truncation, no clipping, as astype does).
+ * The int16 encode of every entry point, exactly: v = stem * 32767.0f in fp32, truncated toward zero, then reduced
+ * modulo 2^16 into [-32768, 32767] -- a stem past full scale wraps (1.5 gives -16386), as numpy's
+ * (stem * maxn).astype('int16') does for |v| < 2^31.  NaN gives 0.  Beyond that the truncation saturates to int32
+ * first: v >= 2^31 and +inf give -1, v < -2^31 and -inf give 0 (numpy's result there depends on the platform). */
 int dcs_separate_pcm16_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const int16_t* h_pcm,
                             int64_t num_samples, int channels, int downmix, float scale_factor,
                             int overlap, int patcher, int16_t* h_out, int64_t out_stride,
@@ -572,8 +576,8 @@ int dcs_separate_audio_channels_wiener(dcs_ctx* ctx, dcs_model* model, dcs_stft*
  * takes for a C-channel stem).  One launch decodes a clip into channels + 1 fp32 planes -- the downmix of
  * dcs_separate_audio_channels, then a_c = pcm/32767 per channel -- the clip is dcs_separate_audio_channels_wiener on
  * those planes with `iterations` and `radius` (dcs_set_wiener and dcs_set_wiener_radius are not read), and one launch
- * encodes its nsrc*channels stem planes as (int16)(int)(stem*32767) (C truncation, no clipping, as in
- * dcs_separate_pcm16_host).  Launches per clip: those of dcs_separate_audio_channels(_wiener) on the clip, plus one
+ * encodes its nsrc*channels stem planes as (int16)(int)(stem*32767) (C truncation, no clipping: wraps modulo 2^16 for
+ * |stem*32767| < 2^31, NaN gives 0, saturating beyond, the encode of dcs_separate_pcm16_host).  Launches per clip: those of dcs_separate_audio_channels(_wiener) on the clip, plus one
  * (the decode forms the downmix in place of the downmix launch, and the encode is added).
  *  - channels = 1: the bytes of dcs_separate_batch_pcm16_host on the same clips (channels 1).
  *  - channels = 2, DCS_ARCH_DSD: the bytes of dcs_separate_batch_pcm16_keep_channels_host with the same iterations and
@@ -633,7 +637,8 @@ int dcs_resample(dcs_resampler* resampler, const float* d_in, int nplanes, int64
  * samples -- channel c is the bits of dcs_resample(to_model) on the plane pcm_c/32767 (fp32), the downmix is
  * dcs_separate_audio_channels' on those planes -- the clip is dcs_separate_audio_channels_wiener on them with
  * `iterations` and `radius`, and one launch resamples and encodes its nsrc*channels stem planes as (int16)(int)(y*32767)
- * with y the fp32 value of dcs_resample(from_model, num_out = L) (C truncation, no clipping).  So per clip the bytes are
+ * with y the fp32 value of dcs_resample(from_model, num_out = L) (C truncation, no clipping: the encode of
+ * dcs_separate_pcm16_host, which wraps modulo 2^16 -- a full-scale clip's resampled stems may overshoot 1.0).  So per clip the bytes are
  * those of (int16)(int)(stem*32767) on the stems of: dcs_resample(to_model) of pcm/32767, then
  * dcs_separate_audio_channels_wiener, then dcs_resample(from_model) trimmed to L.  Launches per clip: those of
  * dcs_separate_audio_channels(_wiener) on a clip of L' samples, plus one -- one fewer than those three calls.
@@ -653,6 +658,37 @@ int dcs_separate_batch_pcm16_channels_resampled_host(dcs_ctx* ctx, dcs_model* mo
                                                      int channels, int iterations, int radius, float scale_factor,
                                                      int overlap, int patcher, int16_t* const* h_out,
                                                      const int64_t* out_strides, void* stream);
+
+/* ---- bring-up and test entries: the int16 conversions of the int16 entry points -------------------------------- */
+/* Each is one launch of the very kernel the int16 batch entry points run, on caller device buffers, on `stream`, which
+ * is synchronised before returning.  resampler NULL: at the clip's rate; else the fused kernels of
+ * dcs_separate_batch_pcm16_channels_resampled_host (C-channel mode only; made on ctx).  Every argument is checked before
+ * anything is queued.
+ * dcs_pcm16_decode: d_pcm int16 [num_samples][channels] interleaved ->
+ *  - mode 0, 1, 2 (the `downmix` of dcs_separate_pcm16_host, channels 1..8): d_out float [num_samples], channel 0 /
+ *    (l + r) * 0.5f / l + r of l = pcm_0 / 32767.0f, r = pcm_1 / 32767.0f (channel 0 whenever channels == 1);
+ *    num_out = num_samples.
+ *  - DCS_PCM16_CHANNELS (channels 1..16): d_out float [channels + 1][num_out], plane 0 the downmix
+ *    (((a_0 + a_1) + a_2) + ...) * (1.0f / channels), plane 1 + c channel c: a_c = pcm_c / 32767.0f, num_out =
+ *    num_samples; with a resampler, a_c = dcs_resample of pcm_c / 32767.0f and num_out in
+ *    [1, dcs_resampled_length(num_samples)].
+ * dcs_pcm16_encode: stem plane p of num_in samples at d_stems + p * stem_stride, the encode of dcs_separate_pcm16_host ->
+ *  - DCS_PCM16_MONO (channels 1, nsrc planes): source s at d_out + s * out_stride, int16 [num_out], num_out = num_in,
+ *    stem_stride and out_stride >= num_in.
+ *  - DCS_PCM16_CHANNELS (channels 1..16, nsrc * channels planes ordered (source, channel), stem_stride >= num_in):
+ *    source s at d_out + s * out_stride as int16 [num_out][channels], out_stride = channels * num_out; num_out = num_in;
+ *    with a resampler the planes are the encode of dcs_resample(num_out) of each plane, stem_stride = num_in and
+ *    num_out in [1, dcs_resampled_length(num_in)].
+ *  d_out needs only 2-byte alignment; nothing outside the values listed is written.
+ * dcs_downmix_f32: nx (1..16) float planes audio_stride (>= num_samples) apart -> d_mono float [num_samples], the
+ *  downmix of DCS_PCM16_CHANNELS on float planes (the float route of dcs_separate_audio_channels). */
+enum { DCS_PCM16_MONO = 0, DCS_PCM16_CHANNELS = 3 };
+int dcs_pcm16_decode(dcs_ctx* ctx, const dcs_resampler* resampler, int mode, const int16_t* d_pcm, int64_t num_samples,
+                     int channels, float* d_out, int64_t num_out, void* stream);
+int dcs_pcm16_encode(dcs_ctx* ctx, const dcs_resampler* resampler, int mode, const float* d_stems, int64_t num_in, int nsrc,
+                     int channels, int64_t stem_stride, int16_t* d_out, int64_t num_out, int64_t out_stride, void* stream);
+int dcs_downmix_f32(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t num_samples, float* d_mono,
+                    void* stream);
 
 #ifdef __cplusplus
 }
