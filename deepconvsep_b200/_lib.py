@@ -91,9 +91,15 @@ _SIGS = {
     "dcs_pcm16_decode": (C.c_int, [_p, _p, C.c_int, _p, _i64, C.c_int, _p, _i64, _p]),
     "dcs_pcm16_encode": (C.c_int, [_p, _p, C.c_int, _p, _i64, C.c_int, C.c_int, _i64, _p, _i64, _i64, _p]),
     "dcs_downmix_f32": (C.c_int, [_p, _p, C.c_int, _i64, _i64, _p, _p]),
+    "dcs_separate_batch_channels_host": (C.c_int, [_p, _p, _p, _p, _p, C.c_int, C.c_int, C.c_int, _p, _p, C.c_int, C.c_int,
+                                                   C.c_int, C.c_float, C.c_int, C.c_int, _p, _p, _p]),
+    "dcs_channels_decode": (C.c_int, [_p, _p, C.c_int, _p, _i64, C.c_int, _p, _i64, _p]),
+    "dcs_channels_encode": (C.c_int, [_p, _p, C.c_int, _p, _i64, C.c_int, C.c_int, _i64, _p, _i64, _i64, _p]),
 }
 # modes of dcs_pcm16_decode / dcs_pcm16_encode beside the downmix 0..2 (include/dcs.h)
 PCM16_MONO, PCM16_CHANNELS = 0, 3
+# sample formats of dcs_separate_batch_channels_host (DCS_SAMPLE_*, include/dcs.h)
+SAMPLE_I16, SAMPLE_I32, SAMPLE_F32 = 0, 1, 2
 
 
 

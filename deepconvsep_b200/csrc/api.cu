@@ -802,9 +802,9 @@ int dcs_pcm16_decode(dcs_ctx* ctx, const dcs_resampler* r, int mode, const int16
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
   if (r)
-    rc = launch_resample_decode_pcm16(r, d_pcm, L, channels, d_out, num_out, st);
+    rc = launch_resample_decode(r, DCS_SAMPLE_I16, d_pcm, L, channels, d_out, num_out, st);
   else if (mode == DCS_PCM16_CHANNELS)
-    rc = launch_pcm_decode_channels(ctx, d_pcm, L, channels, d_out, st);
+    rc = launch_pcm_decode_channels(ctx, DCS_SAMPLE_I16, d_pcm, L, channels, d_out, st);
   else
     rc = launch_pcm_decode(ctx, d_pcm, L, channels, mode, d_out, st);
   return sync_after(fn, rc, st);
@@ -838,12 +838,58 @@ int dcs_pcm16_encode(dcs_ctx* ctx, const dcs_resampler* r, int mode, const float
   cudaStream_t st = (cudaStream_t)stream;
   int rc;
   if (r)
-    rc = launch_resample_encode_pcm16(r, d_stems, num_in, nsrc, channels, d_out, num_out, st);
+    rc = launch_resample_encode(r, DCS_SAMPLE_I16, d_stems, num_in, nsrc, channels, d_out, num_out, st);
   else if (mode == DCS_PCM16_CHANNELS)
-    rc = launch_pcm_encode_channels(ctx, d_stems, num_in, nsrc, channels, stem_stride, d_out, st);
+    rc = launch_pcm_encode_channels(ctx, DCS_SAMPLE_I16, d_stems, num_in, nsrc, channels, stem_stride, d_out, st);
   else
     rc = launch_pcm_encode(ctx, d_stems, num_in, nsrc, stem_stride, d_out, out_stride, st);
   return sync_after(fn, rc, st);
+}
+
+// the C-channel conversions of every sample format, each one launch of the launcher dcs_separate_batch_channels_host
+// calls (two for a decode whose channels take groups), on the caller's buffers
+int dcs_channels_decode(dcs_ctx* ctx, const dcs_resampler* r, int format, const void* d_in, int64_t L, int channels,
+                        float* d_out, int64_t num_out, void* stream) {
+  const char* fn = "dcs_channels_decode";
+  DCS_REQUIRE(ctx && d_in && d_out, "%s: NULL argument", fn);
+  DCS_REQUIRE(!r || resampler_ctx(r) == ctx, "%s: the resampler was made on another ctx", fn);
+  const int b = sample_bytes(format);
+  DCS_REQUIRE(b > 0, "%s: unknown sample format %d", fn, format);
+  DCS_REQUIRE(L >= 1, "%s: num_samples %lld must be >= 1", fn, (long long)L);
+  DCS_REQUIRE((uintptr_t)d_in % b == 0 && (uintptr_t)d_out % 4 == 0, "%s: d_in not %d-byte or d_out not 4-byte aligned", fn,
+              b);
+  DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
+  const int64_t most = r ? resampler_length(r, L) : L;
+  DCS_REQUIRE(num_out >= 1 && num_out <= most && (r || num_out == L), "%s: num_out %lld, want %s%lld", fn, (long long)num_out,
+              r ? "1 .. " : "", (long long)most);
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  return sync_after(fn, r ? launch_resample_decode(r, format, d_in, L, channels, d_out, num_out, st)
+                          : launch_pcm_decode_channels(ctx, format, d_in, L, channels, d_out, st), st);
+}
+
+int dcs_channels_encode(dcs_ctx* ctx, const dcs_resampler* r, int format, const float* d_stems, int64_t num_in, int nsrc,
+                        int channels, int64_t stem_stride, void* d_out, int64_t num_out, int64_t out_stride, void* stream) {
+  const char* fn = "dcs_channels_encode";
+  DCS_REQUIRE(ctx && d_stems && d_out, "%s: NULL argument", fn);
+  DCS_REQUIRE(!r || resampler_ctx(r) == ctx, "%s: the resampler was made on another ctx", fn);
+  const int b = sample_bytes(format);
+  DCS_REQUIRE(b > 0, "%s: unknown sample format %d", fn, format);
+  DCS_REQUIRE(num_in >= 1 && nsrc >= 1, "%s: num_in %lld and nsrc %d must be >= 1", fn, (long long)num_in, nsrc);
+  DCS_REQUIRE((uintptr_t)d_stems % 4 == 0 && (uintptr_t)d_out % b == 0, "%s: d_stems not 4-byte or d_out not %d-byte aligned",
+              fn, b);
+  DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
+  DCS_REQUIRE(r ? stem_stride == num_in : stem_stride >= num_in, "%s: stem_stride %lld, num_in %lld", fn,
+              (long long)stem_stride, (long long)num_in);
+  const int64_t most = r ? resampler_length(r, num_in) : num_in;
+  DCS_REQUIRE(num_out >= 1 && num_out <= most && (r || num_out == num_in), "%s: num_out %lld, want %s%lld", fn,
+              (long long)num_out, r ? "1 .. " : "", (long long)most);
+  DCS_REQUIRE(out_stride == (int64_t)channels * num_out, "%s: out_stride %lld != channels * num_out", fn, (long long)out_stride);
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  return sync_after(fn, r ? launch_resample_encode(r, format, d_stems, num_in, nsrc, channels, d_out, num_out, st)
+                          : launch_pcm_encode_channels(ctx, format, d_stems, num_in, nsrc, channels, stem_stride, d_out, st),
+                    st);
 }
 
 int dcs_downmix_f32(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t L, float* d_mono, void* stream) {
@@ -909,18 +955,20 @@ int dcs_separate_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const int16
 // int16 staging on the device and events for the hand-overs.  The reference's only multi-clip driver starts a Python
 // process per file (examples/dsd100/separate_multiple.ipynb cell 3); per clip this is the wav contract of train_auto
 // (separate_dsd.py:275-287,307-309), exactly dcs_separate_pcm16_host.  Host buffers should be pinned.
-// the pipelined loop of the int16 batch entry points; on any failure the caller drains the copy streams before it
-// returns, because the copies in flight read and write the user's host buffers.  nx == 0: mono stems, the clip decoded
-// into one plane (channel 0 or the downmix of `downmix`), int16 [nsrc][L] out.  nx > 0 (C-channel stems, nx ==
-// channels): the clip is decoded into nx + 1 planes (the downmix, then the channels), separated as
-// dcs_separate_audio_channels_wiener with `iterations` and `radius`, and the stems encoded as interleaved [L][nx] per
-// source.  to / from (nx > 0, both or neither): the clip is at another rate; the decode resamples it to L' =
-// resampler_length(to, L) samples, the clip is separated at L', and the encode resamples its stems back to L
+// the pipelined loop of the int16 and C-channel batch entry points; on any failure the caller drains the copy streams
+// before it returns, because the copies in flight read and write the user's host buffers.  nx == 0: mono stems (int16
+// in and out), the clip decoded into one plane (channel 0 or the downmix of `downmix`), int16 [nsrc][L] out.  nx > 0
+// (C-channel stems, nx == channels): the clip, samples of in_fmt, is decoded into nx + 1 planes (the downmix, then the
+// channels), separated as dcs_separate_audio_channels_wiener with `iterations` and `radius`, and the stems encoded in
+// out_fmt as interleaved [L][nx] per source.  to / from (nx > 0, both or neither): the clip is at another rate; the
+// decode resamples it to L' = resampler_length(to, L) samples, the clip is separated at L', and the encode resamples its
+// stems back to L
 static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to, const dcs_resampler* from,
-                          int nclips, const int16_t* const* h_pcm, const int64_t* num_samples, int channels, int downmix,
-                          int nx, int iterations, int radius, float scale_factor, int overlap, int patcher,
-                          int16_t* const* h_out, const int64_t* out_strides, cudaStream_t st) {
-  const int w = nx > 0 ? nx : 1;   // int16 values per sample of a stem
+                          int in_fmt, int out_fmt, int nclips, const void* const* h_in, const int64_t* num_samples,
+                          int channels, int downmix, int nx, int iterations, int radius, float scale_factor, int overlap,
+                          int patcher, void* const* h_out, const int64_t* out_strides, cudaStream_t st) {
+  const size_t bi = (size_t)sample_bytes(in_fmt), bo = (size_t)sample_bytes(out_fmt);
+  const size_t w = (size_t)(nx > 0 ? nx : 1) * bo;   // bytes per sample of a stem
   float *audio = ctx->audio.as<float>(), *stems = ctx->stems.as<float>();
   // the copy streams start after whatever the caller queued on `st` (and after the memsets of fresh buffers)
   DCS_CUDA(cudaEventRecord(ctx->ev_dec[0], st));
@@ -931,20 +979,20 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_res
     const int64_t L = num_samples[i];
     // H2D of clip i: its staging buffer is free once the decode of clip i-2 has read it
     if (i >= 2) DCS_CUDA(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_dec[b], 0));
-    DCS_CUDA(cudaMemcpyAsync(ctx->pcm_in[b].p, h_pcm[i], (size_t)L * channels * sizeof(int16_t), cudaMemcpyHostToDevice, ctx->s_h2d));
+    DCS_CUDA(cudaMemcpyAsync(ctx->pcm_in[b].p, h_in[i], (size_t)L * channels * bi, cudaMemcpyHostToDevice, ctx->s_h2d));
     DCS_CUDA(cudaEventRecord(ctx->ev_in[b], ctx->s_h2d));
     // kernels of clip i
     DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_in[b], 0));
     const int64_t Lm = to ? resampler_length(to, L) : L;   // the clip's samples at the networks' rate
     if (to) {
-      DCS_TRY(launch_resample_decode_pcm16(to, ctx->pcm_in[b].as<int16_t>(), L, nx, audio, Lm, st));
+      DCS_TRY(launch_resample_decode(to, in_fmt, ctx->pcm_in[b].p, L, nx, audio, Lm, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
       ProfScope ps(ctx, "pcm16_separate", st);
       DCS_TRY(downmix_clip(ctx, m, p, audio, audio + Lm, nx, Lm, Lm, iterations, radius, scale_factor, overlap, patcher, stems,
                            Lm, st));
     } else if (nx > 0) {
       ProfScope ps(ctx, "pcm16_decode_separate", st);   // the clip's kernels up to its stem planes
-      DCS_TRY(launch_pcm_decode_channels(ctx, ctx->pcm_in[b].as<int16_t>(), L, nx, audio, st));
+      DCS_TRY(launch_pcm_decode_channels(ctx, in_fmt, ctx->pcm_in[b].p, L, nx, audio, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
       DCS_TRY(downmix_clip(ctx, m, p, audio, audio + L, nx, L, L, iterations, radius, scale_factor, overlap, patcher, stems, L,
                            st));
@@ -956,40 +1004,39 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_res
     }
     if (i >= 2) DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_out[b], 0));     // D2H of clip i-2 has drained the output staging
     if (from) {
-      DCS_TRY(launch_resample_encode_pcm16(from, stems, Lm, m->nsrc, nx, ctx->pcm_out[b].as<int16_t>(), L, st));
+      DCS_TRY(launch_resample_encode(from, out_fmt, stems, Lm, m->nsrc, nx, ctx->pcm_out[b].p, L, st));
     } else if (nx > 0) {
       ProfScope ps(ctx, "pcm16_encode", st);
-      DCS_TRY(launch_pcm_encode_channels(ctx, stems, L, m->nsrc, nx, L, ctx->pcm_out[b].as<int16_t>(), st));
+      DCS_TRY(launch_pcm_encode_channels(ctx, out_fmt, stems, L, m->nsrc, nx, L, ctx->pcm_out[b].p, st));
     } else
       DCS_TRY(launch_pcm_encode(ctx, stems, L, m->nsrc, L, ctx->pcm_out[b].as<int16_t>(), L, st));
     DCS_CUDA(cudaEventRecord(ctx->ev_enc[b], st));
     // D2H of clip i
     DCS_CUDA(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_enc[b], 0));
-    DCS_CUDA(cudaMemcpy2DAsync(h_out[i], (size_t)w * out_strides[i] * sizeof(int16_t), ctx->pcm_out[b].p,
-                               (size_t)w * L * sizeof(int16_t), (size_t)w * L * sizeof(int16_t), m->nsrc, cudaMemcpyDeviceToHost,
+    DCS_CUDA(cudaMemcpy2DAsync(h_out[i], w * out_strides[i], ctx->pcm_out[b].p, w * L, w * L, m->nsrc, cudaMemcpyDeviceToHost,
                                ctx->s_d2h));
     DCS_CUDA(cudaEventRecord(ctx->ev_out[b], ctx->s_d2h));
   }
   return DCS_OK;
 }
 
-// the checks, resources and drain of every int16 batch entry point around batch_pipeline (nx, iterations, radius, to,
-// from as there; the entry point has checked the resampler pair).  check_model(Lmax): the entry point's own checks of
-// the model, plan and options, run on the longest clip (its length at the networks' rate) after the per-clip checks and
-// before anything is queued
+// the checks, resources and drain of every batch entry point around batch_pipeline (formats, nx, iterations, radius,
+// to, from as there; the entry point has checked the formats and the resampler pair).  check_model(Lmax): the entry
+// point's own checks of the model, plan and options, run on the longest clip (its length at the networks' rate) after
+// the per-clip checks and before anything is queued
 extern "C++" {
 template <class CheckModel>
 static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to,
-                      const dcs_resampler* from, int nclips, const int16_t* const* h_pcm,
+                      const dcs_resampler* from, int in_fmt, int out_fmt, int nclips, const void* const* h_in,
                       const int64_t* num_samples, int channels, int downmix, int nx, int iterations, int radius,
-                      float scale_factor, int overlap, int patcher, int16_t* const* h_out, const int64_t* out_strides,
+                      float scale_factor, int overlap, int patcher, void* const* h_out, const int64_t* out_strides,
                       cudaStream_t st, CheckModel check_model) {
-  DCS_REQUIRE(ctx && m && p && h_pcm && num_samples && h_out && out_strides && nclips >= 0, "%s: bad argument", fn);
+  DCS_REQUIRE(ctx && m && p && h_in && num_samples && h_out && out_strides && nclips >= 0, "%s: bad argument", fn);
   DCS_REQUIRE(nx > 0 || (channels >= 1 && channels <= 8 && downmix >= 0 && downmix <= 2), "bad channels/downmix");
   if (nclips == 0) return DCS_OK;
   int64_t Lmax = 0;
   for (int i = 0; i < nclips; ++i) {
-    DCS_REQUIRE(h_pcm[i] && h_out[i] && num_samples[i] > 0 && out_strides[i] >= num_samples[i], "clip %d: bad buffer / length", i);
+    DCS_REQUIRE(h_in[i] && h_out[i] && num_samples[i] > 0 && out_strides[i] >= num_samples[i], "clip %d: bad buffer / length", i);
     Lmax = std::max(Lmax, num_samples[i]);
   }
   const int64_t Lwork = to ? resampler_length(to, Lmax) : Lmax;   // the longest clip at the networks' rate
@@ -1007,15 +1054,15 @@ static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, c
   // every buffer at the size of the longest clip before the pipeline starts: a grow-only buffer that had to be
   // re-allocated mid-batch would synchronise the stream
   for (int b = 0; b < std::min(nclips, 2); ++b) {
-    DCS_TRY(ctx->pcm_in[b].ensure((size_t)Lmax * channels * sizeof(int16_t), st));
-    DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * (nx > 0 ? nx : 1) * Lmax * sizeof(int16_t), st));
+    DCS_TRY(ctx->pcm_in[b].ensure((size_t)Lmax * channels * sample_bytes(in_fmt), st));
+    DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * (nx > 0 ? nx : 1) * Lmax * sample_bytes(out_fmt), st));
   }
   if (nx > 0)
     DCS_TRY(size_downmix_workspace(ctx, m, p, Lwork, iterations > 0 ? nx : 0, radius, nx, st));
   else
     DCS_TRY(size_workspace(ctx, m, p, Lmax, true, st));
-  const int rc = batch_pipeline(ctx, m, p, to, from, nclips, h_pcm, num_samples, channels, downmix, nx, iterations, radius,
-                                scale_factor, overlap, patcher, h_out, out_strides, st);
+  const int rc = batch_pipeline(ctx, m, p, to, from, in_fmt, out_fmt, nclips, h_in, num_samples, channels, downmix, nx,
+                                iterations, radius, scale_factor, overlap, patcher, h_out, out_strides, st);
   // drain everything, success or not, before the host buffers go back to the caller
   const cudaError_t e0 = cudaStreamSynchronize(ctx->s_h2d), e1 = cudaStreamSynchronize(ctx->s_d2h), e2 = cudaStreamSynchronize(st);
   if (rc != DCS_OK) return rc;
@@ -1030,9 +1077,8 @@ int dcs_separate_batch_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, int n
                                   const int64_t* num_samples, int channels, int downmix, float scale_factor, int overlap,
                                   int patcher, int16_t* const* h_out, const int64_t* out_strides, void* stream) {
   const char* fn = "dcs_separate_batch_pcm16_host";
-  return batch_host(fn, ctx, m, p, nullptr, nullptr, nclips, h_pcm, num_samples, channels, downmix, 0, 0, 0, scale_factor,
-                    overlap, patcher,
-                    h_out, out_strides, (cudaStream_t)stream, [&](int64_t Lmax) {
+  return batch_host(fn, ctx, m, p, nullptr, nullptr, DCS_SAMPLE_I16, DCS_SAMPLE_I16, nclips, (const void* const*)h_pcm,
+                    num_samples, channels, downmix, 0, 0, 0, scale_factor, overlap, patcher, (void* const*)h_out, out_strides, (cudaStream_t)stream, [&](int64_t Lmax) {
                       return check_clip(fn, ctx, m, p, -1, h_pcm, h_out, Lmax, Lmax, Lmax, overlap, patcher);
                     });
 }
@@ -1044,8 +1090,9 @@ int dcs_separate_batch_pcm16_keep_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_
                                                 int overlap, int patcher, int16_t* const* h_out, const int64_t* out_strides,
                                                 void* stream) {
   const char* fn = "dcs_separate_batch_pcm16_keep_channels_host";
-  return batch_host(fn, ctx, m, p, nullptr, nullptr, nclips, h_pcm, num_samples, 2, 1, 2, ctx ? ctx->wiener_iters : 0,
-                    ctx ? ctx->wiener_radius : 0, scale_factor, overlap, patcher, h_out, out_strides, (cudaStream_t)stream,
+  return batch_host(fn, ctx, m, p, nullptr, nullptr, DCS_SAMPLE_I16, DCS_SAMPLE_I16, nclips, (const void* const*)h_pcm,
+                    num_samples, 2, 1, 2, ctx ? ctx->wiener_iters : 0, ctx ? ctx->wiener_radius : 0, scale_factor, overlap,
+                    patcher, (void* const*)h_out, out_strides, (cudaStream_t)stream,
                     [&](int64_t Lmax) {
                       DCS_TRY(check_clip(fn, ctx, m, p, DCS_ARCH_DSD, h_pcm, h_out, Lmax, Lmax, Lmax, overlap, patcher));
                       return check_keep_tap(fn, ctx);
@@ -1194,20 +1241,29 @@ int dcs_separate_audio_channels_wiener(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, 
                       d_stems, stem_stride, (cudaStream_t)stream);
 }
 
-// the int16 batch of C-channel clips: per clip dcs_separate_audio_channels_wiener on the decoded planes, with the checks
-// of that call on the longest clip.  to / from: the resampler pair of a clip rate other than the networks' (NULL: none)
-static int pcm16_channels(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to,
-                          const dcs_resampler* from, int nclips, const int16_t* const* h_pcm, const int64_t* num_samples,
-                          int channels, int iterations, int radius, float scale_factor, int overlap, int patcher,
-                          int16_t* const* h_out, const int64_t* out_strides, void* stream) {
+// the batch of C-channel clips, samples of in_fmt in and out_fmt out: per clip dcs_separate_audio_channels_wiener on
+// the decoded planes, with the checks of that call on the longest clip.  resampled: the clips are at another rate,
+// to / from the resampler pair (refused when NULL); else both are ignored
+static int channels_batch(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, bool resampled, const dcs_resampler* to,
+                          const dcs_resampler* from, int in_fmt, int out_fmt, int nclips, const void* const* h_in,
+                          const int64_t* num_samples, int channels, int iterations, int radius, float scale_factor,
+                          int overlap, int patcher, void* const* h_out, const int64_t* out_strides, void* stream) {
+  DCS_REQUIRE(sample_bytes(in_fmt) > 0 && sample_bytes(out_fmt) > 0, "%s: unknown sample format %d / %d", fn, in_fmt, out_fmt);
+  if (resampled) {
+    DCS_REQUIRE(ctx, "%s: NULL ctx", fn);
+    DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
+    DCS_TRY(check_resample_channels(fn, ctx, to, from, channels, in_fmt));
+  } else {
+    to = from = nullptr;
+  }
   DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
   DCS_REQUIRE(iterations >= 0, "%s: iterations %d must be >= 0", fn, iterations);
   DCS_REQUIRE(radius >= 0, "%s: radius %d must be >= 0", fn, radius);
   DCS_REQUIRE(iterations == 0 || (channels >= 2 && channels <= 8), "%s: the Wiener post-filter needs channels in [2, 8], got %d",
               fn, channels);
-  return batch_host(fn, ctx, m, p, to, from, nclips, h_pcm, num_samples, channels, 0, channels, iterations, radius,
-                    scale_factor, overlap, patcher, h_out, out_strides, (cudaStream_t)stream, [&](int64_t Lmax) {
-                      return check_channels(fn, ctx, m, p, h_pcm, channels, Lmax, Lmax, overlap, patcher, h_out, Lmax,
+  return batch_host(fn, ctx, m, p, to, from, in_fmt, out_fmt, nclips, h_in, num_samples, channels, 0, channels, iterations,
+                    radius, scale_factor, overlap, patcher, h_out, out_strides, (cudaStream_t)stream, [&](int64_t Lmax) {
+                      return check_channels(fn, ctx, m, p, h_in, channels, Lmax, Lmax, overlap, patcher, h_out, Lmax,
                                             iterations, radius);
                     });
 }
@@ -1216,8 +1272,9 @@ int dcs_separate_batch_pcm16_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_stft*
                                            const int64_t* num_samples, int channels, int iterations, int radius,
                                            float scale_factor, int overlap, int patcher, int16_t* const* h_out,
                                            const int64_t* out_strides, void* stream) {
-  return pcm16_channels("dcs_separate_batch_pcm16_channels_host", ctx, m, p, nullptr, nullptr, nclips, h_pcm, num_samples,
-                        channels, iterations, radius, scale_factor, overlap, patcher, h_out, out_strides, stream);
+  return channels_batch("dcs_separate_batch_pcm16_channels_host", ctx, m, p, false, nullptr, nullptr, DCS_SAMPLE_I16,
+                        DCS_SAMPLE_I16, nclips, (const void* const*)h_pcm, num_samples, channels, iterations, radius,
+                        scale_factor, overlap, patcher, (void* const*)h_out, out_strides, stream);
 }
 
 int dcs_separate_batch_pcm16_channels_resampled_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to_model,
@@ -1225,12 +1282,19 @@ int dcs_separate_batch_pcm16_channels_resampled_host(dcs_ctx* ctx, dcs_model* m,
                                                      const int64_t* num_samples, int channels, int iterations, int radius,
                                                      float scale_factor, int overlap, int patcher, int16_t* const* h_out,
                                                      const int64_t* out_strides, void* stream) {
-  const char* fn = "dcs_separate_batch_pcm16_channels_resampled_host";
-  DCS_REQUIRE(ctx, "%s: NULL ctx", fn);
-  DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
-  DCS_TRY(check_resample_pcm16(fn, ctx, to_model, from_model, channels));
-  return pcm16_channels(fn, ctx, m, p, to_model, from_model, nclips, h_pcm, num_samples, channels, iterations, radius,
-                        scale_factor, overlap, patcher, h_out, out_strides, stream);
+  return channels_batch("dcs_separate_batch_pcm16_channels_resampled_host", ctx, m, p, true, to_model, from_model,
+                        DCS_SAMPLE_I16, DCS_SAMPLE_I16, nclips, (const void* const*)h_pcm, num_samples, channels, iterations,
+                        radius, scale_factor, overlap, patcher, (void* const*)h_out, out_strides, stream);
+}
+
+int dcs_separate_batch_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to_model,
+                                     const dcs_resampler* from_model, int in_format, int out_format, int nclips,
+                                     const void* const* h_in, const int64_t* num_samples, int channels, int iterations,
+                                     int radius, float scale_factor, int overlap, int patcher, void* const* h_out,
+                                     const int64_t* out_strides, void* stream) {
+  return channels_batch("dcs_separate_batch_channels_host", ctx, m, p, to_model || from_model, to_model, from_model,
+                        in_format, out_format, nclips, h_in, num_samples, channels, iterations, radius, scale_factor, overlap,
+                        patcher, h_out, out_strides, stream);
 }
 
 // ------------------------------------------------------------------------------------ Wiener post-filter

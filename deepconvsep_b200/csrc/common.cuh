@@ -86,7 +86,8 @@ struct dcs_ctx {
   dcs::DevBuf masks;            // dcs_separate_audio_channels: the downmix's blended masks, nsrc float planes
   dcs::DevBuf net[dcs::NET_SLOTS];
   uint64_t net_sig[dcs::NET_SLOTS] = {0};   // layout signature of what each net[] buffer currently holds
-  // multi-clip scheduler (dcs_separate_batch_pcm16_host): copy streams, double-buffered staging, hand-over events
+  // multi-clip scheduler (dcs_separate_batch_pcm16_host, dcs_separate_batch_channels_host): copy streams,
+  // double-buffered staging, hand-over events
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
   cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_dec[2] = {nullptr, nullptr}, ev_enc[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
   dcs::DevBuf pcm_in[2], pcm_out[2];
@@ -349,28 +350,57 @@ int launch_pcm_decode(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int channel
                       cudaStream_t st);
 int launch_pcm_encode(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int64_t stem_stride, int16_t* d_out,
                       int64_t out_stride, cudaStream_t st);
-// C-channel stems, C in [1, 16]: interleaved int16 [L][C] -> C + 1 float planes L apart (the downmix of
-// launch_downmix, then the C channels); nsrc x C stem planes (source, channel) -> int16 [nsrc][L][C], source s at
-// d_out + s * C * L
-int launch_pcm_decode_channels(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int C, float* d_planes, cudaStream_t st);
-int launch_pcm_encode_channels(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int C, int64_t stem_stride,
-                               int16_t* d_out, cudaStream_t st);
+
+// The sample formats of the C-channel batch (DCS_SAMPLE_*, include/dcs.h): the stored type, the decode of a sample to
+// the fp32 plane and the encode of an fp32 stem value, the rules written in dcs.h
+template <int FMT> struct SampleFormat;
+template <> struct SampleFormat<DCS_SAMPLE_I16> {
+  using T = int16_t;
+  static __device__ __forceinline__ float decode(T x) { return (float)x / 32767.0f; }
+  static __device__ __forceinline__ T encode(float y) { return (int16_t)(int)(y * 32767.0f); }   // wraps modulo 2^16
+};
+template <> struct SampleFormat<DCS_SAMPLE_I32> {
+  using T = int32_t;
+  static __device__ __forceinline__ float decode(T x) { return (float)((double)x / 2147483647.0); }
+  // truncates and saturates; cvt from f64 would give INT_MIN for NaN, so NaN is tested first
+  static __device__ __forceinline__ T encode(float y) { return y == y ? __double2int_rz((double)y * 2147483647.0) : 0; }
+};
+template <> struct SampleFormat<DCS_SAMPLE_F32> {
+  using T = float;
+  static __device__ __forceinline__ float decode(T x) { return x; }
+  static __device__ __forceinline__ T encode(float y) { return y; }
+};
+// bytes of one sample; 0 for an unknown format code
+inline int sample_bytes(int fmt) {
+  return fmt == DCS_SAMPLE_I16 ? 2 : (fmt == DCS_SAMPLE_I32 || fmt == DCS_SAMPLE_F32) ? 4 : 0;
+}
+
+// C-channel stems, C in [1, 16], samples in format fmt: interleaved [L][C] -> C + 1 float planes L apart (the downmix
+// of launch_downmix, then the C channels); nsrc x C stem planes (source, channel) -> [nsrc][L][C], source s at
+// d_out + s * C * L samples
+int launch_pcm_decode_channels(dcs_ctx* ctx, int fmt, const void* d_in, int64_t L, int C, float* d_planes, cudaStream_t st);
+int launch_pcm_encode_channels(dcs_ctx* ctx, int fmt, const float* d_stems, int64_t L, int nsrc, int C, int64_t stem_stride,
+                               void* d_out, cudaStream_t st);
 // nx float planes -> (((a_0 + a_1) + a_2) + ...) * (1.0f / nx): the downmix of launch_pcm_decode_channels, a copy
 // at nx = 1
 int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st);
 
-// the int16 batch at another rate (resample.cu), C in [1, 16], on the resampler's ctx.  check_resample_pcm16: what the
-// batch refuses of its resampler pair (NULL, another ctx, not inverse, no tile that fits).  decode: int16 [L][C] -> C + 1
-// float planes Lout apart at the resampler's output rate (the downmix, then the channels), each channel the bits of
-// dcs_resample on pcm / 32767; encode: nsrc x C stem planes (source, channel) Lin apart -> int16 [nsrc][L][C] at the
-// output rate, (int16_t)(int)(y * 32767) of dcs_resample's y trimmed to L
+// the C-channel batch at another rate (resample.cu), C in [1, 16], on the resampler's ctx.  check_resample_channels:
+// what the batch refuses of its resampler pair (NULL, another ctx, not inverse, no tile that fits for samples in
+// in_fmt).  decode: [L][C] in fmt -> C + 1 float planes Lout apart at the resampler's output rate (the downmix, then the
+// channels), each channel the bits of dcs_resample on the decoded plane; one launch, or two when the 4-byte staging
+// splits the channels into groups (resample_decode_groups > 1: the downmix is then launch_downmix on the resampled
+// planes).  encode: nsrc x C stem planes (source, channel) Lin apart -> [nsrc][L][C] in fmt at the output rate, the
+// encode of dcs_resample's y trimmed to L
 int64_t resampler_length(const dcs_resampler* r, int64_t num_in);
 const dcs_ctx* resampler_ctx(const dcs_resampler* r);
-int check_resample_pcm16(const char* fn, const dcs_ctx* ctx, const dcs_resampler* to, const dcs_resampler* from, int C);
-int launch_resample_decode_pcm16(const dcs_resampler* r, const int16_t* d_pcm, int64_t L, int C, float* d_planes,
-                                 int64_t Lout, cudaStream_t st);
-int launch_resample_encode_pcm16(const dcs_resampler* r, const float* d_stems, int64_t Lin, int nsrc, int C, int16_t* d_out,
-                                 int64_t L, cudaStream_t st);
+int check_resample_channels(const char* fn, const dcs_ctx* ctx, const dcs_resampler* to, const dcs_resampler* from, int C,
+                            int in_fmt);
+int resample_decode_groups(const dcs_resampler* r, int C, int fmt);
+int launch_resample_decode(const dcs_resampler* r, int fmt, const void* d_in, int64_t L, int C, float* d_planes, int64_t Lout,
+                           cudaStream_t st);
+int launch_resample_encode(const dcs_resampler* r, int fmt, const float* d_stems, int64_t Lin, int nsrc, int C, void* d_out,
+                           int64_t L, cudaStream_t st);
 
 // multichannel Wiener post-filter (wiener.cu): nch (2..8) mixture channels, channel c at X + c * x_plane, stem (j, c) at
 // S + (j * nch + c) * src_stride, bins f < F filtered in place by `iterations` EM iterations; radius: the covariance

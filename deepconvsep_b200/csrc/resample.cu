@@ -12,10 +12,12 @@
 // conflict-free and the sample loads nearly so.  The sum is accumulated in fp64 with fma in increasing i and rounded
 // once to fp32: the same bits on every run.
 //
-// The int16 batch at another rate fuses the PCM conversions into the resampler (resample_decode_pcm16_kernel,
-// resample_encode_pcm16_kernel): the same bank, the same work items and the same inner sum (polyphase_sum), so each value
-// has the bits of resample_kernel on the fp32 planes the unfused route would have formed.
+// The C-channel batch at another rate fuses the sample conversions into the resampler (resample_decode_kernel,
+// resample_encode_kernel, one instantiation per sample format): the same bank, the same work items and the same inner
+// sum (polyphase_sum), so each value has the bits of resample_kernel on the fp32 planes the unfused route would have
+// formed.
 #include <algorithm>
+#include <type_traits>
 #include "common.cuh"
 
 struct dcs_resampler {
@@ -93,39 +95,59 @@ resample_kernel(const ResampleArgs a) {
   }
 }
 
-// The int16 batch's conversions fused into the resampler.  Both take the bank and phase constants of a dcs_resampler,
-// tiles of tp periods as resample_kernel does, and a plan per (resampler, C) that fits shared memory.
+// The C-channel batch's conversions fused into the resampler.  Both take the bank and phase constants of a
+// dcs_resampler, tiles of tp periods as resample_kernel does, and a plan per (resampler, C, format) that fits shared
+// memory.
 struct ResamplePcmArgs {
-  const void* in; int64_t num_in;    // decode: int16 [num_in][C]; encode: nsrc*C fp32 planes num_in apart
-  void* out; int64_t num_out;        // decode: C + 1 fp32 planes num_out apart; encode: int16 [nsrc][num_out][C]
+  const void* in; int64_t num_in;    // decode: samples [num_in][C]; encode: nsrc*C fp32 planes num_in apart
+  void* out; int64_t num_out;        // decode: C + 1 fp32 planes num_out apart; encode: samples [nsrc][num_out][C]
   const double* bank;
   int up, down, Q, half_len, c0, tp, span;
   int C, cn, cs;                     // channels; channels per tile and staged values per sample (encode)
   int64_t tiles_t, ntiles;           // tiles along time, all tiles
 };
 
-// int16 [num_in][C] at the clip's rate -> plane 1 + c: resample_kernel on the fp32 plane (float)pcm_c / 32767.0f, and
-// plane 0: (((y_0 + y_1) + y_2) + ...) * (1.0f / C) on those rounded values, downmix_kernel's expression.  A tile is tp
-// periods of all C channels, so one thread forms the downmix of its outputs; its input span is staged as int16, channel
-// by channel ([C][span]), and converted per tap.  A work item is (residue r, RS_V periods) for every channel in turn.
+// the tap value of a staged sample: int16 is converted per tap use, the 4-byte formats are staged already decoded
+__device__ __forceinline__ float staged_tap(int16_t x) { return SampleFormat<DCS_SAMPLE_I16>::decode(x); }
+__device__ __forceinline__ float staged_tap(float x) { return x; }
+
+// [num_in][C] samples of format FMT at the clip's rate -> plane 1 + c: resample_kernel on the fp32 plane of the format's
+// decode of channel c, and plane 0: (((y_0 + y_1) + y_2) + ...) * (1.0f / C) on those rounded values, downmix_kernel's
+// expression.  A tile is tp periods of cn channels; its input span is staged channel by channel ([cn][span]).  A work
+// item is (residue r, RS_V periods) for every channel of the tile in turn, so when the tile holds all C channels
+// (cn = C) one thread forms the downmix of its outputs.
+//  - int16: staged as int16 and converted per tap; cn = C always.
+//  - int32 and float32: staged as their fp32 decode, one conversion per staged sample, so the inner sum is
+//    resample_kernel's on the same values.  Where 4-byte staging leaves no room for all C channels, the channels are
+//    split into equal groups of cn; plane 0 is then not written here but by one downmix_kernel launch on the planes.
+template <int FMT>
 __global__ void __launch_bounds__(RS_THREADS)
-resample_decode_pcm16_kernel(const ResamplePcmArgs a) {
+resample_decode_kernel(const ResamplePcmArgs a) {
+  using In = typename SampleFormat<FMT>::T;
+  constexpr bool kWide = FMT != DCS_SAMPLE_I16;
+  using Staged = typename std::conditional<kWide, float, int16_t>::type;
   extern __shared__ __align__(16) unsigned char rs_smem[];
   double* bank = reinterpret_cast<double*>(rs_smem);
-  int16_t* xs = reinterpret_cast<int16_t*>(bank + (size_t)a.Q * a.up);
-  const int16_t* __restrict__ pcm = static_cast<const int16_t*>(a.in);
+  Staged* xs = reinterpret_cast<Staged*>(bank + (size_t)a.Q * a.up);
+  const In* __restrict__ pcm = static_cast<const In*>(a.in);
   float* __restrict__ planes = static_cast<float*>(a.out);
   for (int k = threadIdx.x; k < a.Q * a.up; k += RS_THREADS) bank[k] = __ldg(a.bank + k);
-  const int C = a.C, items = a.up * (a.tp / RS_V), staged = a.span * C;
+  const int C = a.C, items = a.up * (a.tp / RS_V);
   const float inv = 1.0f / (float)C;
   for (int64_t tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
-    const int64_t P0 = tile * a.tp;
+    const int64_t tt = kWide ? tile % a.tiles_t : tile;
+    const int c_lo = kWide ? (int)(tile / a.tiles_t) * a.cn : 0;
+    const int cn = kWide ? min(a.cn, C - c_lo) : C;
+    const int64_t P0 = tt * a.tp;
     const int64_t jlo = P0 * a.down + a.c0 - (a.Q - 1);
     __syncthreads();
-    for (int k = threadIdx.x; k < staged; k += RS_THREADS) {    // consecutive threads read consecutive int16 values
-      const int jj = k / C, c = k - jj * C;
+    for (int k = threadIdx.x; k < a.span * cn; k += RS_THREADS) {    // consecutive threads read consecutive values
+      const int jj = k / cn, c = k - jj * cn;
       const int64_t j = jlo + jj;
-      xs[c * a.span + jj] = (j >= 0 && j < a.num_in) ? pcm[j * C + c] : (int16_t)0;
+      if constexpr (kWide)
+        xs[c * a.span + jj] = (j >= 0 && j < a.num_in) ? SampleFormat<FMT>::decode(pcm[j * C + c_lo + c]) : 0.f;
+      else
+        xs[c * a.span + jj] = (j >= 0 && j < a.num_in) ? pcm[j * C + c] : (int16_t)0;
     }
     __syncthreads();
     for (int w = threadIdx.x; w < items; w += RS_THREADS) {
@@ -135,11 +157,11 @@ resample_decode_pcm16_kernel(const ResamplePcmArgs a) {
       const int cr = (int)(((int64_t)r * a.down + a.half_len) / a.up);
       const int base = g * RS_V * a.down + cr - a.c0 + a.Q - 1;
       float mix[RS_V];
-      for (int c = 0; c < C; ++c) {
-        const int16_t* xc = xs + c * a.span;
+      for (int c = 0; c < cn; ++c) {
+        const Staged* xc = xs + c * a.span;
         double acc[RS_V];
-        polyphase_sum(bank, a.up, a.down, a.Q, r, base, [&](int k) { return (float)xc[k] / 32767.0f; }, acc);
-        float* y = planes + (int64_t)(1 + c) * a.num_out;
+        polyphase_sum(bank, a.up, a.down, a.Q, r, base, [&](int k) { return staged_tap(xc[k]); }, acc);
+        float* y = planes + (int64_t)(1 + c_lo + c) * a.num_out;
 #pragma unroll
         for (int v = 0; v < RS_V; ++v) {
           const float yv = (float)acc[v];
@@ -148,28 +170,32 @@ resample_decode_pcm16_kernel(const ResamplePcmArgs a) {
           mix[v] = c == 0 ? yv : mix[v] + yv;
         }
       }
+      if (cn == C) {
 #pragma unroll
-      for (int v = 0; v < RS_V; ++v) {
-        const int64_t n = n0 + (int64_t)v * a.up;
-        if (n < a.num_out) planes[n] = mix[v] * inv;
+        for (int v = 0; v < RS_V; ++v) {
+          const int64_t n = n0 + (int64_t)v * a.up;
+          if (n < a.num_out) planes[n] = mix[v] * inv;
+        }
       }
     }
   }
 }
 
-// nsrc*C fp32 stem planes (source s, channel c at (s*C + c) * num_in) at 44.1 kHz -> int16 [nsrc][num_out][C] at the
-// clip's rate: (int16_t)(int)(y * 32767.0f) with y resample_kernel's fp32 value, the truncation of
-// pcm_encode_channels_kernel.  A tile is tp periods of cn channels of one source (cn = C unless the bank leaves too
-// little room); its span is staged interleaved, cs = cn | 1 values per sample so that the staging stores and the tap loads
-// of neighbouring channels fall in different banks.  A work item is (channel, residue, RS_V periods) with the channel
-// fastest, so neighbouring lanes write neighbouring int16 values of the interleaved output.
+// nsrc*C fp32 stem planes (source s, channel c at (s*C + c) * num_in) at 44.1 kHz -> [nsrc][num_out][C] samples of
+// format FMT at the clip's rate: the format's encode of resample_kernel's fp32 value y (for int16 (int16_t)(int)(y *
+// 32767.0f), the truncation of pcm_encode_channels_kernel).  A tile is tp periods of cn channels of one source (cn = C
+// unless the bank leaves too little room); its span is staged interleaved, cs = cn | 1 values per sample so that the
+// staging stores and the tap loads of neighbouring channels fall in different banks.  A work item is (channel, residue,
+// RS_V periods) with the channel fastest, so neighbouring lanes write neighbouring values of the interleaved output.
+template <int FMT>
 __global__ void __launch_bounds__(RS_THREADS)
-resample_encode_pcm16_kernel(const ResamplePcmArgs a) {
+resample_encode_kernel(const ResamplePcmArgs a) {
+  using Out = typename SampleFormat<FMT>::T;
   extern __shared__ __align__(16) unsigned char rs_smem[];
   double* bank = reinterpret_cast<double*>(rs_smem);
   float* xs = reinterpret_cast<float*>(bank + (size_t)a.Q * a.up);
   const float* __restrict__ stems = static_cast<const float*>(a.in);
-  int16_t* __restrict__ out = static_cast<int16_t*>(a.out);
+  Out* __restrict__ out = static_cast<Out*>(a.out);
   for (int k = threadIdx.x; k < a.Q * a.up; k += RS_THREADS) bank[k] = __ldg(a.bank + k);
   const int C = a.C, cs = a.cs, groups = (C + a.cn - 1) / a.cn;
   for (int64_t tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
@@ -187,7 +213,7 @@ resample_encode_pcm16_kernel(const ResamplePcmArgs a) {
     }
     __syncthreads();
     const int items = cn * a.up * (a.tp / RS_V);
-    int16_t* __restrict__ o = out + (int64_t)s * a.num_out * C + c_lo;
+    Out* __restrict__ o = out + (int64_t)s * a.num_out * C + c_lo;
     for (int w = threadIdx.x; w < items; w += RS_THREADS) {
       const int c = w % cn, rg = w / cn;
       const int r = rg % a.up, g = rg / a.up;
@@ -200,7 +226,7 @@ resample_encode_pcm16_kernel(const ResamplePcmArgs a) {
 #pragma unroll
       for (int v = 0; v < RS_V; ++v) {
         const int64_t n = n0 + (int64_t)v * a.up;
-        if (n < a.num_out) o[n * C + c] = (int16_t)(int)((float)acc[v] * 32767.0f);
+        if (n < a.num_out) o[n * C + c] = SampleFormat<FMT>::encode((float)acc[v]);
       }
     }
   }
@@ -217,17 +243,19 @@ static int64_t gcd64(int64_t a, int64_t b) {
 
 namespace dcs {
 
-// the tile of a fused int16 kernel for C channels: periods per tile (a multiple of RS_V, no more work items than 4
-// rounds of the CTA, counting each channel's outputs for the encode), channels per tile and staged values per sample;
-// false when even RS_V periods of one channel do not fit next to the bank
+// the tile of a fused kernel for C channels: periods per tile (a multiple of RS_V, no more work items than 4 rounds of
+// the CTA, counting each channel's outputs for the encode), channels per tile and staged values per sample; false when
+// even RS_V periods of one channel do not fit next to the bank.  The encode stages fp32 stems whatever the format.
+// The int16 decode stages int16 and keeps all C channels in one tile (it forms the downmix); the 4-byte decodes stage
+// fp32 and, like the encode, take the fewest equal channel groups that fit
 struct PcmPlan { int tp, span, cn, cs; size_t smem; };
 
-static bool pcm_plan(const dcs_resampler* r, int C, bool encode, PcmPlan* pl) {
+static bool pcm_plan(const dcs_resampler* r, int C, bool encode, int fmt, PcmPlan* pl) {
   const int64_t bank = (int64_t)r->Q * r->up * (int64_t)sizeof(double);
-  const int64_t bytes = encode ? (int64_t)sizeof(float) : (int64_t)sizeof(int16_t);
-  // encode: the fewest equal channel groups that fit; decode: all C channels in one tile (it forms the downmix)
-  for (int groups = 1; groups <= (encode ? C : 1); ++groups) {
-    const int cn = encode ? (C + groups - 1) / groups : C;
+  const bool wide = encode || fmt != DCS_SAMPLE_I16;
+  const int64_t bytes = wide ? (int64_t)sizeof(float) : (int64_t)sizeof(int16_t);
+  for (int groups = 1; groups <= (wide ? C : 1); ++groups) {
+    const int cn = (C + groups - 1) / groups;
     const int cs = encode ? (cn | 1) : cn;
     const int64_t per_round = (int64_t)r->up * (encode ? cn : 1);
     for (int64_t tp = std::max<int64_t>(1, 4 * RS_THREADS / per_round) * RS_V; tp >= RS_V; tp -= RS_V) {
@@ -263,42 +291,62 @@ static int launch_pcm(const dcs_resampler* r, Kernel kernel, const char* scope, 
 int64_t resampler_length(const dcs_resampler* r, int64_t num_in) { return dcs_resampled_length(num_in, r->up, r->down); }
 const dcs_ctx* resampler_ctx(const dcs_resampler* r) { return r->ctx; }
 
-int check_resample_pcm16(const char* fn, const dcs_ctx* ctx, const dcs_resampler* to, const dcs_resampler* from, int C) {
+int check_resample_channels(const char* fn, const dcs_ctx* ctx, const dcs_resampler* to, const dcs_resampler* from, int C,
+                            int in_fmt) {
   DCS_REQUIRE(to && from, "%s: NULL resampler", fn);
   DCS_REQUIRE(to->ctx == ctx && from->ctx == ctx, "%s: a resampler was made on another ctx", fn);
   DCS_REQUIRE(to->up == from->down && to->down == from->up,
               "%s: the resamplers %d/%d and %d/%d are not inverse (to_model up/down must be from_model down/up)", fn,
               to->up, to->down, from->up, from->down);
   PcmPlan pl;
-  DCS_REQUIRE(pcm_plan(to, C, false, &pl), "%s: %d channels at %d/%d do not fit one tile in shared memory", fn, C, to->up,
-              to->down);
-  DCS_REQUIRE(pcm_plan(from, C, true, &pl), "%s: one channel at %d/%d does not fit one tile in shared memory", fn, from->up,
-              from->down);
+  DCS_REQUIRE(pcm_plan(to, C, false, in_fmt, &pl), "%s: %d channels at %d/%d do not fit one tile in shared memory", fn, C,
+              to->up, to->down);
+  DCS_REQUIRE(pcm_plan(from, C, true, DCS_SAMPLE_F32, &pl), "%s: one channel at %d/%d does not fit one tile in shared memory",
+              fn, from->up, from->down);
   return DCS_OK;
 }
 
-int launch_resample_decode_pcm16(const dcs_resampler* r, const int16_t* d_pcm, int64_t L, int C, float* d_planes,
-                                 int64_t Lout, cudaStream_t st) {
+int resample_decode_groups(const dcs_resampler* r, int C, int fmt) {
   PcmPlan pl;
-  DCS_REQUIRE(L >= 1 && Lout >= 1 && Lout <= resampler_length(r, L) && C >= 1 && C <= 16 && pcm_plan(r, C, false, &pl),
-              "resample_decode_pcm16: bad arguments");
-  ResamplePcmArgs a;
-  a.in = d_pcm; a.num_in = L; a.out = d_planes; a.num_out = Lout; a.C = C;
-  a.tiles_t = ceil_div64(ceil_div64(Lout, r->up), pl.tp);
-  a.ntiles = a.tiles_t;
-  return launch_pcm(r, resample_decode_pcm16_kernel, "resample_decode", pl, a, st);
+  return sample_bytes(fmt) > 0 && C >= 1 && pcm_plan(r, C, false, fmt, &pl) ? (C + pl.cn - 1) / pl.cn : 0;
 }
 
-int launch_resample_encode_pcm16(const dcs_resampler* r, const float* d_stems, int64_t Lin, int nsrc, int C, int16_t* d_out,
-                                 int64_t L, cudaStream_t st) {
+int launch_resample_decode(const dcs_resampler* r, int fmt, const void* d_in, int64_t L, int C, float* d_planes, int64_t Lout,
+                           cudaStream_t st) {
   PcmPlan pl;
-  DCS_REQUIRE(Lin >= 1 && L >= 1 && L <= resampler_length(r, Lin) && nsrc >= 1 && C >= 1 && C <= 16 && pcm_plan(r, C, true, &pl),
-              "resample_encode_pcm16: bad arguments");
+  DCS_REQUIRE(L >= 1 && Lout >= 1 && Lout <= resampler_length(r, L) && C >= 1 && C <= 16 && sample_bytes(fmt) > 0 &&
+                  pcm_plan(r, C, false, fmt, &pl),
+              "resample_decode: bad arguments");
+  ResamplePcmArgs a;
+  a.in = d_in; a.num_in = L; a.out = d_planes; a.num_out = Lout; a.C = C;
+  const int groups = (C + pl.cn - 1) / pl.cn;
+  a.tiles_t = ceil_div64(ceil_div64(Lout, r->up), pl.tp);
+  a.ntiles = a.tiles_t * groups;
+  switch (fmt) {
+    case DCS_SAMPLE_I16: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_I16>, "resample_decode", pl, a, st)); break;
+    case DCS_SAMPLE_I32: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_I32>, "resample_decode", pl, a, st)); break;
+    default: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_F32>, "resample_decode", pl, a, st)); break;
+  }
+  if (groups == 1) return DCS_OK;
+  ProfScope ps(r->ctx, "resample_decode_downmix", st);   // the channel groups' downmix: the same expression, the same bits
+  return launch_downmix(r->ctx, d_planes + Lout, C, Lout, Lout, d_planes, st);
+}
+
+int launch_resample_encode(const dcs_resampler* r, int fmt, const float* d_stems, int64_t Lin, int nsrc, int C, void* d_out,
+                           int64_t L, cudaStream_t st) {
+  PcmPlan pl;
+  DCS_REQUIRE(Lin >= 1 && L >= 1 && L <= resampler_length(r, Lin) && nsrc >= 1 && C >= 1 && C <= 16 && sample_bytes(fmt) > 0 &&
+                  pcm_plan(r, C, true, fmt, &pl),
+              "resample_encode: bad arguments");
   ResamplePcmArgs a;
   a.in = d_stems; a.num_in = Lin; a.out = d_out; a.num_out = L; a.C = C;
   a.tiles_t = ceil_div64(ceil_div64(L, r->up), pl.tp);
   a.ntiles = a.tiles_t * ((C + pl.cn - 1) / pl.cn) * nsrc;
-  return launch_pcm(r, resample_encode_pcm16_kernel, "resample_encode", pl, a, st);
+  switch (fmt) {
+    case DCS_SAMPLE_I16: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_I16>, "resample_encode", pl, a, st);
+    case DCS_SAMPLE_I32: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_I32>, "resample_encode", pl, a, st);
+    default: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_F32>, "resample_encode", pl, a, st);
+  }
 }
 
 }  // namespace dcs

@@ -208,18 +208,21 @@ __global__ void pcm_encode_kernel(const float* __restrict__ stems, int64_t L, in
   out[(int64_t)s * out_stride + i] = (int16_t)(int)v;
 }
 
-// C-channel stems: interleaved int16 [L][C] -> C + 1 float planes L apart: the downmix, then channel c at plane 1 + c.
-// Each channel is pcm / 32767 and the downmix is downmix_kernel's expression on those planes, so at C = 2 it is
-// pcm_decode_kernel's downmix 1 and the network sees what the mono call would see
-__global__ void pcm_decode_channels_kernel(const int16_t* __restrict__ pcm, int64_t L, int C, float* __restrict__ planes) {
+// C-channel stems: interleaved [L][C] samples of format FMT -> C + 1 float planes L apart: the downmix, then channel c at
+// plane 1 + c.  Each channel is the format's decode (pcm / 32767 for int16) and the downmix is downmix_kernel's
+// expression on those planes, so at C = 2 in int16 it is pcm_decode_kernel's downmix 1 and the network sees what the
+// mono call would see
+template <int FMT>
+__global__ void pcm_decode_channels_kernel(const typename SampleFormat<FMT>::T* __restrict__ pcm, int64_t L, int C,
+                                           float* __restrict__ planes) {
+  using S = SampleFormat<FMT>;
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= L) return;
-  const float maxv = 32767.0f;
-  const int16_t* row = pcm + i * C;
-  float a = (float)row[0] / maxv;
+  const typename S::T* row = pcm + i * C;
+  float a = S::decode(row[0]);
   planes[L + i] = a;
   for (int c = 1; c < C; ++c) {
-    const float v = (float)row[c] / maxv;
+    const float v = S::decode(row[c]);
     planes[(int64_t)(1 + c) * L + i] = v;
     a += v;
   }
@@ -239,31 +242,39 @@ __global__ void downmix_kernel(const float* __restrict__ audio, int nx, int64_t 
 constexpr int kPcmEncodeRows = 256;   // rows (samples) of one CTA's tile, one per thread
 constexpr int kPcmMaxChannels = 16;
 
-// stem planes (source s, channel c) at stems + (s C + c) * stem_stride -> int16 [nsrc][L][C] (what
-// scipy.io.wavfile.write takes for a C-channel stem), source s at out + s C L, the truncation rule of
-// pcm_encode_kernel; grid (ceil(L / 256), nsrc).  A thread's C samples are not an aligned vector for most C, so the
-// tile of 256 interleaved rows is staged in shared memory at the byte offset its destination has modulo 16: the
-// 16-byte-aligned middle of the destination then meets 16-byte-aligned shared memory, and each warp stores 512
-// contiguous bytes with 16-byte stores.  The up to 7 values before the first and after the last aligned piece (a
-// source's rows start at s C L 2 bytes, not always a multiple of 16) go out one int16 at a time.
+// stem planes (source s, channel c) at stems + (s C + c) * stem_stride -> [nsrc][L][C] samples of format FMT (what
+// scipy.io.wavfile.write takes for a C-channel stem), source s at out + s C L, the format's encode (for int16 the
+// truncation rule of pcm_encode_kernel); grid (ceil(L / 256), nsrc).  A thread's C samples are not an aligned vector
+// for most C, so the tile of 256 interleaved rows is staged in shared memory at the byte offset its destination has
+// modulo 16: the 16-byte-aligned middle of the destination then meets 16-byte-aligned shared memory, and each warp
+// stores 512 contiguous bytes with 16-byte stores.  The up to 16 / b - 1 values (b bytes each) before the first and
+// after the last aligned piece (a source's rows start at s C L b bytes, not always a multiple of 16) go out one value
+// at a time.  The shift is counted in values: 2-byte units for int16, 4-byte units otherwise (the output is then
+// 4-byte aligned).
+template <int FMT>
 __global__ void __launch_bounds__(kPcmEncodeRows)
-pcm_encode_channels_kernel(const float* __restrict__ stems, int64_t L, int C, int64_t stem_stride, int16_t* __restrict__ out) {
-  __shared__ __align__(16) int16_t tile[kPcmEncodeRows * kPcmMaxChannels + 8];
+pcm_encode_channels_kernel(const float* __restrict__ stems, int64_t L, int C, int64_t stem_stride,
+                           typename SampleFormat<FMT>::T* __restrict__ out) {
+  using S = SampleFormat<FMT>;
+  using T = typename S::T;
+  constexpr int kLog2B = sizeof(T) == 2 ? 1 : 2;                    // log2 of the bytes per value
+  constexpr int kV = 16 >> kLog2B;                                  // values per 16 bytes
+  __shared__ __align__(16) T tile[kPcmEncodeRows * kPcmMaxChannels + kV];
   const int s = blockIdx.y;
   const int64_t i0 = (int64_t)blockIdx.x * kPcmEncodeRows;
   const int rows = (int)(L - i0 < kPcmEncodeRows ? L - i0 : kPcmEncodeRows);
-  int16_t* dst = out + ((int64_t)s * L + i0) * C;                   // the tile's first value
-  const int shift = (int)(((uintptr_t)dst & 15) >> 1);              // in int16 values
+  T* dst = out + ((int64_t)s * L + i0) * C;                         // the tile's first value
+  const int shift = (int)(((uintptr_t)dst & 15) >> kLog2B);         // in values
   if ((int)threadIdx.x < rows) {
     const float* src = stems + (int64_t)s * C * stem_stride + i0 + threadIdx.x;
     for (int c = 0; c < C; ++c)
-      tile[shift + threadIdx.x * C + c] = (int16_t)(int)(src[(int64_t)c * stem_stride] * 32767.0f);
+      tile[shift + threadIdx.x * C + c] = S::encode(src[(int64_t)c * stem_stride]);
   }
   __syncthreads();
   const int n = rows * C;                                           // values of the tile
-  const int head = min(n, (8 - shift) & 7);                         // values before the first 16-byte boundary
-  const int nvec = (n - head) >> 3;
-  const int tail0 = head + nvec * 8;
+  const int head = min(n, (kV - shift) & (kV - 1));                 // values before the first 16-byte boundary
+  const int nvec = (n - head) >> (4 - kLog2B);
+  const int tail0 = head + nvec * kV;
   const uint4* vsrc = reinterpret_cast<const uint4*>(tile + shift + head);
   uint4* vdst = reinterpret_cast<uint4*>(dst + head);
   for (int k = threadIdx.x; k < nvec; k += kPcmEncodeRows) vdst[k] = vsrc[k];
@@ -359,10 +370,30 @@ int launch_pcm_decode(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int channel
   return DCS_OK;
 }
 
-int launch_pcm_decode_channels(dcs_ctx* ctx, const int16_t* d_pcm, int64_t L, int C, float* d_planes, cudaStream_t st) {
+template <int FMT>
+static void pcm_decode_channels_as(const void* d_in, int64_t L, int C, float* d_planes, cudaStream_t st) {
+  pcm_decode_channels_kernel<FMT><<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(
+      static_cast<const typename SampleFormat<FMT>::T*>(d_in), L, C, d_planes);
+}
+
+template <int FMT>
+static void pcm_encode_channels_as(const float* d_stems, int64_t L, int nsrc, int C, int64_t stem_stride, void* d_out,
+                                   cudaStream_t st) {
+  dim3 grid((unsigned)ceil_div64(L, kPcmEncodeRows), (unsigned)nsrc);
+  pcm_encode_channels_kernel<FMT><<<grid, kPcmEncodeRows, 0, st>>>(d_stems, L, C, stem_stride,
+                                                                   static_cast<typename SampleFormat<FMT>::T*>(d_out));
+}
+
+int launch_pcm_decode_channels(dcs_ctx* ctx, int fmt, const void* d_in, int64_t L, int C, float* d_planes, cudaStream_t st) {
   if (L <= 0) return DCS_OK;
   DCS_REQUIRE(C >= 1 && C <= kPcmMaxChannels, "pcm_decode_channels: %d channels not in [1, %d]", C, kPcmMaxChannels);
-  pcm_decode_channels_kernel<<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(d_pcm, L, C, d_planes);
+  DCS_REQUIRE(sample_bytes(fmt) > 0 && (uintptr_t)d_in % sample_bytes(fmt) == 0,
+              "pcm_decode_channels: format %d, or input not aligned to its samples", fmt);
+  switch (fmt) {
+    case DCS_SAMPLE_I16: pcm_decode_channels_as<DCS_SAMPLE_I16>(d_in, L, C, d_planes, st); break;
+    case DCS_SAMPLE_I32: pcm_decode_channels_as<DCS_SAMPLE_I32>(d_in, L, C, d_planes, st); break;
+    default: pcm_decode_channels_as<DCS_SAMPLE_F32>(d_in, L, C, d_planes, st); break;
+  }
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;
@@ -376,13 +407,17 @@ int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_str
   return DCS_OK;
 }
 
-int launch_pcm_encode_channels(dcs_ctx* ctx, const float* d_stems, int64_t L, int nsrc, int C, int64_t stem_stride,
-                               int16_t* d_out, cudaStream_t st) {
+int launch_pcm_encode_channels(dcs_ctx* ctx, int fmt, const float* d_stems, int64_t L, int nsrc, int C, int64_t stem_stride,
+                               void* d_out, cudaStream_t st) {
   if (L <= 0) return DCS_OK;
   DCS_REQUIRE(C >= 1 && C <= kPcmMaxChannels, "pcm_encode_channels: %d channels not in [1, %d]", C, kPcmMaxChannels);
-  DCS_REQUIRE((uintptr_t)d_out % 2 == 0, "pcm_encode_channels: output not 2-byte aligned");
-  dim3 grid((unsigned)ceil_div64(L, kPcmEncodeRows), (unsigned)nsrc);
-  pcm_encode_channels_kernel<<<grid, kPcmEncodeRows, 0, st>>>(d_stems, L, C, stem_stride, d_out);
+  DCS_REQUIRE(sample_bytes(fmt) > 0 && (uintptr_t)d_out % sample_bytes(fmt) == 0,
+              "pcm_encode_channels: format %d, or output not aligned to its samples", fmt);
+  switch (fmt) {
+    case DCS_SAMPLE_I16: pcm_encode_channels_as<DCS_SAMPLE_I16>(d_stems, L, nsrc, C, stem_stride, d_out, st); break;
+    case DCS_SAMPLE_I32: pcm_encode_channels_as<DCS_SAMPLE_I32>(d_stems, L, nsrc, C, stem_stride, d_out, st); break;
+    default: pcm_encode_channels_as<DCS_SAMPLE_F32>(d_stems, L, nsrc, C, stem_stride, d_out, st); break;
+  }
   DCS_CHECK_LAUNCH();
   ctx->launches++;
   return DCS_OK;

@@ -216,6 +216,9 @@ def score_filters(ctx, melody, T, F, start=0, mag=None, ldf=None, stream=None):
 
 # every network was trained on spectra of 44.1 kHz audio; other rates go through a Resampler
 MODEL_RATE = 44100
+# the sample formats of separate_channels_batch: numpy dtype -> DCS_SAMPLE_* (include/dcs.h)
+_SAMPLE_FORMATS = {np.dtype(np.int16): _lib.SAMPLE_I16, np.dtype(np.int32): _lib.SAMPLE_I32,
+                   np.dtype(np.float32): _lib.SAMPLE_F32}
 # the sample rates a Resampler takes: integers in this range whose polyphase bank fits, in both directions
 RESAMPLE_RATES = (8000, 192000)
 
@@ -655,6 +658,49 @@ class Separator(object):
         equal).  At another rate than MODEL_RATE (check_resample_rates) each clip is resampled to 44.1 kHz as it is
         decoded and its stems back to its own rate and length as they are encoded, on the device with this separator's
         resamplers (dcs_separate_batch_pcm16_channels_resampled_host): no more launches per clip than at 44.1 kHz."""
+        ps, ch, args, sample_rate = self._channels_clips("separate_pcm16_channels_batch", clips, (np.int16,), wiener,
+                                                         wiener_radius, sample_rate)
+        if not ps:
+            return []
+        if sample_rate == MODEL_RATE:
+            return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_channels_host, ps, outs, (ch,), args)
+        pre = (self.resampler(sample_rate, MODEL_RATE).handle, self.resampler(MODEL_RATE, sample_rate).handle)
+        return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_channels_resampled_host, ps, outs, (ch,), args, pre)
+
+    def separate_channels_batch(self, clips, outs=None, out_dtype=None, wiener=0, wiener_radius=0, sample_rate=MODEL_RATE):
+        """separate_pcm16_channels_batch for int16, int32 or float32 clips (dcs_separate_batch_channels_host): 24-bit
+        PCM as scipy.io.wavfile reads it (int32, the sample in the top 24 bits), 32-bit PCM, or IEEE float.  clips:
+        list of arrays [L, C] of one dtype and one C in 1..16 -> list of [nsrc, L, C] arrays of out_dtype (default the
+        clips' dtype; int16, int32 or float32), into `outs` when given.  Per clip the stems are
+        encode(separate_channels(decode(clip), wiener, wiener_radius, sample_rate)), with the rules of include/dcs.h:
+        int16 decodes as clip / 32767 and encodes as (stem * 32767) truncated in fp32, wrapping; int32 decodes as
+        (clip / (2^31 - 1)) in fp64 rounded to fp32 and encodes as stem * (2^31 - 1) in fp64, truncated and saturated;
+        float32 is taken and given back as it is, without scaling or clipping.  The conversions run on the device, fused
+        into the resamplers at another rate.  With int16 in and out, the bytes of separate_pcm16_channels_batch."""
+        ps, ch, args, sample_rate = self._channels_clips("separate_channels_batch", clips, tuple(_SAMPLE_FORMATS), wiener,
+                                                         wiener_radius, sample_rate)
+        dtypes = {p_.dtype for p_ in ps}
+        if len(dtypes) > 1:
+            raise ValueError("all clips of a batch must have the same dtype, got %s" % sorted(str(d) for d in dtypes))
+        in_dtype = ps[0].dtype if ps else np.dtype(np.int16)
+        try:
+            out_dtype = in_dtype if out_dtype is None else np.dtype(out_dtype)
+        except TypeError:
+            raise ValueError("separate_channels_batch: out_dtype %r is not a dtype" % (out_dtype,))
+        if out_dtype not in _SAMPLE_FORMATS:
+            raise ValueError("separate_channels_batch encodes int16, int32 or float32 stems, not %s" % out_dtype)
+        if not ps:
+            return []
+        pre = (None, None)
+        if sample_rate != MODEL_RATE:
+            pre = (self.resampler(sample_rate, MODEL_RATE).handle, self.resampler(MODEL_RATE, sample_rate).handle)
+        pre += (_SAMPLE_FORMATS[in_dtype], _SAMPLE_FORMATS[out_dtype])
+        return self._pcm16_batch(self.lib.dcs_separate_batch_channels_host, ps, outs, (ch,), args, pre, out_dtype)
+
+    def _channels_clips(self, call, clips, dtypes, wiener, wiener_radius, sample_rate):
+        """the checks of the C-channel batch calls, before any library call: the network, the filter options, clips
+        [L, C] of one of `dtypes` with one C in 1..16, one sample rate -> (contiguous clips, C, the entry's arguments
+        between the clip lengths and scale_factor, the rate)"""
         check_channels_family(self.model.arch)
         check_wiener_radius(wiener, wiener_radius)
         if wiener < 0:
@@ -662,41 +708,37 @@ class Separator(object):
         ps = []
         for c in clips:
             a = np.asarray(c)
-            if a.dtype != np.int16 or a.ndim != 2:
-                raise ValueError("separate_pcm16_channels_batch needs int16 clips [L, C], got %s %r" % (a.dtype, a.shape))
+            if a.dtype not in dtypes or a.ndim != 2:
+                raise ValueError("%s needs %s clips [L, C], got %s %r"
+                                 % (call, " or ".join(str(np.dtype(d)) for d in dtypes), a.dtype, a.shape))
             ps.append(np.ascontiguousarray(a))
         if not np.isscalar(sample_rate):
             rates = list(sample_rate)
             if len(rates) != len(ps) or any(r != rates[0] for r in rates):
-                raise ValueError("separate_pcm16_channels_batch takes one sample rate per call, got %r for %d clips"
-                                 % (rates, len(ps)))
+                raise ValueError("%s takes one sample rate per call, got %r for %d clips" % (call, rates, len(ps)))
             sample_rate = rates[0] if rates else MODEL_RATE
         if sample_rate != MODEL_RATE:
             check_resample_rates(sample_rate, MODEL_RATE)   # the rate is refused before any library call
         if not ps:
-            return []
+            return ps, 0, (), sample_rate
         ch = ps[0].shape[1]
         if any(p_.shape[1] != ch for p_ in ps):
             raise ValueError("all clips of a batch must have the same channel count, got %r" % sorted({p_.shape[1] for p_ in ps}))
         if not 1 <= ch <= 16:
-            raise ValueError("separate_pcm16_channels_batch takes 1 to 16 channels, got %d" % ch)
+            raise ValueError("%s takes 1 to 16 channels, got %d" % (call, ch))
         if wiener:
             check_wiener_channels(ch)
-        args = (ch, int(wiener), int(wiener_radius))
-        if sample_rate == MODEL_RATE:
-            return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_channels_host, ps, outs, (ch,), args)
-        pre = (self.resampler(sample_rate, MODEL_RATE).handle, self.resampler(MODEL_RATE, sample_rate).handle)
-        return self._pcm16_batch(self.lib.dcs_separate_batch_pcm16_channels_resampled_host, ps, outs, (ch,), args, pre)
+        return ps, ch, (ch, int(wiener), int(wiener_radius)), sample_rate
 
-    def _pcm16_batch(self, entry, ps, outs, channels, args, pre=()):
-        """int16 clips ps through the multi-clip entry point `entry` -> outs, int16 [nsrc, L, *channels] each (made
-        when None).  args: the entry's arguments between the clip lengths and scale_factor; pre: those between the
-        plan and the clip count."""
+    def _pcm16_batch(self, entry, ps, outs, channels, args, pre=(), dtype=np.int16):
+        """clips ps through the multi-clip entry point `entry` -> outs, `dtype` [nsrc, L, *channels] each (made when
+        None).  args: the entry's arguments between the clip lengths and scale_factor; pre: those between the plan and
+        the clip count."""
         n = len(ps)
         Ls = np.array([p_.shape[0] for p_ in ps], dtype=np.int64)
         if outs is None:
-            outs = [np.empty((self.nsrc, int(L)) + channels, dtype=np.int16) for L in Ls]
-        assert all(o.dtype == np.int16 and o.shape == (self.nsrc, int(L)) + channels and o.flags.c_contiguous
+            outs = [np.empty((self.nsrc, int(L)) + channels, dtype=dtype) for L in Ls]
+        assert all(o.dtype == dtype and o.shape == (self.nsrc, int(L)) + channels and o.flags.c_contiguous
                    for o, L in zip(outs, Ls))
         pin = (C.c_void_p * n)(*[p_.ctypes.data for p_ in ps])
         pout = (C.c_void_p * n)(*[o.ctypes.data for o in outs])

@@ -690,6 +690,64 @@ int dcs_pcm16_encode(dcs_ctx* ctx, const dcs_resampler* resampler, int mode, con
 int dcs_downmix_f32(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t num_samples, float* d_mono,
                     void* stream);
 
+/* ---- C-channel clips in int16, int32 or float32 --------------------------------------------------------------- */
+/* Sample formats of dcs_separate_batch_channels_host and of its conversions.  A sample decodes to the fp32 plane the
+ * networks see, and an fp32 stem value y encodes back:
+ *  - DCS_SAMPLE_I16 (2 bytes): decode pcm / 32767.0f; encode (int16)(int)(y * 32767.0f), the product in fp32, C
+ *    truncation, wrapping modulo 2^16 (NaN gives 0, saturating to int32 first beyond +-2^31): the rule of
+ *    dcs_separate_pcm16_host.
+ *  - DCS_SAMPLE_I32 (4 bytes; 24-bit PCM as scipy.io.wavfile reads it, the sample in the top 24 bits): decode
+ *    (float)((double)pcm / 2147483647.0), each step rounded to nearest (the bits of
+ *    (a.astype(float) / iinfo(int32).max).astype(float32)); encode (double)y * 2147483647.0 in fp64, truncated toward
+ *    zero and saturated to [-2^31, 2^31 - 1] (__double2int_rz), NaN gives 0 (tested first: the f64 conversion alone
+ *    would give -2^31).  It saturates where int16 wraps: the wrap
+ *    only reproduces the reference's astype('int16'), and numpy's own int32 result past 2^31 depends on the platform.
+ *  - DCS_SAMPLE_F32 (4 bytes): decode the sample itself, bit for bit (no scaling); encode y itself, bit for bit (no
+ *    clipping, NaN payloads kept).  Non-finite input gives undefined stems and is not checked, as on every float entry.
+ * The downmix is that of dcs_separate_audio_channels on the decoded planes in every format. */
+enum { DCS_SAMPLE_I16 = 0, DCS_SAMPLE_I32 = 1, DCS_SAMPLE_F32 = 2 };
+/* C-channel clips (1 to 16 channels) in any sample format through the multi-clip scheduler: the clips in in_format, the
+ * stems in out_format, chosen independently.  h_in[i]: [num_samples[i]][channels] samples of in_format (pinned for real
+ * overlap) -> source s of clip i at h_out[i] + s*channels*out_strides[i] samples as [num_samples[i]][channels] of
+ * out_format, interleaved: the layouts of dcs_separate_batch_pcm16_channels_host with each value 2 or 4 bytes wide.
+ * to_model and from_model are both NULL (clips at 44.1 kHz) or both set (clips at another rate, the pair of
+ * dcs_separate_batch_pcm16_channels_resampled_host, with its checks).  Per clip the stems are, byte for byte,
+ *     encode_out(dcs_separate_audio_channels_wiener(decode_in(clip), iterations, radius))
+ * at 44.1 kHz, and at another rate encode_out of dcs_resample(from_model, num_out = L) of the stems of that call on
+ * dcs_resample(to_model) of decode_in(clip), per channel.  With DCS_SAMPLE_I16 in and out these are the bytes of
+ * dcs_separate_batch_pcm16_channels_host and dcs_separate_batch_pcm16_channels_resampled_host.
+ * Launches per clip: those of dcs_separate_audio_channels(_wiener) on the clip at 44.1 kHz plus one, in every format.
+ * At another rate, a 4-byte in_format stages each decode tile as fp32; where C channels then do not fit one tile next
+ * to the bank (C >= 11 at some rates, 192 kHz at C = 16 among them) the decode runs on equal channel groups and one
+ * more launch forms the downmix plane, with the same bits.
+ * Workspace: as for dcs_separate_batch_pcm16_channels_host (resampled_host at another rate) with the staging terms
+ *       n B(b_in channels Lmax) + n B(b_out nsrc channels Lmax)
+ * where b_in and b_out are the formats' bytes per sample (2 or 4).
+ * Synchronises before returning, also on an error.  Refused with DCS_EINVAL before anything is queued: an unknown
+ * format code, exactly one resampler NULL, and what the two int16 C-channel batch entries refuse. */
+int dcs_separate_batch_channels_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const dcs_resampler* to_model,
+                                     const dcs_resampler* from_model, int in_format, int out_format, int nclips,
+                                     const void* const* h_in, const int64_t* num_samples, int channels, int iterations,
+                                     int radius, float scale_factor, int overlap, int patcher, void* const* h_out,
+                                     const int64_t* out_strides, void* stream);
+/* Bring-up and test entries: the conversions of dcs_separate_batch_channels_host, the C-channel layout of
+ * dcs_pcm16_decode / dcs_pcm16_encode (DCS_PCM16_CHANNELS) in any format, with the same arguments and checks.  Each is
+ * one launch of the kernel the batch runs (two for a resampled decode whose channels take groups), on caller device
+ * buffers, on `stream`, which is synchronised before returning; every argument is checked before anything is queued.
+ * 4-byte formats need 4-byte-aligned d_in / d_out.
+ * dcs_channels_decode: d_in [num_samples][channels] of `format` -> d_out float [channels + 1][num_out], plane 0 the
+ *  downmix, plane 1 + c the decode of channel c; with a resampler, dcs_resample of it and num_out in
+ *  [1, dcs_resampled_length(num_samples)].
+ * dcs_channels_encode: nsrc * channels fp32 planes (source, channel) stem_stride apart -> source s at
+ *  d_out + s * out_stride samples as [num_out][channels] of `format`, out_stride = channels * num_out; with a resampler
+ *  the planes are the encode of dcs_resample(num_out) of each plane, stem_stride = num_in.  Nothing outside the values
+ *  listed is written. */
+int dcs_channels_decode(dcs_ctx* ctx, const dcs_resampler* resampler, int format, const void* d_in, int64_t num_samples,
+                        int channels, float* d_out, int64_t num_out, void* stream);
+int dcs_channels_encode(dcs_ctx* ctx, const dcs_resampler* resampler, int format, const float* d_stems, int64_t num_in,
+                        int nsrc, int channels, int64_t stem_stride, void* d_out, int64_t num_out, int64_t out_stride,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif
