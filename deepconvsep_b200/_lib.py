@@ -95,11 +95,24 @@ _SIGS = {
                                                    C.c_int, C.c_float, C.c_int, C.c_int, _p, _p, _p]),
     "dcs_channels_decode": (C.c_int, [_p, _p, C.c_int, _p, _i64, C.c_int, _p, _i64, _p]),
     "dcs_channels_encode": (C.c_int, [_p, _p, C.c_int, _p, _i64, C.c_int, C.c_int, _i64, _p, _i64, _i64, _p]),
+    "dcs_long_segments": (_i64, [_i64, _i64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                 _p, _i64]),
+    "dcs_separate_long_channels_host": (C.c_int, [_p, _p, _p, _p, _p, C.c_int, C.c_int, _p, _i64, C.c_int, C.c_int, C.c_int,
+                                                  _i64, C.c_float, C.c_int, C.c_int, _p, _i64, _p]),
+    "dcs_channels_decode_range": (C.c_int, [_p, _p, C.c_int, _p, _i64, _i64, _i64, C.c_int, _p, _i64, _i64, _p]),
+    "dcs_channels_encode_range": (C.c_int, [_p, _p, C.c_int, _p, _i64, _i64, _i64, C.c_int, C.c_int, _p, _i64, _i64, _i64,
+                                            _p]),
 }
 # modes of dcs_pcm16_decode / dcs_pcm16_encode beside the downmix 0..2 (include/dcs.h)
 PCM16_MONO, PCM16_CHANNELS = 0, 3
 # sample formats of dcs_separate_batch_channels_host (DCS_SAMPLE_*, include/dcs.h)
 SAMPLE_I16, SAMPLE_I32, SAMPLE_F32 = 0, 1, 2
+
+
+class Segment(C.Structure):
+    """dcs_segment (include/dcs.h): the in, model and kept ranges of one segment of a long recording."""
+    _fields_ = [("in_start", _i64), ("in_stop", _i64), ("model_start", _i64), ("model_stop", _i64),
+                ("out_start", _i64), ("out_stop", _i64)]
 
 
 

@@ -950,6 +950,17 @@ int dcs_separate_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const int16
                                        &out_stride, stream);
 }
 
+// A clip of the pipeline is a PipeClip: a whole clip (seg NULL), or one segment of a long recording (nx > 0): its in
+// range staged, its model range separated, its kept core encoded and copied into the recording's stems at out_start.
+struct PipeClip {
+  const void* in;            // staged samples: the clip, or the segment's in range
+  int64_t n_in;              // their count
+  void* out;                 // the stems' first kept sample (source 0)
+  int64_t out_stride;        // samples (of nx channels) from one source's stems to the next
+  const dcs_segment* seg;    // the segment, or NULL
+  int64_t rec_len;           // the recording's samples (segments only)
+};
+
 // Multi-clip scheduler: the clips of a batch run through ONE context as a three-stage pipeline -- H2D of clip i+1
 // (copy stream) | kernels of clip i (the caller's stream) | D2H of clip i-1 (second copy stream) -- with double-buffered
 // int16 staging on the device and events for the hand-overs.  The reference's only multi-clip driver starts a Python
@@ -964,11 +975,13 @@ int dcs_separate_pcm16_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const int16
 // decode resamples it to L' = resampler_length(to, L) samples, the clip is separated at L', and the encode resamples its
 // stems back to L
 static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to, const dcs_resampler* from,
-                          int in_fmt, int out_fmt, int nclips, const void* const* h_in, const int64_t* num_samples,
-                          int channels, int downmix, int nx, int iterations, int radius, float scale_factor, int overlap,
-                          int patcher, void* const* h_out, const int64_t* out_strides, cudaStream_t st) {
+                          int in_fmt, int out_fmt, int nclips, const PipeClip* clips, int channels, int downmix, int nx,
+                          int iterations, int radius, float scale_factor, int overlap, int patcher, cudaStream_t st) {
   const size_t bi = (size_t)sample_bytes(in_fmt), bo = (size_t)sample_bytes(out_fmt);
   const size_t w = (size_t)(nx > 0 ? nx : 1) * bo;   // bytes per sample of a stem
+  int pitch_attr = 0;
+  DCS_CUDA(cudaDeviceGetAttribute(&pitch_attr, cudaDevAttrMaxPitch, ctx->device));
+  const size_t max_pitch = (size_t)pitch_attr;
   float *audio = ctx->audio.as<float>(), *stems = ctx->stems.as<float>();
   // the copy streams start after whatever the caller queued on `st` (and after the memsets of fresh buffers)
   DCS_CUDA(cudaEventRecord(ctx->ev_dec[0], st));
@@ -976,16 +989,24 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_res
   DCS_CUDA(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_dec[0], 0));
   for (int i = 0; i < nclips; ++i) {
     const int b = i & 1;
-    const int64_t L = num_samples[i];
+    const PipeClip& cl = clips[i];
+    const dcs_segment* sg = cl.seg;
+    const int64_t L = cl.n_in;
     // H2D of clip i: its staging buffer is free once the decode of clip i-2 has read it
     if (i >= 2) DCS_CUDA(cudaStreamWaitEvent(ctx->s_h2d, ctx->ev_dec[b], 0));
-    DCS_CUDA(cudaMemcpyAsync(ctx->pcm_in[b].p, h_in[i], (size_t)L * channels * bi, cudaMemcpyHostToDevice, ctx->s_h2d));
+    DCS_CUDA(cudaMemcpyAsync(ctx->pcm_in[b].p, cl.in, (size_t)L * channels * bi, cudaMemcpyHostToDevice, ctx->s_h2d));
     DCS_CUDA(cudaEventRecord(ctx->ev_in[b], ctx->s_h2d));
     // kernels of clip i
     DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_in[b], 0));
-    const int64_t Lm = to ? resampler_length(to, L) : L;   // the clip's samples at the networks' rate
+    // the clip's samples at the networks' rate (a segment: its model range) and the samples kept
+    const int64_t Lm = sg ? sg->model_stop - sg->model_start : to ? resampler_length(to, L) : L;
+    const int64_t K = sg ? sg->out_stop - sg->out_start : L;
     if (to) {
-      DCS_TRY(launch_resample_decode(to, in_fmt, ctx->pcm_in[b].p, L, nx, audio, Lm, st));
+      if (sg)
+        DCS_TRY(launch_resample_decode_range(to, in_fmt, ctx->pcm_in[b].p, cl.rec_len, sg->in_start, L, nx, audio,
+                                             sg->model_start, Lm, st));
+      else
+        DCS_TRY(launch_resample_decode(to, in_fmt, ctx->pcm_in[b].p, L, nx, audio, Lm, st));
       DCS_CUDA(cudaEventRecord(ctx->ev_dec[b], st));
       ProfScope ps(ctx, "pcm16_separate", st);
       DCS_TRY(downmix_clip(ctx, m, p, audio, audio + Lm, nx, Lm, Lm, iterations, radius, scale_factor, overlap, patcher, stems,
@@ -1004,19 +1025,69 @@ static int batch_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_res
     }
     if (i >= 2) DCS_CUDA(cudaStreamWaitEvent(st, ctx->ev_out[b], 0));     // D2H of clip i-2 has drained the output staging
     if (from) {
-      DCS_TRY(launch_resample_encode(from, out_fmt, stems, Lm, m->nsrc, nx, ctx->pcm_out[b].p, L, st));
+      if (sg)
+        DCS_TRY(launch_resample_encode_range(from, out_fmt, stems, resampler_length(to, cl.rec_len), sg->model_start, Lm,
+                                             m->nsrc, nx, ctx->pcm_out[b].p, sg->out_start, K, st));
+      else
+        DCS_TRY(launch_resample_encode(from, out_fmt, stems, Lm, m->nsrc, nx, ctx->pcm_out[b].p, L, st));
     } else if (nx > 0) {
-      ProfScope ps(ctx, "pcm16_encode", st);
-      DCS_TRY(launch_pcm_encode_channels(ctx, out_fmt, stems, L, m->nsrc, nx, L, ctx->pcm_out[b].p, st));
+      ProfScope ps(ctx, "pcm16_encode", st);   // a segment: its kept core of the stem planes, Lm apart
+      DCS_TRY(launch_pcm_encode_channels(ctx, out_fmt, stems + (sg ? sg->out_start - sg->model_start : 0), K, m->nsrc, nx, Lm,
+                                         ctx->pcm_out[b].p, st));
     } else
       DCS_TRY(launch_pcm_encode(ctx, stems, L, m->nsrc, L, ctx->pcm_out[b].as<int16_t>(), L, st));
     DCS_CUDA(cudaEventRecord(ctx->ev_enc[b], st));
     // D2H of clip i
     DCS_CUDA(cudaStreamWaitEvent(ctx->s_d2h, ctx->ev_enc[b], 0));
-    DCS_CUDA(cudaMemcpy2DAsync(h_out[i], w * out_strides[i], ctx->pcm_out[b].p, w * L, w * L, m->nsrc, cudaMemcpyDeviceToHost,
-                               ctx->s_d2h));
+    // one 2-D copy, rows = sources; a pitch over the device's limit (cudaDevAttrMaxPitch, 2^31 - 1 bytes: one source of a
+    // long recording's stems can span more) takes one copy per source instead
+    if (w * cl.out_stride <= max_pitch) {
+      DCS_CUDA(cudaMemcpy2DAsync(cl.out, w * cl.out_stride, ctx->pcm_out[b].p, w * K, w * K, m->nsrc, cudaMemcpyDeviceToHost,
+                                 ctx->s_d2h));
+    } else {
+      for (int s = 0; s < m->nsrc; ++s)
+        DCS_CUDA(cudaMemcpyAsync((char*)cl.out + s * w * cl.out_stride, ctx->pcm_out[b].as<char>() + s * w * K, w * K,
+                                 cudaMemcpyDeviceToHost, ctx->s_d2h));
+    }
     DCS_CUDA(cudaEventRecord(ctx->ev_out[b], ctx->s_d2h));
   }
+  return DCS_OK;
+}
+
+// the resources, sizing and drain around batch_pipeline: streams and events made once per ctx, every buffer sized before
+// the pipeline starts (a grow-only buffer re-allocated mid-batch would synchronise the stream) from the longest staged
+// input (Smax samples), the longest clip at the networks' rate (Swork) and the most samples kept of a clip (Kmax)
+static int run_pipeline(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to, const dcs_resampler* from, int in_fmt,
+                        int out_fmt, const std::vector<PipeClip>& clips, int channels, int downmix, int nx, int iterations,
+                        int radius, float scale_factor, int overlap, int patcher, int64_t Smax, int64_t Swork, int64_t Kmax,
+                        cudaStream_t st) {
+  const int nclips = (int)clips.size();
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  // each resource on its own: a call that failed half-way through this block must not leave later calls with null handles
+  if (!ctx->s_h2d) DCS_CUDA(cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
+  if (!ctx->s_d2h) DCS_CUDA(cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking));
+  for (int i = 0; i < 2; ++i) {
+    if (!ctx->ev_in[i]) DCS_CUDA(cudaEventCreateWithFlags(&ctx->ev_in[i], cudaEventDisableTiming));
+    if (!ctx->ev_dec[i]) DCS_CUDA(cudaEventCreateWithFlags(&ctx->ev_dec[i], cudaEventDisableTiming));
+    if (!ctx->ev_enc[i]) DCS_CUDA(cudaEventCreateWithFlags(&ctx->ev_enc[i], cudaEventDisableTiming));
+    if (!ctx->ev_out[i]) DCS_CUDA(cudaEventCreateWithFlags(&ctx->ev_out[i], cudaEventDisableTiming));
+  }
+  for (int b = 0; b < std::min(nclips, 2); ++b) {
+    DCS_TRY(ctx->pcm_in[b].ensure((size_t)Smax * channels * sample_bytes(in_fmt), st));
+    DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * (nx > 0 ? nx : 1) * Kmax * sample_bytes(out_fmt), st));
+  }
+  if (nx > 0)
+    DCS_TRY(size_downmix_workspace(ctx, m, p, Swork, iterations > 0 ? nx : 0, radius, nx, st));
+  else
+    DCS_TRY(size_workspace(ctx, m, p, Smax, true, st));
+  const int rc = batch_pipeline(ctx, m, p, to, from, in_fmt, out_fmt, nclips, clips.data(), channels, downmix, nx, iterations,
+                                radius, scale_factor, overlap, patcher, st);
+  // drain everything, success or not, before the host buffers go back to the caller
+  const cudaError_t e0 = cudaStreamSynchronize(ctx->s_h2d), e1 = cudaStreamSynchronize(ctx->s_d2h), e2 = cudaStreamSynchronize(st);
+  if (rc != DCS_OK) return rc;
+  DCS_CUDA(e0);
+  DCS_CUDA(e1);
+  DCS_CUDA(e2);
   return DCS_OK;
 }
 
@@ -1041,35 +1112,10 @@ static int batch_host(const char* fn, dcs_ctx* ctx, dcs_model* m, dcs_stft* p, c
   }
   const int64_t Lwork = to ? resampler_length(to, Lmax) : Lmax;   // the longest clip at the networks' rate
   DCS_TRY(check_model(Lwork));
-  DCS_CUDA(cudaSetDevice(ctx->device));
-  // each resource on its own: a call that failed half-way through this block must not leave later calls with null handles
-  if (!ctx->s_h2d) DCS_CUDA(cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
-  if (!ctx->s_d2h) DCS_CUDA(cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking));
-  for (int i = 0; i < 2; ++i) {
-    if (!ctx->ev_in[i]) DCS_CUDA(cudaEventCreateWithFlags(&ctx->ev_in[i], cudaEventDisableTiming));
-    if (!ctx->ev_dec[i]) DCS_CUDA(cudaEventCreateWithFlags(&ctx->ev_dec[i], cudaEventDisableTiming));
-    if (!ctx->ev_enc[i]) DCS_CUDA(cudaEventCreateWithFlags(&ctx->ev_enc[i], cudaEventDisableTiming));
-    if (!ctx->ev_out[i]) DCS_CUDA(cudaEventCreateWithFlags(&ctx->ev_out[i], cudaEventDisableTiming));
-  }
-  // every buffer at the size of the longest clip before the pipeline starts: a grow-only buffer that had to be
-  // re-allocated mid-batch would synchronise the stream
-  for (int b = 0; b < std::min(nclips, 2); ++b) {
-    DCS_TRY(ctx->pcm_in[b].ensure((size_t)Lmax * channels * sample_bytes(in_fmt), st));
-    DCS_TRY(ctx->pcm_out[b].ensure((size_t)m->nsrc * (nx > 0 ? nx : 1) * Lmax * sample_bytes(out_fmt), st));
-  }
-  if (nx > 0)
-    DCS_TRY(size_downmix_workspace(ctx, m, p, Lwork, iterations > 0 ? nx : 0, radius, nx, st));
-  else
-    DCS_TRY(size_workspace(ctx, m, p, Lmax, true, st));
-  const int rc = batch_pipeline(ctx, m, p, to, from, in_fmt, out_fmt, nclips, h_in, num_samples, channels, downmix, nx,
-                                iterations, radius, scale_factor, overlap, patcher, h_out, out_strides, st);
-  // drain everything, success or not, before the host buffers go back to the caller
-  const cudaError_t e0 = cudaStreamSynchronize(ctx->s_h2d), e1 = cudaStreamSynchronize(ctx->s_d2h), e2 = cudaStreamSynchronize(st);
-  if (rc != DCS_OK) return rc;
-  DCS_CUDA(e0);
-  DCS_CUDA(e1);
-  DCS_CUDA(e2);
-  return DCS_OK;
+  std::vector<PipeClip> clips((size_t)nclips);
+  for (int i = 0; i < nclips; ++i) clips[(size_t)i] = PipeClip{h_in[i], num_samples[i], h_out[i], out_strides[i], nullptr, 0};
+  return run_pipeline(ctx, m, p, to, from, in_fmt, out_fmt, clips, channels, downmix, nx, iterations, radius, scale_factor,
+                      overlap, patcher, Lmax, Lwork, Lmax, st);
 }
 }  // extern "C++"
 
@@ -1295,6 +1341,176 @@ int dcs_separate_batch_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, co
   return channels_batch("dcs_separate_batch_channels_host", ctx, m, p, to_model || from_model, to_model, from_model,
                         in_format, out_format, nclips, h_in, num_samples, channels, iterations, radius, scale_factor, overlap,
                         patcher, h_out, out_strides, stream);
+}
+
+// ------------------------------------------------------------------------------------ long C-channel recordings
+// The bounds of longclip.plan_segments (deepconvsep_b200/longclip.py documents their derivation) for the core [e0, e1)
+// of a clip of Lm samples: the first frame frame0 (a multiple of step, of lcm(step, chunk) with the windowed Wiener
+// filter) and the stop sample of the range whose separation is exact on the core.
+static int64_t gcd_i64(int64_t a, int64_t b) { while (b) { const int64_t t = a % b; a = b; b = t; } return a; }
+
+int64_t dcs_long_segments(int64_t num_samples, int64_t core_samples, int frame_size, int hop, int time_context, int overlap,
+                          int wiener_reach, int to_up, int to_down, int to_ntaps, int from_ntaps, dcs_segment* out,
+                          int64_t max_segments) {
+  const int64_t L = num_samples, K = core_samples, N = frame_size, H = hop, tc = time_context, step = tc - overlap;
+  if (L < 1 || K < 1 || N < 2 || H < 1 || overlap < 0 || step < 1 || wiener_reach < 0 || to_up < 1 || to_down < 1 ||
+      to_ntaps < 1 || from_ntaps < 1 || max_segments < 0 || (max_segments > 0 && !out))
+    return -1;
+  const bool resampled = !(to_up == 1 && to_down == 1 && to_ntaps == 1 && from_ntaps == 1);
+  const int64_t Lm = resampled ? dcs_resampled_length(L, to_up, to_down) : L;
+  const int64_t CH = DCS_WIENER_CHUNK_FRAMES, R = wiener_reach;
+  const int64_t q = ceil_div64(N / 2, H), s_v = ceil_div64(q, step) * step;
+  const int64_t align = R ? step * CH / gcd_i64(step, CH) : step;
+  const int64_t first_w = CH * (ceil_div64(s_v + overlap, CH) + R);   // longclip._wiener_first_frame(s_v + overlap, R)
+  const int64_t nseg = ceil_div64(L, K);
+  for (int64_t i = 0; i < nseg && i < max_segments; ++i) {
+    dcs_segment& sg = out[i];
+    sg.out_start = i * K;
+    sg.out_stop = std::min(L, sg.out_start + K);
+    // the core at 44.1 kHz: the samples the way back reads for it (from_model is to_down / to_up)
+    int64_t e0 = sg.out_start, e1 = sg.out_stop;
+    if (resampled) {
+      e0 = std::max<int64_t>(0, support_lo(to_down, to_up, from_ntaps, sg.out_start));
+      e1 = std::min<int64_t>(Lm, support_hi(to_down, to_up, from_ntaps, sg.out_stop - 1) + 1);
+    }
+    int64_t g0 = R ? floor_div64(floor_div64(e0 - N / 2, H) + 1 - first_w, align) * align
+                   : floor_div64(floor_div64(e0 - N / 2, H) - s_v - overlap, step) * step;
+    if (i == 0 || g0 <= 0) g0 = 0;   // the margin reaches the start: the true edge is the pipeline's own
+    const int64_t s0 = g0 * H;
+    int64_t s1 = Lm;
+    if (i < nseg - 1) {
+      int64_t G;
+      if (R) {
+        const int64_t b = floor_div64(e1 - 1 - s0 + N / 2, H);   // the last frame the last sample of the core reads
+        G = CH * (floor_div64(b, CH) + R + 1) + q + tc - 2;
+      } else {
+        G = ceil_div64(e1 - s0 + N / 2, H) + q + tc - 1;
+      }
+      s1 = std::min(Lm, s0 + G * H);
+    }
+    sg.model_start = s0;
+    sg.model_stop = s1;
+    sg.in_start = s0;
+    sg.in_stop = s1;
+    if (resampled) {   // the recording's samples the decode of the model range reads
+      sg.in_start = std::max<int64_t>(0, support_lo(to_up, to_down, to_ntaps, s0));
+      sg.in_stop = std::min<int64_t>(L, support_hi(to_up, to_down, to_ntaps, s1 - 1) + 1);
+    }
+  }
+  return nseg;
+}
+
+// the checks of the range entries beyond those of dcs_channels_decode / _encode: a window inside the whole signal's
+// resampling, a staged range inside the signal that covers every input the window reads
+static int check_range(const char* fn, const dcs_resampler* r, int64_t num_samples, int64_t in_first, int64_t num_staged,
+                       int64_t out_first, int64_t num_out) {
+  DCS_REQUIRE(num_samples >= 1, "%s: num_samples %lld must be >= 1", fn, (long long)num_samples);
+  const int64_t most = resampler_length(r, num_samples);
+  DCS_REQUIRE(out_first >= 0 && num_out >= 1 && out_first + num_out <= most, "%s: window [%lld, %lld) not inside [0, %lld)", fn,
+              (long long)out_first, (long long)(out_first + num_out), (long long)most);
+  DCS_REQUIRE(in_first >= 0 && num_staged >= 1 && in_first + num_staged <= num_samples,
+              "%s: staged range [%lld, %lld) not inside [0, %lld)", fn, (long long)in_first, (long long)(in_first + num_staged),
+              (long long)num_samples);
+  int64_t lo, hi;
+  resampler_support(r, out_first, out_first + num_out - 1, num_samples, &lo, &hi);
+  DCS_REQUIRE(lo > hi || (in_first <= lo && in_first + num_staged > hi),
+              "%s: the staged range [%lld, %lld) does not cover the window's inputs [%lld, %lld]", fn, (long long)in_first,
+              (long long)(in_first + num_staged), (long long)lo, (long long)hi);
+  return DCS_OK;
+}
+
+int dcs_channels_decode_range(dcs_ctx* ctx, const dcs_resampler* r, int format, const void* d_in, int64_t num_samples,
+                              int64_t in_first, int64_t num_staged, int channels, float* d_out, int64_t out_first,
+                              int64_t num_out, void* stream) {
+  const char* fn = "dcs_channels_decode_range";
+  DCS_REQUIRE(ctx && r && d_in && d_out, "%s: NULL argument", fn);
+  DCS_REQUIRE(resampler_ctx(r) == ctx, "%s: the resampler was made on another ctx", fn);
+  const int b = sample_bytes(format);
+  DCS_REQUIRE(b > 0, "%s: unknown sample format %d", fn, format);
+  DCS_REQUIRE((uintptr_t)d_in % b == 0 && (uintptr_t)d_out % 4 == 0, "%s: d_in not %d-byte or d_out not 4-byte aligned", fn,
+              b);
+  DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
+  DCS_TRY(check_range(fn, r, num_samples, in_first, num_staged, out_first, num_out));
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  return sync_after(fn, launch_resample_decode_range(r, format, d_in, num_samples, in_first, num_staged, channels, d_out,
+                                                     out_first, num_out, st), st);
+}
+
+int dcs_channels_encode_range(dcs_ctx* ctx, const dcs_resampler* r, int format, const float* d_stems, int64_t num_samples,
+                              int64_t in_first, int64_t num_in, int nsrc, int channels, void* d_out, int64_t out_first,
+                              int64_t num_out, int64_t out_stride, void* stream) {
+  const char* fn = "dcs_channels_encode_range";
+  DCS_REQUIRE(ctx && r && d_stems && d_out, "%s: NULL argument", fn);
+  DCS_REQUIRE(resampler_ctx(r) == ctx, "%s: the resampler was made on another ctx", fn);
+  const int b = sample_bytes(format);
+  DCS_REQUIRE(b > 0, "%s: unknown sample format %d", fn, format);
+  DCS_REQUIRE(nsrc >= 1, "%s: nsrc %d must be >= 1", fn, nsrc);
+  DCS_REQUIRE((uintptr_t)d_stems % 4 == 0 && (uintptr_t)d_out % b == 0, "%s: d_stems not 4-byte or d_out not %d-byte aligned",
+              fn, b);
+  DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
+  DCS_TRY(check_range(fn, r, num_samples, in_first, num_in, out_first, num_out));
+  DCS_REQUIRE(out_stride == (int64_t)channels * num_out, "%s: out_stride %lld != channels * num_out", fn, (long long)out_stride);
+  DCS_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  return sync_after(fn, launch_resample_encode_range(r, format, d_stems, num_samples, in_first, num_in, nsrc, channels, d_out,
+                                                     out_first, num_out, st), st);
+}
+
+int dcs_separate_long_channels_host(dcs_ctx* ctx, dcs_model* m, dcs_stft* p, const dcs_resampler* to_model,
+                                    const dcs_resampler* from_model, int in_format, int out_format, const void* h_in,
+                                    int64_t num_samples, int channels, int iterations, int radius, int64_t core_samples,
+                                    float scale_factor, int overlap, int patcher, void* h_out, int64_t out_stride,
+                                    void* stream) {
+  const char* fn = "dcs_separate_long_channels_host";
+  DCS_REQUIRE(sample_bytes(in_format) > 0 && sample_bytes(out_format) > 0, "%s: unknown sample format %d / %d", fn, in_format,
+              out_format);
+  DCS_REQUIRE(ctx, "%s: NULL ctx", fn);
+  DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
+  const bool resampled = to_model || from_model;
+  if (resampled) DCS_TRY(check_resample_channels(fn, ctx, to_model, from_model, channels, in_format));
+  DCS_REQUIRE(iterations >= 0, "%s: iterations %d must be >= 0", fn, iterations);
+  DCS_REQUIRE(radius >= 0, "%s: radius %d must be >= 0", fn, radius);
+  DCS_REQUIRE(iterations == 0 || (channels >= 2 && channels <= 8), "%s: the Wiener post-filter needs channels in [2, 8], got %d",
+              fn, channels);
+  DCS_REQUIRE(h_in && h_out, "%s: NULL buffer", fn);
+  DCS_REQUIRE(num_samples > 0 && core_samples >= 1 && out_stride >= num_samples,
+              "%s: num_samples %lld, core_samples %lld, out_stride %lld", fn, (long long)num_samples, (long long)core_samples,
+              (long long)out_stride);
+  DCS_TRY(check_model(fn, ctx, m, -1, overlap, patcher));
+  DCS_REQUIRE(p, "%s: NULL argument", fn);
+  DCS_REQUIRE(!ctx->tap && !ctx->pool_tap,
+              "%s: a spectrum or routing tap is set (dcs_set_spectrum_tap / dcs_set_pool_tap); a long recording's segments "
+              "would overwrite it one after another", fn);
+  const int64_t nseg = ceil_div64(num_samples, core_samples);
+  DCS_REQUIRE(nseg <= (int64_t)1 << 24, "%s: %lld segments of %lld samples; take longer cores", fn, (long long)nseg,
+              (long long)core_samples);
+  DCS_REQUIRE(iterations == 0 || radius > 0 || nseg == 1,
+              "%s: the Wiener post-filter with whole-clip covariances (radius 0) needs the whole recording in one segment, "
+              "this one is cut into %lld: set radius >= 1 or core_samples >= num_samples", fn, (long long)nseg);
+  std::vector<dcs_segment> segs((size_t)nseg);
+  const int to_up = resampled ? resampler_up(to_model) : 1, to_down = resampled ? resampler_down(to_model) : 1;
+  DCS_REQUIRE(dcs_long_segments(num_samples, core_samples, p->N, p->hop, m->tc, overlap, iterations * radius, to_up, to_down,
+                                resampled ? resampler_ntaps(to_model) : 1, resampled ? resampler_ntaps(from_model) : 1,
+                                segs.data(), nseg) == nseg,
+              "%s: no segment plan for this geometry", fn);
+  int64_t Smax = 0, Swork = 0, Kmax = 0;
+  for (const dcs_segment& sg : segs) {
+    Smax = std::max(Smax, sg.in_stop - sg.in_start);
+    Swork = std::max(Swork, sg.model_stop - sg.model_start);
+    Kmax = std::max(Kmax, sg.out_stop - sg.out_start);
+  }
+  DCS_TRY(check_channels(fn, ctx, m, p, h_in, channels, Swork, Swork, overlap, patcher, h_out, Swork, iterations, radius));
+  const size_t bi = (size_t)sample_bytes(in_format) * channels, bo = (size_t)sample_bytes(out_format) * channels;
+  std::vector<PipeClip> clips((size_t)nseg);
+  for (int64_t i = 0; i < nseg; ++i) {
+    const dcs_segment& sg = segs[(size_t)i];
+    clips[(size_t)i] = PipeClip{(const char*)h_in + sg.in_start * bi, sg.in_stop - sg.in_start,
+                                (char*)h_out + sg.out_start * bo, out_stride, &segs[(size_t)i], num_samples};
+  }
+  return run_pipeline(ctx, m, p, resampled ? to_model : nullptr, resampled ? from_model : nullptr, in_format, out_format, clips,
+                      channels, 0, channels, iterations, radius, scale_factor, overlap, patcher, Smax, Swork, Kmax,
+                      (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------ Wiener post-filter

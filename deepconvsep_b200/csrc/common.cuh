@@ -394,6 +394,9 @@ int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_str
 // encode of dcs_resample's y trimmed to L
 int64_t resampler_length(const dcs_resampler* r, int64_t num_in);
 const dcs_ctx* resampler_ctx(const dcs_resampler* r);
+int resampler_up(const dcs_resampler* r);
+int resampler_down(const dcs_resampler* r);
+int resampler_ntaps(const dcs_resampler* r);
 int check_resample_channels(const char* fn, const dcs_ctx* ctx, const dcs_resampler* to, const dcs_resampler* from, int C,
                             int in_fmt);
 int resample_decode_groups(const dcs_resampler* r, int C, int fmt);
@@ -401,6 +404,23 @@ int launch_resample_decode(const dcs_resampler* r, int fmt, const void* d_in, in
                            cudaStream_t st);
 int launch_resample_encode(const dcs_resampler* r, int fmt, const float* d_stems, int64_t Lin, int nsrc, int C, void* d_out,
                            int64_t L, cudaStream_t st);
+// the same launches on a window of the whole signal: decode outputs [out_first, out_first + Lout) of the resampling of a
+// recording of L samples staged as its samples [in_first, in_first + num_staged) (zeros elsewhere); encode outputs
+// [out_first, out_first + L) of the resampling of a 44.1 kHz signal of Lm samples whose stems are given at
+// [in_first, in_first + Lin) (zeros elsewhere), the stem planes Lin apart
+int launch_resample_decode_range(const dcs_resampler* r, int fmt, const void* d_in, int64_t L, int64_t in_first,
+                                 int64_t num_staged, int C, float* d_planes, int64_t out_first, int64_t Lout, cudaStream_t st);
+int launch_resample_encode_range(const dcs_resampler* r, int fmt, const float* d_stems, int64_t Lm, int64_t in_first,
+                                 int64_t Lin, int nsrc, int C, void* d_out, int64_t out_first, int64_t L, cudaStream_t st);
+// the inputs output m of a resampler (up, down, ntaps) reads: lo(m) = ceil((m down + half - ntaps + 1) / up) through
+// hi(m) = floor((m down + half) / up), half = (ntaps - 1) / 2, before clipping to the input
+inline int64_t floor_div64(int64_t a, int64_t b) { return a >= 0 ? a / b : -((-a + b - 1) / b); }
+inline int64_t support_lo(int up, int down, int ntaps, int64_t m) {
+  return -floor_div64(-(m * down + (ntaps - 1) / 2 - ntaps + 1), up);
+}
+inline int64_t support_hi(int up, int down, int ntaps, int64_t m) { return floor_div64(m * down + (ntaps - 1) / 2, up); }
+// [lo, hi]: the inputs outputs m_first..m_last read, clipped to [0, num_in) (lo > hi: none)
+void resampler_support(const dcs_resampler* r, int64_t m_first, int64_t m_last, int64_t num_in, int64_t* lo, int64_t* hi);
 
 // multichannel Wiener post-filter (wiener.cu): nch (2..8) mixture channels, channel c at X + c * x_plane, stem (j, c) at
 // S + (j * nch + c) * src_stride, bins f < F filtered in place by `iterations` EM iterations; radius: the covariance

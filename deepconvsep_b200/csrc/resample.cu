@@ -106,6 +106,24 @@ struct ResamplePcmArgs {
   int C, cn, cs;                     // channels; channels per tile and staged values per sample (encode)
   int64_t tiles_t, ntiles;           // tiles along time, all tiles
 };
+// The windowed kernels' arguments (a type of its own: the plain kernels keep their parameter block).  The outputs are
+// [out_first, out_first + num_out) of the whole signal's resampling, their periods counted from p_first =
+// floor(out_first / up); input sample j of the whole signal is at in + (j - in_first) for j in [j_lo, j_hi), and zero
+// elsewhere.
+struct ResampleWindow { int64_t out_first, p_first, in_first, j_lo, j_hi; };
+struct ResampleWinArgs : ResamplePcmArgs { ResampleWindow win; };
+// the window of each argument type; the plain kernels' is the whole signal: periods from 0, input j at j for j in
+// [0, num_in).  The bounds stay in the staging condition's own && (a bool helper changes the plain kernels' SASS)
+__device__ __forceinline__ int64_t first_period(const ResamplePcmArgs&) { return 0; }
+__device__ __forceinline__ int64_t first_period(const ResampleWinArgs& a) { return a.win.p_first; }
+__device__ __forceinline__ int64_t first_out(const ResamplePcmArgs&) { return 0; }
+__device__ __forceinline__ int64_t first_out(const ResampleWinArgs& a) { return a.win.out_first; }
+__device__ __forceinline__ int64_t staged_lo(const ResamplePcmArgs&) { return 0; }
+__device__ __forceinline__ int64_t staged_lo(const ResampleWinArgs& a) { return a.win.j_lo; }
+__device__ __forceinline__ int64_t staged_hi(const ResamplePcmArgs& a) { return a.num_in; }
+__device__ __forceinline__ int64_t staged_hi(const ResampleWinArgs& a) { return a.win.j_hi; }
+__device__ __forceinline__ int64_t staged_at(const ResamplePcmArgs&, int64_t j) { return j; }
+__device__ __forceinline__ int64_t staged_at(const ResampleWinArgs& a, int64_t j) { return j - a.win.in_first; }
 
 // the tap value of a staged sample: int16 is converted per tap use, the 4-byte formats are staged already decoded
 __device__ __forceinline__ float staged_tap(int16_t x) { return SampleFormat<DCS_SAMPLE_I16>::decode(x); }
@@ -120,9 +138,12 @@ __device__ __forceinline__ float staged_tap(float x) { return x; }
 //  - int32 and float32: staged as their fp32 decode, one conversion per staged sample, so the inner sum is
 //    resample_kernel's on the same values.  Where 4-byte staging leaves no room for all C channels, the channels are
 //    split into equal groups of cn; plane 0 is then not written here but by one downmix_kernel launch on the planes.
-template <int FMT>
+// Args = ResampleWinArgs (kWin): a window of the whole recording's resampling; the same sums, tiles aligned to its
+// periods.
+template <int FMT, class Args = ResamplePcmArgs>
 __global__ void __launch_bounds__(RS_THREADS)
-resample_decode_kernel(const ResamplePcmArgs a) {
+resample_decode_kernel(const Args a) {
+  constexpr bool kWin = std::is_same<Args, ResampleWinArgs>::value;
   using In = typename SampleFormat<FMT>::T;
   constexpr bool kWide = FMT != DCS_SAMPLE_I16;
   using Staged = typename std::conditional<kWide, float, int16_t>::type;
@@ -138,21 +159,21 @@ resample_decode_kernel(const ResamplePcmArgs a) {
     const int64_t tt = kWide ? tile % a.tiles_t : tile;
     const int c_lo = kWide ? (int)(tile / a.tiles_t) * a.cn : 0;
     const int cn = kWide ? min(a.cn, C - c_lo) : C;
-    const int64_t P0 = tt * a.tp;
+    const int64_t P0 = first_period(a) + tt * a.tp;
     const int64_t jlo = P0 * a.down + a.c0 - (a.Q - 1);
     __syncthreads();
     for (int k = threadIdx.x; k < a.span * cn; k += RS_THREADS) {    // consecutive threads read consecutive values
       const int jj = k / cn, c = k - jj * cn;
       const int64_t j = jlo + jj;
       if constexpr (kWide)
-        xs[c * a.span + jj] = (j >= 0 && j < a.num_in) ? SampleFormat<FMT>::decode(pcm[j * C + c_lo + c]) : 0.f;
+        xs[c * a.span + jj] = (j >= staged_lo(a) && j < staged_hi(a)) ? SampleFormat<FMT>::decode(pcm[staged_at(a, j) * C + c_lo + c]) : 0.f;
       else
-        xs[c * a.span + jj] = (j >= 0 && j < a.num_in) ? pcm[j * C + c] : (int16_t)0;
+        xs[c * a.span + jj] = (j >= staged_lo(a) && j < staged_hi(a)) ? pcm[staged_at(a, j) * C + c] : (int16_t)0;
     }
     __syncthreads();
     for (int w = threadIdx.x; w < items; w += RS_THREADS) {
       const int r = w % a.up, g = w / a.up;
-      const int64_t n0 = (P0 + (int64_t)g * RS_V) * a.up + r;
+      const int64_t n0 = (P0 + (int64_t)g * RS_V) * a.up + r - first_out(a);   // index in the output planes
       if (n0 >= a.num_out) continue;
       const int cr = (int)(((int64_t)r * a.down + a.half_len) / a.up);
       const int base = g * RS_V * a.down + cr - a.c0 + a.Q - 1;
@@ -166,7 +187,7 @@ resample_decode_kernel(const ResamplePcmArgs a) {
         for (int v = 0; v < RS_V; ++v) {
           const float yv = (float)acc[v];
           const int64_t n = n0 + (int64_t)v * a.up;
-          if (n < a.num_out) y[n] = yv;
+          if ((!kWin || n >= 0) && n < a.num_out) y[n] = yv;
           mix[v] = c == 0 ? yv : mix[v] + yv;
         }
       }
@@ -174,7 +195,7 @@ resample_decode_kernel(const ResamplePcmArgs a) {
 #pragma unroll
         for (int v = 0; v < RS_V; ++v) {
           const int64_t n = n0 + (int64_t)v * a.up;
-          if (n < a.num_out) planes[n] = mix[v] * inv;
+          if ((!kWin || n >= 0) && n < a.num_out) planes[n] = mix[v] * inv;
         }
       }
     }
@@ -187,9 +208,12 @@ resample_decode_kernel(const ResamplePcmArgs a) {
 // unless the bank leaves too little room); its span is staged interleaved, cs = cn | 1 values per sample so that the
 // staging stores and the tap loads of neighbouring channels fall in different banks.  A work item is (channel, residue,
 // RS_V periods) with the channel fastest, so neighbouring lanes write neighbouring values of the interleaved output.
-template <int FMT>
+// Args = ResampleWinArgs (kWin): a window of the resampling of stems placed at [in_first, in_first + num_in) of the 44.1 kHz signal (zeros
+// elsewhere; j_lo = in_first, j_hi = in_first + num_in), the stem planes num_in apart.
+template <int FMT, class Args = ResamplePcmArgs>
 __global__ void __launch_bounds__(RS_THREADS)
-resample_encode_kernel(const ResamplePcmArgs a) {
+resample_encode_kernel(const Args a) {
+  constexpr bool kWin = std::is_same<Args, ResampleWinArgs>::value;
   using Out = typename SampleFormat<FMT>::T;
   extern __shared__ __align__(16) unsigned char rs_smem[];
   double* bank = reinterpret_cast<double*>(rs_smem);
@@ -202,14 +226,14 @@ resample_encode_kernel(const ResamplePcmArgs a) {
     const int64_t tt = tile % a.tiles_t, sg = tile / a.tiles_t;
     const int s = (int)(sg / groups), c_lo = (int)(sg % groups) * a.cn;
     const int cn = min(a.cn, C - c_lo);
-    const int64_t P0 = tt * a.tp;
+    const int64_t P0 = first_period(a) + tt * a.tp;
     const int64_t jlo = P0 * a.down + a.c0 - (a.Q - 1);
     const float* __restrict__ x = stems + ((int64_t)s * C + c_lo) * a.num_in;
     __syncthreads();
     for (int k = threadIdx.x; k < a.span * cn; k += RS_THREADS) {   // plane by plane: coalesced reads
       const int c = k / a.span, jj = k - c * a.span;
       const int64_t j = jlo + jj;
-      xs[jj * cs + c] = (j >= 0 && j < a.num_in) ? __ldg(x + (int64_t)c * a.num_in + j) : 0.f;
+      xs[jj * cs + c] = (j >= staged_lo(a) && j < staged_hi(a)) ? __ldg(x + (int64_t)c * a.num_in + staged_at(a, j)) : 0.f;
     }
     __syncthreads();
     const int items = cn * a.up * (a.tp / RS_V);
@@ -217,7 +241,7 @@ resample_encode_kernel(const ResamplePcmArgs a) {
     for (int w = threadIdx.x; w < items; w += RS_THREADS) {
       const int c = w % cn, rg = w / cn;
       const int r = rg % a.up, g = rg / a.up;
-      const int64_t n0 = (P0 + (int64_t)g * RS_V) * a.up + r;
+      const int64_t n0 = (P0 + (int64_t)g * RS_V) * a.up + r - first_out(a);
       if (n0 >= a.num_out) continue;
       const int cr = (int)(((int64_t)r * a.down + a.half_len) / a.up);
       const int base = g * RS_V * a.down + cr - a.c0 + a.Q - 1;
@@ -226,7 +250,7 @@ resample_encode_kernel(const ResamplePcmArgs a) {
 #pragma unroll
       for (int v = 0; v < RS_V; ++v) {
         const int64_t n = n0 + (int64_t)v * a.up;
-        if (n < a.num_out) o[n * C + c] = SampleFormat<FMT>::encode((float)acc[v]);
+        if ((!kWin || n >= 0) && n < a.num_out) o[n * C + c] = SampleFormat<FMT>::encode((float)acc[v]);
       }
     }
   }
@@ -270,9 +294,8 @@ static bool pcm_plan(const dcs_resampler* r, int C, bool encode, int fmt, PcmPla
   return false;
 }
 
-template <class Kernel>
-static int launch_pcm(const dcs_resampler* r, Kernel kernel, const char* scope, const PcmPlan& pl, ResamplePcmArgs a,
-                      cudaStream_t st) {
+template <class Kernel, class Args>
+static int launch_pcm(const dcs_resampler* r, Kernel kernel, const char* scope, const PcmPlan& pl, Args a, cudaStream_t st) {
   dcs_ctx* ctx = r->ctx;
   a.bank = r->d_bank;
   a.up = r->up; a.down = r->down; a.Q = r->Q; a.half_len = r->half_len; a.c0 = r->c0;
@@ -290,6 +313,9 @@ static int launch_pcm(const dcs_resampler* r, Kernel kernel, const char* scope, 
 
 int64_t resampler_length(const dcs_resampler* r, int64_t num_in) { return dcs_resampled_length(num_in, r->up, r->down); }
 const dcs_ctx* resampler_ctx(const dcs_resampler* r) { return r->ctx; }
+int resampler_up(const dcs_resampler* r) { return r->up; }
+int resampler_down(const dcs_resampler* r) { return r->down; }
+int resampler_ntaps(const dcs_resampler* r) { return r->ntaps; }
 
 int check_resample_channels(const char* fn, const dcs_ctx* ctx, const dcs_resampler* to, const dcs_resampler* from, int C,
                             int in_fmt) {
@@ -311,25 +337,52 @@ int resample_decode_groups(const dcs_resampler* r, int C, int fmt) {
   return sample_bytes(fmt) > 0 && C >= 1 && pcm_plan(r, C, false, fmt, &pl) ? (C + pl.cn - 1) / pl.cn : 0;
 }
 
+// the decode / encode launches of a tile plan; a.tiles_t set, a.ntiles set here.  The decode of channel groups adds
+// the downmix launch
+template <class Args>
+static int decode_launch(const dcs_resampler* r, int fmt, const PcmPlan& pl, Args a, cudaStream_t st) {
+  const int groups = (a.C + pl.cn - 1) / pl.cn;
+  a.ntiles = a.tiles_t * groups;
+  switch (fmt) {
+    case DCS_SAMPLE_I16: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_I16, Args>, "resample_decode", pl, a, st)); break;
+    case DCS_SAMPLE_I32: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_I32, Args>, "resample_decode", pl, a, st)); break;
+    default: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_F32, Args>, "resample_decode", pl, a, st)); break;
+  }
+  if (groups == 1) return DCS_OK;
+  float* planes = static_cast<float*>(a.out);
+  ProfScope ps(r->ctx, "resample_decode_downmix", st);   // the channel groups' downmix: the same expression, the same bits
+  return launch_downmix(r->ctx, planes + a.num_out, a.C, a.num_out, a.num_out, planes, st);
+}
+
+template <class Args>
+static int encode_launch(const dcs_resampler* r, int fmt, const PcmPlan& pl, int nsrc, Args a, cudaStream_t st) {
+  a.ntiles = a.tiles_t * ((a.C + pl.cn - 1) / pl.cn) * nsrc;
+  switch (fmt) {
+    case DCS_SAMPLE_I16: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_I16, Args>, "resample_encode", pl, a, st);
+    case DCS_SAMPLE_I32: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_I32, Args>, "resample_encode", pl, a, st);
+    default: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_F32, Args>, "resample_encode", pl, a, st);
+  }
+}
+
+// the window's arguments: outputs [out_first, out_first + a->num_out), input j of the whole signal at in + (j - in_first)
+// for j in [j_lo, j_hi)
+static void set_window(const dcs_resampler* r, const PcmPlan& pl, int64_t out_first, int64_t in_first, int64_t j_lo,
+                       int64_t j_hi, ResampleWinArgs* a) {
+  a->win.out_first = out_first; a->win.p_first = out_first / r->up;
+  a->win.in_first = in_first; a->win.j_lo = j_lo; a->win.j_hi = j_hi;
+  a->tiles_t = ceil_div64((out_first + a->num_out - 1) / r->up - a->win.p_first + 1, pl.tp);
+}
+
 int launch_resample_decode(const dcs_resampler* r, int fmt, const void* d_in, int64_t L, int C, float* d_planes, int64_t Lout,
                            cudaStream_t st) {
   PcmPlan pl;
   DCS_REQUIRE(L >= 1 && Lout >= 1 && Lout <= resampler_length(r, L) && C >= 1 && C <= 16 && sample_bytes(fmt) > 0 &&
                   pcm_plan(r, C, false, fmt, &pl),
               "resample_decode: bad arguments");
-  ResamplePcmArgs a;
+  ResamplePcmArgs a{};
   a.in = d_in; a.num_in = L; a.out = d_planes; a.num_out = Lout; a.C = C;
-  const int groups = (C + pl.cn - 1) / pl.cn;
   a.tiles_t = ceil_div64(ceil_div64(Lout, r->up), pl.tp);
-  a.ntiles = a.tiles_t * groups;
-  switch (fmt) {
-    case DCS_SAMPLE_I16: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_I16>, "resample_decode", pl, a, st)); break;
-    case DCS_SAMPLE_I32: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_I32>, "resample_decode", pl, a, st)); break;
-    default: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_F32>, "resample_decode", pl, a, st)); break;
-  }
-  if (groups == 1) return DCS_OK;
-  ProfScope ps(r->ctx, "resample_decode_downmix", st);   // the channel groups' downmix: the same expression, the same bits
-  return launch_downmix(r->ctx, d_planes + Lout, C, Lout, Lout, d_planes, st);
+  return decode_launch(r, fmt, pl, a, st);
 }
 
 int launch_resample_encode(const dcs_resampler* r, int fmt, const float* d_stems, int64_t Lin, int nsrc, int C, void* d_out,
@@ -338,15 +391,41 @@ int launch_resample_encode(const dcs_resampler* r, int fmt, const float* d_stems
   DCS_REQUIRE(Lin >= 1 && L >= 1 && L <= resampler_length(r, Lin) && nsrc >= 1 && C >= 1 && C <= 16 && sample_bytes(fmt) > 0 &&
                   pcm_plan(r, C, true, fmt, &pl),
               "resample_encode: bad arguments");
-  ResamplePcmArgs a;
+  ResamplePcmArgs a{};
   a.in = d_stems; a.num_in = Lin; a.out = d_out; a.num_out = L; a.C = C;
   a.tiles_t = ceil_div64(ceil_div64(L, r->up), pl.tp);
-  a.ntiles = a.tiles_t * ((C + pl.cn - 1) / pl.cn) * nsrc;
-  switch (fmt) {
-    case DCS_SAMPLE_I16: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_I16>, "resample_encode", pl, a, st);
-    case DCS_SAMPLE_I32: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_I32>, "resample_encode", pl, a, st);
-    default: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_F32>, "resample_encode", pl, a, st);
-  }
+  return encode_launch(r, fmt, pl, nsrc, a, st);
+}
+
+int launch_resample_decode_range(const dcs_resampler* r, int fmt, const void* d_in, int64_t L, int64_t in_first,
+                                 int64_t num_staged, int C, float* d_planes, int64_t out_first, int64_t Lout, cudaStream_t st) {
+  PcmPlan pl;
+  DCS_REQUIRE(L >= 1 && in_first >= 0 && num_staged >= 1 && in_first + num_staged <= L && out_first >= 0 && Lout >= 1 &&
+                  out_first + Lout <= resampler_length(r, L) && C >= 1 && C <= 16 && sample_bytes(fmt) > 0 &&
+                  pcm_plan(r, C, false, fmt, &pl),
+              "resample_decode_range: bad arguments");
+  ResampleWinArgs a{};
+  a.in = d_in; a.num_in = L; a.out = d_planes; a.num_out = Lout; a.C = C;
+  set_window(r, pl, out_first, in_first, in_first, in_first + num_staged, &a);
+  return decode_launch(r, fmt, pl, a, st);
+}
+
+int launch_resample_encode_range(const dcs_resampler* r, int fmt, const float* d_stems, int64_t Lm, int64_t in_first,
+                                 int64_t Lin, int nsrc, int C, void* d_out, int64_t out_first, int64_t L, cudaStream_t st) {
+  PcmPlan pl;
+  DCS_REQUIRE(Lm >= 1 && in_first >= 0 && Lin >= 1 && in_first + Lin <= Lm && out_first >= 0 && L >= 1 &&
+                  out_first + L <= resampler_length(r, Lm) && nsrc >= 1 && C >= 1 && C <= 16 && sample_bytes(fmt) > 0 &&
+                  pcm_plan(r, C, true, fmt, &pl),
+              "resample_encode_range: bad arguments");
+  ResampleWinArgs a{};
+  a.in = d_stems; a.num_in = Lin; a.out = d_out; a.num_out = L; a.C = C;
+  set_window(r, pl, out_first, in_first, in_first, in_first + Lin, &a);
+  return encode_launch(r, fmt, pl, nsrc, a, st);
+}
+
+void resampler_support(const dcs_resampler* r, int64_t m_first, int64_t m_last, int64_t num_in, int64_t* lo, int64_t* hi) {
+  *lo = std::max<int64_t>(0, support_lo(r->up, r->down, r->ntaps, m_first));
+  *hi = std::min<int64_t>(num_in - 1, support_hi(r->up, r->down, r->ntaps, m_last));
 }
 
 }  // namespace dcs

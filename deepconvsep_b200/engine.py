@@ -4,6 +4,8 @@
 stand-alone scripts (examples/dsd100/separate_dsd.py:239-313).  torch is used only as a
 device-memory / stream container; numpy arrays go through the *_host entry points."""
 import ctypes as C
+import math
+from collections import namedtuple
 from functools import partial
 import numpy as np
 
@@ -221,6 +223,8 @@ _SAMPLE_FORMATS = {np.dtype(np.int16): _lib.SAMPLE_I16, np.dtype(np.int32): _lib
                    np.dtype(np.float32): _lib.SAMPLE_F32}
 # the sample rates a Resampler takes: integers in this range whose polyphase bank fits, in both directions
 RESAMPLE_RATES = (8000, 192000)
+# one segment of Separator.long_segments: the recording's samples staged, the range separated at 44.1 kHz, the core kept
+LongSegment = namedtuple("LongSegment", "in_start in_stop model_start model_stop out_start out_stop")
 
 
 def resample_ratio(rate_in, rate_out):
@@ -696,6 +700,71 @@ class Separator(object):
             pre = (self.resampler(sample_rate, MODEL_RATE).handle, self.resampler(MODEL_RATE, sample_rate).handle)
         pre += (_SAMPLE_FORMATS[in_dtype], _SAMPLE_FORMATS[out_dtype])
         return self._pcm16_batch(self.lib.dcs_separate_batch_channels_host, ps, outs, (ch,), args, pre, out_dtype)
+
+    def long_segments(self, num_samples, wiener=0, wiener_radius=0, sample_rate=MODEL_RATE, segment_seconds=120.0):
+        """The segments separate_long_channels cuts a recording of num_samples samples into (dcs_long_segments): a list
+        of LongSegment (in_start, in_stop, model_start, model_stop, out_start, out_stop) for this separator's geometry,
+        the filter's reach wiener * wiener_radius and the rate's resampler pair."""
+        check_wiener_radius(wiener, wiener_radius)
+        if wiener < 0:
+            raise ValueError("wiener %d: the number of EM iterations cannot be negative" % wiener)
+        core = self._long_core(segment_seconds, sample_rate)
+        if sample_rate != MODEL_RATE:
+            up, down = check_resample_rates(sample_rate, MODEL_RATE)
+            to_taps = from_taps = len(resample_taps(up, down))     # the same length both ways
+        else:
+            up = down = to_taps = from_taps = 1
+        args = (int(num_samples), core, self.frame_size, self.hop, self.model.tc, self.overlap, int(wiener) * int(wiener_radius),
+                up, down, to_taps, from_taps)
+        n = int(self.lib.dcs_long_segments(*args, None, 0))
+        if n < 0:
+            raise ValueError("long_segments: no plan for %d samples in cores of %d" % (int(num_samples), core))
+        segs = (_lib.Segment * n)()
+        self.lib.dcs_long_segments(*args, segs, n)
+        return [LongSegment(s.in_start, s.in_stop, s.model_start, s.model_stop, s.out_start, s.out_stop) for s in segs]
+
+    @staticmethod
+    def _long_core(segment_seconds, sample_rate):
+        """core_samples of segment_seconds at sample_rate; ValueError unless segment_seconds is a finite number > 0"""
+        if isinstance(segment_seconds, bool) or not isinstance(segment_seconds, (int, float, np.integer, np.floating)) \
+                or not (math.isfinite(segment_seconds) and segment_seconds > 0):
+            raise ValueError("segment_seconds %r must be a finite number > 0" % (segment_seconds,))
+        return max(1, int(round(float(segment_seconds) * float(sample_rate))))
+
+    def separate_long_channels(self, recording, out=None, out_dtype=None, wiener=0, wiener_radius=0, sample_rate=MODEL_RATE,
+                               segment_seconds=120.0):
+        """One C-channel recording of any length through the multi-clip scheduler with a device workspace bounded by the
+        segment length (dcs_separate_long_channels_host): recording [L, C] of int16, int32 or float32, C in 1..16 ->
+        [nsrc, L, C] of out_dtype (default the recording's dtype), into `out` when given.  The recording is cut into
+        cores of segment_seconds (long_segments); each segment is separated with the margins that make its core the
+        whole recording's stems (up to the GEMMs' summation order for another patch count), and its core is written
+        straight into the result.  The sample rules, rates and filter options are those of separate_channels_batch; the
+        Wiener post-filter over more than one segment needs wiener_radius >= 1.  120 s keeps the workspace of a
+        6-channel filtered recording near that of a 180 s clip."""
+        ps, ch, args, sample_rate = self._channels_clips("separate_long_channels", [recording], tuple(_SAMPLE_FORMATS), wiener,
+                                                         wiener_radius, sample_rate)
+        core = self._long_core(segment_seconds, sample_rate)
+        x = ps[0]
+        try:
+            out_dtype = x.dtype if out_dtype is None else np.dtype(out_dtype)
+        except TypeError:
+            raise ValueError("separate_long_channels: out_dtype %r is not a dtype" % (out_dtype,))
+        if out_dtype not in _SAMPLE_FORMATS:
+            raise ValueError("separate_long_channels encodes int16, int32 or float32 stems, not %s" % out_dtype)
+        L = x.shape[0]
+        if out is None:
+            out = np.empty((self.nsrc, L, ch), dtype=out_dtype)
+        elif not (isinstance(out, np.ndarray) and out.dtype == out_dtype and out.shape == (self.nsrc, L, ch)
+                  and out.flags.c_contiguous):
+            raise ValueError("separate_long_channels: out must be a contiguous %s array [%d, %d, %d]" % (out_dtype, self.nsrc, L, ch))
+        pre = (None, None)
+        if sample_rate != MODEL_RATE:
+            pre = (self.resampler(sample_rate, MODEL_RATE).handle, self.resampler(MODEL_RATE, sample_rate).handle)
+        _lib.check(self.lib.dcs_separate_long_channels_host(
+            self.ctx.handle, self.model.handle, self.stft.handle, *pre, _SAMPLE_FORMATS[x.dtype], _SAMPLE_FORMATS[out_dtype],
+            x.ctypes.data, L, *args, core, self.scale_factor, self.overlap, self.patcher, out.ctypes.data, L,
+            _stream_ptr(None, self.ctx.device)))
+        return out
 
     def _channels_clips(self, call, clips, dtypes, wiener, wiener_radius, sample_rate):
         """the checks of the C-channel batch calls, before any library call: the network, the filter options, clips

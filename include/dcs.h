@@ -748,6 +748,92 @@ int dcs_channels_encode(dcs_ctx* ctx, const dcs_resampler* resampler, int format
                         int nsrc, int channels, int64_t stem_stride, void* d_out, int64_t num_out, int64_t out_stride,
                         void* stream);
 
+/* ---- long C-channel recordings in bounded device memory ---------------------------------------------------------- */
+/* One segment of a long recording: three sample ranges, half-open.
+ *  - in:    [in_start, in_stop), the recording's samples staged on the device;
+ *  - model: [model_start, model_stop), the range separated at 44.1 kHz (the in range itself at 44.1 kHz);
+ *  - kept:  [out_start, out_stop), the core of the recording written to the output. */
+typedef struct {
+  int64_t in_start, in_stop;
+  int64_t model_start, model_stop;
+  int64_t out_start, out_stop;
+} dcs_segment;
+/* The segments of a recording of num_samples samples cut into cores of core_samples, written to out[0 ..
+ * min(count, max_segments)); returns the count, ceil(num_samples / core_samples), or -1 for bad arguments.  Pure host
+ * arithmetic (no ctx).  frame_size, hop, time_context, overlap: the separation's geometry; wiener_reach: iterations *
+ * radius of the Wiener post-filter (0 without it).  The resampler pair is given as to_model's up, down and ntaps and
+ * from_model's ntaps (from_model is down/up); up = down = ntaps = 1 for a recording at 44.1 kHz.  With half = (n - 1)/2,
+ * output m of a resampler (u, d, n) reads inputs lo(m) = ceil((m d + half - n + 1) / u) .. hi(m) = floor((m d + half) /
+ * u), clipped to the input.  Core i is [o0, o1) = [i K, min(L, (i + 1) K)); then
+ *  1. its exact range at 44.1 kHz: [e0, e1) = [lo_from(o0), hi_from(o1 - 1) + 1) clipped to [0, L'),
+ *     L' = dcs_resampled_length(L, to up, to down) (without resamplers [o0, o1) and L' = L);
+ *  2. the model range: the two bounds of longclip.plan_segments for the core [e0, e1) of a clip of L' samples --
+ *     model_start = frame0 * hop, frame0 the largest multiple of step = time_context - overlap (of lcm(step, 128) when
+ *     wiener_reach > 0) whose margin makes the core exact, 0 for the first core or where the margin reaches the start;
+ *     model_stop = model_start + G * hop with longclip's G, L' for the last core or where that overshoots;
+ *  3. the in range: [lo_to(model_start), hi_to(model_stop - 1) + 1) clipped to [0, L).
+ * The cores tile [0, L) once. */
+int64_t dcs_long_segments(int64_t num_samples, int64_t core_samples, int frame_size, int hop, int time_context, int overlap,
+                          int wiener_reach, int to_up, int to_down, int to_ntaps, int from_ntaps, dcs_segment* out,
+                          int64_t max_segments);
+/* One C-channel recording of any length (1 to 16 channels, any sample formats, 44.1 kHz or any rate of a resampler pair)
+ * through the multi-clip scheduler of dcs_separate_batch_channels_host with a device workspace bounded by the segment
+ * length: h_in [num_samples][channels] of in_format (pinned for real overlap) -> source s at h_out + s*channels*out_stride
+ * samples as [num_samples][channels] of out_format, the layout of the batch.  The recording is cut by dcs_long_segments
+ * (core_samples, the plan's geometry, wiener_reach = iterations * radius, the pair's up/down/ntaps) and each segment is a
+ * clip of the pipeline: H2D of its in range straight from h_in, the decode (at another rate the windowed resampling
+ * decode, whose planes are samples [model_start, model_stop) of the whole recording's), the separation of
+ * dcs_separate_audio_channels_wiener on the model range, the encode of the kept core only (at another rate the windowed
+ * encode of the stems placed at [model_start, model_stop)), and D2H of the core straight to h_out at out_start (one 2-D
+ * copy, rows = sources).  Every output sample is written once; nothing is stitched on the host.
+ * Byte contract, for each segment with X the recording:
+ *  - 44.1 kHz: the kept samples are samples [out_start - in_start, out_stop - in_start) of dcs_separate_batch_channels_host
+ *    on the single clip X[in_start:in_stop] with the same formats and options.
+ *  - another rate: the kept samples are dcs_channels_encode_range(from_model, Y, window [out_start, out_stop)) with
+ *    Y = dcs_separate_audio_channels_wiener on the channel planes of dcs_channels_decode_range(to_model, ...) over the model
+ *    range; those planes are, bit for bit, samples [model_start, model_stop) of dcs_channels_decode(to_model) on the whole
+ *    recording.
+ *  - one segment (core_samples >= num_samples): the bytes of dcs_separate_batch_channels_host on the whole recording.
+ *  - against the whole-recording call the stems differ only by the summation order of the network's GEMMs for another
+ *    patch count (longclip.py).
+ * Launches per segment: those of one clip of dcs_separate_batch_channels_host of the segment's length.
+ * Workspace: every buffer is sized once, before the pipeline starts, from the longest model range S'max, the longest in
+ * range Smax and the longest core Kmax: with B(x) and n = min(segments, 2) as for the batch, a fresh ctx holds
+ *     W(S'max) - B(4 S'max) + B(4 (channels + 1) S'max) + B(4 nsrc channels S'max)
+ *       + n B(b_in channels Smax) + n B(b_out nsrc channels Kmax)
+ * Each model range is at most the core's exact range at 44.1 kHz plus longclip.margins and the rounding of its ends to the
+ * frame grid (under (align + 1) * hop samples each, align = step, or lcm(step, 128) with the filter), so the workspace is
+ * bounded by core_samples and the geometry, not by the recording's length; two recordings with the same core may still
+ * differ by where their cores fall on that grid.
+ * Synchronises before returning, also on an error.  Refused with DCS_EINVAL before anything is queued: what
+ * dcs_separate_batch_channels_host refuses (the model's checks on the longest model range), core_samples < 1,
+ * out_stride < num_samples, a NULL buffer, iterations > 0 with radius 0 over more than one segment (the message names the
+ * radius), a spectrum tap or a routing tap set on the ctx (the segments would overwrite it one after another). */
+int dcs_separate_long_channels_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const dcs_resampler* to_model,
+                                    const dcs_resampler* from_model, int in_format, int out_format, const void* h_in,
+                                    int64_t num_samples, int channels, int iterations, int radius, int64_t core_samples,
+                                    float scale_factor, int overlap, int patcher, void* h_out, int64_t out_stride,
+                                    void* stream);
+/* Bring-up and test entries: the windowed conversions of dcs_separate_long_channels_host at another rate, one launch of
+ * the windowed kernels each (two for a decode whose channels take groups), on `stream`, which is synchronised before
+ * returning; the resampler is required, and the checks of dcs_channels_decode / _encode apply.
+ * dcs_channels_decode_range: outputs [out_first, out_first + num_out) of dcs_channels_decode(resampler) on a recording of
+ *  num_samples samples, of which d_in holds samples [in_first, in_first + num_staged) as [num_staged][channels] (the
+ *  recording is zero outside [0, num_samples)) -> d_out float [channels + 1][num_out].
+ * dcs_channels_encode_range: outputs [out_first, out_first + num_out) of dcs_channels_encode(resampler) on stems of a
+ *  44.1 kHz signal of num_samples samples, of which d_stems holds samples [in_first, in_first + num_in) (nsrc * channels
+ *  planes num_in apart; zeros elsewhere) -> source s at d_out + s * out_stride as [num_out][channels], out_stride =
+ *  channels * num_out.
+ * Both also refuse a window outside [0, dcs_resampled_length(num_samples)), a staged range outside [0, num_samples), and
+ * a staged range that does not cover every input the window reads (lo(out_first) .. hi(out_first + num_out - 1),
+ * clipped). */
+int dcs_channels_decode_range(dcs_ctx* ctx, const dcs_resampler* resampler, int format, const void* d_in,
+                              int64_t num_samples, int64_t in_first, int64_t num_staged, int channels, float* d_out,
+                              int64_t out_first, int64_t num_out, void* stream);
+int dcs_channels_encode_range(dcs_ctx* ctx, const dcs_resampler* resampler, int format, const float* d_stems,
+                              int64_t num_samples, int64_t in_first, int64_t num_in, int nsrc, int channels, void* d_out,
+                              int64_t out_first, int64_t num_out, int64_t out_stride, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
