@@ -107,6 +107,7 @@ _SIGS = {
 PCM16_MONO, PCM16_CHANNELS = 0, 3
 # sample formats of dcs_separate_batch_channels_host (DCS_SAMPLE_*, include/dcs.h)
 SAMPLE_I16, SAMPLE_I32, SAMPLE_F32 = 0, 1, 2
+SAMPLE_I24 = 4   # packed 3-byte PCM; code 3 is not a format
 
 
 class Segment(C.Structure):

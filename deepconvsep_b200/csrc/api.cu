@@ -856,8 +856,8 @@ int dcs_channels_decode(dcs_ctx* ctx, const dcs_resampler* r, int format, const 
   const int b = sample_bytes(format);
   DCS_REQUIRE(b > 0, "%s: unknown sample format %d", fn, format);
   DCS_REQUIRE(L >= 1, "%s: num_samples %lld must be >= 1", fn, (long long)L);
-  DCS_REQUIRE((uintptr_t)d_in % b == 0 && (uintptr_t)d_out % 4 == 0, "%s: d_in not %d-byte or d_out not 4-byte aligned", fn,
-              b);
+  DCS_REQUIRE((uintptr_t)d_in % sample_align(format) == 0 && (uintptr_t)d_out % 4 == 0,
+              "%s: d_in not %d-byte or d_out not 4-byte aligned", fn, sample_align(format));
   DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
   const int64_t most = r ? resampler_length(r, L) : L;
   DCS_REQUIRE(num_out >= 1 && num_out <= most && (r || num_out == L), "%s: num_out %lld, want %s%lld", fn, (long long)num_out,
@@ -876,8 +876,8 @@ int dcs_channels_encode(dcs_ctx* ctx, const dcs_resampler* r, int format, const 
   const int b = sample_bytes(format);
   DCS_REQUIRE(b > 0, "%s: unknown sample format %d", fn, format);
   DCS_REQUIRE(num_in >= 1 && nsrc >= 1, "%s: num_in %lld and nsrc %d must be >= 1", fn, (long long)num_in, nsrc);
-  DCS_REQUIRE((uintptr_t)d_stems % 4 == 0 && (uintptr_t)d_out % b == 0, "%s: d_stems not 4-byte or d_out not %d-byte aligned",
-              fn, b);
+  DCS_REQUIRE((uintptr_t)d_stems % 4 == 0 && (uintptr_t)d_out % sample_align(format) == 0,
+              "%s: d_stems not 4-byte or d_out not %d-byte aligned", fn, sample_align(format));
   DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
   DCS_REQUIRE(r ? stem_stride == num_in : stem_stride >= num_in, "%s: stem_stride %lld, num_in %lld", fn,
               (long long)stem_stride, (long long)num_in);
@@ -1427,8 +1427,8 @@ int dcs_channels_decode_range(dcs_ctx* ctx, const dcs_resampler* r, int format, 
   DCS_REQUIRE(resampler_ctx(r) == ctx, "%s: the resampler was made on another ctx", fn);
   const int b = sample_bytes(format);
   DCS_REQUIRE(b > 0, "%s: unknown sample format %d", fn, format);
-  DCS_REQUIRE((uintptr_t)d_in % b == 0 && (uintptr_t)d_out % 4 == 0, "%s: d_in not %d-byte or d_out not 4-byte aligned", fn,
-              b);
+  DCS_REQUIRE((uintptr_t)d_in % sample_align(format) == 0 && (uintptr_t)d_out % 4 == 0,
+              "%s: d_in not %d-byte or d_out not 4-byte aligned", fn, sample_align(format));
   DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
   DCS_TRY(check_range(fn, r, num_samples, in_first, num_staged, out_first, num_out));
   DCS_CUDA(cudaSetDevice(ctx->device));
@@ -1446,8 +1446,8 @@ int dcs_channels_encode_range(dcs_ctx* ctx, const dcs_resampler* r, int format, 
   const int b = sample_bytes(format);
   DCS_REQUIRE(b > 0, "%s: unknown sample format %d", fn, format);
   DCS_REQUIRE(nsrc >= 1, "%s: nsrc %d must be >= 1", fn, nsrc);
-  DCS_REQUIRE((uintptr_t)d_stems % 4 == 0 && (uintptr_t)d_out % b == 0, "%s: d_stems not 4-byte or d_out not %d-byte aligned",
-              fn, b);
+  DCS_REQUIRE((uintptr_t)d_stems % 4 == 0 && (uintptr_t)d_out % sample_align(format) == 0,
+              "%s: d_stems not 4-byte or d_out not %d-byte aligned", fn, sample_align(format));
   DCS_REQUIRE(channels >= 1 && channels <= 16, "%s: channels %d not in [1, 16]", fn, channels);
   DCS_TRY(check_range(fn, r, num_samples, in_first, num_in, out_first, num_out));
   DCS_REQUIRE(out_stride == (int64_t)channels * num_out, "%s: out_stride %lld != channels * num_out", fn, (long long)out_stride);

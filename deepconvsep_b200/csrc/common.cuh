@@ -370,10 +370,27 @@ template <> struct SampleFormat<DCS_SAMPLE_F32> {
   static __device__ __forceinline__ float decode(T x) { return x; }
   static __device__ __forceinline__ T encode(float y) { return y; }
 };
+// packed 24-bit PCM: a 3-byte POD, so that pcm[j * C + c] is a sample's three byte loads or stores at any address
+struct Pcm24 { uint8_t b[3]; };
+template <> struct SampleFormat<DCS_SAMPLE_I24> {
+  using T = Pcm24;
+  // the int32 rule on v << 8: the bits the int32 route gives for scipy's read of the same WAV data chunk
+  static __device__ __forceinline__ float decode(T x) {
+    return SampleFormat<DCS_SAMPLE_I32>::decode((int32_t)(((uint32_t)x.b[0] << 8) | ((uint32_t)x.b[1] << 16) |
+                                                          ((uint32_t)x.b[2] << 24)));
+  }
+  // the int32 encode's top 24 bits (its arithmetic shift right by 8): saturated to [-2^23, 2^23 - 1], NaN gives 0
+  static __device__ __forceinline__ T encode(float y) {
+    const uint32_t e = (uint32_t)SampleFormat<DCS_SAMPLE_I32>::encode(y);
+    return T{{(uint8_t)(e >> 8), (uint8_t)(e >> 16), (uint8_t)(e >> 24)}};
+  }
+};
 // bytes of one sample; 0 for an unknown format code
 inline int sample_bytes(int fmt) {
-  return fmt == DCS_SAMPLE_I16 ? 2 : (fmt == DCS_SAMPLE_I32 || fmt == DCS_SAMPLE_F32) ? 4 : 0;
+  return fmt == DCS_SAMPLE_I16 ? 2 : (fmt == DCS_SAMPLE_I32 || fmt == DCS_SAMPLE_F32) ? 4 : fmt == DCS_SAMPLE_I24 ? 3 : 0;
 }
+// the alignment a device buffer of the format needs: its sample size, 1 byte for packed 24-bit
+inline int sample_align(int fmt) { return fmt == DCS_SAMPLE_I24 ? 1 : sample_bytes(fmt); }
 
 // C-channel stems, C in [1, 16], samples in format fmt: interleaved [L][C] -> C + 1 float planes L apart (the downmix
 // of launch_downmix, then the C channels); nsrc x C stem planes (source, channel) -> [nsrc][L][C], source s at

@@ -346,6 +346,7 @@ static int decode_launch(const dcs_resampler* r, int fmt, const PcmPlan& pl, Arg
   switch (fmt) {
     case DCS_SAMPLE_I16: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_I16, Args>, "resample_decode", pl, a, st)); break;
     case DCS_SAMPLE_I32: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_I32, Args>, "resample_decode", pl, a, st)); break;
+    case DCS_SAMPLE_I24: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_I24, Args>, "resample_decode", pl, a, st)); break;
     default: DCS_TRY(launch_pcm(r, resample_decode_kernel<DCS_SAMPLE_F32, Args>, "resample_decode", pl, a, st)); break;
   }
   if (groups == 1) return DCS_OK;
@@ -360,6 +361,7 @@ static int encode_launch(const dcs_resampler* r, int fmt, const PcmPlan& pl, int
   switch (fmt) {
     case DCS_SAMPLE_I16: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_I16, Args>, "resample_encode", pl, a, st);
     case DCS_SAMPLE_I32: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_I32, Args>, "resample_encode", pl, a, st);
+    case DCS_SAMPLE_I24: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_I24, Args>, "resample_encode", pl, a, st);
     default: return launch_pcm(r, resample_encode_kernel<DCS_SAMPLE_F32, Args>, "resample_encode", pl, a, st);
   }
 }

@@ -283,6 +283,76 @@ pcm_encode_channels_kernel(const float* __restrict__ stems, int64_t L, int C, in
   if (t < n) dst[t] = tile[shift + t];
 }
 
+// Packed 24-bit PCM (DCS_SAMPLE_I24) has no aligned vector of one sample, so both kernels count the tile of 256 rows in
+// bytes (768 C, a multiple of 16) and stage it in shared memory at the byte offset its global address has modulo 16:
+// the 16-byte-aligned middle then moves with 16-byte loads or stores, and the under 16 bytes before and after it one
+// byte at a time.  The global buffer may sit at any address.
+constexpr int kPcm24TileBytes = kPcmEncodeRows * kPcmMaxChannels * 3;
+
+// the bytes [0, n) at g <-> tile + shift, shift = g mod 16; kLoad: global -> tile, else tile -> global
+template <bool kLoad>
+__device__ __forceinline__ void pcm24_move(uint8_t* tile, int shift, uint8_t* g, int n) {
+  const int head = min(n, (16 - shift) & 15);
+  const int nvec = (n - head) >> 4;
+  const int tail0 = head + nvec * 16;
+  uint4* vt = reinterpret_cast<uint4*>(tile + shift + head);
+  uint4* vg = reinterpret_cast<uint4*>(g + head);
+  for (int k = threadIdx.x; k < nvec; k += blockDim.x) {
+    if constexpr (kLoad) vt[k] = __ldg(vg + k);
+    else vg[k] = vt[k];
+  }
+  const int t = (int)threadIdx.x < head ? (int)threadIdx.x : tail0 + (int)threadIdx.x - head;
+  if ((int)threadIdx.x < head + (n - tail0)) {
+    if constexpr (kLoad) tile[shift + t] = g[t];
+    else g[t] = tile[shift + t];
+  }
+}
+
+// pcm_decode_channels_kernel for DCS_SAMPLE_I24: the tile's 768 C bytes staged as above, then each thread decodes its
+// row from shared memory and writes the C + 1 planes with the same expressions in the same order
+__global__ void __launch_bounds__(kPcmEncodeRows)
+pcm24_decode_channels_kernel(const uint8_t* __restrict__ pcm, int64_t L, int C, float* __restrict__ planes) {
+  using S = SampleFormat<DCS_SAMPLE_I24>;
+  __shared__ __align__(16) uint8_t tile[kPcm24TileBytes + 16];
+  const int64_t i0 = (int64_t)blockIdx.x * kPcmEncodeRows;
+  const int rows = (int)(L - i0 < kPcmEncodeRows ? L - i0 : kPcmEncodeRows);
+  uint8_t* src = const_cast<uint8_t*>(pcm) + i0 * C * 3;
+  const int shift = (int)((uintptr_t)src & 15);
+  pcm24_move<true>(tile, shift, src, rows * C * 3);
+  __syncthreads();
+  if ((int)threadIdx.x >= rows) return;
+  const int64_t i = i0 + threadIdx.x;
+  const Pcm24* row = reinterpret_cast<const Pcm24*>(tile + shift) + threadIdx.x * C;
+  float a = S::decode(row[0]);
+  planes[L + i] = a;
+  for (int c = 1; c < C; ++c) {
+    const float v = S::decode(row[c]);
+    planes[(int64_t)(1 + c) * L + i] = v;
+    a += v;
+  }
+  planes[i] = a * (1.0f / (float)C);
+}
+
+// pcm_encode_channels_kernel for DCS_SAMPLE_I24: each thread encodes its row into the tile, which then goes out as above
+__global__ void __launch_bounds__(kPcmEncodeRows)
+pcm24_encode_channels_kernel(const float* __restrict__ stems, int64_t L, int C, int64_t stem_stride,
+                             uint8_t* __restrict__ out) {
+  using S = SampleFormat<DCS_SAMPLE_I24>;
+  __shared__ __align__(16) uint8_t tile[kPcm24TileBytes + 16];
+  const int s = blockIdx.y;
+  const int64_t i0 = (int64_t)blockIdx.x * kPcmEncodeRows;
+  const int rows = (int)(L - i0 < kPcmEncodeRows ? L - i0 : kPcmEncodeRows);
+  uint8_t* dst = out + ((int64_t)s * L + i0) * C * 3;
+  const int shift = (int)((uintptr_t)dst & 15);
+  if ((int)threadIdx.x < rows) {
+    const float* src = stems + (int64_t)s * C * stem_stride + i0 + threadIdx.x;
+    Pcm24* row = reinterpret_cast<Pcm24*>(tile + shift) + threadIdx.x * C;
+    for (int c = 0; c < C; ++c) row[c] = S::encode(src[(int64_t)c * stem_stride]);
+  }
+  __syncthreads();
+  pcm24_move<false>(tile, shift, dst, rows * C * 3);
+}
+
 template <int N>
 static int launch_stft_n(dcs_stft* p, const float* d_audio, int64_t L, float2* d_X, float* d_mag, float* d_phase,
                          float mag_scale, int64_t ldf, int64_t T, cudaStream_t st) {
@@ -387,11 +457,15 @@ static void pcm_encode_channels_as(const float* d_stems, int64_t L, int nsrc, in
 int launch_pcm_decode_channels(dcs_ctx* ctx, int fmt, const void* d_in, int64_t L, int C, float* d_planes, cudaStream_t st) {
   if (L <= 0) return DCS_OK;
   DCS_REQUIRE(C >= 1 && C <= kPcmMaxChannels, "pcm_decode_channels: %d channels not in [1, %d]", C, kPcmMaxChannels);
-  DCS_REQUIRE(sample_bytes(fmt) > 0 && (uintptr_t)d_in % sample_bytes(fmt) == 0,
+  DCS_REQUIRE(sample_bytes(fmt) > 0 && (uintptr_t)d_in % sample_align(fmt) == 0,
               "pcm_decode_channels: format %d, or input not aligned to its samples", fmt);
   switch (fmt) {
     case DCS_SAMPLE_I16: pcm_decode_channels_as<DCS_SAMPLE_I16>(d_in, L, C, d_planes, st); break;
     case DCS_SAMPLE_I32: pcm_decode_channels_as<DCS_SAMPLE_I32>(d_in, L, C, d_planes, st); break;
+    case DCS_SAMPLE_I24:
+      pcm24_decode_channels_kernel<<<(unsigned)ceil_div64(L, kPcmEncodeRows), kPcmEncodeRows, 0, st>>>(
+          static_cast<const uint8_t*>(d_in), L, C, d_planes);
+      break;
     default: pcm_decode_channels_as<DCS_SAMPLE_F32>(d_in, L, C, d_planes, st); break;
   }
   DCS_CHECK_LAUNCH();
@@ -411,11 +485,15 @@ int launch_pcm_encode_channels(dcs_ctx* ctx, int fmt, const float* d_stems, int6
                                void* d_out, cudaStream_t st) {
   if (L <= 0) return DCS_OK;
   DCS_REQUIRE(C >= 1 && C <= kPcmMaxChannels, "pcm_encode_channels: %d channels not in [1, %d]", C, kPcmMaxChannels);
-  DCS_REQUIRE(sample_bytes(fmt) > 0 && (uintptr_t)d_out % sample_bytes(fmt) == 0,
+  DCS_REQUIRE(sample_bytes(fmt) > 0 && (uintptr_t)d_out % sample_align(fmt) == 0,
               "pcm_encode_channels: format %d, or output not aligned to its samples", fmt);
   switch (fmt) {
     case DCS_SAMPLE_I16: pcm_encode_channels_as<DCS_SAMPLE_I16>(d_stems, L, nsrc, C, stem_stride, d_out, st); break;
     case DCS_SAMPLE_I32: pcm_encode_channels_as<DCS_SAMPLE_I32>(d_stems, L, nsrc, C, stem_stride, d_out, st); break;
+    case DCS_SAMPLE_I24:
+      pcm24_encode_channels_kernel<<<dim3((unsigned)ceil_div64(L, kPcmEncodeRows), (unsigned)nsrc), kPcmEncodeRows, 0, st>>>(
+          d_stems, L, C, stem_stride, static_cast<uint8_t*>(d_out));
+      break;
     default: pcm_encode_channels_as<DCS_SAMPLE_F32>(d_stems, L, nsrc, C, stem_stride, d_out, st); break;
   }
   DCS_CHECK_LAUNCH();

@@ -218,9 +218,12 @@ def score_filters(ctx, melody, T, F, start=0, mag=None, ldf=None, stream=None):
 
 # every network was trained on spectra of 44.1 kHz audio; other rates go through a Resampler
 MODEL_RATE = 44100
+# packed signed 24-bit little-endian PCM, 3 bytes per sample: a clip [L, C] of it is what
+# np.memmap(path, dtype=PCM24, offset=data_offset, shape=(L, C)) gives for the data chunk of a 24-bit WAV
+PCM24 = np.dtype("V3")
 # the sample formats of separate_channels_batch: numpy dtype -> DCS_SAMPLE_* (include/dcs.h)
 _SAMPLE_FORMATS = {np.dtype(np.int16): _lib.SAMPLE_I16, np.dtype(np.int32): _lib.SAMPLE_I32,
-                   np.dtype(np.float32): _lib.SAMPLE_F32}
+                   np.dtype(np.float32): _lib.SAMPLE_F32, PCM24: _lib.SAMPLE_I24}
 # the sample rates a Resampler takes: integers in this range whose polyphase bank fits, in both directions
 RESAMPLE_RATES = (8000, 192000)
 # one segment of Separator.long_segments: the recording's samples staged, the range separated at 44.1 kHz, the core kept
@@ -679,8 +682,11 @@ class Separator(object):
         encode(separate_channels(decode(clip), wiener, wiener_radius, sample_rate)), with the rules of include/dcs.h:
         int16 decodes as clip / 32767 and encodes as (stem * 32767) truncated in fp32, wrapping; int32 decodes as
         (clip / (2^31 - 1)) in fp64 rounded to fp32 and encodes as stem * (2^31 - 1) in fp64, truncated and saturated;
-        float32 is taken and given back as it is, without scaling or clipping.  The conversions run on the device, fused
-        into the resamplers at another rate.  With int16 in and out, the bytes of separate_pcm16_channels_batch."""
+        float32 is taken and given back as it is, without scaling or clipping.  PCM24 (packed 3-byte samples, the bytes of
+        a 24-bit WAV data chunk, util.wav_samples) decodes as the int32 rule on the sample shifted left by 8 and encodes
+        as the int32 encode shifted right by 8: the same values as int32 for 24-bit material, with a quarter fewer
+        bytes over the host link.  The conversions run on the device, fused into the resamplers at another rate.  With
+        int16 in and out, the bytes of separate_pcm16_channels_batch."""
         ps, ch, args, sample_rate = self._channels_clips("separate_channels_batch", clips, tuple(_SAMPLE_FORMATS), wiener,
                                                          wiener_radius, sample_rate)
         dtypes = {p_.dtype for p_ in ps}
@@ -692,7 +698,7 @@ class Separator(object):
         except TypeError:
             raise ValueError("separate_channels_batch: out_dtype %r is not a dtype" % (out_dtype,))
         if out_dtype not in _SAMPLE_FORMATS:
-            raise ValueError("separate_channels_batch encodes int16, int32 or float32 stems, not %s" % out_dtype)
+            raise ValueError("separate_channels_batch encodes int16, int32, float32 or PCM24 (V3) stems, not %s" % out_dtype)
         if not ps:
             return []
         pre = (None, None)
@@ -734,7 +740,7 @@ class Separator(object):
     def separate_long_channels(self, recording, out=None, out_dtype=None, wiener=0, wiener_radius=0, sample_rate=MODEL_RATE,
                                segment_seconds=120.0):
         """One C-channel recording of any length through the multi-clip scheduler with a device workspace bounded by the
-        segment length (dcs_separate_long_channels_host): recording [L, C] of int16, int32 or float32, C in 1..16 ->
+        segment length (dcs_separate_long_channels_host): recording [L, C] of int16, int32, float32 or PCM24, C in 1..16 ->
         [nsrc, L, C] of out_dtype (default the recording's dtype), into `out` when given.  The recording is cut into
         cores of segment_seconds (long_segments); each segment is separated with the margins that make its core the
         whole recording's stems (up to the GEMMs' summation order for another patch count), and its core is written
@@ -750,7 +756,7 @@ class Separator(object):
         except TypeError:
             raise ValueError("separate_long_channels: out_dtype %r is not a dtype" % (out_dtype,))
         if out_dtype not in _SAMPLE_FORMATS:
-            raise ValueError("separate_long_channels encodes int16, int32 or float32 stems, not %s" % out_dtype)
+            raise ValueError("separate_long_channels encodes int16, int32, float32 or PCM24 (V3) stems, not %s" % out_dtype)
         L = x.shape[0]
         if out is None:
             out = np.empty((self.nsrc, L, ch), dtype=out_dtype)

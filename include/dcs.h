@@ -704,12 +704,18 @@ int dcs_downmix_f32(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_st
  *    only reproduces the reference's astype('int16'), and numpy's own int32 result past 2^31 depends on the platform.
  *  - DCS_SAMPLE_F32 (4 bytes): decode the sample itself, bit for bit (no scaling); encode y itself, bit for bit (no
  *    clipping, NaN payloads kept).  Non-finite input gives undefined stems and is not checked, as on every float entry.
- * The downmix is that of dcs_separate_audio_channels on the decoded planes in every format. */
-enum { DCS_SAMPLE_I16 = 0, DCS_SAMPLE_I32 = 1, DCS_SAMPLE_F32 = 2 };
+ *  - DCS_SAMPLE_I24 (3 bytes): packed signed 24-bit little-endian PCM, the samples of a WAV data chunk with a 3-byte
+ *    container.  With v the sign-extended 24-bit value, decode the DCS_SAMPLE_I32 decode of v * 256 (the bits the int32
+ *    route gives for scipy.io.wavfile's read of the same file); encode the DCS_SAMPLE_I32 encode of y shifted right by 8
+ *    bits (arithmetic), its low 3 bytes stored little-endian: the top 24 bits of the int32 stem, saturated to
+ *    [-2^23, 2^23 - 1], NaN gives 0, so the packed stems are the int32 stems shifted right by 8, byte for byte.  Buffers
+ *    of this format need only 1-byte alignment.
+ * The downmix is that of dcs_separate_audio_channels on the decoded planes in every format.  Code 3 is not a format. */
+enum { DCS_SAMPLE_I16 = 0, DCS_SAMPLE_I32 = 1, DCS_SAMPLE_F32 = 2, DCS_SAMPLE_I24 = 4 };
 /* C-channel clips (1 to 16 channels) in any sample format through the multi-clip scheduler: the clips in in_format, the
  * stems in out_format, chosen independently.  h_in[i]: [num_samples[i]][channels] samples of in_format (pinned for real
  * overlap) -> source s of clip i at h_out[i] + s*channels*out_strides[i] samples as [num_samples[i]][channels] of
- * out_format, interleaved: the layouts of dcs_separate_batch_pcm16_channels_host with each value 2 or 4 bytes wide.
+ * out_format, interleaved: the layouts of dcs_separate_batch_pcm16_channels_host with each value 2, 3 or 4 bytes wide.
  * to_model and from_model are both NULL (clips at 44.1 kHz) or both set (clips at another rate, the pair of
  * dcs_separate_batch_pcm16_channels_resampled_host, with its checks).  Per clip the stems are, byte for byte,
  *     encode_out(dcs_separate_audio_channels_wiener(decode_in(clip), iterations, radius))
@@ -717,12 +723,12 @@ enum { DCS_SAMPLE_I16 = 0, DCS_SAMPLE_I32 = 1, DCS_SAMPLE_F32 = 2 };
  * dcs_resample(to_model) of decode_in(clip), per channel.  With DCS_SAMPLE_I16 in and out these are the bytes of
  * dcs_separate_batch_pcm16_channels_host and dcs_separate_batch_pcm16_channels_resampled_host.
  * Launches per clip: those of dcs_separate_audio_channels(_wiener) on the clip at 44.1 kHz plus one, in every format.
- * At another rate, a 4-byte in_format stages each decode tile as fp32; where C channels then do not fit one tile next
+ * At another rate, a 3- or 4-byte in_format stages each decode tile as fp32; where C channels then do not fit one tile next
  * to the bank (C >= 11 at some rates, 192 kHz at C = 16 among them) the decode runs on equal channel groups and one
  * more launch forms the downmix plane, with the same bits.
  * Workspace: as for dcs_separate_batch_pcm16_channels_host (resampled_host at another rate) with the staging terms
  *       n B(b_in channels Lmax) + n B(b_out nsrc channels Lmax)
- * where b_in and b_out are the formats' bytes per sample (2 or 4).
+ * where b_in and b_out are the formats' bytes per sample (2, 3 or 4).
  * Synchronises before returning, also on an error.  Refused with DCS_EINVAL before anything is queued: an unknown
  * format code, exactly one resampler NULL, and what the two int16 C-channel batch entries refuse. */
 int dcs_separate_batch_channels_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* plan, const dcs_resampler* to_model,
@@ -734,7 +740,7 @@ int dcs_separate_batch_channels_host(dcs_ctx* ctx, dcs_model* model, dcs_stft* p
  * dcs_pcm16_decode / dcs_pcm16_encode (DCS_PCM16_CHANNELS) in any format, with the same arguments and checks.  Each is
  * one launch of the kernel the batch runs (two for a resampled decode whose channels take groups), on caller device
  * buffers, on `stream`, which is synchronised before returning; every argument is checked before anything is queued.
- * 4-byte formats need 4-byte-aligned d_in / d_out.
+ * 4-byte formats need 4-byte-aligned d_in / d_out; DCS_SAMPLE_I24 takes any address.
  * dcs_channels_decode: d_in [num_samples][channels] of `format` -> d_out float [channels + 1][num_out], plane 0 the
  *  downmix, plane 1 + c the decode of channel c; with a resampler, dcs_resample of it and num_out in
  *  [1, dcs_resampled_length(num_samples)].
