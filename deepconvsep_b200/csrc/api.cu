@@ -468,6 +468,21 @@ static int separate_clip(dcs_ctx* ctx, const dcs_model* m, dcs_stft* p, const fl
     in = chans;
   }
   if (masks) return run_network(ctx, m, in, plane, nullptr, 0, T, ldf, overlap, patcher, nullptr, stem_stride, st, d_stems);
+  if (m->arch == DCS_ARCH_DSD && nch == 1 && istft_reg_supported(p, d_stems, stem_stride)) {
+    // the mono DSD100 / HHDS net: the network writes its masks (float planes, in the spectra's allocation) and the
+    // register iSTFT forms M_s * X as it reads each row, X shared by the four sources -- the same products the mask
+    // kernel's spectra mode stores, so the same stems, with no masked spectra in memory.  A spectrum tap gets them
+    // from one elementwise pass
+    float* M = reinterpret_cast<float*>(S);
+    DCS_TRY(run_network(ctx, m, in, plane, X, plane, T, ldf, overlap, patcher, nullptr, plane, st, M));
+    if (ctx->tap) {
+      DCS_REQUIRE(ctx->tap_cap >= (int64_t)m->nsrc * plane, "spectrum tap holds %lld elements, this call produced %lld",
+                  (long long)ctx->tap_cap, (long long)m->nsrc * plane);
+      DCS_TRY(launch_masked_spectra(ctx, M, X, m->nsrc, plane, ldf, m->F, ctx->tap, st));
+    }
+    ProfScope ps(ctx, "istft_ola", st);
+    return launch_istft(p, X, nullptr, nullptr, 1.f, m->nsrc, T, ldf, plane, d_stems, L, stem_stride, st, M, plane, 1);
+  }
   DCS_TRY(run_network(ctx, m, in, plane, X, plane, T, ldf, overlap, patcher, S, plane, st));
   if (ctx->wiener_iters > 0 && nch == 2)
     DCS_TRY(launch_wiener(ctx, X, plane, S, plane, m->nsrc, T, ldf, m->F, ctx->wiener_iters, ctx->wiener_radius, st));

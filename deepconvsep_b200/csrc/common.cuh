@@ -208,6 +208,10 @@ int launch_istft(dcs_stft* plan, const float2* d_S, const float* d_mag, const fl
                  int64_t Lout, int64_t out_stride, cudaStream_t st, const float* d_M = nullptr, int64_t m_stride = 0,
                  int nx = 1);
 
+// nsrc mask planes M (plane floats apart) times the one mixture STFT plane X -> nsrc complex planes S, bins >= F zeroed
+int launch_masked_spectra(dcs_ctx* ctx, const float* d_M, const float2* d_X, int nsrc, int64_t plane, int64_t ldf, int F,
+                          float2* d_S, cudaStream_t st);
+
 int launch_stft_reg(dcs_stft* plan, const float* d_audio, int64_t L, float2* d_X, float* d_mag, float* d_phase,
                     float mag_scale, int64_t ldf, int64_t nframes, cudaStream_t st);
 bool istft_reg_supported(const dcs_stft* plan, const float* d_out, int64_t out_stride);

@@ -473,6 +473,32 @@ int launch_pcm_decode_channels(dcs_ctx* ctx, int fmt, const void* d_in, int64_t 
   return DCS_OK;
 }
 
+// the masked spectra of the stems-from-masks route, for the spectrum tap: S[s][t][f] = M_s[t][f] * X[t][f] componentwise
+// (the lone rounded products the masked inverse STFT forms) for f < F, 0 in the pad columns
+__global__ void masked_spectra_kernel(const float* __restrict__ M, const float2* __restrict__ X, int64_t plane, int64_t ldf, int F,
+                                      int64_t n, float2* __restrict__ S) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int64_t e = i % plane, f = e % ldf;
+  if (f < F) {
+    const float m = M[i];
+    const float2 x = X[e];
+    S[i] = make_float2(__fmul_rn(m, x.x), __fmul_rn(m, x.y));
+  } else {
+    S[i] = make_float2(0.f, 0.f);
+  }
+}
+
+int launch_masked_spectra(dcs_ctx* ctx, const float* d_M, const float2* d_X, int nsrc, int64_t plane, int64_t ldf, int F,
+                          float2* d_S, cudaStream_t st) {
+  const int64_t n = (int64_t)nsrc * plane;
+  if (n <= 0) return DCS_OK;
+  masked_spectra_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, st>>>(d_M, d_X, plane, ldf, F, n, d_S);
+  DCS_CHECK_LAUNCH();
+  ctx->launches++;
+  return DCS_OK;
+}
+
 int launch_downmix(dcs_ctx* ctx, const float* d_audio, int nx, int64_t audio_stride, int64_t L, float* d_mono, cudaStream_t st) {
   if (L <= 0) return DCS_OK;
   downmix_kernel<<<(unsigned)ceil_div64(L, 256), 256, 0, st>>>(d_audio, nx, audio_stride, L, d_mono);

@@ -11,9 +11,12 @@
 //     after frame n is added, the oldest hop is complete -> divided by sum(win*syn_win), stored
 //     coalesced, and the window shifts.  No shared accumulator, no atomics: the summation order
 //     is the reference's (ascending frame index) and the result is run-to-run deterministic.
-//     N/hop - 1 halo frames are recomputed at the start of each span.
+//     N/hop - 1 halo frames are recomputed at the start of each span.  Spectrum (and mask) rows reach shared memory
+//     through 2-stage rings filled by bulk async copies on mbarriers, the fetch of frame n+1 in flight while the
+//     group waits for frame n; the masked variant shares one X ring among the groups of all sources of a channel.
 #include "common.cuh"
 #include "fft_reg.cuh"
+#include "tc.cuh"
 
 namespace dcs {
 
@@ -105,33 +108,63 @@ stft_reg_kernel(const float* __restrict__ audio, int64_t L, int hop, const float
   }
 }
 
-// The body of K4 and of its masked variant (MASKED: the spectrum is M_s * X_c, formed as the row is read).  Not masked:
-// group gi owns hops of plane gi / groups_per_src of S.  Masked: S is the mixture STFT (channel c at S + c * src_stride),
-// Mk the masks (source s at Mk + s * m_stride, same ldf), output plane s * nx + c; the source is the fastest-varying part
-// of gi, so the nsrc groups that walk the same frames of one channel are neighbours (same CTA, same wave) and their X
-// rows meet in L2 -- an ordering, not a guarantee.
+// Shared memory of K4 (bytes): per group its FFT scratch, the twiddle tables and the synthesis window, the spectrum
+// row rings (RING stages of ROWP float2 per quad), masked also a mask row ring per group (RING stages of ROWP floats),
+// then the ring barriers (full / empty per quad and stage, masked a full barrier per group and stage).
+constexpr int ISTFT_RING = 2;
+constexpr size_t SM90_SMEM_OPTIN = 232448;   // shared memory a CTA may opt into on sm_90
+template <int T>
+__host__ __device__ constexpr int istft_rowp() { return (32 * T + 1 + 7) / 8 * 8; }
+template <int T>
+__host__ __device__ constexpr size_t istft_smem_bytes(int qpc, bool masked) {
+  constexpr int GPC = ISTFT_THREADS / T, ROWP = istft_rowp<T>();
+  return ((size_t)GPC * FftGroup<T>::SCRATCH + 3 * (size_t)(32 * T) + (size_t)qpc * ISTFT_RING * ROWP) * sizeof(float2) +
+         (masked ? (size_t)GPC * ISTFT_RING * ROWP * sizeof(float) : 0) +
+         ((size_t)qpc * 2 * ISTFT_RING + (masked ? (size_t)GPC * ISTFT_RING : 0)) * sizeof(uint64_t);
+}
+
+// The body of K4 and of its masked variant (MASKED: the spectrum is M_s * X_c, formed as the row is read).
+//
+// Groups are gathered in QUADS of qw neighbouring groups that walk the same frames (qpc quads per CTA, groups past
+// qpc * qw idle: they run the loop on zeros so that every warp reaches the same __syncwarp()s, and store nothing).
+// A quad shares one spectrum row ring in shared memory: one elected lane fetches each row with a bulk async copy that
+// completes on the stage's `full` mbarrier, and every group of the quad arrives on the stage's `empty` mbarrier once it
+// has read the row into registers.  The fetch of frame n+1 is issued at the top of iteration n, before the wait for
+// frame n: two rows per quad in flight while the SM waits on HBM.
+//   Not masked: qw = 1, a quad is one group and owns hops of plane quad / groups_per_src of S.
+//   Masked: S is the mixture STFT (channel c at S + c * src_stride), Mk the masks (source s at Mk + s * m_stride, same
+//   ldf), output plane s * nx + c.  The qw groups of a quad apply the masks of qw consecutive sources (one chunk of the
+//   nsrc sources, ceil(nsrc / qw) chunks) to the same X rows; each group's mask rows go through a ring of its own the
+//   same way (it is their only reader, so no empty barrier).  X is read from HBM once per quad instead of once per group.
 template <int T, int HS, bool MASKED>  // HS = hop / 64: window slots (32 float2 each) per hop
 __device__ __forceinline__ void
 istft_reg_body(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int64_t src_stride,
                const float* __restrict__ wsyn, const float* __restrict__ w2, const float2* __restrict__ tw,
                float* __restrict__ out, int64_t Lout, int64_t out_stride, int hops_per_group, int64_t num_hops,
-               int64_t groups_per_src, int64_t total_groups, const float* __restrict__ Mk, int64_t m_stride, int nsrc,
-               int nx) {
+               int64_t groups_per_src, int64_t total_quads, const float* __restrict__ Mk, int64_t m_stride, int nsrc,
+               int nx, int qw, int qpc) {
   using G = FftGroup<T>;
   constexpr int N2 = G::N2, N = 2 * N2, hop = 64 * HS, R = N / hop, C0 = (N / 2) / hop, GPC = ISTFT_THREADS / T;
+  constexpr int ROWP = istft_rowp<T>();               // float2 per staged row
+  constexpr uint32_t XBYTES = (N2 + 2) / 2 * 16;      // 16-byte pieces covering bins 0..N2
+  constexpr uint32_t MBYTES = (N2 + 4) / 4 * 16;      // masked: 16-byte pieces covering bins 0..N2 of a mask row
   extern __shared__ __align__(16) float2 scratch[];
   const int tid = threadIdx.x, b = tid % T, gl = tid / T;
   float2* scr = scratch + gl * G::SCRATCH;
-  int64_t gi = (int64_t)blockIdx.x * GPC + gl;
-  const bool active = gi < total_groups;
-  if (!active) gi = total_groups - 1;  // keeps the warp convergent; nothing is stored
+  const int qi = gl / qw, mem = gl - qi * qw;          // quad, member
+  const bool in_quad = qi < qpc;
+  int64_t gq = (int64_t)blockIdx.x * qpc + (in_quad ? qi : 0);
+  bool active = in_quad && gq < total_quads;
+  if (gq >= total_quads) gq = total_quads - 1;         // keeps the quad's barriers and the warp convergent; nothing is stored
   int msrc = 0;   // masked: the source whose mask this group applies
   if constexpr (MASKED) {
-    msrc = (int)(gi % nsrc);
-    gi /= nsrc;
+    const int nchunk = (nsrc + qw - 1) / qw;
+    msrc = (int)(gq % nchunk) * qw + mem;
+    gq /= nchunk;
+    if (msrc >= nsrc) { active = false; msrc = nsrc - 1; }
   }
-  const int src = (int)(gi / groups_per_src);   // plane of S (masked: the channel)
-  const int64_t h0 = (gi % groups_per_src) * hops_per_group;
+  const int src = (int)(gq / groups_per_src);   // plane of S (masked: the channel)
+  const int64_t h0 = (gq % groups_per_src) * hops_per_group;
   const float inv_n2 = 1.0f / (float)N2;
   float2 acc[32];
 #pragma unroll
@@ -154,45 +187,67 @@ istft_reg_body(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int64
       cinv[q * HS + kb] = make_float2(c0 == 0.f ? 1.f : 1.f / c0, c1 == 0.f ? 1.f : 1.f / c1);
     }
 
-  // The spectrum row of the NEXT frame is fetched into shared memory with cp.async while the
-  // current frame is transformed and overlap-added: HBM latency is off the critical path.
-  constexpr int ROWP = (N2 + 1 + 7) / 8 * 8;          // float2 per staged row
-  constexpr int CHUNKS = (N2 + 2) / 2;                // 16-byte pieces covering bins 0..N2
-  float2* srow = scratch + GPC * G::SCRATCH + gl * ROWP;
   // shared copies of the twiddle table (N entries, exp(-2 pi i j / N)) and of the synthesis window (as pairs)
-  float2* stw = scratch + GPC * (G::SCRATCH + ROWP);   // tw[0..N2): the real-FFT merge twiddles
+  float2* stw = scratch + GPC * G::SCRATCH;             // tw[0..N2): the real-FFT merge twiddles
   float2* stw2 = stw + N2;                              // inter-stage twiddles, lane-contiguous (FftGroup::fill_tw2)
   float2* swsyn = stw2 + N2;
-  // masked: the group's mask row, ROWP floats, staged like the spectrum row in 16-byte pieces covering bins 0..N2
-  constexpr int MCHUNKS = (N2 + 4) / 4;
-  float* smrow = reinterpret_cast<float*>(swsyn + N2) + gl * ROWP;
+  float2* xring = swsyn + N2 + (in_quad ? qi : 0) * ISTFT_RING * ROWP;            // this quad's spectrum rows
+  float* mring = reinterpret_cast<float*>(swsyn + N2 + qpc * ISTFT_RING * ROWP) + gl * ISTFT_RING * ROWP;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<float*>(swsyn + N2 + qpc * ISTFT_RING * ROWP) +
+                                               (MASKED ? GPC * ISTFT_RING * ROWP : 0));
+  uint64_t* xfull = bars + (in_quad ? qi : 0) * 2 * ISTFT_RING;   // [stage]: the row landed
+  uint64_t* xempty = xfull + ISTFT_RING;                           // [stage]: every group of the quad has read it
+  uint64_t* mfull = bars + qpc * 2 * ISTFT_RING + gl * ISTFT_RING;
   for (int i = tid; i < N2; i += ISTFT_THREADS) stw[i] = __ldg(tw + i);
   G::fill_tw2(stw2, tw, tid, ISTFT_THREADS);
   for (int i = tid; i < N2; i += ISTFT_THREADS) swsyn[i] = __ldg(reinterpret_cast<const float2*>(wsyn) + i);
+  if (tid < qpc * ISTFT_RING) {
+    tc::mbar_init(bars + (tid / ISTFT_RING) * 2 * ISTFT_RING + tid % ISTFT_RING, 1);
+    tc::mbar_init(bars + (tid / ISTFT_RING) * 2 * ISTFT_RING + ISTFT_RING + tid % ISTFT_RING, (uint32_t)qw);
+  }
+  if (MASKED && tid < GPC * ISTFT_RING) tc::mbar_init(bars + qpc * 2 * ISTFT_RING + tid, 1);
+  tc::fence_barrier_init();
   __syncthreads();
-  auto prefetch = [&](int64_t nn) {
-    if (nn >= 0 && nn < nframes) {
-      const float2* rowp = S + (int64_t)src * src_stride + nn * ldf;
-      for (int c = b; c < CHUNKS; c += T) {
-        const uint32_t dst = (uint32_t)__cvta_generic_to_shared(srow + 2 * c);
-        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(rowp + 2 * c) : "memory");
-      }
-      if constexpr (MASKED) {
-        const float* mrowp = Mk + (int64_t)msrc * m_stride + nn * ldf;
-        for (int c = b; c < MCHUNKS; c += T) {
-          const uint32_t dst = (uint32_t)__cvta_generic_to_shared(smrow + 4 * c);
-          asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(mrowp + 4 * c) : "memory");
-        }
-      }
-    }
-    asm volatile("cp.async.commit_group;" ::: "memory");
-  };
+  const bool xlane = in_quad && mem == 0 && b == 0;   // the quad's producer lane
+  const bool glane = in_quad && b == 0;               // the group's lane for its mask rows and its empty arrivals
   const int64_t n_first = h0 + C0 - R + 1, n_last = h0 + hops_per_group - 1 + C0;
-  prefetch(n_first);
+  // frame n into stage (n - n_first) % RING; frames outside the clip complete their stage with no bytes
+  auto fetch_x = [&](int64_t nn) {
+    const int k = (int)(nn - n_first), st = k % ISTFT_RING;
+    if (k >= ISTFT_RING)   // the stage held frame nn - RING: wait until every group of the quad has read it
+      tc::mbar_wait_relaxed(xempty + st, (uint32_t)((k / ISTFT_RING - 1) & 1));
+    if (nn >= 0 && nn < nframes) {
+      tc::mbar_arrive_expect_tx(xfull + st, XBYTES);
+      tc::bulk_copy_g2s(xring + st * ROWP, S + (int64_t)src * src_stride + nn * ldf, XBYTES, xfull + st);
+    } else {
+      tc::mbar_arrive(xfull + st);
+    }
+  };
+  auto fetch_m = [&](int64_t nn) {
+    const int st = (int)(nn - n_first) % ISTFT_RING;
+    if (nn >= 0 && nn < nframes) {
+      tc::mbar_arrive_expect_tx(mfull + st, MBYTES);
+      tc::bulk_copy_g2s(mring + st * ROWP, Mk + (int64_t)msrc * m_stride + nn * ldf, MBYTES, mfull + st);
+    } else {
+      tc::mbar_arrive(mfull + st);
+    }
+  };
+  if (xlane) fetch_x(n_first);
+  if (MASKED && glane) fetch_m(n_first);
   for (int64_t n = n_first; n <= n_last; ++n) {
-    const bool fvalid = n >= 0 && n < nframes;
-    asm volatile("cp.async.wait_group 0;" ::: "memory");
-    __syncwarp();
+    const bool fvalid = in_quad && n >= 0 && n < nframes;
+    const int k = (int)(n - n_first), st = k % ISTFT_RING;
+    const uint32_t par = (uint32_t)((k / ISTFT_RING) & 1);
+    if (n < n_last) {   // frame n+1 goes in flight before this one is waited for
+      if (xlane) fetch_x(n + 1);
+      if (MASKED && glane) fetch_m(n + 1);
+    }
+    const float2* srow = xring + st * ROWP;
+    const float* smrow = mring + st * ROWP;
+    if (in_quad) {
+      tc::mbar_wait(xfull + st, par);
+      if constexpr (MASKED) tc::mbar_wait(mfull + st, par);
+    }
     float2 v[32];
 #pragma unroll
     for (int a = 0; a < 32; ++a) {
@@ -211,7 +266,7 @@ istft_reg_body(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int64
       v[a] = real_pre_conj(xk, xn, stw[idx]);
     }
     __syncwarp();                    // every lane has consumed the row
-    if (n < n_last) prefetch(n + 1);
+    if (glane) tc::mbar_arrive(xempty + st);
     G::template forward<true>(v, scr, stw2, b);
     // z = conj(V)/N2: samples 2n', 2n'+1 of the frame, n' = (b + T q) + 32 kb  <->  v[q*T + kb]
 #pragma unroll
@@ -274,19 +329,20 @@ istft_reg_kernel(const float2* __restrict__ S, int64_t nframes, int64_t ldf, int
                  float* __restrict__ out, int64_t Lout, int64_t out_stride, int hops_per_group, int64_t num_hops,
                  int64_t groups_per_src, int64_t total_groups) {
   istft_reg_body<T, HS, false>(S, nframes, ldf, src_stride, wsyn, w2, tw, out, Lout, out_stride, hops_per_group, num_hops,
-                               groups_per_src, total_groups, nullptr, 0, 1, 1);
+                               groups_per_src, total_groups, nullptr, 0, 1, 1, 1, ISTFT_THREADS / T);
 }
 
-// K4 on M_s * X_c: X complex [nx][nframes][ldf] (x_plane apart), Mk float [nsrc][nframes][ldf] (m_stride apart)
+// K4 on M_s * X_c: X complex [nx][nframes][ldf] (x_plane apart), Mk float [nsrc][nframes][ldf] (m_stride apart); quads
+// of qw groups, qpc of them per CTA
 template <int T, int HS>
 __global__ void __launch_bounds__(ISTFT_THREADS, 1)
 istft_masked_reg_kernel(const float2* __restrict__ X, int64_t nframes, int64_t ldf, int64_t x_plane,
                         const float* __restrict__ Mk, int64_t m_stride, int nsrc, int nx, const float* __restrict__ wsyn,
                         const float* __restrict__ w2, const float2* __restrict__ tw, float* __restrict__ out, int64_t Lout,
                         int64_t out_stride, int hops_per_group, int64_t num_hops, int64_t groups_per_plane,
-                        int64_t total_groups) {
+                        int64_t total_quads, int qw, int qpc) {
   istft_reg_body<T, HS, true>(X, nframes, ldf, x_plane, wsyn, w2, tw, out, Lout, out_stride, hops_per_group, num_hops,
-                              groups_per_plane, total_groups, Mk, m_stride, nsrc, nx);
+                              groups_per_plane, total_quads, Mk, m_stride, nsrc, nx, qw, qpc);
 }
 
 int launch_stft_reg(dcs_stft* p, const float* d_audio, int64_t L, float2* d_X, float* d_mag, float* d_phase,
@@ -327,7 +383,6 @@ template <int T, int HS>
 static int launch_istft_reg_t(dcs_stft* p, const float2* d_S, int nsrc, int64_t nframes, int64_t ldf, int64_t src_stride,
                               float* d_out, int64_t Lout, int64_t out_stride, cudaStream_t st, const float* d_M = nullptr,
                               int64_t m_stride = 0, int nx = 1) {
-  using G = FftGroup<T>;
   constexpr int GPC = ISTFT_THREADS / T;
   const int hop = 64 * HS;
   const int64_t num_hops = ceil_div64(Lout, hop);
@@ -339,17 +394,23 @@ static int launch_istft_reg_t(dcs_stft* p, const float2* d_S, int nsrc, int64_t 
   if (hpg < 12) hpg = 12;
   if (hpg > 64) hpg = 64;
   const int64_t groups_per_src = ceil_div64(num_hops, hpg);
-  const int64_t total = groups_per_src * nplanes;
-  const unsigned grid = (unsigned)ceil_div64(total, GPC);
-  constexpr int ROWP = (G::N2 + 1 + 7) / 8 * 8;
-  const size_t smem = ((size_t)GPC * (G::SCRATCH + ROWP) + 2 * G::N2 + G::N2) * sizeof(float2);   // + twiddles + window
   if (d_M) {
-    const size_t smem_m = smem + (size_t)GPC * ROWP * sizeof(float);   // + a mask row per group: 191232 B (N = 2048), 181760 B (N = 1024)
-    DCS_TRY(ensure_smem_attr(istft_masked_reg_kernel<T, HS>, (int)smem_m));
-    istft_masked_reg_kernel<T, HS><<<grid, ISTFT_THREADS, smem_m, st>>>(
+    // quads of min(nsrc, GPC) groups share an X row ring; as many quads per CTA as fit next to the mask rings:
+    // nsrc = 4 at N = 2048 -> 2 quads, 191 KB; every group busy whenever qw divides GPC and the rings fit
+    const int qw = nsrc < GPC ? nsrc : GPC;
+    int qpc = GPC / qw;
+    while (qpc > 1 && istft_smem_bytes<T>(qpc, true) > SM90_SMEM_OPTIN) --qpc;
+    const int64_t quads = groups_per_src * nx * ((nsrc + qw - 1) / qw);
+    const unsigned grid = (unsigned)ceil_div64(quads, qpc);
+    const size_t smem = istft_smem_bytes<T>(qpc, true);   // 191 232 B + barriers at N = 2048, nsrc = 4
+    DCS_TRY(ensure_smem_attr(istft_masked_reg_kernel<T, HS>, (int)smem));
+    istft_masked_reg_kernel<T, HS><<<grid, ISTFT_THREADS, smem, st>>>(
         d_S, nframes, ldf, src_stride, d_M, m_stride, nsrc, nx, p->d_wsyn, p->d_w2, p->d_tw, d_out, Lout, out_stride,
-        (int)hpg, num_hops, groups_per_src, total);
+        (int)hpg, num_hops, groups_per_src, quads, qw, qpc);
   } else {
+    const int64_t total = groups_per_src * nplanes;
+    const unsigned grid = (unsigned)ceil_div64(total, GPC);
+    const size_t smem = istft_smem_bytes<T>(GPC, false);   // a 2-stage row ring per group: 224 KB (N = 2048)
     DCS_TRY(ensure_smem_attr(istft_reg_kernel<T, HS>, (int)smem));
     istft_reg_kernel<T, HS><<<grid, ISTFT_THREADS, smem, st>>>(
         d_S, nframes, ldf, src_stride, p->d_wsyn, p->d_w2, p->d_tw, d_out, Lout, out_stride, (int)hpg, num_hops,
