@@ -121,6 +121,68 @@ struct FftGroup {
     }
     __syncwarp();  // scratch may be reused by the caller
   }
+
+  // forward<true>() through half the scratch (HALF_SCRATCH float2: 16 rows of PITCH), the transpose in two rounds of
+  // 16 rows, so that a CTA fits more groups next to its row rings.  Every lane sends 16 values and receives 16 a round,
+  // which keeps 32 values live across the transpose as in forward().
+  //   T = 16: round r moves rows ka = 16 r + ka'; the output is forward()'s.
+  //   T = 32: lane i sends row ka' + 16 (hi(i) ^ r) in round r, hi(i) = bit 4 of i (two selects per float, no
+  //   dynamic register index), and lane b receives its 32 second-pass inputs rotated by 16 when hi(b).  A rotation by
+  //   N/2 of a DIF network's input negates its odd outputs exactly (the first stage's differences change sign, every
+  //   later operation is odd), so on return v[kb] is forward()'s value times -1 for odd kb on lanes with hi(b) -- the
+  //   same bits but for the sign of zero results.  The caller folds that sign into the constants it multiplies by.
+  static constexpr int HALF_SCRATCH = 16 * PITCH;
+  __device__ static __forceinline__ void forward_split(float2 (&v)[32], float2* scr, const float2* tw, int b) {
+    fft_dif<32>(v);
+    auto y = [&](int ka) { return ka > 0 ? cmul(v[brev(ka, 5)], tw[ka * T + b]) : v[0]; };
+    if (T == 32) {
+      const bool hi = (b & 16) != 0;
+      float2 later[16];   // the value each lane sends in round 1
+#pragma unroll
+      for (int a = 0; a < 16; ++a) {
+        const float2 lo = y(a), up = y(a + 16);
+        scr[a * PITCH + b] = hi ? up : lo;
+        later[a] = hi ? lo : up;
+      }
+      const float2* row = scr + (b & 15) * PITCH;
+      __syncwarp();
+#pragma unroll
+      for (int i = 0; i < 16; ++i) v[i] = row[(hi ? 16 : 0) + i];
+      __syncwarp();
+#pragma unroll
+      for (int a = 0; a < 16; ++a) scr[a * PITCH + b] = later[a];
+      __syncwarp();
+#pragma unroll
+      for (int i = 0; i < 16; ++i) v[16 + i] = row[(hi ? 0 : 16) + i];
+      fft_dif<32>(v);
+      float2 u[32];
+#pragma unroll
+      for (int kb = 0; kb < 32; ++kb) u[kb] = v[brev(kb, 5)];
+#pragma unroll
+      for (int kb = 0; kb < 32; ++kb) v[kb] = u[kb];
+    } else {
+      float2 u0[16], u1[16];
+#pragma unroll
+      for (int a = 0; a < 16; ++a) scr[a * PITCH + b] = y(a);
+      __syncwarp();
+#pragma unroll
+      for (int i = 0; i < 16; ++i) u0[i] = scr[b * PITCH + i];
+      __syncwarp();
+#pragma unroll
+      for (int a = 0; a < 16; ++a) scr[a * PITCH + b] = y(16 + a);
+      __syncwarp();
+#pragma unroll
+      for (int i = 0; i < 16; ++i) u1[i] = scr[b * PITCH + i];
+      fft_dif<16>(u0);
+      fft_dif<16>(u1);
+#pragma unroll
+      for (int kb = 0; kb < 16; ++kb) {
+        v[kb] = u0[brev(kb, 4)];
+        v[16 + kb] = u1[brev(kb, 4)];
+      }
+    }
+    __syncwarp();  // scratch may be reused by the caller
+  }
 };
 
 }  // namespace dcs
